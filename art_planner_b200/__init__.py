@@ -1,4 +1,4 @@
-"""art_planner_b200 -- B200-native (sm_100a CUDA) implementation of art_planner's batchable hot path:
+"""art_planner_b200 -- CUDA-native (sm_90a, H100) implementation of art_planner's batchable hot path:
 pose validity (ODE box-vs-heightfield torso/feet checks), edge validity over interpolated SE(3) states and
 edge cost, behind a C ABI (include/artp.h) and a host-side mirror of the reference's plugin interface."""
 from . import synth  # noqa: F401

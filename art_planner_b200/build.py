@@ -1,4 +1,4 @@
-"""Build libartp.so (hand-written sm_100a CUDA + the C ABI) in-tree with nvcc."""
+"""Build libartp.so (hand-written sm_90a CUDA + the C ABI) in-tree with nvcc."""
 from __future__ import annotations
 
 import os
@@ -13,7 +13,7 @@ SOURCES = [("artp_capi.cu", ["-fmad=false", "-Xcompiler", "-fPIC,-ffp-contract=o
            ("artp_cnn.cu", ["-Xcompiler", "-fPIC"])]
 HEADERS = ["artp_device.cuh", "artp_kernels.cuh", "artp_sampler.cuh", "artp_tiles.cuh", "artp_basic.cuh", "artp_cnn.h", os.path.join("..", "..", "include", "artp.h")]
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17"]
 
 
 def _stale() -> bool:
@@ -34,7 +34,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         cmd = [nvcc] + NVCC_FLAGS + extra + (["-Xptxas", "-v"] if verbose else []) + ["-c", "-o", obj, os.path.join(CSRC, src)]
         subprocess.run(cmd, check=True)
         objs.append(obj)
-    subprocess.run([nvcc, "-shared", "-o", LIB] + objs, check=True)
+    subprocess.run([nvcc, "-shared"] + NVCC_FLAGS[:2] + ["-o", LIB] + objs, check=True)
     return LIB
 
 

@@ -1,4 +1,4 @@
-// art_planner_b200/csrc/artp_capi.cu -- C ABI (include/artp.h) over the sm_100a kernels.
+// art_planner_b200/csrc/artp_capi.cu -- C ABI (include/artp.h) over the sm_90a kernels.
 // Host side mirrors the reference's checker objects: artp_create ~ StateValidityChecker ctor,
 // artp_set_map ~ setMap + updateHeightField (HeightMapBoxChecker::setHeightField,
 // art_planner/src/validity_checker/height_map_box_checker.cpp:38-54), artp_check_* ~ isValid / checkMotion.
@@ -687,7 +687,7 @@ int check_common(Handle* h, size_t n) {
 
 extern "C" {
 
-const char* artp_version(void) { return "artp 0.1 sm_100a"; }
+const char* artp_version(void) { return "artp 0.1 sm_90a"; }
 
 const char* artp_last_error(const artp_handle* hh) {
   if (!hh) return g_create_error.c_str();
@@ -723,7 +723,7 @@ int artp_create(const artp_params* params, artp_handle** out) {
   h->sm_count = prop.multiProcessorCount;
   cudaFuncAttributes fa;
   if ((e = cudaFuncGetAttributes(&fa, artp::box_tiles_warp_kernel)) != cudaSuccess)
-    return fail("no usable kernel image (built for sm_100a)", e);
+    return fail("no usable kernel image (built for sm_90a)", e);
   {
     // experiment switch ARTP_PIPE_TUNE: bit 0 = the call's own stream (classify) gets the highest priority, the box-stage
     // streams the lowest (measured: no effect); ARTP_PIPE_CAPS: see pipe_cap_g / pipe_cap_f
@@ -853,8 +853,8 @@ int artp_get_last_stage_timing(artp_handle* hh, float* ms5) {
 }
 
 // Pinned host memory for the adapter's staging buffers (the contiguous n x 7 state batch it gathers the OMPL states into,
-// the verdict bytes): cudaHostAlloc'd pages reach the device at PCIe line rate (measured 55 GB/s on the B200 boxes, where
-// memory pinned after the fact -- cudaHostRegister, torch's pin_memory -- reached 17-25 GB/s; profiles/pcie_probe.cu).
+// the verdict bytes): cudaHostAlloc'd pages are allocated pinned and portable, so the copies run as DMA at PCIe line
+// rate without a staging copy.
 void* artp_host_alloc(size_t bytes) {
   void* p = nullptr;
   if (bytes == 0 || cudaHostAlloc(&p, bytes, cudaHostAllocPortable) != cudaSuccess) return nullptr;
@@ -2119,8 +2119,6 @@ int artp_update_features(artp_handle* hh) {
   std::lock_guard<std::recursive_mutex> lk(h->mtx);
   if (!h->has_map) { h->err = "no map set"; return ARTP_E_NOMAP; }
   if (h->win_rows != h->rows) { h->err = "not available on a map window (artp_set_map_window)"; return ARTP_E_INVALID; }
-  artp_cnn::set_base_offset_mode(h->cnn, (h->cnn_mode & 2) ? 1 : 0);
-  artp_cnn::set_conv15_mode(h->cnn, (h->cnn_mode >> 2) & 3);
   return artp_cnn::update_features(h->cnn, h->d_H[0], h->rows, h->cols, h->pitch, h->chk.Lx / h->rows, h->chk.cx, h->chk.cy,
                                    h->stream, h->cnn_mode & 1, h->err);
 }
@@ -2181,7 +2179,9 @@ int artp_get_features(artp_handle* hh, float* out, size_t n_floats, int* hf, int
 
 int artp_set_cnn_mode(artp_handle* hh, int mode) {
   if (!hh) return ARTP_E_INVALID;
-  reinterpret_cast<Handle*>(hh)->cnn_mode = mode;
+  Handle* h = reinterpret_cast<Handle*>(hh);
+  if (mode & ~1) { h->err = "unknown motion-cost network mode (bit 0 is the only mode bit)"; return ARTP_E_INVALID; }
+  h->cnn_mode = mode;
   return ARTP_OK;
 }
 

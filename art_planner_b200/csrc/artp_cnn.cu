@@ -1,4 +1,4 @@
-// art_planner_b200/csrc/artp_cnn.cu -- the learned motion-cost network on sm_100a.
+// art_planner_b200/csrc/artp_cnn.cu -- the learned motion-cost network on sm_90a.
 //
 // Reference: art_planner_motion_cost/src/art_planner_motion_cost/predictor/network_light.py
 //   CNNpart :78-110  conv3x3(1->24)+BN, conv3x3(24->24)+BN+LReLU(0.3), maxpool 2/2, conv3x3(24->48)+BN+LReLU,
@@ -7,21 +7,20 @@
 //
 // Numerics: the reference evaluates in fp16; parity here is against the fp32 evaluation of the same module to 1e-4
 // relative, so everything accumulates in fp32 and the 15x15 convolution -- 83.6 % of the FLOPs, implicit GEMM
-// M = output pixels, N = 48, K = 225 taps x 48 channels -- runs on the 5th-gen tensor cores with an error-compensated
-// fp16 split (a = a_hi + a_lo, w = w_hi + w_lo; D += a_hi*w_hi + a_hi*w_lo + a_lo*w_hi, fp32 accumulate in TMEM),
-// which keeps ~22 mantissa bits per product.
+// M = output pixels, N = 48, K = 225 taps x 48 channels -- runs on the tensor cores (wgmma) with an error-compensated
+// fp16 split (a = a_hi + a_lo, w = w_hi + w_lo; D += a_hi*w_hi + a_hi*w_lo + a_lo*w_hi, fp32 accumulate in
+// registers), which keeps ~22 mantissa bits per product.
 //
-// Tensor-core kernel (conv_tc_kernel<KS,...>, described for the 15x15 layer): one CTA per 16(y) x 8(x) output tile
-// (UMMA M = 128, N = 48).
+// Tensor-core kernel (conv_wgmma_kernel<KS,...>, described for the 15x15 layer): one CTA per 16(y) x 8(x) output tile
+// (M = 128 = two warpgroups of m64 wgmma, N = 48).
 //   * The whole input halo brick [30 y][24 x][64 ch] (hi and lo, 92 KB each) is TMA-loaded ONCE into 128B-swizzled
-//     shared memory; pixels are 128-byte rows, image rows are 24 pixels = 3072 B = 3 swizzle atoms apart, so every one
-//     of the 225 taps is just a shifted view of the same brick: start address += (ky*24 + kx)*128 B, stride between
-//     8-pixel groups (SBO) = 3072 B. Measured on B200: the 128B swizzle XOR is applied on absolute shared-memory
-//     address bits, so the shifted (128 B-aligned, not 1024 B-aligned) start needs descriptor base_offset = 0
-//     (setting it to (shift & 7) double-swizzles; profiles/debug_conv15.py). No per-tap activation traffic.
-//   * Weights [tap][48][64] fp16 hi/lo stream through a 3-stage TMA ring (12 KB per tap).
-//   * Warp 0 = TMA producer, warp 1 = tcgen05.mma issuer (one elected lane), warps 2..5 = epilogue
-//     (tcgen05.ld -> +bias -> LeakyReLU -> fp32 NHWC feature map).
+//     shared memory; pixels are 128-byte rows, image rows are 24 pixels = 3 swizzle atoms apart, so every one of the
+//     225 taps is just a shifted view of the same brick. The A fragments are read from it with ldmatrix at the shifted
+//     pixel rows (swizzle applied in the address), so no per-tap activation traffic leaves shared memory.
+//   * Weights [tap][48][64] fp16 hi/lo stream through a 3-stage TMA ring (12 KB per tap) and are the wgmma B operand
+//     straight from shared memory (K-major, 128B swizzle descriptors).
+//   * Warp 8 = TMA producer; warps 0..7 = two MMA warpgroups, which also run the epilogue (+bias -> LeakyReLU -> fp32
+//     NHWC feature map) from their register accumulators.
 // Layers 2..5 (3x3) use the same kernel with an 18 x 16-pixel brick and 9 taps, writing either fp32 NHWC (before a
 // max-pool) or directly the next layer's fp16 hi/lo NHWC-64 input; layer 1 (Cin = 1) stays on CUDA cores.
 // A complete fp32 CUDA-core path (conv3x3_kernel, conv15_reference_kernel) is kept as the in-library cross-check.
@@ -161,7 +160,7 @@ __global__ void fold_conv_kernel(const float* __restrict__ w, const float* __res
 }
 
 // ------------------------------------------------------------------------------------------------
-// tcgen05 / TMA / mbarrier primitives (inline PTX, sm_100a)
+// wgmma / TMA / mbarrier primitives (inline PTX, sm_90a)
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -170,6 +169,9 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   asm volatile(
@@ -196,55 +198,59 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, u
       "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr));
 }
-__device__ __forceinline__ void tma_load_2d_mc(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(
-          smem_u32(dst)),
-      "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-// K-major, 128B-swizzled shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout).
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t sbo_bytes, uint32_t base_offset) {
+// K-major, 128B-swizzled shared-memory matrix descriptor of the B operand (sm_90 GMMA layout): 128-byte rows, 8-row
+// swizzle atoms 1024 B apart (SBO); the start address advances by 32 B per K = 16 step inside the atom.
+__device__ __forceinline__ uint64_t make_desc_b(uint32_t saddr) {
   uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);             // start address, bits [0,14)
-  d |= (uint64_t)1 << 16;                              // leading byte offset (unused for swizzled K-major), bits [16,30)
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;    // stride byte offset, bits [32,46)
-  d |= (uint64_t)1 << 46;                              // descriptor version 1 (sm_100), bits [46,48)
-  d |= (uint64_t)(base_offset & 7) << 49;              // matrix base offset, bits [49,52)
-  d |= (uint64_t)2 << 61;                              // layout type SWIZZLE_128B, bits [61,64)
+  d |= (uint64_t)((saddr >> 4) & 0x3FFF);     // start address, bits [0,14)
+  d |= (uint64_t)1 << 16;                      // leading byte offset (unused for swizzled K-major), bits [16,30)
+  d |= (uint64_t)(1024 >> 4) << 32;            // stride byte offset, bits [32,46)
+  d |= (uint64_t)1 << 62;                      // layout type SWIZZLE_128B, bits [62,64)
   return d;
 }
 
-constexpr int kTileY = 16, kTileX = 8;           // output tile (UMMA M = 128 = 16 groups of 8 pixels along x)
+// D[64 x N] += A[64 x 16] (registers, the mma.m16n8k16 A fragment per warp) * B[16 x N] (shared memory, K-major),
+// fp16 inputs, fp32 accumulators (thread holds N/2 of them).
+template <int N>
+__device__ __forceinline__ void wgmma_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t bdesc);
+template <>
+__device__ __forceinline__ void wgmma_rs<48>(float (&d)[24], const uint32_t (&a)[4], uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %29, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, "
+      "{%24, %25, %26, %27}, %28, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1)
+      : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_rs<32>(float (&d)[16], const uint32_t (&a)[4], uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "{%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1)
+      : "memory");
+}
+
+constexpr int kTileY = 16, kTileX = 8;           // output tile: M = 128 pixels = two warpgroups of 8 image rows x 8
 constexpr int kWStages = 3;
+constexpr int kConvThreads = 288;                // warps 0..7 = two MMA warpgroups (+ epilogue), warp 8 = TMA producer
 
 template <int KS, int NOUT>
 struct ConvCfg {
@@ -253,25 +259,21 @@ struct ConvCfg {
   static constexpr int kBrickBytes = kBrickY * kBrickX * 128;    // per split term
   static constexpr int kWStageBytes = 2 * NOUT * 128;            // hi + lo weight tile of one tap
   static constexpr int kSmem = 2 * kBrickBytes + kWStages * kWStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-  // instruction descriptor: D = f32 (bits [4,6) = 1), A = B = f16 (0), K-major both, N>>3 at [17,23), M>>4 at [24,29)
-  static constexpr uint32_t kIdesc = (1u << 4) | ((uint32_t)(NOUT >> 3) << 17) | ((128u >> 4) << 24);
+  static_assert(kSmem <= 227 * 1024, "conv tile does not fit the 227 KB of shared memory a block may use");
 };
 
-// Implicit-GEMM convolution on tcgen05 (see the file header). KS x KS taps, KSTEPS x 16 input channels multiplied
-// per tap (channels are stored padded to 64 = one 128-byte swizzle row per pixel), NOUT = UMMA N (multiple of 16),
-// NMAIN fp32 accumulators for the a_hi*w_hi products (tap t -> t % NMAIN) + 1 for the two correction terms.
+// Implicit-GEMM convolution on wgmma (see the file header). KS x KS taps, KSTEPS x 16 input channels multiplied per
+// tap (channels are stored padded to 64 = one 128-byte swizzle row per pixel), NOUT = wgmma N, NMAIN fp32 accumulators
+// for the a_hi*w_hi products (tap t -> t % NMAIN) + 1 for the two correction terms.
 // SPLIT_OUT: write the activation as fp16 hi/lo NHWC-64 (the next layer's TMA source) instead of fp32 NHWC.
-template <int KS, int KSTEPS, int NOUT, int NMAIN, bool SPLIT_OUT, int CLUSTER, int ISSUERS>
-__global__ void __launch_bounds__(192 + 32 * (ISSUERS - 1))
-conv_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_constant__ CUtensorMap map_alo,
-               const __grid_constant__ CUtensorMap map_whi, const __grid_constant__ CUtensorMap map_wlo,
-               const float* __restrict__ bias, float* __restrict__ out, __half* __restrict__ out_hi,
-               __half* __restrict__ out_lo, int OH, int OW, int cout, int use_base_offset) {
+template <int KS, int KSTEPS, int NOUT, int NMAIN, bool SPLIT_OUT>
+__global__ void __launch_bounds__(kConvThreads, 1)
+conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_constant__ CUtensorMap map_alo,
+                  const __grid_constant__ CUtensorMap map_whi, const __grid_constant__ CUtensorMap map_wlo,
+                  const float* __restrict__ bias, float* __restrict__ out, __half* __restrict__ out_hi,
+                  __half* __restrict__ out_lo, int OH, int OW, int cout) {
   using Cfg = ConvCfg<KS, NOUT>;
-  constexpr int kTaps = KS * KS;
-  constexpr int kAcc = NMAIN + ISSUERS;   // ISSUERS correction accumulators (one per MMA-issuing warp)
-  constexpr int kTmemCols = kAcc * 64 <= 64 ? 64 : (kAcc * 64 <= 128 ? 128 : (kAcc * 64 <= 256 ? 256 : 512));
-  static_assert(kAcc * 64 <= 512, "too many accumulators");
+  constexpr int kTaps = KS * KS, kNA = NOUT / 2;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   unsigned char* a_hi = smem;
@@ -280,33 +282,19 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_constan
   uint64_t* bars = reinterpret_cast<uint64_t*>(w_st + kWStages * Cfg::kWStageBytes);
   uint64_t* bar_brick = bars;                 // TMA -> MMA: activations landed
   uint64_t* bar_full = bars + 1;              // [kWStages] TMA -> MMA: weight tap landed
-  uint64_t* bar_empty = bars + 1 + kWStages;  // [kWStages] MMA -> TMA: stage consumed
-  uint64_t* bar_done = bars + 1 + 2 * kWStages;   // MMA -> epilogue: accumulators complete
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 + 2 * kWStages);
+  uint64_t* bar_empty = bars + 1 + kWStages;  // [kWStages] MMA -> TMA: stage consumed (one arrival per MMA warp)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int x0 = blockIdx.x * kTileX, y0 = blockIdx.y * kTileY;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     mbar_init(bar_brick, 1);
-    // CLUSTER = 2: the two CTAs of a pair each fetch half of every weight tile and multicast it to both, so a stage is
-    // free only when BOTH issuers have consumed it (two arrivals on each CTA's empty barrier).
-    for (int s = 0; s < kWStages; ++s) { mbar_init(bar_full + s, 1); mbar_init(bar_empty + s, CLUSTER); }
-    mbar_init(bar_done, ISSUERS);
+    for (int s = 0; s < kWStages; ++s) { mbar_init(bar_full + s, 1); mbar_init(bar_empty + s, 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {   // TMEM allocation: kAcc accumulators x 64 columns (NOUT used of each), one warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(kTmemCols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  if (CLUSTER > 1) cluster_sync_all();   // the peer's barriers are initialised before anything is multicast to it
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t crank = CLUSTER > 1 ? cluster_ctarank() : 0u;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       // activations: one box [64 ch][kBrickX x][kBrickY y] per split term (out-of-range pixels are zero-filled by TMA)
       mbar_expect_tx(bar_brick, 2 * Cfg::kBrickBytes);
@@ -317,284 +305,105 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_constan
         const int s = t % kWStages, round = t / kWStages;
         if (round > 0) mbar_wait(bar_empty + s, (round - 1) & 1);
         mbar_expect_tx(bar_full + s, Cfg::kWStageBytes);
-        if (CLUSTER == 1) {
-          tma_load_2d(w_st + s * Cfg::kWStageBytes, &map_whi, bar_full + s, 0, t * NOUT);
-          tma_load_2d(w_st + s * Cfg::kWStageBytes + NOUT * 128, &map_wlo, bar_full + s, 0, t * NOUT);
-        } else if (crank == 0) {   // rank 0 brings w_hi, rank 1 brings w_lo; each lands in both CTAs
-          tma_load_2d_mc(w_st + s * Cfg::kWStageBytes, &map_whi, bar_full + s, 0, t * NOUT, (uint16_t)3);
-        } else {
-          tma_load_2d_mc(w_st + s * Cfg::kWStageBytes + NOUT * 128, &map_wlo, bar_full + s, 0, t * NOUT, (uint16_t)3);
-        }
-      }
-    }
-  } else if (warp == 1 || (ISSUERS == 2 && warp == 6)) {
-    // MMA issuer(s). With ISSUERS == 2 the taps alternate between two issuing warps (own accumulators each), which
-    // overlaps the per-instruction issue latency of the small N = 48 MMAs.
-    if (lane == 0) {
-      const int me = (warp == 1) ? 0 : 1;
-      mbar_wait(bar_brick, 0);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t ahi = smem_u32(a_hi), alo = smem_u32(a_lo);
-      constexpr int kMainPer = NMAIN / ISSUERS;            // main accumulators per issuer
-      const uint32_t d_corr = tmem_base + (uint32_t)((NMAIN + me) * 64);
-      int mine = 0;
-      for (int t = me; t < kTaps; t += ISSUERS, ++mine) {
-        const int s = t % kWStages, round = t / kWStages;
-        mbar_wait(bar_full + s, round & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int ky = t / KS, kx = t % KS;
-        const uint32_t shift = (uint32_t)(ky * Cfg::kBrickX + kx);           // in pixels = 128-byte rows
-        const uint32_t bo = use_base_offset ? (shift & 7u) : 0u;
-        const uint32_t whi = smem_u32(w_st + s * Cfg::kWStageBytes), wlo = whi + NOUT * 128;
-        // The tensor core truncates when it adds into the fp32 accumulator, so a single accumulator would take
-        // thousands of biased roundings in the 15x15 layer (measured 4e-5 relative). Spread them: the a_hi*w_hi
-        // products go round-robin to NMAIN accumulators, both small correction terms to one more per issuer; the
-        // epilogue sums them in fp32 round-to-nearest.
-        const uint32_t d_main = tmem_base + (uint32_t)((me * kMainPer + (mine % kMainPer)) * 64);
-#pragma unroll
-        for (int j = 0; j < KSTEPS; ++j) {   // KSTEPS x UMMA_K(16) channels; pad channels beyond are never multiplied
-          const uint64_t dah = make_desc(ahi + shift * 128 + j * 32, Cfg::kBrickX * 128, bo);
-          const uint64_t dal = make_desc(alo + shift * 128 + j * 32, Cfg::kBrickX * 128, bo);
-          const uint64_t dwh = make_desc(whi + j * 32, 1024, 0);
-          const uint64_t dwl = make_desc(wlo + j * 32, 1024, 0);
-          umma_f16(d_main, dah, dwh, Cfg::kIdesc, (mine >= kMainPer || j != 0));
-          umma_f16(d_corr, dah, dwl, Cfg::kIdesc, (mine | j) != 0);
-          umma_f16(d_corr, dal, dwh, Cfg::kIdesc, 1);
-        }
-        if (CLUSTER == 1) umma_commit(bar_empty + s);   // frees the weight stage once these MMAs have read it
-        else umma_commit_mc(bar_empty + s, (uint16_t)3);
-      }
-      umma_commit(bar_done);   // bar_done counts ISSUERS arrivals
-    }
-  } else {
-    // epilogue: warp w owns TMEM lanes 32*(w%4) .. +31 = output pixels m = lane index; m = yl*8 + xl
-    mbar_wait(bar_done, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    const int oy = y0 + (m >> 3), ox = x0 + (m & 7);
-    float acc[NOUT];
-#pragma unroll
-    for (int n = 0; n < NOUT; ++n) acc[n] = 0.0f;
-#pragma unroll
-    for (int a = 0; a < kAcc; ++a) {
-      if (a < NMAIN && a >= kTaps) continue;   // accumulator never written (fewer taps than accumulators)
-#pragma unroll
-      for (int c = 0; c < NOUT / 16; ++c) {
-        uint32_t v[16];
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * 64 + c * 16);
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-            : "r"(taddr));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[16 * c + i] += __uint_as_float(v[i]);
-      }
-    }
-    if (oy < OH && ox < OW) {
-      const size_t pix = (size_t)oy * OW + ox;
-      if (SPLIT_OUT) {
-        __half2* ph = reinterpret_cast<__half2*>(out_hi + pix * 64);
-        __half2* pl = reinterpret_cast<__half2*>(out_lo + pix * 64);
-#pragma unroll
-        for (int n2 = 0; n2 < 32; ++n2) {
-          float f[2];
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int n = 2 * n2 + e;
-            float v = 0.0f;
-            if (n < NOUT && n < cout) { v = acc[n < NOUT ? n : 0] * (1.0f / kWScale) + __ldg(bias + n); v = v > 0.0f ? v : 0.3f * v; }
-            f[e] = v;
-          }
-          const __half h0 = __float2half_rn(f[0]), h1 = __float2half_rn(f[1]);
-          ph[n2] = __halves2half2(h0, h1);
-          pl[n2] = __halves2half2(__float2half_rn(f[0] - __half2float(h0)), __float2half_rn(f[1] - __half2float(h1)));
-        }
-      } else {
-        float* op = out + pix * cout;
-#pragma unroll
-        for (int n = 0; n < NOUT; ++n) {
-          if (n < cout) {
-            float f = acc[n] * (1.0f / kWScale) + __ldg(bias + n);
-            op[n] = f > 0.0f ? f : 0.3f * f;
-          }
-        }
-      }
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (CLUSTER > 1) cluster_sync_all();   // no CTA exits while its peer may still multicast into it / arrive on its barriers
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols));
-  }
-}
-
-// 15x15 layer, two-phase variant. The single-phase kernel keeps both activation bricks (a_hi, a_lo: 184 KB) resident,
-// which leaves room for only 3 weight stages: 36 KB in flight per SM against ~1.5 us of L2 latency = 24 GB/s per SM,
-// i.e. the 2.7 MB weight stream takes ~110 us while the MMAs need ~26 us (measured: 113 us; TMA multicast across a CTA
-// pair did not help -- the limit is in-flight bytes, not L2 bandwidth). Here only ONE brick is resident at a time:
-//   phase 1: a_hi brick; per tap a_hi*w_hi -> main accumulators, a_hi*w_lo -> correction accumulator (12 KB/tap)
-//   phase 2: the a_lo brick replaces it; per tap a_lo*w_hi -> correction accumulator (6 KB/tap, two taps per stage)
-// and the freed 92 KB become 8 more weight stages (11 x 12 KB in flight).
-constexpr int kW2Stages = 11;
-struct Conv15Cfg {
-  using B = ConvCfg<15, 48>;
-  static constexpr int kSmem = B::kBrickBytes + kW2Stages * B::kWStageBytes + 1024 + 256;
-};
-
-// NI MMA-issuing warps share the stages round-robin (stage g belongs to issuer g % NI): a single thread issues one
-// small (N = 48) tcgen05.mma about every 100 cycles regardless of the ring depth (measured: 113 us for 2025 MMAs with 1
-// issuer, 78 us with 2), so several issuers are needed to approach the 26 us the tensor pipe itself needs.
-template <int NI>
-__global__ void __launch_bounds__(192 + 32 * (NI - 1), 1)
-conv15_two_phase_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_constant__ CUtensorMap map_alo,
-                        const __grid_constant__ CUtensorMap map_whi, const __grid_constant__ CUtensorMap map_wlo,
-                        const float* __restrict__ bias, float* __restrict__ out, int OH, int OW) {
-  using Cfg = ConvCfg<15, 48>;
-  static_assert(2 * NI <= 8, "two TMEM accumulators (main + correction) of 64 columns per issuer");
-  constexpr int KS = 15, NOUT = 48, KSTEPS = 3, kTaps = 225, kAcc = 2 * NI;
-  constexpr int kTmemCols = kAcc * 64 <= 128 ? 128 : (kAcc * 64 <= 256 ? 256 : 512);
-  constexpr int kPairs = (kTaps + 1) / 2;
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  unsigned char* a_br = smem;
-  unsigned char* w_st = smem + Cfg::kBrickBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(w_st + kW2Stages * Cfg::kWStageBytes);
-  uint64_t* bar_brick = bars;                   // TMA -> MMA: brick landed (phase 0: a_hi, phase 1: a_lo)
-  uint64_t* bar_phase = bars + 1;               // MMA -> TMA: every issuer's phase-1 MMAs finished reading the a_hi brick
-  uint64_t* bar_done = bars + 2;                // MMA -> epilogue (NI arrivals)
-  uint64_t* bar_full = bars + 3;                // [kW2Stages]
-  uint64_t* bar_empty = bars + 3 + kW2Stages;   // [kW2Stages]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 + 2 * kW2Stages);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int x0 = blockIdx.x * kTileX, y0 = blockIdx.y * kTileY;
-  if (warp == 0 && lane == 0) {
-    mbar_init(bar_brick, 1); mbar_init(bar_phase, NI); mbar_init(bar_done, NI);
-    for (int s = 0; s < kW2Stages; ++s) { mbar_init(bar_full + s, 1); mbar_init(bar_empty + s, 1); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(kTmemCols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  const int issuer = (warp == 1) ? 0 : (warp >= 6 ? warp - 5 : -1);
-
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_expect_tx(bar_brick, Cfg::kBrickBytes);
-      tma_load_3d(a_br, &map_ahi, bar_brick, 0, x0, y0);
-      int g = 0;
-      for (int t = 0; t < kTaps; ++t, ++g) {                       // phase 1: w_hi + w_lo of one tap per stage
-        const int s = g % kW2Stages, round = g / kW2Stages;
-        if (round > 0) mbar_wait(bar_empty + s, (round - 1) & 1);
-        mbar_expect_tx(bar_full + s, Cfg::kWStageBytes);
         tma_load_2d(w_st + s * Cfg::kWStageBytes, &map_whi, bar_full + s, 0, t * NOUT);
         tma_load_2d(w_st + s * Cfg::kWStageBytes + NOUT * 128, &map_wlo, bar_full + s, 0, t * NOUT);
       }
-      mbar_wait(bar_phase, 0);                                     // a_hi brick no longer read
-      mbar_expect_tx(bar_brick, Cfg::kBrickBytes);
-      tma_load_3d(a_br, &map_alo, bar_brick, 0, x0, y0);
-      for (int u = 0; u < kPairs; ++u, ++g) {                      // phase 2: w_hi of two taps per stage
-        const int s = g % kW2Stages, round = g / kW2Stages;
-        if (round > 0) mbar_wait(bar_empty + s, (round - 1) & 1);
-        const int t0 = 2 * u, t1 = 2 * u + 1;
-        mbar_expect_tx(bar_full + s, (t1 < kTaps ? 2 : 1) * NOUT * 128);
-        tma_load_2d(w_st + s * Cfg::kWStageBytes, &map_whi, bar_full + s, 0, t0 * NOUT);
-        if (t1 < kTaps) tma_load_2d(w_st + s * Cfg::kWStageBytes + NOUT * 128, &map_whi, bar_full + s, 0, t1 * NOUT);
-      }
     }
-  } else if (issuer >= 0) {
-    if (lane == 0) {
-      const uint32_t abr = smem_u32(a_br);
-      const uint32_t d_main = tmem_base + (uint32_t)(issuer * 128), d_corr = d_main + 64u;
-      mbar_wait(bar_brick, 0);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      bool first = true;
-      for (int g = issuer; g < kTaps; g += NI) {                   // phase 1: g == tap
-        const int s = g % kW2Stages, round = g / kW2Stages, t = g;
-        mbar_wait(bar_full + s, round & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t shift = (uint32_t)((t / KS) * Cfg::kBrickX + (t % KS));
-        const uint32_t whi = smem_u32(w_st + s * Cfg::kWStageBytes), wlo = whi + NOUT * 128;
+    return;   // the MMA warps wait for every stage this warp filled, so the CTA outlives its copies
+  }
+
+  // Warpgroup g owns output pixels m = 64g .. 64g+63 (m = yl*8 + xl); warp q of it the 16 rows 16q .. 16q+15, i.e. image
+  // rows yl = 8g + 2q (+1). ldmatrix.x4 lane l addresses row (l & 7) of 8x8 matrix l >> 3: matrices 0/1 = rows 0-7 / 8-15
+  // at channels 0-7 of the K step, matrices 2/3 the same rows at channels 8-15.
+  const int g = warp >> 2, q = warp & 3;
+  const int mi = lane >> 3;
+  const int yl = 8 * g + 2 * q + (mi & 1), xl = lane & 7, kc = mi >> 1;
+  const uint32_t ahi = smem_u32(a_hi), alo = smem_u32(a_lo);
+  float acc[NMAIN][kNA], corr[kNA];
+#pragma unroll
+  for (int i = 0; i < kNA; ++i) {
+    corr[i] = 0.0f;
+#pragma unroll
+    for (int a = 0; a < NMAIN; ++a) acc[a][i] = 0.0f;
+  }
+  mbar_wait(bar_brick, 0);
+  for (int t0 = 0; t0 < kTaps; t0 += NMAIN) {
+#pragma unroll
+    for (int u = 0; u < NMAIN; ++u) {
+      const int t = t0 + u;
+      if (t < kTaps) {
+        const int s = t % kWStages;
+        mbar_wait(bar_full + s, (t / kWStages) & 1);
+        // every tap is a shifted view of the brick: pixel (yl + ky, xl + kx); the 128B swizzle permutes the 16-byte
+        // chunks of a pixel row by (row index & 7), the brick being 1024-byte aligned
+        const uint32_t p = (uint32_t)((yl + t / KS) * Cfg::kBrickX + xl + t % KS);
+        uint32_t ah[KSTEPS][4], al[KSTEPS][4];
 #pragma unroll
         for (int j = 0; j < KSTEPS; ++j) {
-          const uint64_t da = make_desc(abr + shift * 128 + j * 32, Cfg::kBrickX * 128, 0);
-          umma_f16(d_main, da, make_desc(whi + j * 32, 1024, 0), Cfg::kIdesc, !(first && j == 0));
-          umma_f16(d_corr, da, make_desc(wlo + j * 32, 1024, 0), Cfg::kIdesc, !(first && j == 0));
+          const uint32_t off = p * 128u + ((((uint32_t)(2 * j + kc)) ^ (p & 7u)) << 4);
+          ldsm_x4(ahi + off, ah[j]);
+          ldsm_x4(alo + off, al[j]);
         }
-        first = false;
-        umma_commit(bar_empty + s);
-      }
-      umma_commit(bar_phase);
-      mbar_wait(bar_brick, 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      // phase-2 stages continue the global stage count: g2 = kTaps + u; the issuer of a stage is g2 % NI
-      int u0 = ((issuer - (kTaps % NI)) % NI + NI) % NI;
-      for (int u = u0; u < kPairs; u += NI) {
-        const int g = kTaps + u, s = g % kW2Stages, round = g / kW2Stages;
-        mbar_wait(bar_full + s, round & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+        const uint32_t whi = smem_u32(w_st + s * Cfg::kWStageBytes), wlo = whi + NOUT * 128;
+        wgmma_fence();
+        // The tensor core truncates when it adds into the fp32 accumulator, so a single accumulator would take
+        // thousands of biased roundings in the 15x15 layer. Spread them: the a_hi*w_hi products go round-robin to NMAIN
+        // accumulators, both small correction terms to one more; the epilogue sums them in fp32 round-to-nearest.
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int t = 2 * u + e;
-          if (t < kTaps) {
-            const uint32_t shift = (uint32_t)((t / KS) * Cfg::kBrickX + (t % KS));
-            const uint32_t whi = smem_u32(w_st + s * Cfg::kWStageBytes) + e * NOUT * 128;
-#pragma unroll
-            for (int j = 0; j < KSTEPS; ++j)
-              umma_f16(d_corr, make_desc(abr + shift * 128 + j * 32, Cfg::kBrickX * 128, 0), make_desc(whi + j * 32, 1024, 0),
-                       Cfg::kIdesc, 1);
-          }
+        for (int j = 0; j < KSTEPS; ++j) {   // KSTEPS x 16 channels; pad channels beyond are never multiplied
+          wgmma_rs<NOUT>(acc[u], ah[j], make_desc_b(whi + j * 32));
+          wgmma_rs<NOUT>(corr, ah[j], make_desc_b(wlo + j * 32));
+          wgmma_rs<NOUT>(corr, al[j], make_desc_b(whi + j * 32));
         }
-        umma_commit(bar_empty + s);
-      }
-      umma_commit(bar_done);
-    }
-  } else {
-    mbar_wait(bar_done, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    const int oy = y0 + (m >> 3), ox = x0 + (m & 7);
-    float acc[NOUT];
-#pragma unroll
-    for (int n = 0; n < NOUT; ++n) acc[n] = 0.0f;
-#pragma unroll
-    for (int a = 0; a < kAcc; ++a) {
-#pragma unroll
-      for (int c = 0; c < NOUT / 16; ++c) {
-        uint32_t v[16];
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * 64 + c * 16);
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-            : "r"(taddr));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[16 * c + i] += __uint_as_float(v[i]);
-      }
-    }
-    if (oy < OH && ox < OW) {
-      float* op = out + ((size_t)oy * OW + ox) * 48;
-#pragma unroll
-      for (int n = 0; n < NOUT; ++n) {
-        const float f = acc[n] * (1.0f / kWScale) + __ldg(bias + n);
-        op[n] = f > 0.0f ? f : 0.3f * f;
+        wgmma_commit();
+        wgmma_wait_all();
+        if (lane == 0) mbar_arrive(bar_empty + s);   // frees the weight stage for the producer
       }
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols));
+
+  // epilogue: accumulator element i of lane l sits at row 16q + l/4 + 8*((i/2)&1), column 8*(i/4) + 2*(l&3) + (i&1)
+  float v[kNA];
+#pragma unroll
+  for (int i = 0; i < kNA; ++i) {
+    float sum = 0.0f;
+#pragma unroll
+    for (int a = 0; a < NMAIN; ++a) sum += acc[a][i];
+    v[i] = sum + corr[i];
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int oy = y0 + 8 * g + 2 * q + h, ox = x0 + (lane >> 2);
+    if (oy >= OH || ox >= OW) continue;
+    const size_t pix = (size_t)oy * OW + ox;
+#pragma unroll
+    for (int c8 = 0; c8 < NOUT / 8; ++c8) {
+      const int n = 8 * c8 + 2 * (lane & 3);
+      float f[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float x = 0.0f;
+        if (n + e < cout) { x = v[4 * c8 + 2 * h + e] * (1.0f / kWScale) + __ldg(bias + n + e); x = x > 0.0f ? x : 0.3f * x; }
+        f[e] = x;
+      }
+      if (SPLIT_OUT) {
+        const __half h0 = __float2half_rn(f[0]), h1 = __float2half_rn(f[1]);
+        reinterpret_cast<__half2*>(out_hi + pix * 64)[n / 2] = __halves2half2(h0, h1);
+        reinterpret_cast<__half2*>(out_lo + pix * 64)[n / 2] =
+            __halves2half2(__float2half_rn(f[0] - __half2float(h0)), __float2half_rn(f[1] - __half2float(h1)));
+      } else {
+        float* op = out + pix * cout;
+        if (n < cout) op[n] = f[0];
+        if (n + 1 < cout) op[n + 1] = f[1];
+      }
+    }
+    if (SPLIT_OUT) {   // pad channels of the next layer's input
+      for (int n = NOUT + 2 * (lane & 3); n < 64; n += 8) {
+        reinterpret_cast<__half2*>(out_hi + pix * 64)[n / 2] = __float2half2_rn(0.0f);
+        reinterpret_cast<__half2*>(out_lo + pix * 64)[n / 2] = __float2half2_rn(0.0f);
+      }
+    }
+  }
 }
 
 // First layer (Cin = 1, no activation after its BN) on CUDA cores, reading the map layer directly and writing the
@@ -858,8 +667,6 @@ struct State {
   CUtensorMap maps[6][4];      // per tensor-core layer: activation hi/lo, weight hi/lo (rebuilt when buffers change)
   bool maps_valid = false;
   bool attrs_set = false;
-  int use_base_offset = 0;
-  int conv15_mode = 0;         // 15x15 layer: 0 two-phase (default), 1 single phase, 2 single phase + CTA-pair multicast
   float last_ms[3] = {0, 0, 0};
   cudaEvent_t ev[4] = {};
 };
@@ -891,13 +698,11 @@ void destroy(State* s) {
   delete s;
 }
 
-void set_base_offset_mode(State* s, int on) { s->use_base_offset = on ? 1 : 0; }
-void set_conv15_mode(State* s, int mode) { if (s->conv15_mode != mode) { s->conv15_mode = mode; s->attrs_set = false; } }
 bool has_features(const State* s) { return s->has_features; }
 bool has_weights(const State* s) { return s->has_weights; }
 void last_times(const State* s, float* ms3) { ms3[0] = s->last_ms[0]; ms3[1] = s->last_ms[1]; ms3[2] = s->last_ms[2]; }
 
-static const int kTcNout[6] = {0, 32, 48, 48, 48, 48};   // UMMA N per layer (Cout 24 padded to 32)
+static const int kTcNout[6] = {0, 32, 48, 48, 48, 48};   // wgmma N per layer (Cout 24 padded to 32)
 
 int set_weights(State* s, const float* blob, size_t n, cudaStream_t st, std::string& err) {
   if (n != blob_floats()) { err = "weight blob has the wrong number of floats"; return -1; }
@@ -979,7 +784,7 @@ static int encode_layer_maps(State* s, CUtensorMap* maps, __half* ahi, __half* a
   return 0;
 }
 
-template <int KS, int KSTEPS, int NOUT, int NMAIN, bool SPLIT, int CLUSTER, int ISSUERS = 1>
+template <int KS, int KSTEPS, int NOUT, int NMAIN, bool SPLIT>
 static int launch_tc(State* s, int layer, __half* ahi, __half* alo, int H, int W, float* out, __half* ohi, __half* olo,
                      cudaStream_t st, std::string& err) {
   using Cfg = ConvCfg<KS, NOUT>;
@@ -988,23 +793,13 @@ static int launch_tc(State* s, int layer, __half* ahi, __half* alo, int H, int W
     int rc = encode_layer_maps(s, maps, ahi, alo, H, W, Cfg::kBrickX, Cfg::kBrickY, s->tc[layer].whi, s->tc[layer].wlo, KS * KS, NOUT, err);
     if (rc) return rc;
   }
-  auto kern = conv_tc_kernel<KS, KSTEPS, NOUT, NMAIN, SPLIT, CLUSTER, ISSUERS>;
+  auto kern = conv_wgmma_kernel<KS, KSTEPS, NOUT, NMAIN, SPLIT>;
   if (!s->attrs_set) CNN_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
   const int OH = H - KS + 1, OW = W - KS + 1;
-  const int gx = (OW + kTileX - 1) / kTileX, gy = (OH + kTileY - 1) / kTileY;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(((gx + CLUSTER - 1) / CLUSTER) * CLUSTER, gy);   // padded CTAs compute an out-of-range tile (stores masked)
-  cfg.blockDim = dim3(192 + 32 * (ISSUERS - 1));
-  cfg.dynamicSmemBytes = Cfg::kSmem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CLUSTER; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = CLUSTER > 1 ? 1 : 0;
-  const int cout = kLayers[layer].cout, ubo = s->use_base_offset;
-  const float* bias = s->d_bias[layer];
-  CNN_TRY(cudaLaunchKernelEx(&cfg, kern, maps[0], maps[1], maps[2], maps[3], bias, out, ohi, olo, OH, OW, cout, ubo));
+  const dim3 grid((OW + kTileX - 1) / kTileX, (OH + kTileY - 1) / kTileY);
+  kern<<<grid, kConvThreads, Cfg::kSmem, st>>>(maps[0], maps[1], maps[2], maps[3], s->d_bias[layer], out, ohi, olo, OH, OW,
+                                               kLayers[layer].cout);
+  CNN_TRY(cudaGetLastError());
   return 0;
 }
 
@@ -1061,39 +856,16 @@ int update_features(State* s, const float* d_layer, int rows, int cols, int pitc
   } else {
     int rc;
     conv1_split_kernel<<<g1, 256, 0, st>>>(d_layer, H0, W0, pitch, s->d_wf[0], s->d_bias[0], s->h1, s->l1);
-    if ((rc = launch_tc<3, 2, 32, 1, false, 1>(s, 1, s->h1, s->l1, H1, W1, s->f2, nullptr, nullptr, st, err))) return rc;
+    if ((rc = launch_tc<3, 2, 32, 1, false>(s, 1, s->h1, s->l1, H1, W1, s->f2, nullptr, nullptr, st, err))) return rc;
     maxpool_split_kernel<<<g1, 256, 0, st>>>(s->f2, H2, W2, 24, 2, 2, s->hp2, s->lp2, HP2, WP2);
-    if ((rc = launch_tc<3, 2, 48, 1, true, 1>(s, 2, s->hp2, s->lp2, HP2, WP2, nullptr, s->h3, s->l3, st, err))) return rc;
-    if ((rc = launch_tc<3, 3, 48, 1, false, 1>(s, 3, s->h3, s->l3, H3, W3, s->f4, nullptr, nullptr, st, err))) return rc;
+    if ((rc = launch_tc<3, 2, 48, 1, true>(s, 2, s->hp2, s->lp2, HP2, WP2, nullptr, s->h3, s->l3, st, err))) return rc;
+    if ((rc = launch_tc<3, 3, 48, 1, false>(s, 3, s->h3, s->l3, H3, W3, s->f4, nullptr, nullptr, st, err))) return rc;
     maxpool_split_kernel<<<g1, 256, 0, st>>>(s->f4, H4, W4, 48, 3, 1, s->hp4, s->lp4, HP4, WP4);
-    if ((rc = launch_tc<3, 3, 48, 1, true, 1>(s, 4, s->hp4, s->lp4, HP4, WP4, nullptr, s->h5, s->l5, st, err))) return rc;
+    if ((rc = launch_tc<3, 3, 48, 1, true>(s, 4, s->hp4, s->lp4, HP4, WP4, nullptr, s->h5, s->l5, st, err))) return rc;
     CNN_TRY(cudaGetLastError());
     CNN_TRY(cudaEventRecord(s->ev[1], st));
     CNN_TRY(cudaEventRecord(s->ev[2], st));
-    if (s->conv15_mode == 0) {          // two-phase (default)
-      using Cfg = ConvCfg<15, 48>;
-      CUtensorMap* maps = s->maps[5];
-      if (!s->maps_valid) {
-        rc = encode_layer_maps(s, maps, s->h5, s->l5, H5, W5, Cfg::kBrickX, Cfg::kBrickY, s->tc[5].whi, s->tc[5].wlo, 225, 48, err);
-        if (rc) return rc;
-      }
-      constexpr int kIssuers = 4;
-      if (!s->attrs_set)
-        CNN_TRY(cudaFuncSetAttribute(conv15_two_phase_kernel<kIssuers>, cudaFuncAttributeMaxDynamicSharedMemorySize, Conv15Cfg::kSmem));
-      dim3 grid((W6 + kTileX - 1) / kTileX, (H6 + kTileY - 1) / kTileY);
-      conv15_two_phase_kernel<kIssuers><<<grid, 192 + 32 * (kIssuers - 1), Conv15Cfg::kSmem, st>>>(maps[0], maps[1], maps[2], maps[3],
-                                                                                                   s->d_bias[5], s->feat, H6, W6);
-      CNN_TRY(cudaGetLastError());
-    } else if (s->conv15_mode == 2) {   // single phase, CTA pairs with weight multicast
-      rc = launch_tc<15, 3, 48, 7, false, 2>(s, 5, s->h5, s->l5, H5, W5, s->feat, nullptr, nullptr, st, err);
-      if (rc) return rc;
-    } else if (s->conv15_mode == 3) {   // single phase, two MMA-issuing warps
-      rc = launch_tc<15, 3, 48, 6, false, 1, 2>(s, 5, s->h5, s->l5, H5, W5, s->feat, nullptr, nullptr, st, err);
-      if (rc) return rc;
-    } else {                            // single phase, one CTA per tile
-      rc = launch_tc<15, 3, 48, 7, false, 1>(s, 5, s->h5, s->l5, H5, W5, s->feat, nullptr, nullptr, st, err);
-      if (rc) return rc;
-    }
+    if ((rc = launch_tc<15, 3, 48, 2, false>(s, 5, s->h5, s->l5, H5, W5, s->feat, nullptr, nullptr, st, err))) return rc;
     s->maps_valid = true;
     s->attrs_set = true;
   }

@@ -16,8 +16,6 @@ int update_features(State* s, const float* d_layer, int rows, int cols, int pitc
 int motion_cost(State* s, const float* d_edges, size_t n, float* d_cost3, cudaStream_t st, std::string& err);
 int copy_features(State* s, float* host_out, size_t n_floats, std::string& err);
 void feature_shape(const State* s, int* hf, int* wf);
-void set_base_offset_mode(State* s, int on);
-void set_conv15_mode(State* s, int mode);
 bool has_features(const State* s);
 bool has_weights(const State* s);
 void last_times(const State* s, float* ms3);

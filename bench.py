@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- pose-validity checks/s of the art_planner hot path on B200 (BASELINE.json metric).
+"""bench.py -- pose-validity checks/s of the art_planner hot path on an H100 (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch of synthetic input: BASELINE.json configs[1] -- a
 1 000 000-pose validity batch (torso + 4 feet, yaml robot geometry) on the fBm ("Perlin") 1000x1000 @0.04 m map.
@@ -20,10 +20,16 @@ A "step" is one pass of the hot path over one batch of synthetic input: BASELINE
          (pipelined; the un-pipelined step is reported too); c5 = configs[4] on spatial map shards (strong scaling).
   --impl reference   the reference's own CPU path (oracle/_ref = its compiled ODE when present, else the C port)
          on all host threads, on a bounded sample of the same workload per step.
+  --dump-outputs DIR  after the timed steps, what the last timed step returned to its caller, as .npy files:
+         valid.npy (verdict bytes, float32), valid_bits.npy (the packed 32-bit words as unsigned values, float64),
+         valid_index.npy (the ordered index list of the valid samples, float32, exact below 2^24). The inputs are
+         seeded, so two builds can be compared file by file.
+Runs from the tree as build() left it (the library is not rebuilt here) and writes nothing into it.
 """
 from __future__ import annotations
 
 import argparse
+import atexit
 import json
 import os
 import subprocess
@@ -35,6 +41,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
+sys.dont_write_bytecode = True   # the tree may be read-only
 
 MAP_N = 1000
 MAP_RES = 0.04
@@ -47,11 +54,11 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries; the poller ends with the run)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -65,6 +72,7 @@ class ClockSampler:
                                           "-lms", "10", "-i", str(self.idx)], stdout=subprocess.PIPE, text=True)
             self.t = threading.Thread(target=lambda: [self.lines.append(l) for l in self.proc.stdout], daemon=True)
             self.t.start()
+            atexit.register(self.proc.kill)   # no poller outlives the benchmark, whatever ends it
         except Exception:
             self.proc = None
 
@@ -112,8 +120,6 @@ def make_inputs(rank: int, n: int, workload: str = "c2", world: int = 1):
 def cpu_oracle(params):
     from oracle import orc
     kind = "reference" if orc.available("reference") else "port"
-    if kind == "port":
-        orc.build("port")
     return orc.Oracle(params, kind), kind
 
 
@@ -305,6 +311,8 @@ def main():
     ap.add_argument("--impl", default="b200")
     ap.add_argument("--workload", default="c2", choices=["c2", "c5"],
                     help="c2 = BASELINE configs[1] (default, the metric's config); c5 = configs[4], 4000x4000 map, spatial slabs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)
@@ -313,7 +321,7 @@ def main():
     import torch
     import torch.distributed as dist
     import art_planner_b200 as apb
-    from art_planner_b200 import build, synth
+    from art_planner_b200 import synth
 
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
@@ -322,10 +330,6 @@ def main():
     torch.cuda.set_device(local)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
-    if rank == 0:
-        build.build()
-    if world > 1:
-        dist.barrier()
 
     n = POSES_PER_GPU
     m, poses = make_inputs(rank, n, args.workload, world)
@@ -342,7 +346,7 @@ def main():
     hb_poses.array[:] = poses
     hb_poses32.array[:] = poses.astype(np.float32)        # the cast Pose3FromSE3 does first, done by the adapter
     h_poses, h_poses32, h_valid = (torch.from_numpy(x.array) for x in (hb_poses, hb_poses32, hb_valid))
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")   # > 50 MB L2 of an H100
     # Every step produces the verdict bytes, their bit-packed form and the ordered list of valid sample indices of this
     # rank's shard (32-bit, global numbering). N > 1: the ranks exchange the bit masks with ONE NCCL all-gather (125 KB
     # per rank and 10^6 samples); a consumer that wants the global index list reads the per-rank segments + counts.
@@ -429,6 +433,15 @@ def main():
         dist.barrier()
     wall = time.perf_counter() - wall0
     dev_ms = sum(s.elapsed_time(e) for s, e in ev)
+    if args.dump_outputs and rank == 0:
+        # the last timed step's results (the passes below recompute them into the same buffers)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        cnt = int(loc_cnt.item())
+        dump = {"valid": d_valid, "valid_bits": my_bits[(args.steps - 1) & 1].to(torch.int64) & 0xFFFFFFFF,
+                "valid_index": loc_idx[:cnt]}
+        for name, t_ in dump.items():
+            a_ = t_.cpu().numpy().astype(np.float64 if name == "valid_bits" else np.float32)
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), a_)
     launches = chk.stats()["kernel_launches"] - launches0      # kernels of this library launched inside the timed region
     # second pass, per-stage timing ON (the stages of a round then run one after the other on the call's stream): stage
     # durations from the library's CUDA events, and the throughput of that serial order
@@ -556,7 +569,6 @@ def main():
             m_r = synth.make_fbm_map(MAP_N, MAP_N, MAP_RES, seed=MAP_SEED, **ROUGH_MAP)
             p_r = synth.make_terrain_poses(m_r, n, seed=POSE_SEED, **ROUGH_POSES)
             o_r, kind_r = cpu_oracle(synth.PARAMS_YAML)
-            orc.build("port")
             chk_r = apb.StateValidityChecker(synth.PARAMS_YAML, device=local)
             secondary["c2_rough"] = pose_workload(torch, chk_r, flush, m_r, p_r, 20, o_r, kind_r,
                                                   orc.Oracle(synth.PARAMS_YAML, "port"))
@@ -668,7 +680,7 @@ def main():
             hms = a.elapsed_time(bb) / 100
             secondary["motion_cost_cnn"] = {
                 "workload": "configs[3]: 256x256 elevation patch -> cost CNN trunk, 4096-query batch, seeded random weights",
-                "trunk_ms": float(tms[2]), "conv3x3_stack_ms": float(tms[0]), "conv15x15_tcgen05_ms": float(tms[1]),
+                "trunk_ms": float(tms[2]), "conv3x3_stack_ms": float(tms[0]), "conv15x15_wgmma_ms": float(tms[1]),
                 "trunk_tflops": 13.41e9 / (float(tms[2]) * 1e-3) / 1e12, "conv15_tflops": 11.21e9 / (float(tms[1]) * 1e-3) / 1e12,
                 "head_ms_4096_queries": hms, "edge_cost_evals_per_s": 4096 / (hms * 1e-3)}
         except Exception as ex:   # never let a secondary workload take the headline line down
@@ -710,7 +722,6 @@ def main():
                             "sample": f"N > 1: not timed (see the N = 1 line); rank 0's mask checked against the oracle on its first {n1} poses",
                             "single_thread_value": n1 / t_single, "mask_equals_gpu": bool(np.array_equal(got[:n1], v1))}
         from oracle import orc
-        orc.build("port")
         port = orc.Oracle(synth.PARAMS_YAML, "port")
         port.set_map(m)
         _, zv = port.check_poses(poses[:50_000], want_zone=True)
@@ -723,10 +734,6 @@ def main():
         k0, k_torso, k_reach, k2 = float(sm[0]), float(sm[1]), float(sm[2] + sm[3]), float(sm[4])
         pass_ms = k0 + k_torso + k_reach + k2
         achieved = bytes_per_pose * n / (pass_ms * 1e-3) / 1e9
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tp):
-            traffic = json.load(open(tp)).get("reach_queues_dram_bytes_per_pass")   # group kernel + one-warp-per-box launch
         port_mix = exit_mix(port, poses[:20_000])
         out = {
             "metric": "pose-validity checks/s", "value": value, "unit": "poses/s", "n_gpus": world,
@@ -743,10 +750,10 @@ def main():
             "e2e": {"value": e2e_value, "unit": "poses/s", "h2d_bytes_per_step": n * 28, "d2h_bytes_per_step": n, "mask_equals_device_path": e2e_mask_ok,
                     "ms_per_step": e2e_ms / e2e_steps, "api": "artp_check_poses_f32 (states cast to float by the adapter while it gathers them, exact), buffers from artp_host_alloc",
                     "f64_api_value": world * n * e2e_steps / e2e64_s, "f64_api_h2d_bytes_per_step": n * 56, "two_callers": two_callers,
-                    "note": "PCIe Gen5 x16 moves 53-55 GB/s here (profiles/pcie_probe.cu): 28 MB = 0.52 ms, 56 MB = 1.04 ms, so the double entry point is copy-bound at <= 0.96e9 poses/s"},
+                    "note": "the states cross PCIe inside the timed region: the double entry point moves twice the bytes of the float one"},
             "gpu_launches": int(launches),
             "roofline": {"bound": "hbm", "kernel": "reach_groups_kernel + box_tiles_warp_kernel (the two reach-box queues)", "achieved": achieved, "peak": peak,
-                         "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                         "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
                          "algorithmic_bytes_per_pose": bytes_per_pose, "kernel_ms": k_reach,
                          "classify_kernel_ms": k0, "torso_queue_kernel_ms": k_torso, "group_kernel_ms": k2, "pass_ms": pass_ms,
                          "serial_order_value": world * n * args.steps / (fork_ms * 1e-3),
@@ -756,11 +763,9 @@ def main():
                          "queued_warp_stage": stats_last["last_queued_warp_stage"],
                          "queued_reach_stage": stats_last["last_queued_reach_stage"],
                          "queued_reach_groups": stats_last["last_reach_plane_stage"],
-                         "actual_dram_GBps_dominant_kernel": (traffic / (k_reach * 1e-3) / 1e9) if traffic else None,
                          "note": "achieved = ALGORITHMIC bytes (the zone vertices the reference scans, SURVEY 8d) / sum of the stage "
                                  "durations; the range tables, plane tables and vertex probes answer most of those scans without reading "
-                                 "them, so frac exceeds 1 while real DRAM traffic (traffic, ncu) stays near 1 % of peak: the pipeline is "
-                                 "instruction-issue bound (group kernel: 68 % of issue slots busy, 20 of 32 lanes; profiles/r02_v6_*)"},
+                                 "them, so frac can exceed 1 while the real DRAM traffic is far smaller"},
             "cpu_baseline": cpu_baseline,
             "clocks": clocks, "wall_s_timed_region": wall, "secondary": secondary, "exchange_ok": exchange_ok,
             "exchange": {"unpipelined_value": world * n * args.steps / (serial_ms * 1e-3), "unpipelined_ms_per_step": serial_ms / args.steps,

@@ -1,5 +1,5 @@
 /*
- * include/artp.h -- C ABI of the B200-native art_planner hot path (libartp.so).
+ * include/artp.h -- C ABI of the CUDA-native art_planner hot path (libartp.so).
  *
  * Drop-in boundary (SURVEY.md section 8b): everything the reference's OMPL plugins for this path need,
  * as plain C: pointers + sizes, no C++/torch types, no exceptions across the boundary. Every entry point
@@ -320,13 +320,13 @@ int artp_motion_cost_states(artp_handle* h, const double* s_start, const double*
  * cost[i] = w_e*E + w_t*T + w_r*R, feasible[i] = R <= risk_threshold (weights / threshold from artp_params). */
 int artp_combine_cost(artp_handle* h, const float* cost3, size_t n, double* cost, uint8_t* feasible);
 /* Test hooks: feature map copy-out ([Hf][Wf][48] fp32, channels last), kernel selection (bit 0: CUDA-core fp32
- * reference for the 15x15 layer instead of tcgen05; bit 1: set the smem-descriptor base_offset, a known-wrong variant kept for the record; bits 2-3: 15x15 layer variant, 0 = two-phase (default), 1 = single phase, 2 = single phase with CTA-pair weight multicast), trunk timings
+ * reference for every layer instead of the tensor-core (wgmma) kernels; any other bit is ARTP_E_INVALID), trunk timings
  * ms3 = (3x3 stack, 15x15 layer, whole trunk) of the last artp_update_features. */
 int artp_get_features(artp_handle* h, float* out, size_t n_floats, int* hf, int* wf);
 int artp_set_cnn_mode(artp_handle* h, int mode);
 int artp_get_cnn_timing(artp_handle* h, float* ms3);
 
-/* Version string of the library / kernel image ("artp <ver> sm_100a"). */
+/* Version string of the library / kernel image ("artp <ver> sm_90a"). */
 const char* artp_version(void);
 
 #ifdef __cplusplus

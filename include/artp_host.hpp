@@ -1,4 +1,4 @@
-// include/artp_host.hpp -- C++ host side of the B200-native art_planner hot path, above the C ABI (artp.h).
+// include/artp_host.hpp -- C++ host side of the CUDA-native art_planner hot path, above the C ABI (artp.h).
 //
 // Header-only mirror of the reference's plugin classes for this path -- same class and method names, argument meaning
 // and error behaviour -- so that art_planner's planners and facade keep calling what they call today:

@@ -35,7 +35,7 @@ def setup():
     return m, obj, orc, feat, golden
 
 
-@pytest.mark.parametrize("mode", [1, 0, 4, 8, 12], ids=["cuda-core", "tcgen05-two-phase", "tcgen05-single-phase", "tcgen05-multicast-pairs", "tcgen05-two-issuers"])
+@pytest.mark.parametrize("mode", [1, 0], ids=["cuda-core", "wgmma"])
 def test_feature_map(setup, mode):
     m, obj, orc, feat, golden = setup
     obj.setMode(mode)
@@ -85,6 +85,9 @@ def test_errors_without_weights_or_features():
     obj.setWeights(costnet.make_state_dict(seed=5))
     with pytest.raises(ap.ArtpError):
         obj.costQuery(np.zeros((4, 6), np.float32))   # features not computed
+    for mode in (2, 4, 8, 12):
+        with pytest.raises(ap.ArtpError):
+            obj.setMode(mode)           # bit 0 is the only mode bit
 
 
 @pytest.mark.parametrize("shape", [(300, 260), (1000, 1000), (121, 97)], ids=["300x260-partial-tiles", "1000x1000-metric-map", "121x97-odd"])
