@@ -37,6 +37,7 @@ struct Handle {
   float* d_H[2] = {nullptr, nullptr};
   float2* d_T[2][artp::kMaxLevel + 1] = {};
   uint32_t* d_NF[2][artp::kMaxLevel + 1] = {};   // bit-packed window flags (2 bits per entry)
+  uint32_t* d_C[2][artp::kMaxLevel + 1] = {};    // compact conservative copies of d_T (Field::C)
   int pitch = 0;
   int rows = 0, cols = 0;           // full map
   int win_row0 = 0, win_rows = 0;   // rows held by this handle (artp_set_map_window); whole map: 0, rows
@@ -161,6 +162,49 @@ __global__ void build_level_kernel(const float* __restrict__ H, const float2* __
     T[i] = make_float2(mx, mn);
     NF[i] = nf;
   }
+}
+
+// Compact table level from T (encoding at artp::Field::C): maxCode = the smallest code c >= 1 with dec(c) >= max,
+// minCode = the largest c with dec(c) <= min, both found by bisection over the non-decreasing dec(). A height the
+// codes cannot cover (above dec(kCodeMax)) takes the reserved code 65535, which sends its zones to the exact tables.
+__global__ void build_codes_kernel(const float2* __restrict__ T, uint32_t* __restrict__ C, size_t n, float base, float step) {
+  const float top = artp::code_dec(base, step, artp::kCodeMax);
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float2 v = T[i];
+    uint32_t cM = 0, cm = 0xFFFFu;
+    if (v.x > top) cM = 0xFFFFu;
+    else if (v.x > -CUDART_INF_F) {
+      uint32_t lo = 1, hi = artp::kCodeMax;
+      while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (artp::code_dec(base, step, mid) >= v.x) hi = mid; else lo = mid + 1;
+      }
+      cM = lo;
+    }
+    if (v.y <= top) {
+      uint32_t lo = 0, hi = artp::kCodeMax;
+      while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1) >> 1;
+        if (artp::code_dec(base, step, mid) <= v.y) lo = mid; else hi = mid - 1;
+      }
+      cm = lo;
+    }
+    C[i] = (cM << 16) | cm;
+  }
+}
+
+// Encoding of the compact tables of one layer: base = the smallest finite height, step = the smallest power of two
+// with dec(kCodeMax) >= the largest finite height (checked with the device's own dec()).
+void code_scale(const float* layer, size_t n, float& base, float& step) {
+  float lo = HUGE_VALF, hi = -HUGE_VALF;
+  for (size_t i = 0; i < n; ++i) {
+    const float v = layer[i] * 1.0f + 0.0f;   // the stored height (reverse_columns_kernel)
+    if (std::fabs(v) < HUGE_VALF) { lo = std::min(lo, v); hi = std::max(hi, v); }
+  }
+  base = lo <= hi ? lo : 0.0f;
+  int e = -126;
+  while (e < 127 && artp::code_dec(base, std::ldexp(1.0f, e), artp::kCodeMax) < hi) ++e;
+  step = std::ldexp(1.0f, e);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -798,7 +842,7 @@ void artp_destroy(artp_handle* hh) {
   for (int i = 0; i < kMaxSlices; ++i) if (h->slice_ev[i]) cudaEventDestroy(h->slice_ev[i]);
   if (h->box_ev) cudaEventDestroy(h->box_ev);
   cudaFree(h->d_slices);
-  for (int k = 0; k < 2; ++k) for (int l = 0; l <= artp::kMaxLevel; ++l) { cudaFree(h->d_T[k][l]); cudaFree(h->d_NF[k][l]); }
+  for (int k = 0; k < 2; ++k) for (int l = 0; l <= artp::kMaxLevel; ++l) { cudaFree(h->d_T[k][l]); cudaFree(h->d_NF[k][l]); cudaFree(h->d_C[k][l]); }
   cudaFree(h->d_H[0]); cudaFree(h->d_H[1]); cudaFree(h->d_ctr); cudaFree(h->d_defer); cudaFree(h->d_stage);
   cudaFree(h->d_block_counts); cudaFree(h->d_recs); cudaFree(h->d_recs_f); cudaFree(h->d_recs_g); cudaFree(h->d_samp_layers); cudaFree(h->d_samp_scratch);
   if (h->h_small_out) cudaFreeHost(h->h_small_out);
@@ -958,7 +1002,10 @@ int artp_set_map_window(artp_handle* hh, const float* elevation, const float* el
   if (h->win_rows != nrows || h->cols != cols) {
     for (int k = 0; k < 2; ++k) {
       cudaFree(h->d_H[k]); h->d_H[k] = nullptr;
-      for (int l = 0; l <= artp::kMaxLevel; ++l) { cudaFree(h->d_T[k][l]); cudaFree(h->d_NF[k][l]); h->d_T[k][l] = nullptr; h->d_NF[k][l] = nullptr; }
+      for (int l = 0; l <= artp::kMaxLevel; ++l) {
+        cudaFree(h->d_T[k][l]); cudaFree(h->d_NF[k][l]); cudaFree(h->d_C[k][l]);
+        h->d_T[k][l] = nullptr; h->d_NF[k][l] = nullptr; h->d_C[k][l] = nullptr;
+      }
       CU_TRY(h, cudaMalloc(&h->d_H[k], npad * sizeof(float)));
     }
   }
@@ -967,10 +1014,13 @@ int artp_set_map_window(artp_handle* hh, const float* elevation, const float* el
       if (!h->d_T[k][l]) {
         CU_TRY(h, cudaMalloc(&h->d_T[k][l], npad * sizeof(float2)));
         CU_TRY(h, cudaMalloc(&h->d_NF[k][l], ((npad + 15) / 16) * sizeof(uint32_t)));
+        CU_TRY(h, cudaMalloc(&h->d_C[k][l], npad * sizeof(uint32_t)));
       }
   int rc = ensure_stage(h, ncell * sizeof(float));
   if (rc) return rc;
   const float* src[2] = {elevation, elevation_masked};
+  float cbase[2], cstep[2];
+  for (int k = 0; k < 2; ++k) code_scale(src[k], ncell, cbase[k], cstep[k]);
   // plane tables (temporary): 4 slots per cell = load factor 0.5 for the 2 triangles of a cell
   size_t cap = 1;
   while (cap < 4 * ncell) cap <<= 1;
@@ -997,8 +1047,9 @@ int artp_set_map_window(artp_handle* hh, const float* elevation, const float* el
                                                                   l > 1 ? nf_prev : nullptr, d_merge, h->d_T[k][l], nf_cur, nrows,
                                                                   cols, pitch, 1 << (l - 1));
       pack_flags_kernel<<<h->sm_count * 4, 256, 0, h->stream>>>(nf_cur, npad, h->d_NF[k][l]);
+      build_codes_kernel<<<h->sm_count * 4, 256, 0, h->stream>>>(h->d_T[k][l], h->d_C[k][l], npad, cbase[k], cstep[k]);
       CU_TRY(h, cudaGetLastError());
-      h->stats.kernel_launches += 2;
+      h->stats.kernel_launches += 3;
     }
   }
   CU_TRY(h, cudaStreamSynchronize(h->stream));
@@ -1009,9 +1060,11 @@ int artp_set_map_window(artp_handle* hh, const float* elevation, const float* el
   for (int k = 0; k < 2; ++k) {
     f.H = h->d_H[k] - row0;                 // indexed with GLOBAL vertex indices x in [x_lo, x_hi]
     f.kmax = kmax[k];
+    f.cbase = cbase[k]; f.cstep = cstep[k];
     for (int l = 0; l <= artp::kMaxLevel; ++l) {
       f.T[l] = (l >= 1 && l <= kmax[k]) ? h->d_T[k][l] - row0 : nullptr;
       f.NF[l] = (l >= 1 && l <= kmax[k]) ? h->d_NF[k][l] : nullptr;   // bit-packed: indexed with LOCAL entry numbers, see below
+      f.C[l] = (l >= 1 && l <= kmax[k]) ? h->d_C[k][l] - row0 : nullptr;
     }
     h->chk.f[k] = f;
   }

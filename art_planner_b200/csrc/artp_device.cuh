@@ -27,6 +27,12 @@ struct Field {
   // triangle whose plane matches (within eps) the plane of another triangle of the map. Built at artp_set_map, k = 1..kmax.
   const float2* T[kMaxLevel + 1];
   const uint32_t* NF[kMaxLevel + 1];   // 2 flag bits per entry, 16 entries per word: 32x smaller than the (max, min) tables, cache resident
+  // Conservative copies of T[k] at half the size (the classify stage's random lookups then stay in L2):
+  // C[k][i] = (maxCode << 16) | minCode with max in [dec(maxCode - 1), dec(maxCode)] and min in [dec(minCode), dec(minCode + 1)],
+  // dec(c) = cbase + c * cstep (code_dec). Finite heights take max codes 1..65533 and min codes 0..65534; a window without
+  // a finite height has max code 0 (max -inf) and min code 65535 (min +inf). Same pitch and row shift as T.
+  const uint32_t* C[kMaxLevel + 1];
+  float cbase, cstep;   // smallest finite height of the stored window; a power of two
   int kmax;
   float W, D, hW, hD, sW, sD, asp, iW, iD;
   float px, py;    // heightfield body position (float casts of the map centre)
@@ -63,6 +69,12 @@ struct BoxCtx {
 __device__ __forceinline__ int window_flags(const uint32_t* __restrict__ nf, size_t idx) {
   return (int)((__ldg(nf + (idx >> 4)) >> ((idx & 15) * 2)) & 3u);
 }
+
+// Height of code c of the compact range tables. The host builds the codes with this same function (both sides are
+// compiled without FMA contraction): c * step is exact, and the rounded sum is non-decreasing in c, so every bound
+// the codes state holds by construction.
+constexpr uint32_t kCodeMax = 65533;   // largest code of a finite max; the host picks cstep so that dec(kCodeMax) >= max
+__host__ __device__ __forceinline__ float code_dec(float base, float step, uint32_t c) { return base + (float)c * step; }
 
 // nextafterf(x, -inf) / nextafterf(x, +inf) for finite x (dNextAfter, ode/include/ode/common.h:296), as integer ops.
 __device__ __forceinline__ float next_down(float x) {

@@ -183,6 +183,36 @@ __device__ __forceinline__ int zone_early_out(const BoxCtx& b, float maxY, float
   return -1;
 }
 
+// zone_early_out on the compact tables' intervals: maxY in [dec(cM - 1), dec(cM)], minY in [dec(cm), dec(cm + 1)].
+// Every subtraction and comparison of the tests is monotone in maxY and minY, so each test is evaluated at the interval
+// ends as true, false or unknown, in zone_early_out's order. Returns its answer when the first test that is not false is
+// true (or all are false), kZoneUnknown when an unknown comes first -- always for the single-plane test, which needs
+// the exact minY -- and for zones without a finite height (reserved codes).
+constexpr int kZoneUnknown = -4;
+__device__ __forceinline__ int zone_early_out_codes(const Field& f, const BoxCtx& b, uint32_t cM, uint32_t cm,
+                                                    bool allFinite) {
+  if (cM == 0 || cM == 0xFFFFu || cm == 0xFFFFu) return kZoneUnknown;
+  const float mxLo = code_dec(f.cbase, f.cstep, cM - 1), mxHi = code_dec(f.cbase, f.cstep, cM);
+  const float mnLo = code_dec(f.cbase, f.cstep, cm), mnHi = code_dec(f.cbase, f.cstep, cm + 1);
+  if (b.minB - mxHi > -ARTP_EPS) return R_FREE;                                            // above
+  if (!(b.minB - mxLo > -ARTP_EPS)) {
+    if (mnLo - b.maxB > -ARTP_EPS) return R_FREE;                                          // under
+    if (!(mnHi - b.maxB > -ARTP_EPS)) {
+      if (allFinite) {
+        if (mnLo - b.minB > -ARTP_EPS && b.maxB - mxHi > -ARTP_EPS) return R_HIT;           // spans
+        if (!(mnHi - b.minB > -ARTP_EPS && b.maxB - mxLo > -ARTP_EPS) && !(mxLo - mnHi < ARTP_EPS)) {   // single plane
+          if (b.x1 - b.x0 < 1 || b.z1 - b.z0 < 1) return R_FREE;
+          return -1;
+        }
+      } else {
+        if (b.x1 - b.x0 < 1 || b.z1 - b.z0 < 1) return R_FREE;
+        return -1;
+      }
+    }
+  }
+  return kZoneUnknown;
+}
+
 // Zone min / max / all-finite (heightfield.cpp:1002-1026). Fast path: exact range tables -- the zone is covered
 // by <= 32 overlapping 2^k x 2^k windows (one table entry per lane; max/min/or are idempotent so overlap is
 // harmless). Fallback (tiny or very elongated zones, e.g. clipped at the map border): stride the zone itself.
@@ -698,35 +728,52 @@ __device__ __forceinline__ int classify_box(const Checker& c, const float R[9], 
     if (force_all || kk < 1 || kk > f.kmax || cx * cz > 32) {
       r = -1; fl |= REC_NEEDS_REDUCE;
     } else {
-      const float2* __restrict__ T = f.T[kk];
+      // Zone codes from the compact tables first (half the bytes of T: they stay in L2); the exact T entries are read only
+      // when the codes' intervals leave a test open.
+      const uint32_t* __restrict__ C = f.C[kk];
       const uint32_t* __restrict__ NF = f.NF[kk];
       const int sW = 1 << kk;
-      float mx = -CUDART_INF_F, mn = CUDART_INF_F;
+      uint32_t cM = 0, cm = 0xFFFFu;
       int nf = 0;
-      if (cx <= 2 && cz <= 2) {
+      const bool quad = cx <= 2 && cz <= 2;
+      const int xs0 = b.x0, xs1 = b.x1 - sW + 1, zs0 = b.z0, zs1 = b.z1 - sW + 1;
+      const size_t i00 = (size_t)zs0 * f.pitch + xs0, i01 = (size_t)zs0 * f.pitch + xs1,
+                   i10 = (size_t)zs1 * f.pitch + xs0, i11 = (size_t)zs1 * f.pitch + xs1;
+      if (quad) {
         // the common case (window edge > half the zone edge): all four windows are requested before any is used
-        const int xs0 = b.x0, xs1 = b.x1 - sW + 1, zs0 = b.z0, zs1 = b.z1 - sW + 1;
-        const size_t i00 = (size_t)zs0 * f.pitch + xs0, i01 = (size_t)zs0 * f.pitch + xs1,
-                     i10 = (size_t)zs1 * f.pitch + xs0, i11 = (size_t)zs1 * f.pitch + xs1;
-        const float2 v0 = __ldg(T + i00), v1 = __ldg(T + i01), v2 = __ldg(T + i10), v3 = __ldg(T + i11);
+        const uint32_t w0 = __ldg(C + i00), w1 = __ldg(C + i01), w2 = __ldg(C + i10), w3 = __ldg(C + i11);
         const int n0 = window_flags(NF, i00 - f.x_lo), n1 = window_flags(NF, i01 - f.x_lo), n2 = window_flags(NF, i10 - f.x_lo), n3 = window_flags(NF, i11 - f.x_lo);
-        mx = fmaxf(fmaxf(v0.x, v1.x), fmaxf(v2.x, v3.x));
-        mn = fminf(fminf(v0.y, v1.y), fminf(v2.y, v3.y));
+        cM = max(max(w0 >> 16, w1 >> 16), max(w2 >> 16, w3 >> 16));
+        cm = min(min(w0 & 0xFFFFu, w1 & 0xFFFFu), min(w2 & 0xFFFFu, w3 & 0xFFFFu));
         nf = n0 | n1 | n2 | n3;
       } else {
         for (int iz = 0; iz < cz; ++iz) {
-          const int zs = min(b.z0 + iz * sW, b.z1 - sW + 1);
+          const int zs = min(b.z0 + iz * sW, zs1);
           for (int ix = 0; ix < cx; ++ix) {
-            const int xs = min(b.x0 + ix * sW, b.x1 - sW + 1);
-            const size_t idx = (size_t)zs * f.pitch + xs;
-            const float2 v = __ldg(T + idx);
-            mx = fmaxf(mx, v.x); mn = fminf(mn, v.y);
+            const size_t idx = (size_t)zs * f.pitch + min(b.x0 + ix * sW, xs1);
+            const uint32_t wv = __ldg(C + idx);
+            cM = max(cM, wv >> 16); cm = min(cm, wv & 0xFFFFu);
             nf |= window_flags(NF, idx - f.x_lo);
           }
         }
       }
       const bool allFinite = (nf & 1) == 0;
-      r = zone_early_out(b, mx, mn, allFinite);
+      r = zone_early_out_codes(f, b, cM, cm, allFinite);
+      if (r == kZoneUnknown) {
+        // exact zone max / min (the max and min codes commute with the reductions; the exact values do too)
+        const float2* __restrict__ T = f.T[kk];
+        float mx = -CUDART_INF_F, mn = CUDART_INF_F;
+#pragma unroll 1
+        for (int iz = 0; iz < cz; ++iz) {
+          const int zs = min(b.z0 + iz * sW, b.z1 - sW + 1);
+#pragma unroll 1
+          for (int ix = 0; ix < cx; ++ix) {
+            const float2 v = __ldg(T + (size_t)zs * f.pitch + min(b.x0 + ix * sW, b.x1 - sW + 1));
+            mx = fmaxf(mx, v.x); mn = fminf(mn, v.y);
+          }
+        }
+        r = zone_early_out(b, mx, mn, allFinite);
+      }
       if (allFinite) fl |= REC_ALLFINITE;
       if ((nf & 2) == 0) fl |= REC_MERGEFREE;   // no two triangles of the zone lie in one plane: greedy grouping is the identity
       if (r == -1 && allFinite && nX >= 2 && nZ >= 2 && (probe & (foot ? 1 : 2))) {
