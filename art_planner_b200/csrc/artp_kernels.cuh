@@ -810,11 +810,7 @@ __device__ __forceinline__ int classify_box(const Checker& c, const float R[9], 
 __global__ void __launch_bounds__(128, 8)
 classify_items_kernel(const Checker c, const Work w, BoxRec* __restrict__ recs_w, BoxRec* __restrict__ recs_f,
                       BoxRec* __restrict__ recs_g, uint32_t* __restrict__ count_w, uint32_t* __restrict__ count_f,
-                      uint32_t* __restrict__ count_g, int flags) {
-  const int force_all = flags & 1;      // every in-map box goes to the grouping stage (artp_set_mode 1)
-  // Vertex probes here only for reach boxes (one cell, most lanes busy); an undecided torso is rare (a few lanes of a
-  // warp) and its probes run lane-parallel at the head of the warp stage instead. ARTP_K0_FLAGS=2 turns probes off.
-  const int probe = (flags & 2) ? 0 : 1;
+                      uint32_t* __restrict__ count_g, int force_all) {   // force_all: every in-map box goes to the grouping stage (artp_set_mode 1)
   const uint32_t item = w.item_base + blockIdx.x * blockDim.x + threadIdx.x;
   const bool in_range = item < w.n_items;
   const int lane = threadIdx.x & 31;
@@ -843,7 +839,10 @@ classify_items_kernel(const Checker c, const Work w, BoxRec* __restrict__ recs_w
       BoxCtx b;
       uint32_t fl;
       const bool foot = k > 0;
-      const int r = classify_box(c, R, R1, t, k, force_all, probe, b, fl);
+      // Vertex probes here only for reach boxes (one cell, most lanes busy); an undecided torso is rare (a few lanes of a
+      // warp) and its probes run lane-parallel at the head of the warp stage instead. Classify without the probes measured
+      // slower: the boxes they decide land in the queues.
+      const int r = classify_box(c, R, R1, t, k, force_all, 1, b, fl);
       if (r == kBoxOutside) {
         if (foot && c.unknown_untraversable) result = 0;
         continue;

@@ -248,18 +248,12 @@ int artp_poll_error(artp_handle* h);
 /* Test hook: cap the plane store at max_triangles (0 = no cap) from the next artp_set_map on. */
 int artp_debug_set_group_capacity(artp_handle* h, int max_triangles);
 
-/* Environment switches (read at artp_create unless noted; experiments and A/B measurements, never needed in production):
+/* Environment switch (a test hook, never needed in production):
  *   ARTP_NO_GROUPS=1        (read at artp_set_map) every undecided reach box takes the one-warp-per-box queue instead of the
  *                           8-lane-group kernel -- same verdicts (tests/test_pose_gpu.py runs both)
- *   ARTP_SLICE_ITEMS=n      host-buffer calls: equal H2D slices of n states instead of the built-in schedules
- *   ARTP_SLICE_SCHEDULE=a,b,...  host-buffer calls: slice fractions of a round (e.g. 0.1,0.2,0.3,0.4)
- *   ARTP_TRACE=1            host-buffer calls print the GPU timeline of their slices (copy landed, classify, box stages)
- *   ARTP_K0_FLAGS=2         classify stage without its reach-box vertex probes (measured slower: the boxes land in the queues)
- *   ARTP_FORK_ITEMS=n       rounds of up to n items run their three box kernels side by side on internal streams
- *                           (default: always; 0 = serial order)
- *   ARTP_PIPE_CAPS=g,f      host-buffer calls: grid caps of the per-slice reach kernels in half SM counts (default 4,4)
- * artp_set_timing(h, 1) makes the host-buffer calls run their slices back to back (the per-stage events need one stream):
- * leave it off when measuring end-to-end throughput. */
+ * artp_set_timing(h, 1) makes the host-buffer calls copy their states before the kernels start and run the kernels in
+ * order on one stream (the per-stage events need one stream), so that, as for the *_device calls, the events cover the
+ * call's whole last round of up to 2^20 states: leave it off when measuring end-to-end throughput. */
 
 /* Kernel timing for roofline reporting: when enabled, CUDA events are recorded on the launch stream around the three
  * stages of every check call; artp_get_last_timing waits for the last call's kernels and returns

@@ -1,4 +1,4 @@
-"""e2e probe: host-buffer API throughput for 1M poses vs H2D slice size (env ARTP_SLICE_ITEMS), plus raw H2D bandwidth."""
+"""e2e probe: host-buffer API throughput for 1M poses, plus raw H2D bandwidth."""
 import os, sys, time
 R = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, R)
 import numpy as np, torch
@@ -25,4 +25,4 @@ for f32, h in ((True, hp32), (False, hp)):
     t = time.perf_counter()
     for _ in range(30): chk.isValidHostPtr(h.data_ptr(), len(poses), hv.data_ptr(), f32=f32)
     dt = (time.perf_counter() - t) / 30
-    print(f"slice {os.environ.get('ARTP_SLICE_ITEMS','default')} f32={f32}: {dt*1e3:.3f} ms  {len(poses)/dt/1e9:.3f} e9 poses/s")
+    print(f"f32={f32}: {dt*1e3:.3f} ms  {len(poses)/dt/1e9:.3f} e9 poses/s")
