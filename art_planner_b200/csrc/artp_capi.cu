@@ -494,7 +494,7 @@ int launch_classify(Handle* h, artp::Work w, size_t lo, size_t hi, cudaStream_t 
   w.item_base = (uint32_t)lo;
   w.n_items = (uint32_t)hi;
   BoxQueues* q = &h->d_ctr->q;   // every round appends to the round's queues
-  artp::classify_items_kernel<<<(unsigned)((hi - lo + 127) / 128), 128, 0, s>>>(
+  artp::classify_items_kernel<<<(unsigned)((hi - lo + artp::kClassifyItems - 1) / artp::kClassifyItems), artp::kClassifyItems, 0, s>>>(
       h->chk, w, h->d_recs, h->d_recs_f, h->group_grid ? h->d_recs_g : nullptr, &q->big.end, &q->reach.end, &q->group.end,
       h->mode == 1);
   CU_TRY(h, cudaGetLastError());
