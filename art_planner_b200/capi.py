@@ -118,6 +118,8 @@ def load():
     lib.artp_motion_cost.argtypes = [vp, vp, sz, vp]
     lib.artp_motion_cost_device.argtypes = [vp, vp, sz, vp, vp]
     lib.artp_combine_cost.argtypes = [vp, vp, sz, vp, vp]
+    lib.artp_motion_cost_split.argtypes = [vp, vp, vp, sz, dbl, vp]
+    lib.artp_motion_cost_split_device.argtypes = [vp, vp, vp, sz, vp, sz, vp, vp, vp, vp]
     lib.artp_get_features.argtypes = [vp, vp, sz, C.POINTER(i32), C.POINTER(i32)]
     lib.artp_set_cnn_mode.argtypes = [vp, i32]
     lib.artp_get_cnn_timing.argtypes = [vp, C.POINTER(C.c_float)]

@@ -554,6 +554,68 @@ class MotionCostObjective:
         h.check(h.lib.artp_motion_cost_states(h.h, a.ctypes.data, b.ctypes.data, n, cost.ctypes.data, feas.ctypes.data, c3.ctypes.data))
         return cost, feas, c3
 
+    def motionCost(self, s1, s2) -> float:
+        """MotionCostObjective::motionCost (motion_cost_objective.cpp:36-95) of one edge: a batch of one."""
+        a = np.ascontiguousarray(s1, dtype=np.float64).reshape(1, 7)
+        b = np.ascontiguousarray(s2, dtype=np.float64).reshape(1, 7)
+        return float(self.motionCostBatch(a, b)[0])
+
+    def motionCostBatch(self, s1, s2, max_query_edge_length: float = 0.5, out=None, rows=None, cost3=None):
+        """MotionCostObjective::motionCost for n edges [n, 7] -> float64 [n]: each edge split into
+        (unsigned)(lateralDistance / max_query_edge_length) + 1 pieces, every piece queried, +inf if a piece is too
+        risky, else the ordered sum of getCost. numpy arrays use the host entry point; CUDA float64 tensors the device
+        entry point on the current stream, with the per-edge piece offsets built by torch. rows [>= pieces, 6] float32
+        and cost3 [>= pieces, 3] float32 (CUDA only, optional) receive the piece rows and their (energy, time, risk)."""
+        h, lib = self._c.handle, self._c.handle.lib
+        if _is_torch_cuda(s1):
+            import torch
+            assert s1.dtype == torch.float64 and s2.dtype == torch.float64 and s1.is_contiguous() and s2.is_contiguous()
+            if not max_query_edge_length > 0:
+                raise capi.ArtpError(capi.ARTP_E_INVALID, "max_query_edge_length must be > 0")
+            n = s1.shape[0]
+            if out is None:
+                out = torch.empty(n, dtype=torch.float64, device=s1.device)
+            if n == 0:
+                return out
+            d = torch.sqrt((s2[:, 0] - s1[:, 0]) ** 2 + (s2[:, 1] - s1[:, 1]) ** 2)   # lateralDistance, utils.h:52-61
+            q = d / max_query_edge_length
+            if not bool((q < 2.0 ** 32).all()):
+                raise capi.ArtpError(capi.ARTP_E_INVALID, "edge too long or not finite (n_interp must fit 32 bits)")
+            off = torch.zeros(n + 1, dtype=torch.int64, device=s1.device)
+            off[1:] = torch.cumsum(q.to(torch.int64) + 1, 0)
+            total = int(off[-1].item())
+            if total >= 2 ** 32:
+                raise capi.ArtpError(capi.ARTP_E_INVALID, "too many pieces (>= 2^32)")
+            off32 = off.to(torch.int32)      # two's-complement wrap: the uint32 offsets' bits
+            if rows is None:
+                rows = torch.empty((total, 6), dtype=torch.float32, device=s1.device)
+            if cost3 is None:
+                cost3 = torch.empty((total, 3), dtype=torch.float32, device=s1.device)
+            assert rows.shape[0] >= total and cost3.shape[0] >= total and rows.is_contiguous() and cost3.is_contiguous()
+            h.check(lib.artp_motion_cost_split_device(
+                h.h, C.c_void_p(s1.data_ptr()), C.c_void_p(s2.data_ptr()), n, C.c_void_p(off32.data_ptr()), total,
+                C.c_void_p(rows.data_ptr()), C.c_void_p(cost3.data_ptr()), C.c_void_p(out.data_ptr()), _stream_ptr()))
+            return out
+        a = np.ascontiguousarray(s1, dtype=np.float64)
+        b = np.ascontiguousarray(s2, dtype=np.float64)
+        n = a.shape[0]
+        if out is None:
+            out = np.empty(n, dtype=np.float64)
+        h.check(lib.artp_motion_cost_split(h.h, a.ctypes.data, b.ctypes.data, n, float(max_query_edge_length),
+                                           out.ctypes.data))
+        return out
+
+    def pathCost(self, states, max_query_edge_length: float = 0.5) -> float:
+        """PathGeometric::cost(obj) for this objective (OMPL 1.4.2): 0 for fewer than two states, else the left-to-right
+        sum of motionCost over consecutive states (initial and terminal cost are the identity 0), one batch call."""
+        if len(states) < 2:
+            return 0.0
+        c = self.motionCostBatch(states[:-1], states[1:], max_query_edge_length)
+        total = 0.0
+        for v in c.tolist():   # not sum(): Python's float sum is compensated, the reference's is not
+            total += v
+        return total
+
     def getCost(self, cost3):
         """(cost, feasible) per edge: w_e*E + w_t*T + w_r*R and R <= risk_threshold (motion_cost_objective.h:54-66)."""
         h = self._c.handle

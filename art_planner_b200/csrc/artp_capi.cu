@@ -1403,6 +1403,58 @@ __global__ void combine_cost_kernel(const float* __restrict__ cost3, size_t n, f
   }
 }
 
+// MotionCostObjective::motionCost (motion_cost_objective.cpp:36-95) splits edge e into the pieces piece_off[e] ..
+// piece_off[e+1] - 1 (n_interp + 1 of them). Knot j of the edge is s1 for j = 0, s2 for j = n_interp + 1 (copied, not
+// interpolated) and interpolate(s1, s2, j * (1.0 / (n_interp + 1))) in between (:49, :67); piece i's row is
+// [x y yaw](knot i+1) ++ [x y yaw](knot i) with the casts of edge_matrix_kernel. Built here, in the translation unit
+// without FMA contraction, so that the rows equal the host's bit for bit; the head's translation unit contracts.
+__device__ __forceinline__ void knot_row(const double* s, float* o) {
+  o[0] = (float)s[0]; o[1] = (float)s[1];
+  o[2] = (float)atan2(2 * (s[6] * s[5] + s[3] * s[4]), 1 - 2 * (s[4] * s[4] + s[5] * s[5]));
+}
+__device__ __forceinline__ void split_knot_row(const double* a, const double* b, uint32_t j, uint32_t n_pieces, float* o) {
+  if (j == 0) {
+    knot_row(a, o);
+  } else if (j == n_pieces) {
+    knot_row(b, o);
+  } else {   // no pointer select between a, b and k: that would put all three in local memory
+    double k[7];
+    artp::se3_interpolate(a, b, (double)j * (1.0 / (double)n_pieces), k);
+    knot_row(k, o);
+  }
+}
+__global__ void split_rows_kernel(const double* __restrict__ s1, const double* __restrict__ s2, uint32_t n_edges,
+                                  const uint32_t* __restrict__ piece_off, size_t total, float* __restrict__ rows) {
+  for (size_t p = blockIdx.x * (size_t)blockDim.x + threadIdx.x; p < total; p += (size_t)gridDim.x * blockDim.x) {
+    uint32_t lo = 0, hi = n_edges;          // largest e with piece_off[e] <= p, as load_item_state
+    while (hi - lo > 1) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (__ldg(piece_off + mid) <= p) lo = mid; else hi = mid;
+    }
+    const uint32_t o0 = __ldg(piece_off + lo), n_pieces = __ldg(piece_off + lo + 1) - o0, i = (uint32_t)p - o0;
+    double a[7], b[7];
+#pragma unroll
+    for (int k = 0; k < 7; ++k) { a[k] = s1[(size_t)lo * 7 + k]; b[k] = s2[(size_t)lo * 7 + k]; }
+    split_knot_row(a, b, i + 1, n_pieces, rows + 6 * p);
+    split_knot_row(a, b, i, n_pieces, rows + 6 * p + 3);
+  }
+}
+// The rest of motionCost per edge, one thread walking its pieces in order: +inf at the first piece whose risk is above
+// the threshold (isFeasible), else the left-to-right double sum of getCost from 0.0, the expression of combine_cost_kernel.
+__global__ void split_reduce_kernel(const float* __restrict__ cost3, const uint32_t* __restrict__ piece_off, size_t n,
+                                    float we, float wt, float wr, float thr, double* __restrict__ cost) {
+  for (size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x; e < n; e += (size_t)gridDim.x * blockDim.x) {
+    const uint32_t o0 = piece_off[e], o1 = piece_off[e + 1];
+    double c = 0.0;
+    for (uint32_t k = o0; k < o1; ++k) {
+      const float ce = cost3[3 * (size_t)k], ct = cost3[3 * (size_t)k + 1], cr = cost3[3 * (size_t)k + 2];
+      if ((double)cr > (double)thr) { c = CUDART_INF; break; }
+      c += (double)ce * (double)we + (double)ct * (double)wt + (double)cr * (double)wr;
+    }
+    cost[e] = c;
+  }
+}
+
 int artp_edge_matrix_from_states(const double* s_start, const double* s_target, size_t n, float* edges) {
   if (n && (!s_start || !s_target || !edges)) return ARTP_E_INVALID;
   for (size_t i = 0; i < n; ++i) {
@@ -1972,6 +2024,78 @@ int artp_combine_cost(artp_handle* hh, const float* cost3, size_t n, double* cos
     feasible[i] = (double)cr <= (double)h->p.risk_threshold ? 1 : 0;   // isFeasible (getRisk returns double)
   }
   return ARTP_OK;
+}
+
+static int check_cost_net(Handle* h) {
+  if (!artp_cnn::has_weights(h->cnn)) { h->err = "motion-cost weights not set"; return ARTP_E_NOWEIGHTS; }
+  if (!artp_cnn::has_features(h->cnn)) {
+    h->err = "features not computed (call artp_update_features after artp_set_map)";
+    return ARTP_E_NOWEIGHTS;
+  }
+  return ARTP_OK;
+}
+
+// Touches no per-handle scratch (the head reads the feature map and weights only), so, like artp_motion_cost_device, it
+// joins no scratch group.
+int artp_motion_cost_split_device(artp_handle* hh, const double* d_s1, const double* d_s2, size_t n,
+                                  const uint32_t* d_piece_off, size_t total_pieces, float* d_rows, float* d_cost3,
+                                  double* d_cost, void* stream) {
+  LOCK_HANDLE(h, hh);
+  if (n == 0) return ARTP_OK;
+  if (!d_s1 || !d_s2 || !d_piece_off || !d_rows || !d_cost3 || !d_cost) { h->err = "null buffer"; return ARTP_E_INVALID; }
+  if (total_pieces < n || total_pieces > 0xFFFFFFFFull) {
+    h->err = "total_pieces must lie in [n, 2^32) (every edge has at least one piece)";
+    return ARTP_E_INVALID;
+  }
+  int rc = check_cost_net(h);
+  if (rc) return rc;
+  CU_TRY(h, cudaSetDevice(h->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  split_rows_kernel<<<(unsigned)std::min<size_t>((total_pieces + 255) / 256, (size_t)h->sm_count * 8), 256, 0, s>>>(
+      d_s1, d_s2, (uint32_t)n, d_piece_off, total_pieces, d_rows);
+  CU_TRY(h, cudaGetLastError());
+  if ((rc = artp_cnn::motion_cost(h->cnn, d_rows, total_pieces, d_cost3, s, h->err))) return rc;
+  split_reduce_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)h->sm_count * 8), 256, 0, s>>>(
+      d_cost3, d_piece_off, n, h->p.cost_w_energy, h->p.cost_w_time, h->p.cost_w_risk, h->p.risk_threshold, d_cost);
+  CU_TRY(h, cudaGetLastError());
+  h->stats.kernel_launches += 3;
+  h->stats.last_launches = 3;
+  return ARTP_OK;
+}
+
+int artp_motion_cost_split(artp_handle* hh, const double* s1, const double* s2, size_t n, double max_query_edge_length,
+                           double* cost) {
+  LOCK_HANDLE(h, hh);
+  if (n == 0) return ARTP_OK;
+  if (!s1 || !s2 || !cost) { h->err = "null buffer"; return ARTP_E_INVALID; }
+  if (!(max_query_edge_length > 0.0)) { h->err = "max_query_edge_length must be > 0"; return ARTP_E_INVALID; }
+  int rc = check_cost_net(h);
+  if (rc) return rc;
+  std::vector<uint32_t> off(n + 1);
+  size_t total = 0;
+  for (size_t e = 0; e < n; ++e) {
+    off[e] = (uint32_t)total;
+    // n_interp = (unsigned)(lateralDistance (utils.h:52-61) / max_query_edge_length), motion_cost_objective.cpp:40-45
+    const double dx = s2[7 * e] - s1[7 * e], dy = s2[7 * e + 1] - s1[7 * e + 1];
+    const double q = std::sqrt(dx * dx + dy * dy) / max_query_edge_length;
+    if (!(q < 4294967296.0)) { h->err = "edge too long or not finite (n_interp must fit 32 bits)"; return ARTP_E_INVALID; }
+    total += (size_t)(unsigned int)q + 1;
+    if (total > 0xFFFFFFFFull) { h->err = "too many pieces (>= 2^32)"; return ARTP_E_INVALID; }
+  }
+  off[n] = (uint32_t)total;
+  const size_t sb = n * 7 * sizeof(double);
+  char* r[6];   // s1 | s2 | piece offsets | rows | cost3 | cost
+  rc = host_call_begin(h, {sb, sb, (n + 1) * sizeof(uint32_t), total * 6 * sizeof(float), total * 3 * sizeof(float),
+                           n * sizeof(double)}, r);
+  if (rc) return rc;
+  CU_TRY(h, cudaMemcpyAsync(r[0], s1, sb, cudaMemcpyHostToDevice, h->stream));
+  CU_TRY(h, cudaMemcpyAsync(r[1], s2, sb, cudaMemcpyHostToDevice, h->stream));
+  CU_TRY(h, cudaMemcpyAsync(r[2], off.data(), (n + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
+  rc = artp_motion_cost_split_device(hh, (const double*)r[0], (const double*)r[1], n, (const uint32_t*)r[2], total,
+                                     (float*)r[3], (float*)r[4], (double*)r[5], h->stream);
+  if (rc) return rc;
+  CU_TRY(h, cudaMemcpyAsync(cost, r[5], n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  return host_call_end(h);   // `off` outlives its H2D copy: the call synchronises before it returns
 }
 
 int artp_get_features(artp_handle* hh, float* out, size_t n_floats, int* hf, int* wf) {

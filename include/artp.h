@@ -39,6 +39,10 @@
  *                                   art_planner_motion_cost/scripts/cost_query_server.py:145-169,
  *                                   predictor/predictor.py:28-44, predictor/cost_query.py:39-69)
  *   artp_combine_cost               MotionCostObjective::getCost / isFeasible (motion_cost_objective.h:54-66)
+ *   artp_motion_cost_split[_device] ompl::base::OptimizationObjective::motionCost -> MotionCostObjective::motionCost
+ *                                   (objectives/motion_cost_objective.cpp:36-95), the objective planner_ros.cpp:313-317
+ *                                   installs; callers: path.cost(obj) in Planner::getSolutionPath (planner.cpp:281-283),
+ *                                   opt_->motionCost (lazy_prm_star_min_update.cpp:436)
  */
 #ifndef ARTP_H
 #define ARTP_H
@@ -313,6 +317,20 @@ int artp_motion_cost_states(artp_handle* h, const double* s_start, const double*
 /* MotionCostObjective::getCost / isFeasible (motion_cost_objective.h:54-66) on host arrays:
  * cost[i] = w_e*E + w_t*T + w_r*R, feasible[i] = R <= risk_threshold (weights / threshold from artp_params). */
 int artp_combine_cost(artp_handle* h, const float* cost3, size_t n, double* cost, uint8_t* feasible);
+/* MotionCostObjective::motionCost (motion_cost_objective.cpp:36-95) for n edges: split, query, sum. HOST buffers.
+ * Edge e is split into n_interp + 1 pieces, n_interp = (unsigned)(lateralDistance(s1, s2) / max_query_edge_length)
+ * (params.h:54: 0.5), at the knots s1, interpolate(s1, s2, j * (1.0 / (n_interp + 1))) for j = 1..n_interp, s2; each piece
+ * is one edge-matrix row through the network. cost[e] = +inf when a piece's risk is above risk_threshold, else the
+ * left-to-right double sum of getCost over the pieces. Needs artp_set_cost_weights + artp_update_features (else
+ * ARTP_E_NOWEIGHTS); max_query_edge_length > 0; total pieces < 2^32 (else ARTP_E_INVALID). */
+int artp_motion_cost_split(artp_handle* h, const double* s1, const double* s2, size_t n,
+                           double max_query_edge_length, double* cost);
+/* DEVICE buffers on `stream`: d_piece_off = n + 1 exclusive prefix sums of the per-edge piece counts (n_interp + 1),
+ * total_pieces = d_piece_off[n]; d_rows (total_pieces x 6 floats) and d_cost3 (total_pieces x 3) are caller scratch
+ * that receive the piece rows and their (energy, time, risk). */
+int artp_motion_cost_split_device(artp_handle* h, const double* d_s1, const double* d_s2, size_t n,
+                                  const uint32_t* d_piece_off, size_t total_pieces, float* d_rows, float* d_cost3,
+                                  double* d_cost, void* stream);
 /* Test hooks: feature map copy-out ([Hf][Wf][48] fp32, channels last), kernel selection (bit 0: CUDA-core fp32
  * reference for every layer instead of the tensor-core (wgmma) kernels; any other bit is ARTP_E_INVALID), trunk timings
  * ms3 = (3x3 stack, 15x15 layer, whole trunk) of the last artp_update_features. */

@@ -387,6 +387,7 @@ class MotionCostObjective {
 
   explicit MotionCostObjective(const StateValidityCheckerPtr& checker, std::unique_ptr<MotionCostFunc> func = nullptr)
       : checker_(checker), motion_cost_func_(std::move(func)) {
+    custom_func_ = motion_cost_func_ != nullptr;
     if (!motion_cost_func_) {
       HandlePtr h = checker_->handle();
       motion_cost_func_.reset(new MotionCostFunc([h](const EdgeMatrix& edges, EdgeMatrix* costs) {
@@ -441,6 +442,33 @@ class MotionCostObjective {
   }
   double motionCostHeuristic(const State*, const State*) const { return 0.0; }   // motion_cost_objective.cpp:99-103
 
+  // motionCost for a batch of edges: split, query and sum on the device in one call (artp_motion_cost_split), the same
+  // cost per edge as motionCost. A caller-supplied MotionCostFunc (e.g. the ROS transport) stays the only cost source:
+  // the batch then loops over motionCost. Throws "Motion cost call failed" like motionCost.
+  void motionCostBatch(const std::vector<State>& s1, const std::vector<State>& s2, std::vector<double>* cost) const {
+    if (s1.size() != s2.size()) throw std::invalid_argument("motionCostBatch: size mismatch");
+    cost->resize(s1.size());
+    if (s1.empty()) return;
+    if (custom_func_) {
+      for (size_t e = 0; e < s1.size(); ++e) (*cost)[e] = motionCost(&s1[e], &s2[e]);
+      return;
+    }
+    const auto& h = checker_->handle();
+    if (artp_motion_cost_split(h->get(), &s1[0].x, &s2[0].x, s1.size(), h->params().planner.prm_motion_cost.max_query_edge_length,
+                               cost->data()) != ARTP_OK)
+      throw std::runtime_error("Motion cost call failed");
+  }
+  // ompl::geometric::PathGeometric::cost(obj) (OMPL 1.4.2) for this objective: initial and terminal cost are the identity
+  // 0, so the cost is 0 for fewer than two states, else the left-to-right sum of motionCost over consecutive states.
+  double pathCost(const std::vector<State>& path) const {
+    if (path.size() < 2) return 0.0;
+    std::vector<double> c;
+    motionCostBatch(std::vector<State>(path.begin(), path.end() - 1), std::vector<State>(path.begin() + 1, path.end()), &c);
+    double cost = 0.0;
+    for (double v : c) cost += v;
+    return cost;
+  }
+
   // PRMMotionCostMaintainer::updateEdges / computeCostForVertexEdges (prm_motion_cost.cpp:27-128) for a batch of graph
   // edges (source = v1, target = v2): edge matrix -> cost query -> per edge isFeasible ? getCost : +inf, in one device call.
   // Returns false where the reference's functor would (then the graph is left alone, :69-72 / :124-127).
@@ -480,6 +508,7 @@ class MotionCostObjective {
  private:
   StateValidityCheckerPtr checker_;
   std::unique_ptr<MotionCostFunc> motion_cost_func_;
+  bool custom_func_{false};   // motion_cost_func_ came from the caller
 };
 
 }  // namespace artp_host
