@@ -45,7 +45,6 @@ struct Handle {
   artp::Checker chk;
   float* d_H[2] = {nullptr, nullptr};
   float2* d_T[2][artp::kMaxLevel + 1] = {};
-  uint32_t* d_NF[2][artp::kMaxLevel + 1] = {};   // bit-packed window flags (2 bits per entry)
   uint32_t* d_C[2][artp::kMaxLevel + 1] = {};    // compact conservative copies of d_T (Field::C)
   int pitch = 0;
   int rows = 0, cols = 0;           // full map
@@ -167,15 +166,16 @@ __global__ void build_level_kernel(const float* __restrict__ H, const float2* __
   }
 }
 
-// Compact table level from T (encoding at artp::Field::C): maxCode = the smallest code c >= 1 with dec(c) >= max,
-// minCode = the largest c with dec(c) <= min, both found by bisection over the non-decreasing dec(). A height the
-// codes cannot cover (above dec(kCodeMax)) takes the reserved code 65535, which sends its zones to the exact tables.
-__global__ void build_codes_kernel(const float2* __restrict__ T, uint32_t* __restrict__ C, size_t n, float base, float step) {
+// Compact table level from T and the window flags NF (encoding at artp::Field::C): maxCode = the smallest code c >= 1 with
+// dec(c) >= max, minCode = the largest c with dec(c) <= min, both found by bisection over the non-decreasing dec(). A height
+// the codes cannot cover (above dec(kCodeMax)) takes the reserved code kCodeNone, which sends its zones to the exact tables.
+__global__ void build_codes_kernel(const float2* __restrict__ T, const unsigned char* __restrict__ NF, uint32_t* __restrict__ C,
+                                   size_t n, float base, float step) {
   const float top = artp::code_dec(base, step, artp::kCodeMax);
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const float2 v = T[i];
-    uint32_t cM = 0, cm = 0xFFFFu;
-    if (v.x > top) cM = 0xFFFFu;
+    uint32_t cM = 0, cm = artp::kCodeNone;
+    if (v.x > top) cM = artp::kCodeNone;
     else if (v.x > -CUDART_INF_F) {
       uint32_t lo = 1, hi = artp::kCodeMax;
       while (lo < hi) {
@@ -192,7 +192,7 @@ __global__ void build_codes_kernel(const float2* __restrict__ T, uint32_t* __res
       }
       cm = lo;
     }
-    C[i] = (cM << 16) | cm;
+    C[i] = artp::code_word(cM, cm, NF[i] & 3u);
   }
 }
 
@@ -290,19 +290,6 @@ __global__ void plane_table_query_kernel(const artp::Field f, int x_off, const P
           }
         }
     if (dup) mergeable[(size_t)z * f.pitch + x] = 2;   // races write the same value
-  }
-}
-
-// 16 flag bytes (values 0..3) -> one word of 2-bit fields; the tail of the last word is zero
-__global__ void pack_flags_kernel(const unsigned char* __restrict__ nf, size_t n, uint32_t* __restrict__ out) {
-  const size_t words = (n + 15) / 16;
-  for (size_t w = blockIdx.x * (size_t)blockDim.x + threadIdx.x; w < words; w += (size_t)gridDim.x * blockDim.x) {
-    uint32_t v = 0;
-    for (int i = 0; i < 16; ++i) {
-      const size_t e = w * 16 + i;
-      if (e < n) v |= (uint32_t)(nf[e] & 3) << (2 * i);
-    }
-    out[w] = v;
   }
 }
 
@@ -876,7 +863,7 @@ void artp_destroy(artp_handle* hh) {
   }
   if (h->box_ev) cudaEventDestroy(h->box_ev);
   cudaFree(h->d_slices);
-  for (int k = 0; k < 2; ++k) for (int l = 0; l <= artp::kMaxLevel; ++l) { cudaFree(h->d_T[k][l]); cudaFree(h->d_NF[k][l]); cudaFree(h->d_C[k][l]); }
+  for (int k = 0; k < 2; ++k) for (int l = 0; l <= artp::kMaxLevel; ++l) { cudaFree(h->d_T[k][l]); cudaFree(h->d_C[k][l]); }
   cudaFree(h->d_H[0]); cudaFree(h->d_H[1]); cudaFree(h->d_ctr); cudaFree(h->d_defer); cudaFree(h->d_stage);
   cudaFree(h->d_block_counts); cudaFree(h->d_recs); cudaFree(h->d_recs_f); cudaFree(h->d_recs_g); cudaFree(h->d_samp_layers); cudaFree(h->d_samp_scratch);
   if (h->h_small_out) cudaFreeHost(h->h_small_out);
@@ -1025,8 +1012,8 @@ int artp_set_map_window(artp_handle* hh, const float* elevation, const float* el
     for (int k = 0; k < 2; ++k) {
       cudaFree(h->d_H[k]); h->d_H[k] = nullptr;
       for (int l = 0; l <= artp::kMaxLevel; ++l) {
-        cudaFree(h->d_T[k][l]); cudaFree(h->d_NF[k][l]); cudaFree(h->d_C[k][l]);
-        h->d_T[k][l] = nullptr; h->d_NF[k][l] = nullptr; h->d_C[k][l] = nullptr;
+        cudaFree(h->d_T[k][l]); cudaFree(h->d_C[k][l]);
+        h->d_T[k][l] = nullptr; h->d_C[k][l] = nullptr;
       }
       CU_TRY(h, cudaMalloc(&h->d_H[k], npad * sizeof(float)));
     }
@@ -1035,7 +1022,6 @@ int artp_set_map_window(artp_handle* hh, const float* elevation, const float* el
     for (int l = 1; l <= kmax[k]; ++l)
       if (!h->d_T[k][l]) {
         CU_TRY(h, cudaMalloc(&h->d_T[k][l], npad * sizeof(float2)));
-        CU_TRY(h, cudaMalloc(&h->d_NF[k][l], ((npad + 15) / 16) * sizeof(uint32_t)));
         CU_TRY(h, cudaMalloc(&h->d_C[k][l], npad * sizeof(uint32_t)));
       }
   int rc = grow(h, h->d_stage, h->stage_cap, ncell * sizeof(float));
@@ -1068,10 +1054,9 @@ int artp_set_map_window(artp_handle* hh, const float* elevation, const float* el
       build_level_kernel<<<h->sm_count * 4, 256, 0, h->stream>>>(h->d_H[k], l > 1 ? h->d_T[k][l - 1] : nullptr,
                                                                   l > 1 ? nf_prev : nullptr, d_merge, h->d_T[k][l], nf_cur, nrows,
                                                                   cols, pitch, 1 << (l - 1));
-      pack_flags_kernel<<<h->sm_count * 4, 256, 0, h->stream>>>(nf_cur, npad, h->d_NF[k][l]);
-      build_codes_kernel<<<h->sm_count * 4, 256, 0, h->stream>>>(h->d_T[k][l], h->d_C[k][l], npad, cbase[k], cstep[k]);
+      build_codes_kernel<<<h->sm_count * 4, 256, 0, h->stream>>>(h->d_T[k][l], nf_cur, h->d_C[k][l], npad, cbase[k], cstep[k]);
       CU_TRY(h, cudaGetLastError());
-      h->stats.kernel_launches += 3;
+      h->stats.kernel_launches += 2;
     }
   }
   CU_TRY(h, cudaStreamSynchronize(h->stream));
@@ -1085,7 +1070,6 @@ int artp_set_map_window(artp_handle* hh, const float* elevation, const float* el
     f.cbase = cbase[k]; f.cstep = cstep[k];
     for (int l = 0; l <= artp::kMaxLevel; ++l) {
       f.T[l] = (l >= 1 && l <= kmax[k]) ? h->d_T[k][l] - row0 : nullptr;
-      f.NF[l] = (l >= 1 && l <= kmax[k]) ? h->d_NF[k][l] : nullptr;   // bit-packed: indexed with LOCAL entry numbers, see below
       f.C[l] = (l >= 1 && l <= kmax[k]) ? h->d_C[k][l] - row0 : nullptr;
     }
     h->chk.f[k] = f;

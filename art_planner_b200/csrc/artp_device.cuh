@@ -22,21 +22,22 @@ struct Field {
   int nx, nz;      // m_nWidthSamples (rows), m_nDepthSamples (cols)
   int pitch;       // row stride in floats (multiple of 4 -> 16 B aligned rows)
   // Range tables (exact, idempotent reductions): level k holds, for every (x,z), the reduction over the
-  // 2^k x 2^k vertex window starting there: T[k][x + z*pitch] = (max h, min over finite h or +inf),
-  // NF[k], entry x + z*pitch (bit-packed, see window_flags): bit 0 = the window holds a non-finite height, bit 1 = a cell starting in the window has a
-  // triangle whose plane matches (within eps) the plane of another triangle of the map. Built at artp_set_map, k = 1..kmax.
+  // 2^k x 2^k vertex window starting there: T[k][x + z*pitch] = (max h, min over finite h or +inf). Built at
+  // artp_set_map, k = 1..kmax.
   const float2* T[kMaxLevel + 1];
-  const uint32_t* NF[kMaxLevel + 1];   // 2 flag bits per entry, 16 entries per word: 32x smaller than the (max, min) tables, cache resident
-  // Conservative copies of T[k] at half the size (the classify stage's random lookups then stay in L2):
-  // C[k][i] = (maxCode << 16) | minCode with max in [dec(maxCode - 1), dec(maxCode)] and min in [dec(minCode), dec(minCode + 1)],
-  // dec(c) = cbase + c * cstep (code_dec). Finite heights take max codes 1..65533 and min codes 0..65534; a window without
-  // a finite height has max code 0 (max -inf) and min code 65535 (min +inf). Same pitch and row shift as T.
+  // Conservative copies of T[k] at half the size that also carry the window's flags (the classify stage's random lookups
+  // then stay in L2, one load per window): C[k][i] = (maxCode << 17) | (minCode << 2) | flags (see code_max / code_min /
+  // code_flags) with max in [dec(maxCode - 1), dec(maxCode)] and min in [dec(minCode), dec(minCode + 1)],
+  // dec(c) = cbase + c * cstep (code_dec). Finite heights take max codes 1..kCodeMax and min codes 0..kCodeMax; a window
+  // without a finite height has max code 0 (max -inf) and min code kCodeNone (min +inf). Flag bit 0 = the window holds a
+  // non-finite height, bit 1 = a cell starting in the window has a triangle whose plane matches (within eps) the plane of
+  // another triangle of the map. Same pitch and row shift as T.
   const uint32_t* C[kMaxLevel + 1];
   float cbase, cstep;   // smallest finite height of the stored window; a power of two
   int kmax;
   float W, D, hW, hD, sW, sD, asp, iW, iD;
   float px, py;    // heightfield body position (float casts of the map centre)
-  // Map window (artp_set_map_window): only vertices x in [x_lo, x_hi] are stored (H, T, NF are shifted by -x_lo so that
+  // Map window (artp_set_map_window): only vertices x in [x_lo, x_hi] are stored (H, T, C are shifted by -x_lo so that
   // global indices keep working); nx and all geometry are those of the full map. Whole map: 0, nx - 1.
   int x_lo, x_hi;
 };
@@ -64,17 +65,21 @@ struct BoxCtx {
   int x0, x1, z0, z1;
 };
 
-// flags of range-table entry idx (bit 0 non-finite, bit 1 mergeable); idx is LOCAL to the handle's map window
-// (global entry - x_lo: the packed words cannot be shifted by a pointer offset the way the float2 tables are)
-__device__ __forceinline__ int window_flags(const uint32_t* __restrict__ nf, size_t idx) {
-  return (int)((__ldg(nf + (idx >> 4)) >> ((idx & 15) * 2)) & 3u);
-}
-
 // Height of code c of the compact range tables. The host builds the codes with this same function (both sides are
 // compiled without FMA contraction): c * step is exact, and the rounded sum is non-decreasing in c, so every bound
 // the codes state holds by construction.
-constexpr uint32_t kCodeMax = 65533;   // largest code of a finite max; the host picks cstep so that dec(kCodeMax) >= max
+constexpr uint32_t kCodeMax = 32765;    // largest code of a finite max; the host picks cstep so that dec(kCodeMax) >= max
+constexpr uint32_t kCodeNone = 32767;   // reserved: a max above dec(kCodeMax) / a window without a finite min
 __host__ __device__ __forceinline__ float code_dec(float base, float step, uint32_t c) { return base + (float)c * step; }
+__host__ __device__ __forceinline__ uint32_t code_word(uint32_t cM, uint32_t cm, uint32_t flags) {
+  return (cM << 17) | (cm << 2) | flags;
+}
+// A zone's codes from its windows' words: the max code is the top field, so it is the top field of the words' unsigned max;
+// the min code over the words' low 17 bits (min code and flags) is the min code of their minimum; the flags reduce by OR.
+__device__ __forceinline__ uint32_t code_max(uint32_t max_of_words) { return max_of_words >> 17; }
+__device__ __forceinline__ uint32_t code_min_key(uint32_t w) { return w & 0x1FFFFu; }
+__device__ __forceinline__ uint32_t code_min(uint32_t min_of_keys) { return min_of_keys >> 2; }
+__device__ __forceinline__ uint32_t code_flags(uint32_t or_of_words) { return or_of_words & 3u; }
 
 // nextafterf(x, -inf) / nextafterf(x, +inf) for finite x (dNextAfter, ode/include/ode/common.h:296), as integer ops.
 __device__ __forceinline__ float next_down(float x) {

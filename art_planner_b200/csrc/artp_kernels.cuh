@@ -121,12 +121,15 @@ __device__ __forceinline__ void load_item_state(const Work& w, uint32_t item, do
     return;
   }
   if (!w.edge_mode) {
+    // Each state is read once: streaming loads (evict first in L1 and L2), so the pose stream does not push the range
+    // tables that classify reads at random out of L2. (Edge mode keeps the default: every step of an edge reads its
+    // endpoints again.)
     if (w.s2f) {
 #pragma unroll
-      for (int k = 0; k < 7; ++k) s[k] = (double)w.s2f[(size_t)item * 7 + k];   // exact; cast back to float downstream
+      for (int k = 0; k < 7; ++k) s[k] = (double)__ldcs(w.s2f + (size_t)item * 7 + k);   // exact; cast back to float downstream
     } else {
 #pragma unroll
-      for (int k = 0; k < 7; ++k) s[k] = w.s2[(size_t)item * 7 + k];
+      for (int k = 0; k < 7; ++k) s[k] = __ldcs(w.s2 + (size_t)item * 7 + k);
     }
     return;
   }
@@ -191,7 +194,7 @@ __device__ __forceinline__ int zone_early_out(const BoxCtx& b, float maxY, float
 constexpr int kZoneUnknown = -4;
 __device__ __forceinline__ int zone_early_out_codes(const Field& f, const BoxCtx& b, uint32_t cM, uint32_t cm,
                                                     bool allFinite) {
-  if (cM == 0 || cM == 0xFFFFu || cm == 0xFFFFu) return kZoneUnknown;
+  if (cM == 0 || cM == kCodeNone || cm == kCodeNone) return kZoneUnknown;
   const float mxLo = code_dec(f.cbase, f.cstep, cM - 1), mxHi = code_dec(f.cbase, f.cstep, cM);
   const float mnLo = code_dec(f.cbase, f.cstep, cm), mnHi = code_dec(f.cbase, f.cstep, cm + 1);
   if (b.minB - mxHi > -ARTP_EPS) return R_FREE;                                            // above
@@ -697,35 +700,37 @@ __device__ __forceinline__ int zone_classify(const Checker& c, const BoxCtx& b, 
     if (force_all || kk < 1 || kk > f.kmax || cx * cz > 32) {
       r = -1; fl |= REC_NEEDS_REDUCE;
     } else {
-      // Zone codes from the compact tables first (half the bytes of T: they stay in L2); the exact T entries are read only
-      // when the codes' intervals leave a test open.
+      // Zone codes and flags from the compact tables first (one word per window, half the bytes of T: they stay in L2);
+      // the exact T entries are read only when the codes' intervals leave a test open.
       const uint32_t* __restrict__ C = f.C[kk];
-      const uint32_t* __restrict__ NF = f.NF[kk];
       const int sW = 1 << kk;
-      uint32_t cM = 0, cm = 0xFFFFu;
-      int nf = 0;
-      const bool quad = cx <= 2 && cz <= 2;
-      const int xs0 = b.x0, xs1 = b.x1 - sW + 1, zs0 = b.z0, zs1 = b.z1 - sW + 1;
-      const size_t i00 = (size_t)zs0 * f.pitch + xs0, i01 = (size_t)zs0 * f.pitch + xs1,
-                   i10 = (size_t)zs1 * f.pitch + xs0, i11 = (size_t)zs1 * f.pitch + xs1;
-      if (quad) {
-        // the common case (window edge > half the zone edge): all four windows are requested before any is used
-        const uint32_t w0 = __ldg(C + i00), w1 = __ldg(C + i01), w2 = __ldg(C + i10), w3 = __ldg(C + i11);
-        const int n0 = window_flags(NF, i00 - f.x_lo), n1 = window_flags(NF, i01 - f.x_lo), n2 = window_flags(NF, i10 - f.x_lo), n3 = window_flags(NF, i11 - f.x_lo);
-        cM = max(max(w0 >> 16, w1 >> 16), max(w2 >> 16, w3 >> 16));
-        cm = min(min(w0 & 0xFFFFu, w1 & 0xFFFFu), min(w2 & 0xFFFFu, w3 & 0xFFFFu));
-        nf = n0 | n1 | n2 | n3;
+      const int xs1 = b.x1 - sW + 1, zs1 = b.z1 - sW + 1;   // the last window starts
+      uint32_t wmax = 0, wmin = 0xFFFFFFFFu, wor = 0;
+      if (cx * cz <= 8) {
+        // The short side of the zone holds at most two windows (kk is the floor of its log2), so the windows start on a
+        // 4 x 2 grid (8 x 1 when the short side holds one), long side first. All eight words are requested before any
+        // is used; a start past the zone's last window clamps to that window (max, min and OR are idempotent).
+        const bool zlong = cz > cx;
+        const int sh = min(cx, cz) - 1;
+        uint32_t wv[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int a = j >> sh, s = j & sh;   // window along the long / short side
+          const int ix = zlong ? s : a, iz = zlong ? a : s;
+          wv[j] = __ldg(C + (size_t)min(b.z0 + iz * sW, zs1) * f.pitch + min(b.x0 + ix * sW, xs1));
+        }
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { wmax = max(wmax, wv[j]); wmin = min(wmin, code_min_key(wv[j])); wor |= wv[j]; }
       } else {
         for (int iz = 0; iz < cz; ++iz) {
           const int zs = min(b.z0 + iz * sW, zs1);
           for (int ix = 0; ix < cx; ++ix) {
-            const size_t idx = (size_t)zs * f.pitch + min(b.x0 + ix * sW, xs1);
-            const uint32_t wv = __ldg(C + idx);
-            cM = max(cM, wv >> 16); cm = min(cm, wv & 0xFFFFu);
-            nf |= window_flags(NF, idx - f.x_lo);
+            const uint32_t wv = __ldg(C + (size_t)zs * f.pitch + min(b.x0 + ix * sW, xs1));
+            wmax = max(wmax, wv); wmin = min(wmin, code_min_key(wv)); wor |= wv;
           }
         }
       }
+      const uint32_t cM = code_max(wmax), cm = code_min(wmin), nf = code_flags(wor);
       const bool allFinite = (nf & 1) == 0;
       r = zone_early_out_codes(f, b, cM, cm, allFinite);
       if (r == kZoneUnknown) {

@@ -31,6 +31,7 @@ import bench
 from art_planner_b200 import synth
 
 SUB = 250   # cells per side of the sub-square
+CODE_MAX = 32765   # artp::kCodeMax: the largest code of a finite max in the compact range tables
 
 
 def sub_square_poses(m, n):
@@ -98,9 +99,9 @@ def fallback_rate(m, poses):
         fin_all = L[np.isfinite(L)].astype(np.float32)
         base, top = fin_all.min(), fin_all.max()
         e = -126
-        while base + np.float32(65533) * np.float32(2.0 ** e) < top:
+        while base + np.float32(CODE_MAX) * np.float32(2.0 ** e) < top:
             e += 1
-        dec = base + np.arange(65536, dtype=np.float32) * np.float32(2.0 ** e)
+        dec = base + np.arange(CODE_MAX + 3, dtype=np.float32) * np.float32(2.0 ** e)
         sel = np.nonzero((x1 - x0 >= 1) & (z1 - z0 >= 1))[0]
         mx = np.full(len(sel), -np.inf, np.float32)
         mn = np.full(len(sel), np.inf, np.float32)
@@ -112,9 +113,9 @@ def fallback_rate(m, poses):
             if f.any():
                 mx[a], mn[a] = zone[f].max(), zone[f].min()
         ok = np.isfinite(mx)
-        cM = np.searchsorted(dec[1:65534], mx, "left") + 1
-        cm = np.searchsorted(dec[:65534], mn, "right") - 1
-        cM, cm = np.clip(cM, 1, 65533), np.clip(cm, 0, 65533)
+        cM = np.searchsorted(dec[1:CODE_MAX + 1], mx, "left") + 1
+        cm = np.searchsorted(dec[:CODE_MAX + 1], mn, "right") - 1
+        cM, cm = np.clip(cM, 1, CODE_MAX), np.clip(cm, 0, CODE_MAX)
         mxLo, mxHi, mnLo, mnHi = dec[cM - 1], dec[cM], dec[cm], dec[cm + 1]
         minB, maxB = lo_b[sel].astype(np.float32), hi_b[sel].astype(np.float32)
         above_t, above_f = minB - mxHi > -eps, ~(minB - mxLo > -eps)
