@@ -3,7 +3,8 @@ pose validity (ODE box-vs-heightfield torso/feet checks), edge validity over int
 edge cost, behind a C ABI (include/artp.h) and a host-side mirror of the reference's plugin interface."""
 from . import synth  # noqa: F401
 from .capi import ArtpError  # noqa: F401
-from .checker import (MotionCostObjective, MotionValidator, PathLengthObjective, SE3FromSE2Sampler,  # noqa: F401
-                      StateValidityChecker)
+from .checker import (GoalStateRegion, MotionCostObjective, MotionValidator, PathLengthObjective,  # noqa: F401
+                      SE3FromSE2Sampler, StartState, StateValidityChecker)
 
-__all__ = ["synth", "ArtpError", "StateValidityChecker", "MotionValidator", "PathLengthObjective", "MotionCostObjective", "SE3FromSE2Sampler"]
+__all__ = ["synth", "ArtpError", "StateValidityChecker", "MotionValidator", "PathLengthObjective", "MotionCostObjective", "SE3FromSE2Sampler",
+           "StartState", "GoalStateRegion"]

@@ -91,6 +91,11 @@ def load():
     lib.artp_sample_states_device.argtypes = [vp, vp, u64, u64, sz, vp, vp, vp]
     lib.artp_sample_valid.argtypes = [vp, u64, u64, sz, vp, sz, C.POINTER(C.c_size_t)]
     lib.artp_sample_valid_device.argtypes = [vp, u64, u64, sz, vp, sz, vp, vp]
+    u32 = C.c_uint32
+    lib.artp_find_valid_near.argtypes = [vp, vp, sz, vp, u32, vp, u64, u64, vp, vp]
+    lib.artp_find_valid_near_device.argtypes = [vp, vp, sz, vp, u32, vp, u64, u64, vp, vp, vp]
+    lib.artp_ball_offsets.argtypes = [vp, u64, u64, sz, u32, vp, vp]
+    lib.artp_pose_from_2d.argtypes = [vp, vp, sz, vp, vp]
     lib.artp_path_length_cost.argtypes = [vp, vp, vp, sz, vp]
     lib.artp_path_length_cost_device.argtypes = [vp, vp, vp, sz, vp, vp]
     lib.artp_compact_valid_device.argtypes = [vp, vp, sz, C.c_int64, vp, vp, vp]

@@ -194,6 +194,59 @@ class StateValidityChecker:
                                                           None if row is None else row.ctypes.data))
         return (cum, row) if want_host else None
 
+    def findValidNear(self, centres, radius, n_iter: int, offsets=None, seed: int = 0, first_draw: int = 0):
+        """StartState / GoalStateRegion::sampleGoal (start.cpp:7-41, goal.cpp:11-41) for n queries in one call: the first
+        valid of the centre and the centre moved in x / y by offsets 1..n_iter; none valid -> the last candidate. centres
+        [n, 7] float64, radius scalar or [n], offsets [n, n_iter, 2] or None (the Philox "ARTB" stream from first_draw,
+        see artp.h). Returns (states [n, 7], index int32 [n]: candidate k, or -1). CUDA float64 tensors go through the
+        device entry point on the current stream (radius and offsets then CUDA tensors too)."""
+        lib, h = self._h.lib, self._h
+        if not 0 <= int(n_iter) < 2 ** 32:
+            raise capi.ArtpError(capi.ARTP_E_INVALID, "n_iter must lie in [0, 2^32)")
+        if _is_torch_cuda(centres):
+            import torch
+            assert centres.dtype == torch.float64 and centres.is_contiguous() and centres.shape[-1] == 7
+            n = centres.shape[0]
+            r = torch.as_tensor(radius, dtype=torch.float64, device=centres.device).expand(n).contiguous()
+            off = None if offsets is None else offsets.contiguous()
+            assert off is None or (off.dtype == torch.float64 and off.numel() == n * int(n_iter) * 2)
+            out = torch.empty((n, 7), dtype=torch.float64, device=centres.device)
+            idx = torch.empty(n, dtype=torch.int32, device=centres.device)
+            h.check(lib.artp_find_valid_near_device(h.h, C.c_void_p(centres.data_ptr()), n, C.c_void_p(r.data_ptr()), int(n_iter),
+                                                    None if off is None else C.c_void_p(off.data_ptr()), int(seed), int(first_draw),
+                                                    C.c_void_p(out.data_ptr()), C.c_void_p(idx.data_ptr()), _stream_ptr()))
+            return out, idx
+        c = np.ascontiguousarray(centres, dtype=np.float64).reshape(-1, 7)
+        n = c.shape[0]
+        r = np.ascontiguousarray(np.broadcast_to(np.asarray(radius, dtype=np.float64), (n,)))
+        off = None
+        if offsets is not None:
+            off = np.ascontiguousarray(offsets, dtype=np.float64)
+            assert off.size == n * int(n_iter) * 2
+        out = np.empty((n, 7), np.float64)
+        idx = np.empty(n, np.int32)
+        h.check(lib.artp_find_valid_near(h.h, c.ctypes.data, n, r.ctypes.data, int(n_iter), None if off is None else off.ctypes.data,
+                                         int(seed), int(first_draw), out.ctypes.data, idx.ctypes.data))
+        return out, idx
+
+    def ballOffsets(self, seed: int, first_draw: int, n: int, n_iter: int, radius):
+        """The [n, n_iter, 2] offsets findValidNear draws from its stream (offsets=None) for the same seed / first_draw."""
+        lib, h = self._h.lib, self._h
+        r = np.ascontiguousarray(np.broadcast_to(np.asarray(radius, dtype=np.float64), (n,)))
+        out = np.empty((n, int(n_iter), 2), np.float64)
+        h.check(lib.artp_ball_offsets(h.h, int(seed), int(first_draw), n, int(n_iter), r.ctypes.data, out.ctypes.data))
+        return out
+
+    def poseFrom2D(self, states):
+        """The goal projection of Planner::plan (planner.cpp:223-237, Map::get3DPoseFrom2D map.cpp:77-90) on the device:
+        states [n, 7] -> (states [n, 7], inside uint8 [n]); states off the map come back unchanged with inside == 0.
+        Needs the current map's normals (estimateNormals, or a sampler set with host normal layers)."""
+        s = np.ascontiguousarray(states, dtype=np.float64).reshape(-1, 7)
+        out = np.empty_like(s)
+        inside = np.empty(s.shape[0], np.uint8)
+        self._h.check(self._h.lib.artp_pose_from_2d(self._h.h, s.ctypes.data, s.shape[0], out.ctypes.data, inside.ctypes.data))
+        return out, inside
+
     def isValidBatchBits(self, states, out_valid, out_bits):
         """One shard step of the multi-GPU path: verdict bytes + bit-packed mask (CUDA float64 states), one call."""
         n = states.shape[0]
@@ -362,6 +415,45 @@ class SE3FromSE2Sampler:
         h, lib = self._c.handle, self._c.handle.lib
         h.check(lib.artp_sample_valid_device(h.h, self.seed, int(first), n_draw, C.c_void_p(out.data_ptr()), out.shape[0],
                                              C.c_void_p(count.data_ptr()), _stream_ptr()))
+
+
+class StartState:
+    """art_planner::StartState (start.h, start.cpp:7-41): the start pose repaired by a disc search around it, one device
+    call per sampleGoal. Offsets come from the Philox "ARTB" stream of `seed`; the draw position advances by what the
+    reference's loop consumes: k draws when candidate k is returned, n_iter when none is valid, none for a valid centre."""
+
+    def __init__(self, checker: StateValidityChecker, seed: int = 0):
+        self._c = checker
+        self.seed = int(seed)
+        self.draw = 0
+        self._state = None
+        self.threshold = 0.0
+        self.max_num_samples = 0
+
+    def setState(self, state) -> None:
+        self._state = np.array(state, dtype=np.float64).reshape(7)
+
+    def setThreshold(self, threshold: float) -> None:
+        self.threshold = float(threshold)
+
+    def setMaxNumSamples(self, n: int) -> None:
+        self.max_num_samples = int(n)
+
+    def sampleGoal(self, state=None):
+        """The repaired state (written into `state` [7] if given) and its candidate index (-1: none valid; the state is
+        then the last candidate drawn, like the reference)."""
+        out, idx = self._c.findValidNear(self._state.reshape(1, 7), self.threshold, self.max_num_samples, seed=self.seed,
+                                         first_draw=self.draw)
+        k = int(idx[0])
+        self.draw += k if k >= 0 else self.max_num_samples
+        if state is not None:
+            state[:] = out[0]
+            return state, k
+        return out[0], k
+
+
+class GoalStateRegion(StartState):
+    """art_planner::GoalStateRegion (goal.h, goal.cpp:11-41): the same search, called by OMPL from inside solve()."""
 
 
 class MotionValidator:

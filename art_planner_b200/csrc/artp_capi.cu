@@ -85,6 +85,7 @@ struct Handle {
   bool has_sampler = false;
   bool has_device_normals = false;  // artp_estimate_normals filled normal_x/y/z/std_dev of d_samp_layers for this map
   bool has_device_cdf = false;      // artp_compute_sample_cdf filled cum_prob / cum_row of d_samp_layers for this map
+  bool has_normals = false;         // normal_x/y/z of d_samp_layers hold this map's normals (device-estimated or the caller's)
   char* d_samp_scratch = nullptr;
   size_t samp_scratch_cap = 0;
   uint8_t* h_small_out = nullptr;   // mapped pinned host bytes the latency-path kernel writes its verdicts to
@@ -1144,6 +1145,7 @@ int artp_set_map_window(artp_handle* hh, const float* elevation, const float* el
   h->has_sampler = false;      // its layers belong to the previous map
   h->has_device_normals = false;
   h->has_device_cdf = false;
+  h->has_normals = false;
   return ARTP_OK;
 }
 
@@ -1588,8 +1590,19 @@ static int ensure_sampler_layers(Handle* h) {
   if (h->samp_layers_cap < need) {   // the layers computed on the device go with the old buffer
     h->has_device_normals = false;
     h->has_device_cdf = false;
+    h->has_normals = false;
   }
   return grow(h, h->d_samp_layers, h->samp_layers_cap, need);
+}
+
+// The map fields of the sampler's view (geometry, elevation, normal and plane-fit layers of d_samp_layers).
+static void sampler_map_view(Handle* h, artp::SamplerDev& m) {
+  const size_t ncell = (size_t)h->rows * h->cols;
+  float* base = h->d_samp_layers;
+  m.elevation_rev = h->d_H[0]; m.pitch = h->pitch;
+  m.normal_x = base; m.normal_y = base + ncell; m.normal_z = base + 2 * ncell; m.std_dev = base + 3 * ncell;
+  m.rows = h->rows; m.cols = h->cols;
+  m.res = h->chk.Lx / h->rows; m.cx = h->chk.cx; m.cy = h->chk.cy;
 }
 
 int artp_estimate_normals(artp_handle* hh, double estimation_radius, float* normal_x, float* normal_y, float* normal_z,
@@ -1615,6 +1628,7 @@ int artp_estimate_normals(artp_handle* hh, double estimation_radius, float* norm
     if (dst[k]) CU_TRY(h, cudaMemcpyAsync(dst[k], base + k * ncell, ncell * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
   if ((rc = host_call_end(h))) return rc;
   h->has_device_normals = true;
+  h->has_normals = true;
   h->has_sampler = false;          // the sampler must be (re)armed with artp_set_sampler
   h->stats.kernel_launches += 1;
   h->stats.last_launches = 1;
@@ -1682,13 +1696,11 @@ int artp_set_sampler(artp_handle* hh, const artp_sampler_params* sp, const float
     for (int k = 0; k < 4; ++k)
       CU_TRY(h, cudaMemcpyAsync(base + k * ncell, src[k], ncell * sizeof(float), cudaMemcpyHostToDevice, h->stream));
     h->has_device_normals = false;   // overwritten by the caller's layers
+    h->has_normals = true;
   }
   artp::SamplerDev& m = h->samp;
-  m.elevation_rev = h->d_H[0]; m.pitch = h->pitch;
-  m.normal_x = base; m.normal_y = base + ncell; m.normal_z = base + 2 * ncell; m.std_dev = base + 3 * ncell;
+  sampler_map_view(h, m);
   m.cum_prob = nullptr; m.cum_row = nullptr;
-  m.rows = h->rows; m.cols = h->cols;
-  m.res = h->chk.Lx / h->rows; m.cx = h->chk.cx; m.cy = h->chk.cy;
   m.max_roll_pert = sp->max_roll_pert; m.max_pitch_pert = sp->max_pitch_pert;
   m.from_distribution = sp->sample_from_distribution ? 1 : 0;
   m.low[0] = sp->low[0]; m.low[1] = sp->low[1]; m.high[0] = sp->high[0]; m.high[1] = sp->high[1];
@@ -1870,6 +1882,133 @@ int artp_sample_valid(artp_handle* hh, uint64_t seed, uint64_t first_sample, siz
   }
   *n_valid = cnt;      // > capacity means the output was truncated to `capacity` states
   return rc;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Start / goal repair: StartState / GoalStateRegion::sampleGoal (start.cpp:7-41, goal.cpp:11-41), and the goal's
+// projection onto the map (planner.cpp:223-237, map.cpp:77-90)
+// ---------------------------------------------------------------------------------------------------------------
+// Argument checks shared by both forms; `radius` only when it is a host buffer.
+static int ball_search_args(Handle* h, size_t n, uint32_t n_iter, const double* radius) {
+  if (!h->has_map) { h->err = "no map set"; return ARTP_E_NOMAP; }
+  if ((uint64_t)n >= (1ull << 32) || n * ((uint64_t)n_iter + 1) >= (1ull << 32)) {
+    h->err = "n * (n_iter + 1) candidates must be < 2^32"; return ARTP_E_INVALID;
+  }
+  if (radius)
+    for (size_t q = 0; q < n; ++q)
+      if (!(radius[q] >= 0.0 && std::isfinite(radius[q]))) { h->err = "radius must be finite and >= 0"; return ARTP_E_INVALID; }
+  return ARTP_OK;
+}
+
+int artp_find_valid_near_device(artp_handle* hh, const double* d_centres, size_t n, const double* d_radius, uint32_t n_iter,
+                                const double* d_offsets, uint64_t seed, uint64_t first_draw, double* d_states_out,
+                                int32_t* d_index, void* stream) {
+  LOCK_HANDLE(h, hh);
+  int rc = ball_search_args(h, n, n_iter, nullptr);
+  if (rc) return rc;
+  if (n == 0) return ARTP_OK;
+  if (!d_centres || !d_radius || !d_states_out || !d_index) { h->err = "null buffer"; return ARTP_E_INVALID; }
+  CU_TRY(h, cudaSetDevice(h->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  ChainScope cs(h, 0, s);
+  if (cs.rc) return cs.rc;
+  const uint64_t total = n * ((uint64_t)n_iter + 1);
+  const size_t chunk = (size_t)std::min<uint64_t>(total, kSampleChunk);
+  // scratch: candidate states f32 | verdicts | first valid candidate per query
+  const size_t o_val = (chunk * 7 * sizeof(float) + 255) & ~(size_t)255, o_best = o_val + ((chunk + 255) & ~(size_t)255);
+  if ((rc = grow(h, h->d_samp_scratch, h->samp_scratch_cap, o_best + n * sizeof(uint32_t)))) return rc;
+  float* d_sf = (float*)h->d_samp_scratch;
+  uint8_t* d_val = (uint8_t*)(h->d_samp_scratch + o_val);
+  uint32_t* d_best = (uint32_t*)(h->d_samp_scratch + o_best);
+  artp::BallSearch b{d_centres, d_radius, d_offsets, seed, first_draw, n_iter};
+  CU_TRY(h, cudaMemsetAsync(d_best, 0xFF, n * sizeof(uint32_t), s));
+  uint32_t launches = 0;
+  for (uint64_t c0 = 0; c0 < total; c0 += chunk) {
+    const size_t m = (size_t)std::min<uint64_t>(chunk, total - c0);
+    artp::ball_candidates_kernel<<<grid_for(h, m, 128), 128, 0, s>>>(b, c0, m, d_sf);
+    CU_TRY(h, cudaGetLastError());
+    artp::Work w;
+    w.s1 = nullptr; w.s2 = nullptr; w.s2f = d_sf; w.valid = d_val; w.item_base = 0; w.n_items = (uint32_t)m; w.steps = 0;
+    w.edge_mode = 0;
+    if ((rc = run_items(h, w, s))) return rc;
+    launches += h->stats.last_launches + 2;
+    artp::ball_first_valid_kernel<<<grid_for(h, m, 256), 256, 0, s>>>(d_val, c0, m, n_iter, d_best);
+    CU_TRY(h, cudaGetLastError());
+    h->stats.kernel_launches += 2;
+    h->stats.poses_checked += m;
+  }
+  artp::ball_result_kernel<<<grid_for(h, n, 128), 128, 0, s>>>(b, n, d_best, d_states_out, d_index);
+  CU_TRY(h, cudaGetLastError());
+  h->stats.kernel_launches += 1;
+  h->stats.last_launches = launches + 1;
+  return ARTP_OK;
+}
+
+int artp_find_valid_near(artp_handle* hh, const double* centres, size_t n, const double* radius, uint32_t n_iter,
+                         const double* offsets, uint64_t seed, uint64_t first_draw, double* states_out, int32_t* index) {
+  LOCK_HANDLE(h, hh);
+  if (n && (!centres || !radius || !states_out || !index)) { h->err = "null buffer"; return ARTP_E_INVALID; }
+  int rc = ball_search_args(h, n, n_iter, radius);
+  if (rc) return rc;
+  if (n == 0) return ARTP_OK;
+  const size_t sb = n * 7 * sizeof(double), ob = offsets ? n * (size_t)n_iter * 2 * sizeof(double) : 0;
+  char* r[5];   // centres | radius | offsets | states | index
+  if ((rc = host_call_begin(h, {sb, n * sizeof(double), ob, sb, n * sizeof(int32_t)}, r))) return rc;
+  CU_TRY(h, cudaMemcpyAsync(r[0], centres, sb, cudaMemcpyHostToDevice, h->stream));
+  CU_TRY(h, cudaMemcpyAsync(r[1], radius, n * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  if (ob) CU_TRY(h, cudaMemcpyAsync(r[2], offsets, ob, cudaMemcpyHostToDevice, h->stream));
+  rc = artp_find_valid_near_device(hh, (const double*)r[0], n, (const double*)r[1], n_iter, offsets ? (const double*)r[2] : nullptr,
+                                   seed, first_draw, (double*)r[3], (int32_t*)r[4], h->stream);
+  if (rc) return rc;
+  CU_TRY(h, cudaMemcpyAsync(states_out, r[3], sb, cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(h, cudaMemcpyAsync(index, r[4], n * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+  return host_call_end(h, true);
+}
+
+int artp_ball_offsets(artp_handle* hh, uint64_t seed, uint64_t first_draw, size_t n, uint32_t n_iter, const double* radius,
+                      double* offsets) {
+  LOCK_HANDLE(h, hh);
+  const size_t total = n * (size_t)n_iter;
+  if (total == 0) return ARTP_OK;
+  if (!radius || !offsets) { h->err = "null buffer"; return ARTP_E_INVALID; }
+  if ((uint64_t)n >= (1ull << 32)) { h->err = "n must be < 2^32"; return ARTP_E_INVALID; }
+  char* r[2];   // radius | offsets
+  int rc = host_call_begin(h, {n * sizeof(double), total * 2 * sizeof(double)}, r);
+  if (rc) return rc;
+  CU_TRY(h, cudaMemcpyAsync(r[0], radius, n * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  artp::ball_offsets_kernel<<<grid_for(h, total, 256), 256, 0, h->stream>>>(seed, first_draw, n, n_iter, (const double*)r[0],
+                                                                            (double*)r[1]);
+  CU_TRY(h, cudaGetLastError());
+  CU_TRY(h, cudaMemcpyAsync(offsets, r[1], total * 2 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if ((rc = host_call_end(h))) return rc;
+  h->stats.kernel_launches += 1;
+  h->stats.last_launches = 1;
+  return ARTP_OK;
+}
+
+int artp_pose_from_2d(artp_handle* hh, const double* states_in, size_t n, double* states_out, uint8_t* inside) {
+  LOCK_HANDLE(h, hh);
+  if (!h->has_map) { h->err = "no map set"; return ARTP_E_NOMAP; }
+  if (h->win_rows != h->rows) { h->err = "not available on a map window (artp_set_map_window)"; return ARTP_E_INVALID; }
+  if (!h->has_normals) {
+    h->err = "no normal layers for this map (artp_estimate_normals or artp_set_sampler after artp_set_map)"; return ARTP_E_INVALID;
+  }
+  if (n == 0) return ARTP_OK;
+  if (!states_in || !states_out) { h->err = "null buffer"; return ARTP_E_INVALID; }
+  char* r[3];   // states in | states out | inside
+  int rc = host_call_begin(h, {n * 7 * sizeof(double), n * 7 * sizeof(double), n}, r);
+  if (rc) return rc;
+  artp::SamplerDev m{};
+  sampler_map_view(h, m);
+  CU_TRY(h, cudaMemcpyAsync(r[0], states_in, n * 7 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  artp::pose_from_2d_kernel<<<grid_for(h, n, 128), 128, 0, h->stream>>>(m, (const double*)r[0], n, (double*)r[1], (uint8_t*)r[2]);
+  CU_TRY(h, cudaGetLastError());
+  CU_TRY(h, cudaMemcpyAsync(states_out, r[1], n * 7 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (inside) CU_TRY(h, cudaMemcpyAsync(inside, r[2], n, cudaMemcpyDeviceToHost, h->stream));
+  if ((rc = host_call_end(h))) return rc;
+  h->stats.kernel_launches += 1;
+  h->stats.last_launches = 1;
+  return ARTP_OK;
 }
 
 // cv::circle(kernel, (r, r), r, 255, FILLED) on a size x size zero image, r = size / 2 (utils.cpp:106-111): OpenCV's

@@ -26,6 +26,13 @@
  *                                   ompl::base::StateSampler::sampleUniform -> SE3FromSE2Sampler::sampleUniform
  *                                   (src/sampler.cpp:82-131, positions :40-77) and the rejection loops around it
  *                                   (prm_motion_cost.cpp:171-194, lazy_prm_star_min_update.cpp:549-556)
+ *   artp_find_valid_near[_device], artp_ball_offsets
+ *                                   StartState::sampleGoal (src/start.cpp:7-41, called from Planner::setStartAndGoal,
+ *                                   planner.cpp:167-189) and GoalStateRegion::sampleGoal (src/goal.cpp:11-41, called by
+ *                                   OMPL inside ss_->solve): the centre, then up to n_iter uniformInBall offsets in x / y,
+ *                                   each through isValid, first valid wins
+ *   artp_pose_from_2d               the goal's projection in Planner::plan (planner.cpp:223-237): grid_map isInside, then
+ *                                   Map::get3DPoseFrom2D (src/map/map.cpp:77-90) + setSO3FromRPY (utils.h:101-115)
  *   artp_estimate_normals           art_planner::estimateNormals (src/utils.cpp:213-324; processors::Basic, basic.cpp:47)
  *   artp_compute_sample_cdf         computeCumulativeProbabilityDistribution
  *                                   (src/map/processors/probability_distribution.cpp:20-46)
@@ -210,6 +217,38 @@ int artp_sample_valid(artp_handle* h, uint64_t seed, uint64_t first_sample, size
                       size_t capacity, size_t* n_valid);
 int artp_sample_valid_device(artp_handle* h, uint64_t seed, uint64_t first_sample, size_t n_draw, double* d_states_out,
                              size_t capacity, uint32_t* d_count, void* stream);
+
+/* ---- StartState / GoalStateRegion::sampleGoal (src/start.cpp:7-41, src/goal.cpp:11-41) on the device ---------------
+ * n independent searches. For query q, candidate 0 is centres[q] unchanged; candidate k = 1..n_iter is centres[q] with
+ * x += off[q][k-1][0], y += off[q][k-1][1] (double adds; z and the quaternion stay). states_out[q] = the first candidate, in
+ * the order 0, 1, .., n_iter, that isValid accepts, and index[q] = its k. When none is valid, states_out[q] = candidate
+ * n_iter (the last drawn one: what the reference's caller is left holding, since its `state = nullptr` only clears a
+ * local) and index[q] = -1. All n * (n_iter + 1) candidates are checked in one pass.
+ * Offsets: offsets != NULL gives them (n x n_iter x 2 doubles); NULL draws them from the counter-based stream
+ *   Philox4x32-10(key = seed, counter = (draw lo, draw hi, q, "ARTB")), draw = first_draw + k - 1,
+ *   u0, u1 = the two doubles of that block taken as in artp_sampler_uniforms, off = radius[q] * sqrt(u1) * (cos 2 pi u0,
+ *   sin 2 pi u0).
+ * That is the distribution of OMPL's RNG::uniformInBall(radius) in 2-D (uniform direction, radius r * u^(1/2)) but not its
+ * stream, which is a serial mt19937: feed OMPL's own offsets to reproduce a reference run exactly. The reference draws k
+ * offsets when it returns candidate k, n_iter when none is valid, none when the centre is valid.
+ * radius: n doubles, finite and >= 0 (host form: else ARTP_E_INVALID; the device form does not read them back to check).
+ * n < 2^32 and n * (n_iter + 1) < 2^32, else ARTP_E_INVALID. On a map window a candidate whose boxes leave the window is
+ * invalid and the call raises ARTP_E_WINDOW, as every check does. */
+int artp_find_valid_near(artp_handle* h, const double* centres, size_t n, const double* radius, uint32_t n_iter,
+                         const double* offsets, uint64_t seed, uint64_t first_draw, double* states_out, int32_t* index);
+int artp_find_valid_near_device(artp_handle* h, const double* d_centres, size_t n, const double* d_radius, uint32_t n_iter,
+                                const double* d_offsets, uint64_t seed, uint64_t first_draw, double* d_states_out,
+                                int32_t* d_index, void* stream);
+/* The stream's offsets (n x n_iter x 2 doubles, host) that artp_find_valid_near draws with offsets == NULL. */
+int artp_ball_offsets(artp_handle* h, uint64_t seed, uint64_t first_draw, size_t n, uint32_t n_iter, const double* radius,
+                      double* offsets);
+/* The goal projection of Planner::plan (planner.cpp:223-237): for a state whose (x, y) lies on the map (grid_map isInside
+ * and getIndexFromPosition), z = the cell's "elevation", roll = -atan2(nb.y, nb.z), pitch = atan2(nb.x, nb.z) with
+ * nb = AngleAxisd(yaw, UnitZ)^-1 * the cell's normal, yaw = getYawFromSO3 (double atan2 returned as float), and the
+ * quaternion from setSO3FromRPY; x and y are not moved. Other states are copied unchanged with inside[i] = 0 (nullable).
+ * HOST buffers. Needs the normal layers of the current map (artp_estimate_normals, or artp_set_sampler with host layers),
+ * else ARTP_E_INVALID; ARTP_E_INVALID on a map window. The bounds clip before it (enforceBounds) stays with OMPL. */
+int artp_pose_from_2d(artp_handle* h, const double* states_in, size_t n, double* states_out, uint8_t* inside);
 
 /* PathLengthObjective::motionCost for n edges -> cost[n] (double). */
 int artp_path_length_cost(artp_handle* h, const double* s1, const double* s2, size_t n, double* cost);

@@ -189,6 +189,29 @@ class StateValidityChecker {
     return drawn;
   }
 
+  // StartState / GoalStateRegion::sampleGoal (start.cpp:7-41, goal.cpp:11-41) for a batch of queries in one device call
+  // (artp_find_valid_near): per query the first valid of the centre and the centre moved in x / y by offsets 1..n_iter,
+  // else the last candidate with index -1. offsets: n x n_iter x 2 doubles, or nullptr for the "ARTB" Philox stream.
+  void findValidNearBatch(const std::vector<State>& centres, const std::vector<double>& radius, uint32_t n_iter,
+                          const double* offsets, uint64_t seed, uint64_t first_draw, std::vector<State>* states,
+                          std::vector<int32_t>* index) const {
+    if (radius.size() != centres.size()) throw std::invalid_argument("findValidNearBatch: size mismatch");
+    states->resize(centres.size());
+    index->resize(centres.size());
+    if (centres.empty()) return;
+    handle_->check(artp_find_valid_near(handle_->get(), &centres[0].x, centres.size(), radius.data(), n_iter, offsets, seed,
+                                        first_draw, &(*states)[0].x, index->data()), "artp_find_valid_near");
+  }
+
+  // The goal projection of Planner::plan (planner.cpp:223-237): states on the map get z and roll / pitch from the map
+  // (Map::get3DPoseFrom2D, map.cpp:77-90), the others are copied with inside = 0. Needs the map's normals (estimateNormals).
+  void poseFrom2D(const std::vector<State>& in, std::vector<State>* out, std::vector<uint8_t>* inside) const {
+    out->resize(in.size());
+    inside->resize(in.size());
+    if (in.empty()) return;
+    handle_->check(artp_pose_from_2d(handle_->get(), &in[0].x, in.size(), &(*out)[0].x, inside->data()), "artp_pose_from_2d");
+  }
+
   const HandlePtr& handle() const { return handle_; }
 
  private:
@@ -196,6 +219,41 @@ class StateValidityChecker {
   std::shared_ptr<Map> map_;
 };
 using StateValidityCheckerPtr = std::shared_ptr<StateValidityChecker>;
+
+// art_planner::StartState (start.h, start.cpp:7-41): the start repaired by a disc search around it, in one device call.
+// Offsets come from the "ARTB" Philox stream of `seed` (artp.h); the draw position advances by what the reference's loop
+// consumes from its RNG: k draws when candidate k is returned, n_iter when none is valid, none for a valid centre.
+// sampleGoal writes the repaired state (the last candidate when none is valid, like the reference) and returns its
+// candidate index, -1 when none is valid.
+class StartState {
+ public:
+  StartState(const StateValidityCheckerPtr& checker, uint64_t seed) : checker_(checker), seed_(seed) {}
+  void setState(const State& state) { state_ = state; }
+  void setThreshold(double threshold) { threshold_ = threshold; }
+  void setMaxNumSamples(const unsigned int& num_samples) { max_num_samples_ = num_samples; }
+  int sampleGoal(State* state) const {
+    std::vector<State> out;
+    std::vector<int32_t> index;
+    checker_->findValidNearBatch({state_}, {threshold_}, max_num_samples_, nullptr, seed_, next_, &out, &index);
+    *state = out[0];
+    next_ += index[0] >= 0 ? static_cast<uint64_t>(index[0]) : max_num_samples_;
+    return index[0];
+  }
+  uint64_t nextDraw() const { return next_; }
+ private:
+  StateValidityCheckerPtr checker_;
+  uint64_t seed_;
+  mutable uint64_t next_{0};
+  State state_;
+  double threshold_{0.0};
+  unsigned int max_num_samples_{0};
+};
+
+// art_planner::GoalStateRegion (goal.h, goal.cpp:11-41): the same search; OMPL calls it from inside solve().
+class GoalStateRegion : public StartState {
+ public:
+  using StartState::StartState;
+};
 
 // art_planner::SE3FromSE2Sampler (sampler.cpp:13-131): sampleUniform on the device, one candidate per Philox counter,
 // and the rejection loop around it (prm_motion_cost.cpp:171-194) as one fused sample -> isValid -> compact call.
@@ -518,7 +576,9 @@ class MotionCostObjective {
 #include <ompl/base/MotionValidator.h>
 #include <ompl/base/SpaceInformation.h>
 #include <ompl/base/StateValidityChecker.h>
+#include <ompl/base/goals/GoalState.h>
 #include <ompl/base/objectives/PathLengthOptimizationObjective.h>
+#include <ompl/util/RandomNumbers.h>
 #include <ompl/base/spaces/SE3StateSpace.h>
 namespace artp_host {
 namespace ob = ompl::base;
@@ -556,6 +616,37 @@ class OmplMotionValidator : public ob::MotionValidator {
  private:
   StateValidityCheckerPtr c_;
 };
+// StartState / GoalStateRegion as OMPL goals (start.h, goal.h: ob::GoalState with setThreshold / setMaxNumSamples).
+// sampleGoal draws its n_iter offsets from its own ompl::RNG::uniformInBall, as the reference loop does, and checks all
+// candidates in one call with those offsets: the result is the reference's for the same RNG. Only the RNG's position
+// afterwards differs, since this draws all n_iter offsets every time.
+class OmplDiscSearchGoal : public ob::GoalState {
+ public:
+  OmplDiscSearchGoal(const ob::SpaceInformationPtr& si, const StateValidityCheckerPtr& c) : ob::GoalState(si), c_(c) {}
+  void setMaxNumSamples(const unsigned int& num_samples) { max_num_samples_ = num_samples; }
+  void sampleGoal(ob::State* state) const override {
+    std::vector<double> off(2 * static_cast<size_t>(max_num_samples_)), o(2);
+    for (unsigned int i = 0; i < max_num_samples_; ++i) {
+      rng_.uniformInBall(threshold_, o);
+      off[2 * i] = o[0]; off[2 * i + 1] = o[1];
+    }
+    const std::vector<State> centre{fromOmpl(state_)};
+    std::vector<State> out;
+    std::vector<int32_t> index;
+    c_->findValidNearBatch(centre, {threshold_}, max_num_samples_, off.data(), 0, 0, &out, &index);
+    si_->copyState(state, state_);
+    auto* s = state->as<ob::SE3StateSpace::StateType>();
+    s->setX(out[0].x);
+    s->setY(out[0].y);
+  }
+ private:
+  StateValidityCheckerPtr c_;
+  unsigned int max_num_samples_{0};
+  mutable ompl::RNG rng_;
+};
+class OmplStartState : public OmplDiscSearchGoal { public: using OmplDiscSearchGoal::OmplDiscSearchGoal; };
+class OmplGoalStateRegion : public OmplDiscSearchGoal { public: using OmplDiscSearchGoal::OmplDiscSearchGoal; };
+
 class OmplPathLengthObjective : public ob::PathLengthOptimizationObjective {
  public:
   OmplPathLengthObjective(const ob::SpaceInformationPtr& si, const StateValidityCheckerPtr& c)
