@@ -118,7 +118,10 @@ def load():
     lib.artp_get_last_stage_timing.argtypes = [vp, C.POINTER(C.c_float)]
     lib.artp_version.restype = C.c_char_p
     lib.artp_cost_weights_size.restype = C.c_size_t
+    lib.artp_cost_weights_size_for.restype = C.c_size_t
+    lib.artp_cost_weights_size_for.argtypes = [i32]
     lib.artp_set_cost_weights.argtypes = [vp, vp, sz]
+    lib.artp_get_cost_network.argtypes = [vp, C.POINTER(i32)]
     lib.artp_update_features.argtypes = [vp]
     lib.artp_motion_cost.argtypes = [vp, vp, sz, vp]
     lib.artp_motion_cost_device.argtypes = [vp, vp, sz, vp, vp]

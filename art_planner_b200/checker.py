@@ -596,13 +596,23 @@ class MotionCostObjective:
         self._c = checker
 
     def setWeights(self, state_dict) -> None:
-        """Parameters keyed like the reference module's state_dict (numpy arrays or torch tensors)."""
+        """Parameters keyed like the reference module's state_dict (numpy arrays or torch tensors) of either
+        network_light or network: a torch.load of either kind of .pt goes straight in. The state dict picks the network
+        (init_conv1 has 24 or 32 output channels); call updateFeatures again after a change of network."""
         from . import costnet
         sd = {k: (v.detach().cpu().numpy() if hasattr(v, "detach") else np.asarray(v)) for k, v in state_dict.items()}
         blob = costnet.pack_blob(sd)
         h = self._c.handle
-        assert blob.size == h.lib.artp_cost_weights_size()
+        assert blob.size == h.lib.artp_cost_weights_size_for(costnet.NETWORKS[costnet.network_of(sd)][1])
         h.check(h.lib.artp_set_cost_weights(h.h, blob.ctypes.data, blob.size))
+
+    def network(self) -> str:
+        """"light" (network_light.py) or "full" (network.py): the architecture of the loaded weights."""
+        from . import costnet
+        h = self._c.handle
+        net = C.c_int()
+        h.check(h.lib.artp_get_cost_network(h.h, C.byref(net)))
+        return next(name for name, (_, v) in costnet.NETWORKS.items() if v == net.value)
 
     def updateFeatures(self) -> None:
         """CostPredictor.updateFeatures over the checker's current map (predictor.py:28-36)."""
@@ -719,11 +729,13 @@ class MotionCostObjective:
         return cost, feas
 
     def features(self):
-        """[Hf, Wf, 48] float32 feature map (test hook)."""
+        """[Hf, Wf, C] float32 feature map (test hook); C = 48 for network_light, 64 for network."""
+        from . import costnet
         h = self._c.handle
         hf, wf = C.c_int(), C.c_int()
         h.check(h.lib.artp_get_features(h.h, None, 0, C.byref(hf), C.byref(wf)))
-        out = np.empty((hf.value, wf.value, 48), dtype=np.float32)
+        ch = costnet.NETWORKS[self.network()][0][5][2]   # init_flatten's output channels
+        out = np.empty((hf.value, wf.value, ch), dtype=np.float32)
         h.check(h.lib.artp_get_features(h.h, out.ctypes.data, out.size, C.byref(hf), C.byref(wf)))
         return out
 

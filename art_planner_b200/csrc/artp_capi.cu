@@ -2097,7 +2097,20 @@ int artp_process_basic(artp_handle* hh, const float* elevation, const float* tra
   return ARTP_OK;
 }
 
-size_t artp_cost_weights_size(void) { return artp_cnn::blob_floats(); }
+static_assert(ARTP_COST_NET_LIGHT == artp_cnn::kNetLight && ARTP_COST_NET_FULL == artp_cnn::kNetFull,
+              "the ABI's network numbers are the library's");
+
+size_t artp_cost_weights_size(void) { return artp_cnn::blob_floats(ARTP_COST_NET_LIGHT); }
+
+size_t artp_cost_weights_size_for(int network) { return artp_cnn::blob_floats(network); }
+
+int artp_get_cost_network(artp_handle* hh, int* network) {
+  LOCK_HANDLE(h, hh);
+  if (!network) return ARTP_E_INVALID;
+  *network = artp_cnn::network(h->cnn);
+  if (*network < 0) { h->err = "motion-cost weights not set"; return ARTP_E_NOWEIGHTS; }
+  return ARTP_OK;
+}
 
 int artp_set_cost_weights(artp_handle* hh, const float* blob, size_t n_floats) {
   LOCK_HANDLE(h, hh);

@@ -4,6 +4,8 @@
 //   CNNpart :78-110  conv3x3(1->24)+BN, conv3x3(24->24)+BN+LReLU(0.3), maxpool 2/2, conv3x3(24->48)+BN+LReLU,
 //                    conv3x3(48->48)+BN+LReLU, maxpool 3/1, conv3x3(48->48)+BN+LReLU, conv15x15(48->48)+BN+LReLU
 //   FCpart  :113-165 and CostQuery.__call__ (cost_query.py:39-69), server centring (cost_query_server.py:160-161)
+// and the full-width network.py (same file but for the widths: 32 where light has 24, 64 where it has 48, out0 80->64,
+// out1 64->32 x 3). The weight blob's length picks the network (kNets); every kernel below is instantiated for both.
 //
 // Numerics: the reference evaluates in fp16; parity here is against the fp32 evaluation of the same module to 1e-4
 // relative, so everything accumulates in fp32 and the 15x15 convolution -- 83.6 % of the FLOPs, implicit GEMM
@@ -48,17 +50,36 @@ namespace artp_cnn {
     if (_e != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(_e); return -3; } \
   } while (0)
 
+// The widths that tell the two architectures apart: c1 = init_conv1/2, c3 = init_conv3..5 and init_flatten (the
+// feature channels), nh = out0_conv1, b = out1_conv1..3 (the out2 convs read b and give 1 each).
+struct NetDims { int c1, c3, nh, b[3]; };
+constexpr NetDims kNets[kNumNetworks] = {{24, 48, 48, {24, 24, 36}},    // kNetLight: network_light.py
+                                         {32, 64, 64, {32, 32, 32}}};   // kNetFull: network.py
+
 struct LayerDef { int cout, cin, k; bool bn; };
-static const LayerDef kLayers[14] = {
-    {24, 1, 3, true},  {24, 24, 3, true}, {48, 24, 3, true}, {48, 48, 3, true}, {48, 48, 3, true}, {48, 48, 15, true},
-    {16, 10, 1, true}, {48, 64, 1, true}, {24, 48, 1, true}, {24, 48, 1, true}, {36, 48, 1, true},
-    {1, 24, 1, false}, {1, 24, 1, false}, {1, 36, 1, false}};
+// Layer l of the blob order: init_conv1..5, init_flatten, tar0_conv1, out0_conv1, out1_conv1..3, out2_conv1..3.
+static LayerDef layer_def(int net, int l) {
+  const NetDims& d = kNets[net];
+  if (l == 0) return {d.c1, 1, 3, true};
+  if (l == 1) return {d.c1, d.c1, 3, true};
+  if (l == 2) return {d.c3, d.c1, 3, true};
+  if (l <= 4) return {d.c3, d.c3, 3, true};
+  if (l == 5) return {d.c3, d.c3, 15, true};
+  if (l == 6) return {16, 10, 1, true};
+  if (l == 7) return {d.nh, d.c3 + 16, 1, true};
+  if (l <= 10) return {d.b[l - 8], d.nh, 1, true};
+  return {1, d.b[l - 11], 1, false};
+}
 static const float kBnEps = 1e-5f;
 __device__ constexpr float kWScale = 1024.0f;   // undone exactly in the 15x15 epilogue
 
-size_t blob_floats() {
+size_t blob_floats(int net) {
+  if (net < 0 || net >= kNumNetworks) return 0;
   size_t n = 0;
-  for (const auto& l : kLayers) n += (size_t)l.cout * l.cin * l.k * l.k + (l.bn ? 4 * l.cout : l.cout);
+  for (int i = 0; i < 14; ++i) {
+    const LayerDef l = layer_def(net, i);
+    n += (size_t)l.cout * l.cin * l.k * l.k + (l.bn ? 4 * l.cout : l.cout);
+  }
   return n;
 }
 
@@ -247,10 +268,25 @@ __device__ __forceinline__ void wgmma_rs<32>(float (&d)[16], const uint32_t (&a)
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1)
       : "memory");
 }
+template <>
+__device__ __forceinline__ void wgmma_rs<64>(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+      "%24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(1)
+      : "memory");
+}
 
 constexpr int kTileY = 16, kTileX = 8;           // output tile: M = 128 pixels = two warpgroups of 8 image rows x 8
-constexpr int kWStages = 3;
 constexpr int kConvThreads = 288;                // warps 0..7 = two MMA warpgroups (+ epilogue), warp 8 = TMA producer
+constexpr int kMaxSmem = 227 * 1024;             // dynamic shared memory one block may use on sm_90
 
 template <int KS, int NOUT>
 struct ConvCfg {
@@ -258,8 +294,12 @@ struct ConvCfg {
   static constexpr int kBrickX = ((kTileX + KS - 1) + 7) & ~7;   // row pitch = whole swizzle atoms (8 pixels = 1024 B)
   static constexpr int kBrickBytes = kBrickY * kBrickX * 128;    // per split term
   static constexpr int kWStageBytes = 2 * NOUT * 128;            // hi + lo weight tile of one tap
-  static constexpr int kSmem = 2 * kBrickBytes + kWStages * kWStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-  static_assert(kSmem <= 227 * 1024, "conv tile does not fit the 227 KB of shared memory a block may use");
+  static constexpr int kFixed = 2 * kBrickBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  // A three-deep weight ring where it fits. The full network's 15x15 layer (two 92 KB bricks, 16 KB per tap at N = 64)
+  // would need 234 752 B with three stages, over the limit, so it runs with two (DESIGN.md section 4.3).
+  static constexpr int kWStages = kFixed + 3 * kWStageBytes <= kMaxSmem ? 3 : 2;
+  static constexpr int kSmem = kFixed + kWStages * kWStageBytes;
+  static_assert(kSmem <= kMaxSmem, "conv tile does not fit the 227 KB of shared memory a block may use");
 };
 
 // Implicit-GEMM convolution on wgmma (see the file header). KS x KS taps, KSTEPS x 16 input channels multiplied per
@@ -273,7 +313,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
                   const float* __restrict__ bias, float* __restrict__ out, __half* __restrict__ out_hi,
                   __half* __restrict__ out_lo, int OH, int OW, int cout) {
   using Cfg = ConvCfg<KS, NOUT>;
-  constexpr int kTaps = KS * KS, kNA = NOUT / 2;
+  constexpr int kTaps = KS * KS, kNA = NOUT / 2, kWStages = Cfg::kWStages;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   unsigned char* a_hi = smem;
@@ -408,12 +448,14 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
 
 // First layer (Cin = 1, no activation after its BN) on CUDA cores, reading the map layer directly and writing the
 // fp16 hi/lo NHWC-64 input of the second layer. One thread per (pixel, group of 8 output channels): the eight threads of
-// a pixel write its two 128-byte rows as sixteen 16-byte stores; channels 24..63 are zero.
+// a pixel write its two 128-byte rows as sixteen 16-byte stores; channels C1..63 are zero.
+template <int C1>
 __global__ void __launch_bounds__(256) conv1_split_kernel(const float* __restrict__ layer, int H, int W, int pitch,
-                                                          const float* __restrict__ wf /*[9][1][24]*/, const float* __restrict__ bias,
+                                                          const float* __restrict__ wf /*[9][1][C1]*/, const float* __restrict__ bias,
                                                           __half* __restrict__ hi, __half* __restrict__ lo) {
-  __shared__ float sw[9 * 24 + 24];
-  for (int i = threadIdx.x; i < 9 * 24 + 24; i += blockDim.x) sw[i] = i < 216 ? wf[i] : bias[i - 216];
+  static_assert(C1 % 8 == 0 && C1 <= 64, "C1 output channels fill whole 8-channel groups of a 64-channel pixel row");
+  __shared__ float sw[9 * C1 + C1];
+  for (int i = threadIdx.x; i < 9 * C1 + C1; i += blockDim.x) sw[i] = i < 9 * C1 ? wf[i] : bias[i - 9 * C1];
   __syncthreads();
   const int OH = H - 2, OW = W - 2;
   const size_t total = (size_t)OH * OW * 8;
@@ -424,7 +466,7 @@ __global__ void __launch_bounds__(256) conv1_split_kernel(const float* __restric
     const int oy = (int)(p % OH), ox = (int)(p / OH);
     const size_t pix = (size_t)oy * OW + ox;
     __half2 hh[4], ll[4];
-    if (v4 < 3) {
+    if (v4 < C1 / 8) {
       float in[9];
 #pragma unroll
       for (int t = 0; t < 9; ++t) in[t] = __ldg(layer + (size_t)(ox + t % 3) * pitch + (H - 1 - (oy + t / 3)));   // E[r][c]
@@ -434,9 +476,9 @@ __global__ void __launch_bounds__(256) conv1_split_kernel(const float* __restric
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int n = 8 * v4 + 2 * e2 + e;
-          float a = sw[216 + n];
+          float a = sw[9 * C1 + n];
 #pragma unroll
-          for (int t = 0; t < 9; ++t) a = fmaf(in[t], sw[t * 24 + n], a);
+          for (int t = 0; t < 9; ++t) a = fmaf(in[t], sw[t * C1 + n], a);
           f[e] = a;
         }
         const __half h0 = __float2half_rn(f[0]), h1 = __float2half_rn(f[1]);
@@ -509,20 +551,22 @@ __global__ void fold_tc_kernel(const float* __restrict__ w /*[cout][cin][taps]*/
   }
 }
 
-// Reference implementation of the 15x15 layer on CUDA cores (fp32), used by the self-check entry point only.
-__global__ void conv15_reference_kernel(const float* __restrict__ in /*[H][W][48]*/, int H, int W,
-                                        const float* __restrict__ wf /*[225][48][48]*/, const float* __restrict__ bias,
+// Reference implementation of the 15x15 layer on CUDA cores (fp32, C channels in and out), used by the self-check
+// entry point only.
+template <int C>
+__global__ void conv15_reference_kernel(const float* __restrict__ in /*[H][W][C]*/, int H, int W,
+                                        const float* __restrict__ wf /*[225][C][C]*/, const float* __restrict__ bias,
                                         float* __restrict__ out) {
   const int OH = H - 14, OW = W - 14;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= OH * OW * 48) return;
-  const int n = i % 48, p = i / 48, ox = p % OW, oy = p / OW;
+  if (i >= OH * OW * C) return;
+  const int n = i % C, p = i / C, ox = p % OW, oy = p / OW;
   float acc = 0.0f;
   for (int ky = 0; ky < 15; ++ky)
     for (int kx = 0; kx < 15; ++kx) {
-      const float* ip = in + ((size_t)(oy + ky) * W + ox + kx) * 48;
-      const float* wp = wf + (size_t)(ky * 15 + kx) * 48 * 48 + n;
-      for (int c = 0; c < 48; ++c) acc = fmaf(ip[c], wp[c * 48], acc);
+      const float* ip = in + ((size_t)(oy + ky) * W + ox + kx) * C;
+      const float* wp = wf + (size_t)(ky * 15 + kx) * C * C + n;
+      for (int c = 0; c < C; ++c) acc = fmaf(ip[c], wp[c * C], acc);
     }
   const float f = acc + bias[n];
   out[i] = f > 0.0f ? f : 0.3f * f;
@@ -531,14 +575,20 @@ __global__ void conv15_reference_kernel(const float* __restrict__ in /*[H][W][48
 // ------------------------------------------------------------------------------------------------
 // Query head: CostQuery.__call__ + FCpart, one thread per query, folded weights in shared memory.
 // ------------------------------------------------------------------------------------------------
-// folded head weights: tar0 [10][16]+b[16], out0 [64][48]+b[48], o11 [48][24]+b, o12 [48][24]+b, o13 [48][36]+b,
-// o21 [24]+b[1], o22 [24]+b[1], o23 [36]+b[1]
-constexpr int kHeadFloats = 10 * 16 + 16 + 64 * 48 + 48 + 48 * 24 + 24 + 48 * 24 + 24 + 48 * 36 + 36 + 24 + 1 + 24 + 1 + 36 + 1;
+// folded head weights (CF feature channels, out0 width NH, out1 widths B1..B3; light: 48, 48, 24/24/36): tar0
+// [10][16]+b[16], out0 [CF+16][NH]+b[NH], o11 [NH][B1]+b, o12 [NH][B2]+b, o13 [NH][B3]+b, o21 [B1]+b[1], o22 [B2]+b[1],
+// o23 [B3]+b[1]
+__host__ __device__ constexpr int head_floats(int cf, int nh, int b1, int b2, int b3) {
+  return 10 * 16 + 16 + (cf + 16) * nh + nh + (nh + 1) * (b1 + b2 + b3) + (b1 + b2 + b3) + 3;
+}
 
-__global__ void __launch_bounds__(128) head_kernel(const float* __restrict__ feats /*[Hf][Wf][48]*/, int Hf, int Wf,
+// The widths are template parameters so that x / h stay in registers, fully unrolled, for either network.
+template <int CF, int NH, int B1, int B2, int B3>
+__global__ void __launch_bounds__(128) head_kernel(const float* __restrict__ feats /*[Hf][Wf][CF]*/, int Hf, int Wf,
                                                     const float* __restrict__ hw, const float* __restrict__ edges, size_t n,
                                                     float* __restrict__ cost3, double res, double Lx, double Ly, double cx,
                                                     double cy) {
+  constexpr int kIn = CF + 16, kHeadFloats = head_floats(CF, NH, B1, B2, B3);
   extern __shared__ float sw[];
   for (int i = threadIdx.x; i < kHeadFloats; i += blockDim.x) sw[i] = hw[i];
   __syncthreads();
@@ -555,11 +605,11 @@ __global__ void __launch_bounds__(128) head_kernel(const float* __restrict__ fea
   rr = fmin(fmax(rr, 1.0), (double)(Hf - 2));
   cc = fmin(fmax(cc, 1.0), (double)(Wf - 2));
   const int row = (int)rr, col = (int)cc;   // .long() truncation
-  float x[64];
+  float x[kIn];
   {
-    const float4* fp = reinterpret_cast<const float4*>(feats + ((size_t)row * Wf + col) * 48);
+    const float4* fp = reinterpret_cast<const float4*>(feats + ((size_t)row * Wf + col) * CF);
 #pragma unroll
-    for (int i = 0; i < 12; ++i) { const float4 v = __ldg(fp + i); x[4 * i] = v.x; x[4 * i + 1] = v.y; x[4 * i + 2] = v.z; x[4 * i + 3] = v.w; }
+    for (int i = 0; i < CF / 4; ++i) { const float4 v = __ldg(fp + i); x[4 * i] = v.x; x[4 * i + 1] = v.y; x[4 * i + 2] = v.z; x[4 * i + 3] = v.w; }
   }
   const float dx = (float)tx, dy = (float)ty;
   float ang = (float)tyaw;
@@ -575,35 +625,35 @@ __global__ void __launch_bounds__(128) head_kernel(const float* __restrict__ fea
     float a = w[160 + o];
 #pragma unroll
     for (int i = 0; i < 10; ++i) a = fmaf(info[i], w[i * 16 + o], a);
-    x[48 + o] = a;
+    x[CF + o] = a;
   }
   w += 176;
-  float h[48];
+  float h[NH];
 #pragma unroll
-  for (int o = 0; o < 48; ++o) h[o] = w[64 * 48 + o];
-  for (int i = 0; i < 64; ++i) {
+  for (int o = 0; o < NH; ++o) h[o] = w[kIn * NH + o];
+  for (int i = 0; i < kIn; ++i) {
     const float v = x[i];
 #pragma unroll
-    for (int o = 0; o < 48; ++o) h[o] = fmaf(v, w[i * 48 + o], h[o]);
+    for (int o = 0; o < NH; ++o) h[o] = fmaf(v, w[i * NH + o], h[o]);
   }
 #pragma unroll
-  for (int o = 0; o < 48; ++o) h[o] = h[o] > 0.0f ? h[o] : 0.3f * h[o];
-  w += 64 * 48 + 48;
+  for (int o = 0; o < NH; ++o) h[o] = h[o] > 0.0f ? h[o] : 0.3f * h[o];
+  w += kIn * NH + NH;
   float outv[3];
-  const int widths[3] = {24, 24, 36};
-  const float* w2 = w + (48 * 24 + 24) * 2 + 48 * 36 + 36;
+  const int widths[3] = {B1, B2, B3};
+  const float* w2 = w + NH * (B1 + B2 + B3) + (B1 + B2 + B3);
   for (int b = 0; b < 3; ++b) {
     const int nb = widths[b];
     float acc2 = 0.0f;
     for (int o = 0; o < nb; ++o) {
-      float a = w[48 * nb + o];
-      for (int i = 0; i < 48; ++i) a = fmaf(h[i], w[i * nb + o], a);
+      float a = w[NH * nb + o];
+      for (int i = 0; i < NH; ++i) a = fmaf(h[i], w[i * nb + o], a);
       a = a > 0.0f ? a : 0.3f * a;
       acc2 = fmaf(a, w2[o], acc2);
     }
     acc2 += w2[nb];
     outv[b] = acc2;
-    w += 48 * nb + nb;
+    w += NH * nb + nb;
     w2 += nb + 1;
   }
   cost3[3 * q + 0] = fmaxf(outv[0], 0.0f);                        // power  (ReLU)
@@ -612,9 +662,12 @@ __global__ void __launch_bounds__(128) head_kernel(const float* __restrict__ fea
 }
 
 // Fold the head's 1x1 convs (+BN) into [Cin][Cout] matrices + bias, in head_kernel's order.
-__global__ void fold_head_kernel(const float* __restrict__ blob, const size_t* __restrict__ offs, float* __restrict__ hw) {
+struct HeadDims { int cin[8], cout[8]; };   // blob layers 6..13
+__global__ void fold_head_kernel(const float* __restrict__ blob, const size_t* __restrict__ offs, HeadDims d,
+                                 float* __restrict__ hw) {
   // offs[l] = offset of layer l (6..13) in the blob; single block
-  const int cin[8] = {10, 64, 48, 48, 48, 24, 24, 36}, cout[8] = {16, 48, 24, 24, 36, 1, 1, 1};
+  const int* cin = d.cin;
+  const int* cout = d.cout;
   int o = 0;
   for (int l = 0; l < 8; ++l) {
     const float* w = blob + offs[l];
@@ -648,15 +701,19 @@ struct TcLayer { __half *whi = nullptr, *wlo = nullptr; int nout = 0; };
 struct State {
   int device = 0, sm_count = 0;
   bool has_weights = false, has_features = false;
+  // The loaded network (-1: none yet). Weight buffers, activation buffers, tensor maps and kernel attributes are all
+  // sized for it and are released when a blob of the other network arrives.
+  int net = -1;
+  LayerDef layers[14];
   float* d_blob = nullptr;
   size_t layer_off[14];
   float* d_wf[5] = {};     // folded fp32 3x3 weights [9][cin][cout] (layer 0 always; 1..4 for the CUDA-core check path)
   float* d_bias[6] = {};   // folded biases (layers 0..5)
-  float* d_wf6 = nullptr;  // folded fp32 15x15 weights [225][48][48] (CUDA-core check path only)
+  float* d_wf6 = nullptr;  // folded fp32 15x15 weights [225][c3][c3] (CUDA-core check path only)
   TcLayer tc[6];           // tensor-core weights of layers 1..5 (index = layer)
   float* d_head = nullptr;
   size_t* d_offs = nullptr;
-  // activations (sized for the current map); h* / l* = fp16 hi / lo NHWC-64, f* = fp32 NHWC
+  // activations (sized for the current map and network); h* / l* = fp16 hi / lo NHWC-64, f* = fp32 NHWC
   int rows = 0, cols = 0;
   __half *h1 = nullptr, *l1 = nullptr, *hp2 = nullptr, *lp2 = nullptr, *h3 = nullptr, *l3 = nullptr, *hp4 = nullptr,
          *lp4 = nullptr, *h5 = nullptr, *l5 = nullptr;
@@ -686,59 +743,89 @@ static void free_acts(State* s) {
   s->f1 = s->f2 = s->fp2 = s->f3 = s->f4 = s->fp4 = s->f5 = s->feat = nullptr;
 }
 
+static void free_weights(State* s) {
+  cudaFree(s->d_blob);
+  for (auto& p : s->d_wf) { cudaFree(p); p = nullptr; }
+  for (auto& p : s->d_bias) { cudaFree(p); p = nullptr; }
+  for (auto& t : s->tc) { cudaFree(t.whi); cudaFree(t.wlo); t = TcLayer(); }
+  cudaFree(s->d_wf6); cudaFree(s->d_head); cudaFree(s->d_offs);
+  s->d_blob = s->d_wf6 = s->d_head = nullptr;
+  s->d_offs = nullptr;
+}
+
 void destroy(State* s) {
   if (!s) return;
   free_acts(s);
-  cudaFree(s->d_blob);
-  for (auto p : s->d_wf) cudaFree(p);
-  for (auto p : s->d_bias) cudaFree(p);
-  for (auto& t : s->tc) { cudaFree(t.whi); cudaFree(t.wlo); }
-  cudaFree(s->d_wf6); cudaFree(s->d_head); cudaFree(s->d_offs);
+  free_weights(s);
   for (auto e : s->ev) if (e) cudaEventDestroy(e);
   delete s;
 }
 
 bool has_features(const State* s) { return s->has_features; }
 bool has_weights(const State* s) { return s->has_weights; }
+int network(const State* s) { return s->has_weights ? s->net : -1; }
 void last_times(const State* s, float* ms3) { ms3[0] = s->last_ms[0]; ms3[1] = s->last_ms[1]; ms3[2] = s->last_ms[2]; }
 
-static const int kTcNout[6] = {0, 32, 48, 48, 48, 48};   // wgmma N per layer (Cout 24 padded to 32)
+// wgmma N of tensor-core layer l (1..5): Cout rounded up to a multiple of 16 (light init_conv2: 24 -> 32)
+static int tc_nout(const LayerDef& l) { return (l.cout + 15) / 16 * 16; }
+
+static int head_floats(int net) {
+  const NetDims& d = kNets[net];
+  return head_floats(d.c3, d.nh, d.b[0], d.b[1], d.b[2]);
+}
 
 int set_weights(State* s, const float* blob, size_t n, cudaStream_t st, std::string& err) {
-  if (n != blob_floats()) { err = "weight blob has the wrong number of floats"; return -1; }
+  int net = -1;
+  for (int k = 0; k < kNumNetworks; ++k) if (n == blob_floats(k)) net = k;
+  if (net < 0) { err = "weight blob has the wrong number of floats (neither network_light nor network)"; return -1; }
   CNN_TRY(cudaSetDevice(s->device));
+  if (s->net != net) {
+    // Another architecture: every buffer, tensor map and kernel attribute sized for the old one goes.
+    CNN_TRY(cudaStreamSynchronize(st));
+    free_weights(s);
+    free_acts(s);
+    s->rows = s->cols = 0;
+    s->maps_valid = false;
+    s->attrs_set = false;
+    s->has_weights = s->has_features = false;
+    s->net = net;
+    for (int l = 0; l < 14; ++l) s->layers[l] = layer_def(net, l);
+  }
+  const LayerDef* L = s->layers;
   if (!s->d_blob) {
     CNN_TRY(cudaMalloc(&s->d_blob, n * sizeof(float)));
-    for (int l = 0; l < 5; ++l) CNN_TRY(cudaMalloc(&s->d_wf[l], (size_t)9 * kLayers[l].cin * kLayers[l].cout * sizeof(float)));
-    for (int l = 0; l < 6; ++l) CNN_TRY(cudaMalloc(&s->d_bias[l], kLayers[l].cout * sizeof(float)));
-    CNN_TRY(cudaMalloc(&s->d_wf6, (size_t)225 * 48 * 48 * sizeof(float)));
+    for (int l = 0; l < 5; ++l) CNN_TRY(cudaMalloc(&s->d_wf[l], (size_t)9 * L[l].cin * L[l].cout * sizeof(float)));
+    for (int l = 0; l < 6; ++l) CNN_TRY(cudaMalloc(&s->d_bias[l], L[l].cout * sizeof(float)));
+    CNN_TRY(cudaMalloc(&s->d_wf6, (size_t)225 * L[5].cin * L[5].cout * sizeof(float)));
     for (int l = 1; l < 6; ++l) {
-      const size_t cnt = (size_t)kLayers[l].k * kLayers[l].k * kTcNout[l] * 64;
-      s->tc[l].nout = kTcNout[l];
+      s->tc[l].nout = tc_nout(L[l]);
+      const size_t cnt = (size_t)L[l].k * L[l].k * s->tc[l].nout * 64;
       CNN_TRY(cudaMalloc(&s->tc[l].whi, cnt * sizeof(__half)));
       CNN_TRY(cudaMalloc(&s->tc[l].wlo, cnt * sizeof(__half)));
     }
-    CNN_TRY(cudaMalloc(&s->d_head, kHeadFloats * sizeof(float)));
+    CNN_TRY(cudaMalloc(&s->d_head, head_floats(net) * sizeof(float)));
     CNN_TRY(cudaMalloc(&s->d_offs, 8 * sizeof(size_t)));
   }
   size_t off = 0;
   for (int l = 0; l < 14; ++l) {
     s->layer_off[l] = off;
-    off += (size_t)kLayers[l].cout * kLayers[l].cin * kLayers[l].k * kLayers[l].k + (kLayers[l].bn ? 4 * kLayers[l].cout : kLayers[l].cout);
+    off += (size_t)L[l].cout * L[l].cin * L[l].k * L[l].k + (L[l].bn ? 4 * L[l].cout : L[l].cout);
   }
   CNN_TRY(cudaMemcpyAsync(s->d_blob, blob, n * sizeof(float), cudaMemcpyHostToDevice, st));
   CNN_TRY(cudaMemcpyAsync(s->d_offs, s->layer_off + 6, 8 * sizeof(size_t), cudaMemcpyHostToDevice, st));
   for (int l = 0; l < 6; ++l) {
-    const int kk = kLayers[l].k * kLayers[l].k;
+    const int kk = L[l].k * L[l].k;
     const float* w = s->d_blob + s->layer_off[l];
-    const float* bn = w + (size_t)kLayers[l].cout * kLayers[l].cin * kk;
+    const float* bn = w + (size_t)L[l].cout * L[l].cin * kk;
     // fp32 folded weights (first layer + the CUDA-core check path) and biases
-    fold_conv_kernel<<<256, 256, 0, st>>>(w, bn, kLayers[l].cout, kLayers[l].cin, kk, l < 5 ? s->d_wf[l] : s->d_wf6, s->d_bias[l]);
+    fold_conv_kernel<<<256, 256, 0, st>>>(w, bn, L[l].cout, L[l].cin, kk, l < 5 ? s->d_wf[l] : s->d_wf6, s->d_bias[l]);
     if (l >= 1)
-      fold_tc_kernel<<<256, 256, 0, st>>>(w, bn, kLayers[l].cout, kLayers[l].cin, kk, kTcNout[l], s->tc[l].whi, s->tc[l].wlo,
+      fold_tc_kernel<<<256, 256, 0, st>>>(w, bn, L[l].cout, L[l].cin, kk, s->tc[l].nout, s->tc[l].whi, s->tc[l].wlo,
                                           s->d_bias[l]);
   }
-  fold_head_kernel<<<1, 256, 0, st>>>(s->d_blob, s->d_offs, s->d_head);
+  HeadDims hd;
+  for (int l = 0; l < 8; ++l) { hd.cin[l] = L[6 + l].cin; hd.cout[l] = L[6 + l].cout; }
+  fold_head_kernel<<<1, 256, 0, st>>>(s->d_blob, s->d_offs, hd, s->d_head);
   CNN_TRY(cudaGetLastError());
   CNN_TRY(cudaStreamSynchronize(st));
   s->has_weights = true;
@@ -798,8 +885,61 @@ static int launch_tc(State* s, int layer, __half* ahi, __half* alo, int H, int W
   const int OH = H - KS + 1, OW = W - KS + 1;
   const dim3 grid((OW + kTileX - 1) / kTileX, (OH + kTileY - 1) / kTileY);
   kern<<<grid, kConvThreads, Cfg::kSmem, st>>>(maps[0], maps[1], maps[2], maps[3], s->d_bias[layer], out, ohi, olo, OH, OW,
-                                               kLayers[layer].cout);
+                                               s->layers[layer].cout);
   CNN_TRY(cudaGetLastError());
+  return 0;
+}
+
+// Extents of every trunk activation for a rows x cols map.
+struct TrunkDims {
+  int H0, W0, H1, W1, H2, W2, HP2, WP2, H3, W3, H4, W4, HP4, WP4, H5, W5, H6, W6;
+  TrunkDims(int rows, int cols) : H0(rows), W0(cols) {
+    H1 = H0 - 2; W1 = W0 - 2; H2 = H1 - 2; W2 = W1 - 2; HP2 = H2 / 2; WP2 = W2 / 2;
+    H3 = HP2 - 2; W3 = WP2 - 2; H4 = H3 - 2; W4 = W3 - 2; HP4 = H4 - 2; WP4 = W4 - 2;
+    H5 = HP4 - 2; W5 = WP4 - 2; H6 = H5 - 14; W6 = W5 - 14;
+  }
+};
+
+// The trunk's launches for one network: C1 channels after init_conv1/2, C3 after init_conv3..5 and init_flatten. Events
+// ev[0..3] bracket the 3x3 stack and the 15x15 layer.
+template <int NET>
+static int run_trunk(State* s, const float* d_layer, int pitch, const TrunkDims& d, cudaStream_t st, int use_cuda_core_path,
+                     std::string& err) {
+  constexpr int C1 = kNets[NET].c1, C3 = kNets[NET].c3;
+  constexpr int K2 = (C1 + 15) / 16, N2 = 16 * K2, K4 = C3 / 16;   // wgmma K steps / N of init_conv2 and the C3 layers
+  static_assert(C3 % 16 == 0, "C3 channels are whole K = 16 steps");
+  auto grid2 = [](int oh, int ow) { return dim3((ow + 15) / 16, (oh + 15) / 16); };
+  const int g1 = s->sm_count * 8;
+  CNN_TRY(cudaEventRecord(s->ev[0], st));
+  if (use_cuda_core_path) {
+    conv3x3_kernel<1, C1, 1, false, true><<<grid2(d.H1, d.W1), 256, 0, st>>>(d_layer, d.H0, d.W0, pitch, s->d_wf[0], s->d_bias[0], s->f1);
+    conv3x3_kernel<C1, C1, 8, true, false><<<grid2(d.H2, d.W2), 256, 0, st>>>(s->f1, d.H1, d.W1, 0, s->d_wf[1], s->d_bias[1], s->f2);
+    maxpool_kernel<<<g1, 256, 0, st>>>(s->f2, d.H2, d.W2, C1, 2, 2, s->fp2, d.HP2, d.WP2);
+    conv3x3_kernel<C1, C3, 8, true, false><<<grid2(d.H3, d.W3), 256, 0, st>>>(s->fp2, d.HP2, d.WP2, 0, s->d_wf[2], s->d_bias[2], s->f3);
+    conv3x3_kernel<C3, C3, 8, true, false><<<grid2(d.H4, d.W4), 256, 0, st>>>(s->f3, d.H3, d.W3, 0, s->d_wf[3], s->d_bias[3], s->f4);
+    maxpool_kernel<<<g1, 256, 0, st>>>(s->f4, d.H4, d.W4, C3, 3, 1, s->fp4, d.HP4, d.WP4);
+    conv3x3_kernel<C3, C3, 8, true, false><<<grid2(d.H5, d.W5), 256, 0, st>>>(s->fp4, d.HP4, d.WP4, 0, s->d_wf[4], s->d_bias[4], s->f5);
+    CNN_TRY(cudaGetLastError());
+    CNN_TRY(cudaEventRecord(s->ev[1], st));
+    CNN_TRY(cudaEventRecord(s->ev[2], st));
+    conv15_reference_kernel<C3><<<(d.H6 * d.W6 * C3 + 255) / 256, 256, 0, st>>>(s->f5, d.H5, d.W5, s->d_wf6, s->d_bias[5], s->feat);
+    CNN_TRY(cudaGetLastError());
+  } else {
+    int rc;
+    conv1_split_kernel<C1><<<g1, 256, 0, st>>>(d_layer, d.H0, d.W0, pitch, s->d_wf[0], s->d_bias[0], s->h1, s->l1);
+    if ((rc = launch_tc<3, K2, N2, 1, false>(s, 1, s->h1, s->l1, d.H1, d.W1, s->f2, nullptr, nullptr, st, err))) return rc;
+    maxpool_split_kernel<<<g1, 256, 0, st>>>(s->f2, d.H2, d.W2, C1, 2, 2, s->hp2, s->lp2, d.HP2, d.WP2);
+    if ((rc = launch_tc<3, K2, C3, 1, true>(s, 2, s->hp2, s->lp2, d.HP2, d.WP2, nullptr, s->h3, s->l3, st, err))) return rc;
+    if ((rc = launch_tc<3, K4, C3, 1, false>(s, 3, s->h3, s->l3, d.H3, d.W3, s->f4, nullptr, nullptr, st, err))) return rc;
+    maxpool_split_kernel<<<g1, 256, 0, st>>>(s->f4, d.H4, d.W4, C3, 3, 1, s->hp4, s->lp4, d.HP4, d.WP4);
+    if ((rc = launch_tc<3, K4, C3, 1, true>(s, 4, s->hp4, s->lp4, d.HP4, d.WP4, nullptr, s->h5, s->l5, st, err))) return rc;
+    CNN_TRY(cudaGetLastError());
+    CNN_TRY(cudaEventRecord(s->ev[1], st));
+    CNN_TRY(cudaEventRecord(s->ev[2], st));
+    if ((rc = launch_tc<15, K4, C3, 2, false>(s, 5, s->h5, s->l5, d.H5, d.W5, s->feat, nullptr, nullptr, st, err))) return rc;
+    s->maps_valid = true;
+    s->attrs_set = true;
+  }
   return 0;
 }
 
@@ -810,71 +950,40 @@ int update_features(State* s, const float* d_layer, int rows, int cols, int pitc
   if (!s->has_weights) { err = "motion-cost weights not set"; return -5; }
   if (rows < 64 || cols < 64) { err = "map too small for the motion-cost network (needs >= 64 x 64 cells)"; return -1; }
   CNN_TRY(cudaSetDevice(s->device));
-  const int H0 = rows, W0 = cols;
-  const int H1 = H0 - 2, W1 = W0 - 2, H2 = H1 - 2, W2 = W1 - 2, HP2 = H2 / 2, WP2 = W2 / 2;
-  const int H3 = HP2 - 2, W3 = WP2 - 2, H4 = H3 - 2, W4 = W3 - 2, HP4 = H4 - 2, WP4 = W4 - 2;
-  const int H5 = HP4 - 2, W5 = WP4 - 2, H6 = H5 - 14, W6 = W5 - 14;
+  const TrunkDims d(rows, cols);
   if (rows != s->rows || cols != s->cols) {
     free_acts(s);
     auto hl = [&](__half** h, __half** l, int hh, int ww) -> cudaError_t {
       cudaError_t e = cudaMalloc(h, (size_t)hh * ww * 64 * 2);
       return e != cudaSuccess ? e : cudaMalloc(l, (size_t)hh * ww * 64 * 2);
     };
-    CNN_TRY(hl(&s->h1, &s->l1, H1, W1));
-    CNN_TRY(hl(&s->hp2, &s->lp2, HP2, WP2));
-    CNN_TRY(hl(&s->h3, &s->l3, H3, W3));
-    CNN_TRY(hl(&s->hp4, &s->lp4, HP4, WP4));
-    CNN_TRY(hl(&s->h5, &s->l5, H5, W5));
-    CNN_TRY(cudaMalloc(&s->f1, (size_t)H1 * W1 * 24 * 4));
-    CNN_TRY(cudaMalloc(&s->f2, (size_t)H2 * W2 * 24 * 4));
-    CNN_TRY(cudaMalloc(&s->fp2, (size_t)HP2 * WP2 * 24 * 4));
-    CNN_TRY(cudaMalloc(&s->f3, (size_t)H3 * W3 * 48 * 4));
-    CNN_TRY(cudaMalloc(&s->f4, (size_t)H4 * W4 * 48 * 4));
-    CNN_TRY(cudaMalloc(&s->fp4, (size_t)HP4 * WP4 * 48 * 4));
-    CNN_TRY(cudaMalloc(&s->f5, (size_t)H5 * W5 * 48 * 4));
-    CNN_TRY(cudaMalloc(&s->feat, (size_t)H6 * W6 * 48 * 4));
+    const size_t c1 = s->layers[0].cout, c3 = s->layers[2].cout;
+    CNN_TRY(hl(&s->h1, &s->l1, d.H1, d.W1));
+    CNN_TRY(hl(&s->hp2, &s->lp2, d.HP2, d.WP2));
+    CNN_TRY(hl(&s->h3, &s->l3, d.H3, d.W3));
+    CNN_TRY(hl(&s->hp4, &s->lp4, d.HP4, d.WP4));
+    CNN_TRY(hl(&s->h5, &s->l5, d.H5, d.W5));
+    CNN_TRY(cudaMalloc(&s->f1, (size_t)d.H1 * d.W1 * c1 * 4));
+    CNN_TRY(cudaMalloc(&s->f2, (size_t)d.H2 * d.W2 * c1 * 4));
+    CNN_TRY(cudaMalloc(&s->fp2, (size_t)d.HP2 * d.WP2 * c1 * 4));
+    CNN_TRY(cudaMalloc(&s->f3, (size_t)d.H3 * d.W3 * c3 * 4));
+    CNN_TRY(cudaMalloc(&s->f4, (size_t)d.H4 * d.W4 * c3 * 4));
+    CNN_TRY(cudaMalloc(&s->fp4, (size_t)d.HP4 * d.WP4 * c3 * 4));
+    CNN_TRY(cudaMalloc(&s->f5, (size_t)d.H5 * d.W5 * c3 * 4));
+    CNN_TRY(cudaMalloc(&s->feat, (size_t)d.H6 * d.W6 * c3 * 4));
     s->rows = rows; s->cols = cols;
     s->maps_valid = false;
   }
   if (!s->ev[0]) for (auto& e : s->ev) CNN_TRY(cudaEventCreate(&e));
-  auto grid2 = [](int oh, int ow) { return dim3((ow + 15) / 16, (oh + 15) / 16); };
-  const int g1 = s->sm_count * 8;
-  CNN_TRY(cudaEventRecord(s->ev[0], st));
-  if (use_cuda_core_path) {
-    conv3x3_kernel<1, 24, 1, false, true><<<grid2(H1, W1), 256, 0, st>>>(d_layer, H0, W0, pitch, s->d_wf[0], s->d_bias[0], s->f1);
-    conv3x3_kernel<24, 24, 8, true, false><<<grid2(H2, W2), 256, 0, st>>>(s->f1, H1, W1, 0, s->d_wf[1], s->d_bias[1], s->f2);
-    maxpool_kernel<<<g1, 256, 0, st>>>(s->f2, H2, W2, 24, 2, 2, s->fp2, HP2, WP2);
-    conv3x3_kernel<24, 48, 8, true, false><<<grid2(H3, W3), 256, 0, st>>>(s->fp2, HP2, WP2, 0, s->d_wf[2], s->d_bias[2], s->f3);
-    conv3x3_kernel<48, 48, 8, true, false><<<grid2(H4, W4), 256, 0, st>>>(s->f3, H3, W3, 0, s->d_wf[3], s->d_bias[3], s->f4);
-    maxpool_kernel<<<g1, 256, 0, st>>>(s->f4, H4, W4, 48, 3, 1, s->fp4, HP4, WP4);
-    conv3x3_kernel<48, 48, 8, true, false><<<grid2(H5, W5), 256, 0, st>>>(s->fp4, HP4, WP4, 0, s->d_wf[4], s->d_bias[4], s->f5);
-    CNN_TRY(cudaGetLastError());
-    CNN_TRY(cudaEventRecord(s->ev[1], st));
-    CNN_TRY(cudaEventRecord(s->ev[2], st));
-    conv15_reference_kernel<<<(H6 * W6 * 48 + 255) / 256, 256, 0, st>>>(s->f5, H5, W5, s->d_wf6, s->d_bias[5], s->feat);
-    CNN_TRY(cudaGetLastError());
-  } else {
-    int rc;
-    conv1_split_kernel<<<g1, 256, 0, st>>>(d_layer, H0, W0, pitch, s->d_wf[0], s->d_bias[0], s->h1, s->l1);
-    if ((rc = launch_tc<3, 2, 32, 1, false>(s, 1, s->h1, s->l1, H1, W1, s->f2, nullptr, nullptr, st, err))) return rc;
-    maxpool_split_kernel<<<g1, 256, 0, st>>>(s->f2, H2, W2, 24, 2, 2, s->hp2, s->lp2, HP2, WP2);
-    if ((rc = launch_tc<3, 2, 48, 1, true>(s, 2, s->hp2, s->lp2, HP2, WP2, nullptr, s->h3, s->l3, st, err))) return rc;
-    if ((rc = launch_tc<3, 3, 48, 1, false>(s, 3, s->h3, s->l3, H3, W3, s->f4, nullptr, nullptr, st, err))) return rc;
-    maxpool_split_kernel<<<g1, 256, 0, st>>>(s->f4, H4, W4, 48, 3, 1, s->hp4, s->lp4, HP4, WP4);
-    if ((rc = launch_tc<3, 3, 48, 1, true>(s, 4, s->hp4, s->lp4, HP4, WP4, nullptr, s->h5, s->l5, st, err))) return rc;
-    CNN_TRY(cudaGetLastError());
-    CNN_TRY(cudaEventRecord(s->ev[1], st));
-    CNN_TRY(cudaEventRecord(s->ev[2], st));
-    if ((rc = launch_tc<15, 3, 48, 2, false>(s, 5, s->h5, s->l5, H5, W5, s->feat, nullptr, nullptr, st, err))) return rc;
-    s->maps_valid = true;
-    s->attrs_set = true;
-  }
+  const int rc = s->net == kNetFull ? run_trunk<kNetFull>(s, d_layer, pitch, d, st, use_cuda_core_path, err)
+                                    : run_trunk<kNetLight>(s, d_layer, pitch, d, st, use_cuda_core_path, err);
+  if (rc) return rc;
   CNN_TRY(cudaEventRecord(s->ev[3], st));
   CNN_TRY(cudaStreamSynchronize(st));
   cudaEventElapsedTime(&s->last_ms[0], s->ev[0], s->ev[1]);   // layers 1..5
   cudaEventElapsedTime(&s->last_ms[1], s->ev[2], s->ev[3]);   // 15x15 layer
   cudaEventElapsedTime(&s->last_ms[2], s->ev[0], s->ev[3]);   // whole trunk
-  s->Hf = H6; s->Wf = W6;
+  s->Hf = d.H6; s->Wf = d.W6;
   s->res = res; s->Lx = rows * res; s->Ly = cols * res; s->cx = cx; s->cy = cy;
   s->has_features = true;
   return 0;
@@ -888,15 +997,24 @@ int motion_cost(State* s, const float* d_edges, size_t n, float* d_cost3, cudaSt
   // One thread per query. Small batches (config 4: 4096 queries) use one-warp CTAs so that the batch spreads over the
   // SMs (128 CTAs instead of 32: 39 -> ~10 us); big batches amortise the 29 KB weight load over 128 queries per CTA.
   const int bt = n <= (size_t)s->sm_count * 128 ? 32 : 128;
-  head_kernel<<<(unsigned)((n + bt - 1) / bt), bt, kHeadFloats * sizeof(float), st>>>(s->feat, s->Hf, s->Wf, s->d_head, d_edges, n,
-                                                                                       d_cost3, s->res, s->Lx, s->Ly, s->cx, s->cy);
+  const unsigned grid = (unsigned)((n + bt - 1) / bt);
+  const size_t smem = head_floats(s->net) * sizeof(float);   // 30 KB light, 46.8 KB full: under the 48 KB default
+  if (s->net == kNetFull) {
+    constexpr NetDims D = kNets[kNetFull];
+    head_kernel<D.c3, D.nh, D.b[0], D.b[1], D.b[2]><<<grid, bt, smem, st>>>(s->feat, s->Hf, s->Wf, s->d_head, d_edges, n, d_cost3,
+                                                                           s->res, s->Lx, s->Ly, s->cx, s->cy);
+  } else {
+    constexpr NetDims D = kNets[kNetLight];
+    head_kernel<D.c3, D.nh, D.b[0], D.b[1], D.b[2]><<<grid, bt, smem, st>>>(s->feat, s->Hf, s->Wf, s->d_head, d_edges, n, d_cost3,
+                                                                           s->res, s->Lx, s->Ly, s->cx, s->cy);
+  }
   CNN_TRY(cudaGetLastError());
   return 0;
 }
 
 int copy_features(State* s, float* host_out, size_t n_floats, std::string& err) {
   if (!s->has_features) { err = "features not computed"; return -5; }
-  if (n_floats != (size_t)s->Hf * s->Wf * 48) { err = "feature buffer size mismatch"; return -1; }
+  if (n_floats != (size_t)s->Hf * s->Wf * s->layers[5].cout) { err = "feature buffer size mismatch"; return -1; }
   CNN_TRY(cudaMemcpy(host_out, s->feat, n_floats * sizeof(float), cudaMemcpyDeviceToHost));
   return 0;
 }

@@ -331,12 +331,24 @@ int artp_process_basic(artp_handle* h, const float* elevation, const float* trav
 int artp_debug_circular_kernel(int size, uint8_t* out);
 
 /* ---- learned motion cost (MotionCostFunc, objectives/motion_cost_objective.h:22-23) ------------------------------
- * Weights: ONE flat fp32 blob in the layer order of the reference's `network` module (network_light.py:9-63):
- * init_conv1..5, init_flatten, tar0_conv1, out0_conv1, out1_conv1..3 -- each conv.weight [Cout][Cin][kh][kw] followed by
- * its BatchNorm weight, bias, running_mean, running_var -- then out2_conv1..3 as conv.weight followed by conv.bias.
- * artp_cost_weights_size() floats in total (583 767 parameters + BN buffers). */
+ * Weights: ONE flat fp32 blob in the layer order of the reference's `network` module: init_conv1..5, init_flatten,
+ * tar0_conv1, out0_conv1, out1_conv1..3 -- each conv.weight [Cout][Cin][kh][kw] followed by its BatchNorm weight, bias,
+ * running_mean, running_var -- then out2_conv1..3 as conv.weight followed by conv.bias. Two architectures share this
+ * layout and differ only in their widths; the blob's length picks the one that runs:
+ *   ARTP_COST_NET_LIGHT  network_light.py:9-63 (init 24/48 channels, out0 64->48, out1 48->24/24/36):
+ *                        584 543 floats (583 767 parameters + BN buffers) = artp_cost_weights_size()
+ *   ARTP_COST_NET_FULL   network.py:9-63 (init 32/64 channels, out0 80->64, out1 64->32/32/32):
+ *                        1 036 771 floats (1 035 779 parameters + BN buffers)
+ * artp_set_cost_weights takes either length (any other is ARTP_E_INVALID); a blob of the other architecture replaces
+ * the loaded one, and artp_update_features must run again before the next cost query. */
+#define ARTP_COST_NET_LIGHT 0
+#define ARTP_COST_NET_FULL  1
 size_t artp_cost_weights_size(void);
+/* Blob length of `network` (ARTP_COST_NET_*), 0 for any other value. */
+size_t artp_cost_weights_size_for(int network);
 int artp_set_cost_weights(artp_handle* h, const float* blob, size_t n_floats);
+/* The architecture of the loaded weights (ARTP_COST_NET_*); ARTP_E_NOWEIGHTS before any artp_set_cost_weights. */
+int artp_get_cost_network(artp_handle* h, int* network);
 /* CostPredictor.updateFeatures (predictor.py:28-36): run the CNN trunk over the `elevation` layer of the current map
  * (orientation as cost_query_server.py:74). Call after artp_set_map whenever the map changed. */
 int artp_update_features(artp_handle* h);
@@ -370,7 +382,8 @@ int artp_motion_cost_split(artp_handle* h, const double* s1, const double* s2, s
 int artp_motion_cost_split_device(artp_handle* h, const double* d_s1, const double* d_s2, size_t n,
                                   const uint32_t* d_piece_off, size_t total_pieces, float* d_rows, float* d_cost3,
                                   double* d_cost, void* stream);
-/* Test hooks: feature map copy-out ([Hf][Wf][48] fp32, channels last), kernel selection (bit 0: CUDA-core fp32
+/* Test hooks: feature map copy-out ([Hf][Wf][C] fp32, channels last, C = 48 light / 64 full: n_floats = Hf*Wf*C),
+ * kernel selection (bit 0: CUDA-core fp32
  * reference for every layer instead of the tensor-core (wgmma) kernels; any other bit is ARTP_E_INVALID), trunk timings
  * ms3 = (3x3 stack, 15x15 layer, whole trunk) of the last artp_update_features. */
 int artp_get_features(artp_handle* h, float* out, size_t n_floats, int* hf, int* wf);

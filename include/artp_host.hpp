@@ -454,6 +454,7 @@ class MotionCostObjective {
       }));
     }
   }
+  // Either network's blob (artp.h, above artp_cost_weights_size): its length picks network_light or network.
   void setWeights(const std::vector<float>& blob) {
     checker_->handle()->check(artp_set_cost_weights(checker_->handle()->get(), blob.data(), blob.size()), "artp_set_cost_weights");
   }
