@@ -1,4 +1,4 @@
-"""GPU (-m gpu): the classify stage decides most boxes from the compact range tables (a 16-bit code interval around the
+"""GPU (-m gpu): the classify stage decides most boxes from the compact range tables (a 15-bit code interval around the
 exact zone max / min) and falls back to the exact tables when an interval leaves a test open. These poses put box
 bottoms and tops within about one code step of their zone's max or min, on a map whose codes are coarse (heights
 around +300 m, -inf patches in the masked layer), so both outcomes of every interval test occur. Masks must equal the
@@ -23,11 +23,12 @@ def offset_map():
 
 
 def code_step(layer):
-    """The compact tables' step: the smallest power of two with base + 65533 * step >= the largest finite height."""
+    """The compact tables' step: the smallest power of two with base + 32765 * step >= the largest finite height
+    (kCodeMax, artp_device.cuh)."""
     h = layer[np.isfinite(layer)]
     base, top = np.float32(h.min()), np.float32(h.max())
     e = -126
-    while base + np.float32(65533) * np.float32(2.0 ** e) < top:
+    while base + np.float32(32765) * np.float32(2.0 ** e) < top:
         e += 1
     return 2.0 ** e
 

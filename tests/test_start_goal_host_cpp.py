@@ -13,21 +13,22 @@ import start_goal_cases as sgc
 from art_planner_b200 import synth
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EXE = os.path.join(ROOT, "tests", "host_cpp", "start_goal")
 
 
 @pytest.fixture(scope="module")
-def exe():
+def exe(tmp_path_factory):
+    """The driver, compiled into a temporary directory: the source tree may be read-only."""
     from art_planner_b200 import build, capi
     if not os.path.exists(capi.LIB_PATH):
         if shutil.which("nvcc") is None:
             pytest.skip("libartp.so not built and nvcc absent")
         build.build()
     libdir = os.path.dirname(capi.LIB_PATH)
+    exe_path = str(tmp_path_factory.mktemp("host_cpp") / "start_goal")
     subprocess.run(["g++", "-std=c++14", "-O1", "-Wall", "-I", os.path.join(ROOT, "include"),
-                    os.path.join(ROOT, "tests", "host_cpp", "start_goal.cpp"), "-o", EXE,
+                    os.path.join(ROOT, "tests", "host_cpp", "start_goal.cpp"), "-o", exe_path,
                     "-L", libdir, "-l:libartp.so", f"-Wl,-rpath,{libdir}"], check=True)
-    return EXE
+    return exe_path
 
 
 def test_start_goal_mirror_compiles_and_fails_loudly_without_gpu(exe):
