@@ -44,6 +44,11 @@ class ArtpBasicParams(C.Structure):
         "foothold_margin_min_step", "foothold_size")]
 
 
+class ArtpSampleDistributionParams(C.Structure):
+    _fields_ = [("use_inverse_vertex_density", C.c_int), ("density_blur_radius", C.c_double),
+                ("use_max_prob_unknown_samples", C.c_int), ("max_prob_unknown_samples", C.c_double)]
+
+
 class ArtpStats(C.Structure):
     _fields_ = [("poses_checked", C.c_uint64), ("poses_deferred", C.c_uint64), ("kernel_launches", C.c_uint64),
                 ("last_deferred", C.c_uint32), ("last_launches", C.c_uint32), ("last_queued_boxes", C.c_uint32),
@@ -109,6 +114,10 @@ def load():
     lib.artp_poll_error.argtypes = [vp]
     lib.artp_process_basic.argtypes = [vp, vp, vp, vp, i32, i32, dbl, C.POINTER(ArtpBasicParams), vp, vp]
     lib.artp_debug_circular_kernel.argtypes = [i32, vp]
+    lib.artp_set_sample_filter.argtypes = [vp, vp, vp, vp]
+    lib.artp_update_sample_distribution.argtypes = [vp, C.POINTER(ArtpSampleDistributionParams), vp, sz, vp, vp, vp]
+    lib.artp_update_sample_distribution_device.argtypes = [vp, C.POINTER(ArtpSampleDistributionParams), vp, sz, vp]
+    lib.artp_debug_gaussian_kernel.argtypes = [i32, dbl, vp]
     lib.artp_host_alloc.restype = C.c_void_p
     lib.artp_host_alloc.argtypes = [sz]
     lib.artp_host_free.argtypes = [vp]

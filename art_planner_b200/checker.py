@@ -194,6 +194,45 @@ class StateValidityChecker:
                                                           None if row is None else row.ctypes.data))
         return (cum, row) if want_host else None
 
+    def setSampleFilter(self, traversability_thresholded=None, observed=None, want_host: bool = True):
+        """Basic::setTraversabilityFilter (basic.cpp:110-125) on the device for the current map, with the "observed" layer the
+        unknown-space cap reads; both stay resident for updateSampleDistribution. None: the layer the last processBasic on
+        this checker received (observed) / produced (traversability_thresholded). Returns traversability_sample_filter
+        (float32 F-order) or None."""
+        rows, cols = self._map.elevation.shape
+        f = lambda a: None if a is None else np.asfortranarray(a, dtype=np.float32)
+        t, o = f(traversability_thresholded), f(observed)
+        for a in (t, o):
+            if a is not None and a.shape != (rows, cols):
+                raise capi.ArtpError(capi.ARTP_E_INVALID, "layer shape differs from the map's")
+        out = np.empty((rows, cols), np.float32, order="F") if want_host else None
+        self._h.check(self._h.lib.artp_set_sample_filter(self._h.h, *[None if a is None else a.ctypes.data for a in (t, o, out)]))
+        return out
+
+    def updateSampleDistribution(self, vertex_states, dp, want_host: bool = True):
+        """computeInverseSampleDensity -> applyBaseSampleDistribution -> applyMaxUnknownProbability ->
+        computeCumulativeProbabilityDistribution (planner.cpp:39-58) on the device for the roadmap's vertex states [n, 7]
+        (only x, y read). dp: an object with the fields of artp_sample_distribution_params. The CDF stays resident: re-arm
+        the sampler afterwards (SE3FromSE2Sampler.updateDistribution does both). A CUDA float64 tensor goes through the
+        device entry point on the current stream and returns None; else returns (sample_probability, cum_prob,
+        cum_prob_rowwise) when want_host."""
+        lib, h = self._h.lib, self._h
+        p = capi.ArtpSampleDistributionParams(int(dp.use_inverse_vertex_density), float(dp.density_blur_radius),
+                                              int(dp.use_max_prob_unknown_samples), float(dp.max_prob_unknown_samples))
+        if _is_torch_cuda(vertex_states):
+            import torch
+            assert vertex_states.dtype == torch.float64 and vertex_states.is_contiguous() and vertex_states.shape[-1] == 7
+            h.check(lib.artp_update_sample_distribution_device(h.h, C.byref(p), C.c_void_p(vertex_states.data_ptr()),
+                                                               vertex_states.shape[0], _stream_ptr()))
+            return None
+        v = np.ascontiguousarray(vertex_states, dtype=np.float64).reshape(-1, 7)
+        rows, cols = self._map.elevation.shape
+        outs = [np.empty((rows, cols), np.float32, order="F"), np.empty((rows, cols), np.float32, order="F"),
+                np.empty(rows, np.float32)] if want_host else [None] * 3
+        h.check(lib.artp_update_sample_distribution(h.h, C.byref(p), v.ctypes.data, v.shape[0],
+                                                    *[None if a is None else a.ctypes.data for a in outs]))
+        return tuple(outs) if want_host else None
+
     def findValidNear(self, centres, radius, n_iter: int, offsets=None, seed: int = 0, first_draw: int = 0):
         """StartState / GoalStateRegion::sampleGoal (start.cpp:7-41, goal.cpp:11-41) for n queries in one call: the first
         valid of the centre and the centre moved in x / y by offsets 1..n_iter; none valid -> the last candidate. centres
@@ -350,6 +389,20 @@ class SE3FromSE2Sampler:
         p = capi.ArtpSamplerParams(float(sp.max_roll_pert), float(sp.max_pitch_pert), int(sp.sample_from_distribution),
                                    (C.c_double * 2)(*sp.low), (C.c_double * 2)(*sp.high))
         h.check(lib.artp_set_sampler(h.h, C.byref(p), *[None if a is None else a.ctypes.data for a in keep]))
+        self._sp, self._params, self._normals = sp, p, keep[:4]
+
+    def updateDistribution(self, vertex_states) -> None:
+        """The reApplyPreprocessing step of PRMMotionCostMaintainer::sampleGraph (prm_motion_cost.cpp:190-193): the sampling
+        distribution from the roadmap's vertex states (with the filter / observed layers of the checker's setSampleFilter),
+        then the sampler re-armed on the new device CDF. Parameters from `sp` (use_inverse_vertex_density,
+        use_max_prob_unknown_samples, max_prob_unknown_samples) and the blur radius of planner.cpp:48."""
+        h, lib = self._c.handle, self._c.handle.lib
+        rp = h.params
+        dp = capi.ArtpSampleDistributionParams(int(self._sp.use_inverse_vertex_density), (rp.torso_length + rp.torso_width) * 0.25,
+                                               int(self._sp.use_max_prob_unknown_samples), float(self._sp.max_prob_unknown_samples))
+        self._c.updateSampleDistribution(vertex_states, dp, want_host=False)
+        h.check(lib.artp_set_sampler(h.h, C.byref(self._params), *[None if a is None else a.ctypes.data for a in self._normals],
+                                     None, None))
 
     def uniforms(self, first: int, n: int) -> np.ndarray:
         """The [n, 6] uniform01 variates of samples first..first+n-1 of this sampler's Philox stream."""

@@ -24,6 +24,7 @@
 #include "artp_tiles.cuh"
 #include "artp_sampler.cuh"
 #include "artp_basic.cuh"
+#include "artp_distribution.cuh"
 
 namespace {
 
@@ -88,6 +89,18 @@ struct Handle {
   bool has_normals = false;         // normal_x/y/z of d_samp_layers hold this map's normals (device-estimated or the caller's)
   char* d_samp_scratch = nullptr;
   size_t samp_scratch_cap = 0;
+  double res = 0.0;                 // map resolution as artp_set_map received it
+  // sampling distribution (artp_distribution.cuh): the layers artp_set_sample_filter keeps for this map ...
+  float* d_dist_layers = nullptr;   // traversability_sample_filter | observed
+  size_t dist_layers_cap = 0;       // floats
+  bool has_sample_filter = false, has_dist_observed = false;
+  char* d_dist_scratch = nullptr;   // n_samples | blur pass | sample_probability | cap row sums | words (artp_update_sample_distribution)
+  size_t dist_scratch_cap = 0;
+  // ... and the layers of the last artp_process_basic, its NULL-layer inputs
+  float* d_basic_keep = nullptr;    // observed | traversability_thresholded
+  size_t basic_keep_cap = 0;        // floats
+  int basic_rows = 0, basic_cols = 0;
+  bool has_basic_layers = false, has_basic_observed = false;
   uint8_t* h_small_out = nullptr;   // mapped pinned host bytes the latency-path kernel writes its verdicts to
   int timing = 0;
   cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // classify | warp | reach vertex | reach plane | group
@@ -867,6 +880,7 @@ void artp_destroy(artp_handle* hh) {
   for (int k = 0; k < 2; ++k) for (int l = 0; l <= artp::kMaxLevel; ++l) { cudaFree(h->d_T[k][l]); cudaFree(h->d_C[k][l]); }
   cudaFree(h->d_H[0]); cudaFree(h->d_H[1]); cudaFree(h->d_ctr); cudaFree(h->d_defer); cudaFree(h->d_stage);
   cudaFree(h->d_block_counts); cudaFree(h->d_recs); cudaFree(h->d_recs_f); cudaFree(h->d_recs_g); cudaFree(h->d_samp_layers); cudaFree(h->d_samp_scratch);
+  cudaFree(h->d_dist_layers); cudaFree(h->d_dist_scratch); cudaFree(h->d_basic_keep);
   if (h->h_small_out) cudaFreeHost(h->h_small_out);
   if (h->h_err) cudaFreeHost(h->h_err);
   for (int g = 0; g < 2; ++g) if (h->chain_ev[g]) cudaEventDestroy(h->chain_ev[g]);
@@ -1146,6 +1160,9 @@ int artp_set_map_window(artp_handle* hh, const float* elevation, const float* el
   h->has_device_normals = false;
   h->has_device_cdf = false;
   h->has_normals = false;
+  h->has_sample_filter = false;
+  h->has_dist_observed = false;
+  h->res = res;
   return ARTP_OK;
 }
 
@@ -1635,6 +1652,18 @@ int artp_estimate_normals(artp_handle* hh, double estimation_radius, float* norm
   return ARTP_OK;
 }
 
+// computeCumulativeProbabilityDistribution of a device-resident probability layer into cum_prob / cum_row of
+// d_samp_layers (ensure_sampler_layers first). Two launches on s.
+static int launch_sample_cdf(Handle* h, const float* d_prob, cudaStream_t s) {
+  const size_t ncell = (size_t)h->rows * h->cols;
+  float* d_cum = h->d_samp_layers + 4 * ncell;
+  float* d_row = h->d_samp_layers + 5 * ncell;
+  artp::cdf_rows_kernel<<<(h->rows + 63) / 64, 64, 0, s>>>(d_prob, h->rows, h->cols, d_cum, d_row);
+  artp::cdf_rowwise_kernel<<<1, 32, 0, s>>>(d_row, h->rows);
+  CU_TRY(h, cudaGetLastError());
+  return ARTP_OK;
+}
+
 int artp_compute_sample_cdf(artp_handle* hh, const float* sample_probability, float* cum_prob, float* cum_prob_rowwise) {
   LOCK_HANDLE(h, hh);
   if (!h->has_map) { h->err = "no map set"; return ARTP_E_NOMAP; }
@@ -1649,9 +1678,7 @@ int artp_compute_sample_cdf(artp_handle* hh, const float* sample_probability, fl
   float* d_cum = h->d_samp_layers + 4 * ncell;
   float* d_row = h->d_samp_layers + 5 * ncell;
   CU_TRY(h, cudaMemcpyAsync(d_prob, sample_probability, ncell * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-  artp::cdf_rows_kernel<<<(h->rows + 63) / 64, 64, 0, h->stream>>>((const float*)d_prob, h->rows, h->cols, d_cum, d_row);
-  artp::cdf_rowwise_kernel<<<1, 32, 0, h->stream>>>(d_row, h->rows);
-  CU_TRY(h, cudaGetLastError());
+  if ((rc = launch_sample_cdf(h, (const float*)d_prob, h->stream))) return rc;
   if (cum_prob) CU_TRY(h, cudaMemcpyAsync(cum_prob, d_cum, ncell * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
   if (cum_prob_rowwise)
     CU_TRY(h, cudaMemcpyAsync(cum_prob_rowwise, d_row, (size_t)h->rows * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
@@ -2049,6 +2076,13 @@ int artp_debug_circular_kernel(int size, uint8_t* out) {   // test hook: the siz
   return k.size;
 }
 
+// cv::dilate / cv::erode of a rows x cols layer with getCircularKernel(size), one launch on s.
+static void launch_morph(bool dilate, const float* src, float* dst, int rows, int cols, int size, unsigned grid, cudaStream_t s) {
+  const artp::MorphKernel k = make_circular_kernel(size);
+  if (dilate) artp::morph_kernel<true><<<grid, 256, 0, s>>>(src, dst, rows, cols, k);
+  else artp::morph_kernel<false><<<grid, 256, 0, s>>>(src, dst, rows, cols, k);
+}
+
 int artp_process_basic(artp_handle* hh, const float* elevation, const float* traversability, const float* observed, int rows,
                        int cols, double res, const artp_basic_params* bp, float* elevation_masked, float* traversability_thresholded) {
   LOCK_HANDLE(h, hh);
@@ -2067,17 +2101,15 @@ int artp_process_basic(artp_handle* hh, const float* elevation, const float* tra
   char* stage;
   int rc = host_call_begin(h, {9 * lb}, &stage);
   if (rc) return rc;
+  h->has_basic_layers = false;
+  if ((rc = grow(h, h->d_basic_keep, h->basic_keep_cap, 2 * n))) return rc;
   float* L = (float*)stage;   // 0 elev, 1 trav, 2 observed, 3 T0, 4 A, 5 B, 6 elev eroded, 7 elev dilated, 8 out
   cudaStream_t s = h->stream;
   CU_TRY(h, cudaMemcpyAsync(L, elevation, lb, cudaMemcpyHostToDevice, s));
   CU_TRY(h, cudaMemcpyAsync(L + n, traversability, lb, cudaMemcpyHostToDevice, s));
   if (observed) CU_TRY(h, cudaMemcpyAsync(L + 2 * n, observed, lb, cudaMemcpyHostToDevice, s));
   const unsigned grid = (unsigned)std::min<size_t>((n + 255) / 256, (size_t)h->sm_count * 16);
-  auto morph = [&](bool dil, const float* src, float* dst, int size) {
-    const artp::MorphKernel k = make_circular_kernel(size);
-    if (dil) artp::morph_kernel<true><<<grid, 256, 0, s>>>(src, dst, rows, cols, k);
-    else artp::morph_kernel<false><<<grid, 256, 0, s>>>(src, dst, rows, cols, k);
-  };
+  auto morph = [&](bool dil, const float* src, float* dst, int size) { launch_morph(dil, src, dst, rows, cols, size, grid, s); };
   float *E = L, *T0 = L + 3 * n, *A = L + 4 * n, *B = L + 5 * n, *Elo = L + 6 * n, *Ehi = L + 7 * n, *O = L + 8 * n;
   artp::basic_threshold_kernel<<<grid, 256, 0, s>>>(L + n, L + 2 * n, bp->unknown_space_untraversable ? 1 : 0, bp->traversability_thres, n, T0);
   morph(true, T0, A, hole); morph(false, A, B, hole);                    // dilateAndErode: close holes (:72)
@@ -2091,10 +2123,218 @@ int artp_process_basic(artp_handle* hh, const float* elevation, const float* tra
   CU_TRY(h, cudaGetLastError());
   CU_TRY(h, cudaMemcpyAsync(elevation_masked, O, lb, cudaMemcpyDeviceToHost, s));
   if (traversability_thresholded) CU_TRY(h, cudaMemcpyAsync(traversability_thresholded, B, lb, cudaMemcpyDeviceToHost, s));
+  // kept for artp_set_sample_filter(h, NULL, NULL, ...)
+  if (observed) CU_TRY(h, cudaMemcpyAsync(h->d_basic_keep, L + 2 * n, lb, cudaMemcpyDeviceToDevice, s));
+  CU_TRY(h, cudaMemcpyAsync(h->d_basic_keep + n, B, lb, cudaMemcpyDeviceToDevice, s));
   if ((rc = host_call_end(h))) return rc;
+  h->basic_rows = rows; h->basic_cols = cols;
+  h->has_basic_layers = true;
+  h->has_basic_observed = observed != nullptr;
   h->stats.kernel_launches += 11;
   h->stats.last_launches = 11;
   return ARTP_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// The sampler's distribution (artp_distribution.cuh): Basic::setTraversabilityFilter, then computeInverseSampleDensity ->
+// applyBaseSampleDistribution -> applyMaxUnknownProbability -> computeCumulativeProbabilityDistribution
+// (planner.cpp:39-58), the chain sampleGraph re-applies every recompute_density_after_n_samples vertices.
+// ---------------------------------------------------------------------------------------------------------------
+int artp_set_sample_filter(artp_handle* hh, const float* traversability_thresholded, const float* observed,
+                           float* traversability_sample_filter) {
+  LOCK_HANDLE(h, hh);
+  if (!h->has_map) { h->err = "no map set"; return ARTP_E_NOMAP; }
+  if (h->win_rows != h->rows) { h->err = "not available on a map window (artp_set_map_window)"; return ARTP_E_INVALID; }
+  const int rows = h->rows, cols = h->cols;
+  const bool basic_fits = h->has_basic_layers && h->basic_rows == rows && h->basic_cols == cols;
+  if (!traversability_thresholded && !basic_fits) {
+    h->err = "no traversability_thresholded layer: pass it, or run artp_process_basic on a map of this size first";
+    return ARTP_E_INVALID;
+  }
+  const bool basic_observed = !observed && basic_fits && h->has_basic_observed;
+  // basic.cpp:116-122, with the implicit double -> int conversions of the int size parameters
+  const artp_params& p = h->p;
+  const int reach = (int)(std::sqrt(p.reach_x * p.reach_x + p.reach_y * p.reach_y) / h->res);
+  const int wall = (int)(std::min((p.torso_length - p.reach_x) * 0.5, (p.torso_width - p.reach_y) * 0.5) / h->res);
+  if (std::max(reach, wall) > artp::kMaxMorph) { h->err = "structuring element larger than 64 cells"; return ARTP_E_LIMIT; }
+  const size_t n = (size_t)rows * cols, lb = n * sizeof(float);
+  char* r[3];   // caller's traversability_thresholded | dilated | closed
+  int rc = host_call_begin(h, {lb, lb, lb}, r);
+  if (rc) return rc;
+  h->has_sample_filter = h->has_dist_observed = false;
+  if ((rc = grow(h, h->d_dist_layers, h->dist_layers_cap, 2 * n))) return rc;
+  cudaStream_t s = h->stream;
+  float *filter = h->d_dist_layers, *obs = h->d_dist_layers + n;
+  const float* thr = traversability_thresholded ? (const float*)r[0] : h->d_basic_keep + n;
+  if (traversability_thresholded) CU_TRY(h, cudaMemcpyAsync(r[0], traversability_thresholded, lb, cudaMemcpyHostToDevice, s));
+  if (observed) CU_TRY(h, cudaMemcpyAsync(obs, observed, lb, cudaMemcpyHostToDevice, s));
+  if (basic_observed) CU_TRY(h, cudaMemcpyAsync(obs, h->d_basic_keep, lb, cudaMemcpyDeviceToDevice, s));
+  const unsigned grid = grid_for(h, n, 256);
+  launch_morph(true, thr, (float*)r[1], rows, cols, reach, grid, s);              // dilateAndErode: step over small obstacles
+  launch_morph(false, (float*)r[1], (float*)r[2], rows, cols, reach, grid, s);
+  launch_morph(false, (float*)r[2], filter, rows, cols, wall, grid, s);           // erode: keep away from walls
+  CU_TRY(h, cudaGetLastError());
+  if (traversability_sample_filter)
+    CU_TRY(h, cudaMemcpyAsync(traversability_sample_filter, filter, lb, cudaMemcpyDeviceToHost, s));
+  if ((rc = host_call_end(h))) return rc;
+  h->has_sample_filter = true;
+  h->has_dist_observed = observed || basic_observed;
+  h->stats.kernel_launches += 3;
+  h->stats.last_launches = 3;
+  return ARTP_OK;
+}
+
+// getGaussianKernel(ksize, sigma, CV_32F) for sigma > 0: exp(-x^2 / (2 sigma^2)) at x = i - (ksize - 1) / 2, normalised
+// by the double sum, then cast to float -- equal to OpenCV's coefficients (tests/test_sample_distribution_cpu.py).
+static artp::GaussTaps gauss_taps(int ksize, double sigma) {
+  artp::GaussTaps k;
+  std::memset(&k, 0, sizeof(k));
+  std::vector<double> v(ksize);
+  const double scale2X = -0.5 / (sigma * sigma);
+  double sum = 0.0;
+  for (int i = 0; i < ksize; ++i) {
+    const double x = i - (ksize - 1) * 0.5;
+    v[i] = std::exp(scale2X * (x * x));
+    sum += v[i];
+  }
+  const double inv = 1.0 / sum;
+  k.half = ksize / 2;
+  for (int t = 0; t <= k.half; ++t) k.w[t] = (float)(v[k.half + t] * inv);
+  return k;
+}
+
+int artp_debug_gaussian_kernel(int ksize, double sigma, float* out) {   // test hook: the ksize coefficients
+  if (ksize < 1 || ksize > artp::kMaxGaussTaps || !(ksize & 1) || !(sigma > 0) || !out) return ARTP_E_INVALID;
+  const artp::GaussTaps k = gauss_taps(ksize, sigma);
+  for (int i = 0; i < ksize; ++i) out[i] = k.w[std::abs(i - k.half)];
+  return ksize;
+}
+
+// Argument checks shared by both forms; the blur's kernel size and sigma in cells (sample_density.cpp:33-35).
+static int distribution_args(Handle* h, const artp_sample_distribution_params* dp, int* ksize, double* sigma) {
+  if (!h->has_map) { h->err = "no map set"; return ARTP_E_NOMAP; }
+  if (h->win_rows != h->rows) { h->err = "not available on a map window (artp_set_map_window)"; return ARTP_E_INVALID; }
+  if (!dp) { h->err = "null distribution params"; return ARTP_E_INVALID; }
+  *ksize = 0; *sigma = 0.0;
+  if (dp->use_inverse_vertex_density) {
+    if (!(dp->density_blur_radius > 0.0 && std::isfinite(dp->density_blur_radius))) {
+      h->err = "density_blur_radius must be finite and > 0"; return ARTP_E_INVALID;
+    }
+    const double cells = 6 * dp->density_blur_radius / h->res;
+    if (!(cells < artp::kMaxGaussTaps + 1)) { h->err = "Gaussian kernel larger than 1023 cells"; return ARTP_E_LIMIT; }
+    int k = (int)cells;
+    if (k % 2 == 0) k += 1;
+    if (k > artp::kMaxGaussTaps) { h->err = "Gaussian kernel larger than 1023 cells"; return ARTP_E_LIMIT; }
+    *ksize = k;
+    *sigma = dp->density_blur_radius / h->res;
+  }
+  if (dp->use_max_prob_unknown_samples) {
+    if (!(dp->max_prob_unknown_samples >= 0.0 && dp->max_prob_unknown_samples <= 1.0)) {
+      h->err = "max_prob_unknown_samples must lie in [0, 1]"; return ARTP_E_INVALID;
+    }
+    if (!h->has_dist_observed) {
+      h->err = "the unknown-space cap needs the observed layer (artp_set_sample_filter after artp_set_map)"; return ARTP_E_INVALID;
+    }
+  }
+  return ARTP_OK;
+}
+
+// Scratch of one update: n_samples | blur pass | sample_probability | known row sums | unknown row sums | max bits, mult[2].
+struct DistScratch { float *n_samples, *pass, *prob; double *known, *unknown; unsigned int* max_bits; float* mult; };
+static int dist_scratch(Handle* h, DistScratch* d) {
+  const size_t lb = ((size_t)h->rows * h->cols * sizeof(float) + 255) & ~(size_t)255, rb = ((size_t)h->rows * sizeof(double) + 255) & ~(size_t)255;
+  int rc = grow(h, h->d_dist_scratch, h->dist_scratch_cap, 3 * lb + 2 * rb + 256);
+  if (rc) return rc;
+  char* b = h->d_dist_scratch;
+  d->n_samples = (float*)b; d->pass = (float*)(b + lb); d->prob = (float*)(b + 2 * lb);
+  d->known = (double*)(b + 3 * lb); d->unknown = (double*)(b + 3 * lb + rb);
+  d->max_bits = (unsigned int*)(b + 3 * lb + 2 * rb); d->mult = (float*)(b + 3 * lb + 2 * rb + 64);
+  return ARTP_OK;
+}
+
+// The chain on s into d->prob and the sampler's CDF layers; arguments checked by distribution_args.
+static int update_distribution(Handle* h, const artp_sample_distribution_params* dp, int ksize, double sigma,
+                               const double* d_states, size_t n, cudaStream_t s, DistScratch* d) {
+  int rc;
+  if ((rc = ensure_sampler_layers(h)) || (rc = dist_scratch(h, d))) return rc;
+  const int rows = h->rows, cols = h->cols;
+  const size_t ncell = (size_t)rows * cols;
+  const unsigned grid = grid_for(h, ncell, 256);
+  uint32_t launches = 0;
+  const float* n_blur = nullptr;
+  if (dp->use_inverse_vertex_density) {                                          // sample_density.cpp:21-42
+    CU_TRY(h, cudaMemsetAsync(d->n_samples, 0, ncell * sizeof(float), s));
+    CU_TRY(h, cudaMemsetAsync(d->max_bits, 0, sizeof(unsigned int), s));
+    if (n) {
+      artp::SamplerDev m{};
+      sampler_map_view(h, m);
+      artp::vertex_histogram_kernel<<<grid_for(h, n, 256), 256, 0, s>>>(m, d_states, n, d->n_samples);
+      ++launches;
+    }
+    const artp::GaussTaps k = gauss_taps(ksize, sigma);
+    artp::gauss_pass_kernel<0><<<grid, 256, 0, s>>>(d->n_samples, d->pass, rows, cols, k);
+    artp::gauss_pass_kernel<1><<<grid, 256, 0, s>>>(d->pass, d->n_samples, rows, cols, k);
+    artp::abs_max_kernel<<<grid, 256, 0, s>>>(d->n_samples, ncell, d->max_bits);
+    launches += 3;
+    n_blur = d->n_samples;
+  }
+  artp::combine_kernel<<<grid, 256, 0, s>>>(n_blur, d->max_bits, h->has_sample_filter ? h->d_dist_layers : nullptr, ncell, d->prob);
+  ++launches;
+  if (dp->use_max_prob_unknown_samples) {                                        // probability_distribution.cpp:50-91
+    const float* obs = h->d_dist_layers + ncell;
+    artp::cap_rows_kernel<<<(rows + 63) / 64, 64, 0, s>>>(d->prob, obs, rows, cols, d->known, d->unknown);
+    artp::cap_mult_kernel<<<1, 32, 0, s>>>(d->known, d->unknown, rows, dp->max_prob_unknown_samples, d->mult);
+    artp::cap_apply_kernel<<<grid, 256, 0, s>>>(d->prob, obs, d->mult, ncell);
+    launches += 3;
+  }
+  CU_TRY(h, cudaGetLastError());
+  if ((rc = launch_sample_cdf(h, d->prob, s))) return rc;
+  launches += 2;
+  h->has_device_cdf = true;
+  h->has_sampler = false;          // the sampler must be (re)armed with artp_set_sampler
+  h->stats.kernel_launches += launches;
+  h->stats.last_launches = launches;
+  return ARTP_OK;
+}
+
+int artp_update_sample_distribution_device(artp_handle* hh, const artp_sample_distribution_params* dp,
+                                           const double* d_vertex_states, size_t n, void* stream) {
+  LOCK_HANDLE(h, hh);
+  int ksize;
+  double sigma;
+  int rc = distribution_args(h, dp, &ksize, &sigma);
+  if (rc) return rc;
+  if (n && !d_vertex_states) { h->err = "null buffer"; return ARTP_E_INVALID; }
+  CU_TRY(h, cudaSetDevice(h->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  ChainScope cs(h, 0, s);
+  if (cs.rc) return cs.rc;
+  DistScratch d;
+  return update_distribution(h, dp, ksize, sigma, d_vertex_states, n, s, &d);
+}
+
+int artp_update_sample_distribution(artp_handle* hh, const artp_sample_distribution_params* dp, const double* vertex_states,
+                                    size_t n, float* sample_probability, float* cum_prob, float* cum_prob_rowwise) {
+  LOCK_HANDLE(h, hh);
+  int ksize;
+  double sigma;
+  int rc = distribution_args(h, dp, &ksize, &sigma);
+  if (rc) return rc;
+  if (n && !vertex_states) { h->err = "null buffer"; return ARTP_E_INVALID; }
+  const size_t sb = n * 7 * sizeof(double), ncell = (size_t)h->rows * h->cols;
+  char* r[1];
+  if ((rc = host_call_begin(h, {sb}, r))) return rc;
+  if (n) CU_TRY(h, cudaMemcpyAsync(r[0], vertex_states, sb, cudaMemcpyHostToDevice, h->stream));
+  DistScratch d;
+  if ((rc = update_distribution(h, dp, ksize, sigma, (const double*)r[0], n, h->stream, &d))) return rc;
+  if (sample_probability)
+    CU_TRY(h, cudaMemcpyAsync(sample_probability, d.prob, ncell * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  if (cum_prob)
+    CU_TRY(h, cudaMemcpyAsync(cum_prob, h->d_samp_layers + 4 * ncell, ncell * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  if (cum_prob_rowwise)
+    CU_TRY(h, cudaMemcpyAsync(cum_prob_rowwise, h->d_samp_layers + 5 * ncell, (size_t)h->rows * sizeof(float),
+                              cudaMemcpyDeviceToHost, h->stream));
+  return host_call_end(h);
 }
 
 static_assert(ARTP_COST_NET_LIGHT == artp_cnn::kNetLight && ARTP_COST_NET_FULL == artp_cnn::kNetFull,

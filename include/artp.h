@@ -330,6 +330,46 @@ int artp_process_basic(artp_handle* h, const float* elevation, const float* trav
  * edge length (3 for size <= 0: OpenCV's default box). */
 int artp_debug_circular_kernel(int size, uint8_t* out);
 
+/* ---- the sampler's distribution (Planner::setUpMapProcessors, planner.cpp:39-58) ----------------------------------
+ * The chain the reference builds with sample_from_distribution, and re-applies from PRMMotionCostMaintainer::sampleGraph
+ * every recompute_density_after_n_samples vertices (prm_motion_cost.cpp:190-193), on the device:
+ *   artp_set_sample_filter           Basic::setTraversabilityFilter (basic.cpp:110-125): dilateAndErode of
+ *                                    "traversability_thresholded" by (int)(sqrt(reach.x^2 + reach.y^2) / res), then erode by
+ *                                    (int)(min((torso.length - reach.x) / 2, (torso.width - reach.y) / 2) / res) cells
+ *                                    (geometry from artp_params); the result and the "observed" layer stay on the device.
+ *   artp_update_sample_distribution  computeInverseSampleDensity (sample_density.cpp:12-43: histogram of the vertices'
+ *                                    (x, y), Gaussian blur, max - n), applyBaseSampleDistribution (x the filter, when one is
+ *                                    set), applyMaxUnknownProbability (probability_distribution.cpp:50-91) and the CDF of
+ *                                    artp_compute_sample_cdf, which stays resident: re-arm the sampler with
+ *                                    artp_set_sampler(h, sp, ..., NULL, NULL) afterwards.
+ * Every layer is bit-identical to oracle/sample_distribution_oracle.py; the blur is within 2e-6 x max(layer) of
+ * cv::GaussianBlur (DESIGN.md 4.4). A stateless call: with no vertex on the map the density is the uniform 1 (the
+ * reference would keep its previous layer). artp_set_map drops the filter and observed layers; a map window is
+ * ARTP_E_INVALID. */
+typedef struct artp_sample_distribution_params {
+  int    use_inverse_vertex_density;      /* params.h:82 */
+  double density_blur_radius;             /* planner.cpp:48: (torso.length + torso.width) * 0.25; > 0 */
+  int    use_max_prob_unknown_samples;    /* params.h:83 */
+  double max_prob_unknown_samples;        /* params.h:84; in [0, 1] */
+} artp_sample_distribution_params;
+/* HOST grid_map layers of the current map's rows x cols. NULL = the layer the last artp_process_basic on this handle
+ * received (observed) / produced (traversability_thresholded), when it ran on a map of the same size (else
+ * ARTP_E_INVALID for traversability_thresholded; no observed layer for observed). traversability_sample_filter: nullable
+ * HOST out. Structuring elements above 64 cells: ARTP_E_LIMIT. */
+int artp_set_sample_filter(artp_handle* h, const float* traversability_thresholded, const float* observed,
+                           float* traversability_sample_filter);
+/* vertex_states: the roadmap's vertices, n x 7 doubles (only x, y read; order irrelevant; off-map or NaN positions are
+ * not counted). Blur kernel (int)(6 r / res) (+1 if even) above 1023 cells: ARTP_E_LIMIT. The cap without an observed
+ * layer, or bad parameters: ARTP_E_INVALID. sample_probability, cum_prob (rows x cols) and cum_prob_rowwise (rows):
+ * nullable HOST outs. The _device form reads DEVICE vertex states and runs asynchronously on `stream`. */
+int artp_update_sample_distribution(artp_handle* h, const artp_sample_distribution_params* dp,
+                                    const double* vertex_states, size_t n, float* sample_probability,
+                                    float* cum_prob, float* cum_prob_rowwise);
+int artp_update_sample_distribution_device(artp_handle* h, const artp_sample_distribution_params* dp,
+                                           const double* d_vertex_states, size_t n, void* stream);
+/* Test hook: getGaussianKernel(ksize, sigma, CV_32F) as the blur uses it (odd ksize <= 1023, sigma > 0); returns ksize. */
+int artp_debug_gaussian_kernel(int ksize, double sigma, float* out);
+
 /* ---- learned motion cost (MotionCostFunc, objectives/motion_cost_objective.h:22-23) ------------------------------
  * Weights: ONE flat fp32 blob in the layer order of the reference's `network` module: init_conv1..5, init_flatten,
  * tar0_conv1, out0_conv1, out1_conv1..3 -- each conv.weight [Cout][Cin][kh][kw] followed by its BatchNorm weight, bias,

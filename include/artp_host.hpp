@@ -48,6 +48,9 @@ struct Params {
     double max_pitch_pert{10.0 / 180 * 3.14159265358979323846};   // params.h:79
     double max_roll_pert{3.33 / 180 * 3.14159265358979323846};    // params.h:80
     bool sample_from_distribution{true};                            // params.h:81
+    bool use_inverse_vertex_density{false};                         // params.h:82
+    bool use_max_prob_unknown_samples{false};                       // params.h:83
+    double max_prob_unknown_samples{0.1};                           // params.h:84
   } sampler;
   int device{0};   // not in the reference: CUDA device ordinal
 };
@@ -64,6 +67,8 @@ struct Map {
   // layers the sampler reads (Map::getNormal / getPlaneFitStdDev map.h:94-116, probability_distribution.cpp:20-46);
   // cum_prob_rowwise = column 0 of "cum_prob_rowwise_hack". Empty when no sampler is used.
   std::vector<float> normal_x, normal_y, normal_z, plane_fit_std_dev, cum_prob, cum_prob_rowwise;
+  // the sampler's distribution (planner.cpp:39-58): inputs from processors::Basic, outputs of the device chain
+  std::vector<float> traversability_thresholded, observed, traversability_sample_filter, sample_probability;
 };
 
 inline artp_params toArtp(const Params& p) {
@@ -167,6 +172,40 @@ class StateValidityChecker {
                                            map_->cum_prob_rowwise.data()), "artp_compute_sample_cdf");
   }
 
+  // Basic::setTraversabilityFilter (basic.cpp:110-125) on the device: fills the map's traversability_sample_filter from its
+  // traversability_thresholded layer and keeps it, with the map's observed layer (empty: none), for updateSampleDistribution.
+  void setSampleFilter() {
+    if (!map_) throw std::runtime_error("setSampleFilter: no map");
+    const size_t ncell = static_cast<size_t>(map_->rows) * map_->cols;
+    if (map_->traversability_thresholded.size() != ncell || (!map_->observed.empty() && map_->observed.size() != ncell))
+      throw std::invalid_argument("setSampleFilter: layer size mismatch");
+    map_->traversability_sample_filter.resize(ncell);
+    handle_->check(artp_set_sample_filter(handle_->get(), map_->traversability_thresholded.data(),
+                                          map_->observed.empty() ? nullptr : map_->observed.data(),
+                                          map_->traversability_sample_filter.data()), "artp_set_sample_filter");
+  }
+
+  // computeInverseSampleDensity -> applyBaseSampleDistribution -> applyMaxUnknownProbability ->
+  // computeCumulativeProbabilityDistribution (planner.cpp:39-58) on the device for the roadmap's vertices, with the
+  // sampler parameters and blur radius the reference's Planner uses; fills sample_probability / cum_prob /
+  // cum_prob_rowwise and keeps the CDF resident (re-arm SE3FromSE2Sampler: updateDistribution does both).
+  void updateSampleDistribution(const std::vector<State>& vertices) {
+    if (!map_) throw std::runtime_error("updateSampleDistribution: no map");
+    const Params& p = handle_->params();
+    artp_sample_distribution_params dp{};
+    dp.use_inverse_vertex_density = p.sampler.use_inverse_vertex_density ? 1 : 0;
+    dp.density_blur_radius = (p.robot.torso.length + p.robot.torso.width) * 0.25;
+    dp.use_max_prob_unknown_samples = p.sampler.use_max_prob_unknown_samples ? 1 : 0;
+    dp.max_prob_unknown_samples = p.sampler.max_prob_unknown_samples;
+    const size_t ncell = static_cast<size_t>(map_->rows) * map_->cols;
+    map_->sample_probability.resize(ncell);
+    map_->cum_prob.resize(ncell);
+    map_->cum_prob_rowwise.resize(map_->rows);
+    handle_->check(artp_update_sample_distribution(handle_->get(), &dp, vertices.empty() ? nullptr : &vertices[0].x,
+                                                   vertices.size(), map_->sample_probability.data(), map_->cum_prob.data(),
+                                                   map_->cum_prob_rowwise.data()), "artp_update_sample_distribution");
+  }
+
   // The rejection-sampling loop `do { sampleUniform(s) } while (!isValid(s))` (prm_motion_cost.cpp:171-194,
   // lazy_prm_star_min_update.cpp:549-556) in batches: draw `batch` candidates with the caller's sampler, check them in
   // one call, keep the valid ones in draw order; repeat until n_wanted states are collected or max_draws candidates
@@ -262,16 +301,24 @@ class SE3FromSE2Sampler {
   // bounds: SE3 position bounds x,y (planner.cpp:148-160); only read when !sample_from_distribution.
   SE3FromSE2Sampler(const StateValidityCheckerPtr& checker, const std::shared_ptr<Map>& map, uint64_t seed,
                     const double low[2], const double high[2])
-      : checker_(checker), seed_(seed) {
+      : checker_(checker), map_(map), seed_(seed) {
     const auto& h = checker_->handle();
     const Params& p = h->params();
-    artp_sampler_params sp{};
-    sp.max_roll_pert = p.sampler.max_roll_pert; sp.max_pitch_pert = p.sampler.max_pitch_pert;
-    sp.sample_from_distribution = p.sampler.sample_from_distribution ? 1 : 0;
-    sp.low[0] = low[0]; sp.low[1] = low[1]; sp.high[0] = high[0]; sp.high[1] = high[1];
-    h->check(artp_set_sampler(h->get(), &sp, map->normal_x.data(), map->normal_y.data(), map->normal_z.data(),
+    sp_.max_roll_pert = p.sampler.max_roll_pert; sp_.max_pitch_pert = p.sampler.max_pitch_pert;
+    sp_.sample_from_distribution = p.sampler.sample_from_distribution ? 1 : 0;
+    sp_.low[0] = low[0]; sp_.low[1] = low[1]; sp_.high[0] = high[0]; sp_.high[1] = high[1];
+    h->check(artp_set_sampler(h->get(), &sp_, map->normal_x.data(), map->normal_y.data(), map->normal_z.data(),
                               map->plane_fit_std_dev.data(), map->cum_prob.empty() ? nullptr : map->cum_prob.data(),
                               map->cum_prob_rowwise.empty() ? nullptr : map->cum_prob_rowwise.data()), "artp_set_sampler");
+  }
+  // The reApplyPreprocessing step of PRMMotionCostMaintainer::sampleGraph (prm_motion_cost.cpp:190-193): the distribution
+  // from the roadmap's vertices (StateValidityChecker::updateSampleDistribution), then the sampler re-armed on the
+  // device-resident CDF.
+  void updateDistribution(const std::vector<State>& vertices) {
+    checker_->updateSampleDistribution(vertices);
+    const auto& h = checker_->handle();
+    h->check(artp_set_sampler(h->get(), &sp_, map_->normal_x.data(), map_->normal_y.data(), map_->normal_z.data(),
+                              map_->plane_fit_std_dev.data(), nullptr, nullptr), "artp_set_sampler");
   }
   void sampleUniform(State* state) {                                             // sampler.cpp:82-131
     const auto& h = checker_->handle();
@@ -309,6 +356,8 @@ class SE3FromSE2Sampler {
   uint64_t nextIndex() const { return next_; }
  private:
   StateValidityCheckerPtr checker_;
+  std::shared_ptr<Map> map_;
+  artp_sampler_params sp_{};
   uint64_t seed_;
   uint64_t next_{0};
 };
