@@ -9,9 +9,14 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libartp.so")
 # (source, extra flags): the geometric kernels need bit-exact fp32 (no FMA contraction, SURVEY.md section 7);
 # the motion-cost network does not.
-SOURCES = [("artp_capi.cu", ["-fmad=false", "-Xcompiler", "-fPIC,-ffp-contract=off"]),
+# The three units of the C ABI all build rows, costs and states that must equal the host's bit for bit.
+GEOMETRY_FLAGS = ["-fmad=false", "-Xcompiler", "-fPIC,-ffp-contract=off"]
+SOURCES = [("artp_capi.cu", GEOMETRY_FLAGS), ("artp_sampling.cu", GEOMETRY_FLAGS), ("artp_cost.cu", GEOMETRY_FLAGS),
            ("artp_cnn.cu", ["-Xcompiler", "-fPIC"])]
-HEADERS = ["artp_device.cuh", "artp_kernels.cuh", "artp_sampler.cuh", "artp_tiles.cuh", "artp_basic.cuh", "artp_distribution.cuh", "artp_cnn.h", os.path.join("..", "..", "include", "artp.h")]
+HEADERS = ["artp_internal.h", "artp_device.cuh", "artp_kernels.cuh", "artp_sampler.cuh", "artp_tiles.cuh", "artp_basic.cuh",
+           "artp_distribution.cuh", "artp_cnn.h", "artp.map", os.path.join("..", "..", "include", "artp.h")]
+# The library exports the C ABI (artp_*) and nothing else.
+VERSION_SCRIPT = os.path.join(CSRC, "artp.map")
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17"]
 
@@ -34,7 +39,8 @@ def build(force: bool = False, verbose: bool = False) -> str:
         cmd = [nvcc] + NVCC_FLAGS + extra + (["-Xptxas", "-v"] if verbose else []) + ["-c", "-o", obj, os.path.join(CSRC, src)]
         subprocess.run(cmd, check=True)
         objs.append(obj)
-    subprocess.run([nvcc, "-shared"] + NVCC_FLAGS[:2] + ["-o", LIB] + objs, check=True)
+    subprocess.run([nvcc, "-shared"] + NVCC_FLAGS[:2] + ["-Xlinker", "--version-script=" + VERSION_SCRIPT, "-o", LIB] + objs,
+                   check=True)
     return LIB
 
 

@@ -1,0 +1,335 @@
+// art_planner_b200/csrc/artp_cost.cu -- the cost half of the C ABI (include/artp.h): PathLengthObjective::motionCost, the
+// MotionCostFunc edge matrix, the learned motion cost of edge rows, of states and of whole edges split the way
+// MotionCostObjective::motionCost splits them, and the network's weights, features and mode (artp_cnn.cu runs the network).
+// Compiled without FMA contraction like artp_capi.cu, so that the rows and costs built here equal the host's bit for bit.
+#include <cmath>
+#include <vector>
+
+#include "artp_internal.h"
+
+using namespace artp_api;
+
+namespace {
+
+// PathLengthObjective::motionCost (art_planner/src/objectives/path_length_objective.cpp:26-70), double.
+__global__ void path_length_kernel(const double* __restrict__ s1, const double* __restrict__ s2, size_t n,
+                                   double* __restrict__ cost, int directional, double v_lon, double v_lat,
+                                   double v_ang) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const double* a = s1 + 7 * i;
+    const double* b = s2 + 7 * i;
+    const double x_dif = b[0] - a[0], y_dif = b[1] - a[1], z_dif = b[2] - a[2];
+    if (!directional) {
+      cost[i] = sqrt(x_dif * x_dif + y_dif * y_dif + z_dif * z_dif) / v_lon;
+      continue;
+    }
+    const double yaw1 = (double)artp::so3_yaw(a);
+    const double yaw2 = (double)artp::so3_yaw(b);
+    const double d = fabs(yaw1 - yaw2);
+    const double yaw_dif = (d > 3.14159265358979323846) ? 2.0 * 3.14159265358979323846 - d : d;
+    const double lon_dif = cos(yaw1) * x_dif + sin(yaw1) * y_dif;
+    const double lat_dif = -sin(yaw1) * x_dif + cos(yaw1) * y_dif;
+    const double t_yaw = fabs(yaw_dif) / v_ang, t_lon = fabs(lon_dif) / v_lon, t_lat = fabs(lat_dif) / v_lat;
+    const double m = t_lon > t_lat ? t_lon : t_lat;
+    cost[i] = m > t_yaw ? m : t_yaw;
+  }
+}
+
+// Row [x y yaw] of knot s of the MotionCostFunc edge matrix as PRMMotionCostMaintainer::updateEdges /
+// computeCostForVertexEdges fill it (prm_motion_cost.cpp:27-128): x, y cast double -> float by the assignment into the
+// float matrix, yaw = getYawFromSO3. An edge's row is knot_row(target) ++ knot_row(start).
+__host__ __device__ __forceinline__ void knot_row(const double* s, float* o) {
+  o[0] = (float)s[0]; o[1] = (float)s[1];
+  o[2] = artp::so3_yaw(s);
+}
+
+// getCost (motion_cost_objective.h:54-66): getEnergy/getTime/getRisk return double (:30-46), so the weighted sum is
+// evaluated in double on exact float products.
+__host__ __device__ __forceinline__ double get_cost(float ce, float ct, float cr, float we, float wt, float wr) {
+  return (double)ce * (double)we + (double)ct * (double)wt + (double)cr * (double)wr;
+}
+
+__global__ void edge_matrix_kernel(const double* __restrict__ s_start, const double* __restrict__ s_target, size_t n,
+                                   float* __restrict__ edges) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    knot_row(s_target + 7 * i, edges + 6 * i);
+    knot_row(s_start + 7 * i, edges + 6 * i + 3);
+  }
+}
+// getCost / isFeasible per row (motion_cost_objective.h:54-66); infeasible edges get +inf like updateEdges (:56-59)
+__global__ void combine_cost_kernel(const float* __restrict__ cost3, size_t n, float we, float wt, float wr, float thr,
+                                    double* __restrict__ cost, uint8_t* __restrict__ feasible) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float ce = cost3[3 * i], ct = cost3[3 * i + 1], cr = cost3[3 * i + 2];
+    const bool ok = (double)cr <= (double)thr;
+    feasible[i] = ok ? 1 : 0;
+    cost[i] = ok ? get_cost(ce, ct, cr, we, wt, wr) : CUDART_INF;
+  }
+}
+
+// MotionCostObjective::motionCost (motion_cost_objective.cpp:36-95) splits edge e into the pieces piece_off[e] ..
+// piece_off[e+1] - 1 (n_interp + 1 of them). Knot j of the edge is s1 for j = 0, s2 for j = n_interp + 1 (copied, not
+// interpolated) and interpolate(s1, s2, j * (1.0 / (n_interp + 1))) in between (:49, :67); piece i's row is
+// knot_row(knot i+1) ++ knot_row(knot i).
+__device__ __forceinline__ void split_knot_row(const double* a, const double* b, uint32_t j, uint32_t n_pieces, float* o) {
+  if (j == 0) {
+    knot_row(a, o);
+  } else if (j == n_pieces) {
+    knot_row(b, o);
+  } else {   // no pointer select between a, b and k: that would put all three in local memory
+    double k[7];
+    artp::se3_interpolate(a, b, (double)j * (1.0 / (double)n_pieces), k);
+    knot_row(k, o);
+  }
+}
+__global__ void split_rows_kernel(const double* __restrict__ s1, const double* __restrict__ s2, uint32_t n_edges,
+                                  const uint32_t* __restrict__ piece_off, size_t total, float* __restrict__ rows) {
+  for (size_t p = blockIdx.x * (size_t)blockDim.x + threadIdx.x; p < total; p += (size_t)gridDim.x * blockDim.x) {
+    uint32_t lo = 0, hi = n_edges;          // largest e with piece_off[e] <= p, as load_item_state
+    while (hi - lo > 1) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (__ldg(piece_off + mid) <= p) lo = mid; else hi = mid;
+    }
+    const uint32_t o0 = __ldg(piece_off + lo), n_pieces = __ldg(piece_off + lo + 1) - o0, i = (uint32_t)p - o0;
+    double a[7], b[7];
+#pragma unroll
+    for (int k = 0; k < 7; ++k) { a[k] = s1[(size_t)lo * 7 + k]; b[k] = s2[(size_t)lo * 7 + k]; }
+    split_knot_row(a, b, i + 1, n_pieces, rows + 6 * p);
+    split_knot_row(a, b, i, n_pieces, rows + 6 * p + 3);
+  }
+}
+// The rest of motionCost per edge, one thread walking its pieces in order: +inf at the first piece whose risk is above
+// the threshold (isFeasible), else the left-to-right double sum of getCost from 0.0.
+__global__ void split_reduce_kernel(const float* __restrict__ cost3, const uint32_t* __restrict__ piece_off, size_t n,
+                                    float we, float wt, float wr, float thr, double* __restrict__ cost) {
+  for (size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x; e < n; e += (size_t)gridDim.x * blockDim.x) {
+    const uint32_t o0 = piece_off[e], o1 = piece_off[e + 1];
+    double c = 0.0;
+    for (uint32_t k = o0; k < o1; ++k) {
+      const float ce = cost3[3 * (size_t)k], ct = cost3[3 * (size_t)k + 1], cr = cost3[3 * (size_t)k + 2];
+      if ((double)cr > (double)thr) { c = CUDART_INF; break; }
+      c += get_cost(ce, ct, cr, we, wt, wr);
+    }
+    cost[e] = c;
+  }
+}
+
+// The network's head over n edge rows on s, counted as one launch.
+int launch_cost_head(Handle* h, const float* d_edges, size_t n, float* d_cost3, cudaStream_t s) {
+  const int rc = artp_cnn::motion_cost(h->cnn, d_edges, n, d_cost3, s, h->err);
+  return rc || n == 0 ? rc : count_launch(h);
+}
+
+int path_length_cost(Handle* h, const double* d_s1, const double* d_s2, size_t n, double* d_cost, cudaStream_t s) {
+  return launch(h, path_length_kernel, grid_for(h, n, 256, 8), 256, 0, s, d_s1, d_s2, n, d_cost, h->p.use_directional_cost,
+                h->p.max_lon_vel, h->p.max_lat_vel, h->p.max_ang_vel);
+}
+
+int check_cost_net(Handle* h) {
+  if (!artp_cnn::has_weights(h->cnn)) { h->err = "motion-cost weights not set"; return ARTP_E_NOWEIGHTS; }
+  if (!artp_cnn::has_features(h->cnn)) {
+    h->err = "features not computed (call artp_update_features after artp_set_map)";
+    return ARTP_E_NOWEIGHTS;
+  }
+  return ARTP_OK;
+}
+
+// The split cost of n edges with total_pieces pieces on s: piece rows, the head, the per-edge reduction.
+int motion_cost_split(Handle* h, const double* d_s1, const double* d_s2, size_t n, const uint32_t* d_piece_off, size_t total_pieces,
+                      float* d_rows, float* d_cost3, double* d_cost, cudaStream_t s) {
+  TRY(launch(h, split_rows_kernel, grid_for(h, total_pieces, 256, 8), 256, 0, s, d_s1, d_s2, (uint32_t)n, d_piece_off,
+             total_pieces, d_rows));
+  TRY(launch_cost_head(h, d_rows, total_pieces, d_cost3, s));
+  return launch(h, split_reduce_kernel, grid_for(h, n, 256, 8), 256, 0, s, d_cost3, d_piece_off, n, h->p.cost_w_energy,
+                h->p.cost_w_time, h->p.cost_w_risk, h->p.risk_threshold, d_cost);
+}
+
+}  // namespace
+
+static_assert(ARTP_COST_NET_LIGHT == artp_cnn::kNetLight && ARTP_COST_NET_FULL == artp_cnn::kNetFull,
+              "the ABI's network numbers are the library's");
+
+extern "C" {
+
+int artp_edge_matrix_from_states(const double* s_start, const double* s_target, size_t n, float* edges) {
+  if (n && (!s_start || !s_target || !edges)) return ARTP_E_INVALID;
+  for (size_t i = 0; i < n; ++i) {
+    knot_row(s_target + 7 * i, edges + 6 * i);
+    knot_row(s_start + 7 * i, edges + 6 * i + 3);
+  }
+  return ARTP_OK;
+}
+
+int artp_motion_cost_states(artp_handle* hh, const double* s_start, const double* s_target, size_t n, double* cost,
+                            uint8_t* feasible, float* cost3) {
+  LOCK_CALL(h, hh);
+  if (n == 0) return ARTP_OK;
+  if (!s_start || !s_target || !cost || !feasible) return null_buffer(h);
+  const size_t sb = n * 7 * sizeof(double);
+  char* r[6];   // s_start | s_target | edge matrix | cost3 | cost | feasible
+  TRY(host_call_begin(h, {sb, sb, n * 6 * sizeof(float), n * 3 * sizeof(float), n * sizeof(double), n}, r));
+  float* d_edges = (float*)r[2];
+  float* d_c3 = (float*)r[3];
+  CU_TRY(h, cudaMemcpyAsync(r[0], s_start, sb, cudaMemcpyHostToDevice, h->stream));
+  CU_TRY(h, cudaMemcpyAsync(r[1], s_target, sb, cudaMemcpyHostToDevice, h->stream));
+  const unsigned grid = grid_for(h, n, 256, 8);
+  TRY(launch(h, edge_matrix_kernel, grid, 256, 0, h->stream, (const double*)r[0], (const double*)r[1], n, d_edges));
+  TRY(launch_cost_head(h, d_edges, n, d_c3, h->stream));
+  TRY(launch(h, combine_cost_kernel, grid, 256, 0, h->stream, d_c3, n, h->p.cost_w_energy, h->p.cost_w_time, h->p.cost_w_risk,
+      h->p.risk_threshold, (double*)r[4], (uint8_t*)r[5]));
+  CU_TRY(h, cudaMemcpyAsync(cost, r[4], n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(h, cudaMemcpyAsync(feasible, r[5], n, cudaMemcpyDeviceToHost, h->stream));
+  if (cost3) CU_TRY(h, cudaMemcpyAsync(cost3, d_c3, n * 3 * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  return host_call_end(h);
+}
+
+int artp_path_length_cost_device(artp_handle* hh, const double* d_s1, const double* d_s2, size_t n, double* d_cost,
+                                 void* stream) {
+  LOCK_CALL(h, hh);
+  if (n == 0) return ARTP_OK;
+  if (!d_s1 || !d_s2 || !d_cost) return null_buffer(h);
+  CU_TRY(h, cudaSetDevice(h->device));
+  return path_length_cost(h, d_s1, d_s2, n, d_cost, (cudaStream_t)stream);
+}
+
+int artp_path_length_cost(artp_handle* hh, const double* s1, const double* s2, size_t n, double* cost) {
+  LOCK_CALL(h, hh);
+  if (n == 0) return ARTP_OK;
+  if (!s1 || !s2 || !cost) return null_buffer(h);
+  const size_t sb = n * 7 * sizeof(double);
+  char* r[3];
+  TRY(host_call_begin(h, {sb, sb, n * sizeof(double)}, r));
+  CU_TRY(h, cudaMemcpyAsync(r[0], s1, sb, cudaMemcpyHostToDevice, h->stream));
+  CU_TRY(h, cudaMemcpyAsync(r[1], s2, sb, cudaMemcpyHostToDevice, h->stream));
+  TRY(path_length_cost(h, (const double*)r[0], (const double*)r[1], n, (double*)r[2], h->stream));
+  CU_TRY(h, cudaMemcpyAsync(cost, r[2], n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  return host_call_end(h);
+}
+
+size_t artp_cost_weights_size(void) { return artp_cnn::blob_floats(ARTP_COST_NET_LIGHT); }
+
+size_t artp_cost_weights_size_for(int network) { return artp_cnn::blob_floats(network); }
+
+int artp_get_cost_network(artp_handle* hh, int* network) {
+  LOCK_HANDLE(h, hh);
+  if (!network) return ARTP_E_INVALID;
+  *network = artp_cnn::network(h->cnn);
+  if (*network < 0) { h->err = "motion-cost weights not set"; return ARTP_E_NOWEIGHTS; }
+  return ARTP_OK;
+}
+
+int artp_set_cost_weights(artp_handle* hh, const float* blob, size_t n_floats) {
+  LOCK_HANDLE(h, hh);
+  if (!blob) return ARTP_E_INVALID;
+  return artp_cnn::set_weights(h->cnn, blob, n_floats, h->stream, h->err);
+}
+
+int artp_update_features(artp_handle* hh) {
+  LOCK_HANDLE(h, hh);
+  TRY(require_whole_map(h));
+  return artp_cnn::update_features(h->cnn, h->d_H[0], h->rows, h->cols, h->pitch, h->chk.Lx / h->rows, h->chk.cx, h->chk.cy,
+                                   h->stream, h->cnn_mode & 1, h->err);
+}
+
+int artp_motion_cost_device(artp_handle* hh, const float* d_edges, size_t n, float* d_cost3, void* stream) {
+  LOCK_CALL(h, hh);
+  if (n && (!d_edges || !d_cost3)) return null_buffer(h);
+  return launch_cost_head(h, d_edges, n, d_cost3, (cudaStream_t)stream);
+}
+
+int artp_motion_cost(artp_handle* hh, const float* edges, size_t n, float* cost3) {
+  LOCK_CALL(h, hh);
+  if (n == 0) return ARTP_OK;
+  if (!edges || !cost3) return null_buffer(h);
+  char* r[2];   // edges | cost3
+  TRY(host_call_begin(h, {n * 6 * sizeof(float), n * 3 * sizeof(float)}, r));
+  CU_TRY(h, cudaMemcpyAsync(r[0], edges, n * 6 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  TRY(launch_cost_head(h, (const float*)r[0], n, (float*)r[1], h->stream));
+  CU_TRY(h, cudaMemcpyAsync(cost3, r[1], n * 3 * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  return host_call_end(h);
+}
+
+// Reads only the parameters fixed at artp_create, so it takes no lock.
+int artp_combine_cost(artp_handle* hh, const float* cost3, size_t n, double* cost, uint8_t* feasible) {
+  if (!hh || (n && (!cost3 || !cost || !feasible))) return ARTP_E_INVALID;
+  const artp_params& p = reinterpret_cast<Handle*>(hh)->p;
+  for (size_t i = 0; i < n; ++i) {
+    const float ce = cost3[3 * i], ct = cost3[3 * i + 1], cr = cost3[3 * i + 2];
+    cost[i] = get_cost(ce, ct, cr, p.cost_w_energy, p.cost_w_time, p.cost_w_risk);
+    feasible[i] = (double)cr <= (double)p.risk_threshold ? 1 : 0;   // isFeasible (getRisk returns double)
+  }
+  return ARTP_OK;
+}
+
+// Touches no per-handle scratch (the head reads the feature map and weights only), so, like artp_motion_cost_device, it
+// joins no scratch group.
+int artp_motion_cost_split_device(artp_handle* hh, const double* d_s1, const double* d_s2, size_t n,
+                                  const uint32_t* d_piece_off, size_t total_pieces, float* d_rows, float* d_cost3,
+                                  double* d_cost, void* stream) {
+  LOCK_CALL(h, hh);
+  if (n == 0) return ARTP_OK;
+  if (!d_s1 || !d_s2 || !d_piece_off || !d_rows || !d_cost3 || !d_cost) return null_buffer(h);
+  if (total_pieces < n || total_pieces > 0xFFFFFFFFull) {
+    h->err = "total_pieces must lie in [n, 2^32) (every edge has at least one piece)";
+    return ARTP_E_INVALID;
+  }
+  TRY(check_cost_net(h));
+  CU_TRY(h, cudaSetDevice(h->device));
+  return motion_cost_split(h, d_s1, d_s2, n, d_piece_off, total_pieces, d_rows, d_cost3, d_cost, (cudaStream_t)stream);
+}
+
+int artp_motion_cost_split(artp_handle* hh, const double* s1, const double* s2, size_t n, double max_query_edge_length,
+                           double* cost) {
+  LOCK_CALL(h, hh);
+  if (n == 0) return ARTP_OK;
+  if (!s1 || !s2 || !cost) return null_buffer(h);
+  if (!(max_query_edge_length > 0.0)) { h->err = "max_query_edge_length must be > 0"; return ARTP_E_INVALID; }
+  TRY(check_cost_net(h));
+  std::vector<uint32_t> off(n + 1);
+  size_t total = 0;
+  for (size_t e = 0; e < n; ++e) {
+    off[e] = (uint32_t)total;
+    // n_interp = (unsigned)(lateralDistance (utils.h:52-61) / max_query_edge_length), motion_cost_objective.cpp:40-45
+    const double dx = s2[7 * e] - s1[7 * e], dy = s2[7 * e + 1] - s1[7 * e + 1];
+    const double q = std::sqrt(dx * dx + dy * dy) / max_query_edge_length;
+    if (!(q < 4294967296.0)) { h->err = "edge too long or not finite (n_interp must fit 32 bits)"; return ARTP_E_INVALID; }
+    total += (size_t)(unsigned int)q + 1;
+    if (total > 0xFFFFFFFFull) { h->err = "too many pieces (>= 2^32)"; return ARTP_E_INVALID; }
+  }
+  off[n] = (uint32_t)total;
+  const size_t sb = n * 7 * sizeof(double);
+  char* r[6];   // s1 | s2 | piece offsets | rows | cost3 | cost
+  TRY(host_call_begin(h, {sb, sb, (n + 1) * sizeof(uint32_t), total * 6 * sizeof(float), total * 3 * sizeof(float),
+                          n * sizeof(double)}, r));
+  CU_TRY(h, cudaMemcpyAsync(r[0], s1, sb, cudaMemcpyHostToDevice, h->stream));
+  CU_TRY(h, cudaMemcpyAsync(r[1], s2, sb, cudaMemcpyHostToDevice, h->stream));
+  CU_TRY(h, cudaMemcpyAsync(r[2], off.data(), (n + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
+  TRY(motion_cost_split(h, (const double*)r[0], (const double*)r[1], n, (const uint32_t*)r[2], total, (float*)r[3],
+      (float*)r[4], (double*)r[5], h->stream));
+  CU_TRY(h, cudaMemcpyAsync(cost, r[5], n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  return host_call_end(h);   // `off` outlives its H2D copy: the call synchronises before it returns
+}
+
+int artp_get_features(artp_handle* hh, float* out, size_t n_floats, int* hf, int* wf) {
+  LOCK_HANDLE(h, hh);
+  if (!hf || !wf) return ARTP_E_INVALID;
+  artp_cnn::feature_shape(h->cnn, hf, wf);
+  if (!out) return ARTP_OK;
+  return artp_cnn::copy_features(h->cnn, out, n_floats, h->err);
+}
+
+int artp_set_cnn_mode(artp_handle* hh, int mode) {
+  LOCK_HANDLE(h, hh);
+  if (mode & ~1) { h->err = "unknown motion-cost network mode (bit 0 is the only mode bit)"; return ARTP_E_INVALID; }
+  h->cnn_mode = mode;
+  return ARTP_OK;
+}
+
+int artp_get_cnn_timing(artp_handle* hh, float* ms3) {
+  LOCK_HANDLE(h, hh);
+  if (!ms3) return ARTP_E_INVALID;
+  artp_cnn::last_times(h->cnn, ms3);
+  return ARTP_OK;
+}
+
+}  // extern "C"

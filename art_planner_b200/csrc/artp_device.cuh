@@ -56,6 +56,56 @@ struct Checker {
   int reach_tw, reach_th;
 };
 
+// TMA tile of a box queue (artp_tiles.cuh).
+struct TileCfg {
+  int tw, th;              // tile extent in floats (tw a multiple of 4; a zone may be at most tw - 3 wide, th high)
+  uint32_t bytes, stride;  // tw * th * 4, and that rounded up to 128 bytes
+  int x_off;               // first stored vertex column of the layer (map window), a multiple of 4
+  int slots;               // tile slots per warp: 2 = the next box's tile is prefetched while this one is decided, 1 = none
+};
+struct SamplerDev {
+  const float* elevation_rev;   // Field::H of the elevation layer: H[x + z*pitch] = layer(x, cols-1-z)
+  int pitch;
+  const float* normal_x;        // grid_map layout: (row, col) at row + col*rows
+  const float* normal_y;
+  const float* normal_z;
+  const float* std_dev;
+  const float* cum_prob;        // may be null (uniform mode)
+  const float* cum_row;         // rows floats
+  int rows, cols;
+  double res, cx, cy;
+  double max_roll_pert, max_pitch_pert;
+  int from_distribution;
+  double low[2], high[2];
+  double reach_z;
+};
+
+// OMPL 1.4.2 SE3StateSpace::interpolate (RealVector lerp + SO3 slerp), double.
+__device__ __forceinline__ void se3_interpolate(const double* a, const double* b, double t, double* out) {
+  for (int i = 0; i < 3; ++i) out[i] = a[i] + (b[i] - a[i]) * t;
+  const double dq = a[3] * b[3] + a[4] * b[4] + a[5] * b[5] + a[6] * b[6];
+  const double dqa = fabs(dq);
+  const double theta = (dqa > 1.0 - 1e-9) ? 0.0 : acos(dqa);
+  if (theta > 2.220446049250313e-16) {
+    const double d = 1.0 / sin(theta);
+    const double s0 = sin((1.0 - t) * theta);
+    double s1 = sin(t * theta);
+    if (dq < 0) s1 = -s1;
+    out[3] = (a[3] * s0 + b[3] * s1) * d;
+    out[4] = (a[4] * s0 + b[4] * s1) * d;
+    out[5] = (a[5] * s0 + b[5] * s1) * d;
+    out[6] = (a[6] * s0 + b[6] * s1) * d;
+  } else {
+    out[3] = a[3]; out[4] = a[4]; out[5] = a[5]; out[6] = a[6];
+  }
+}
+
+// getYawFromSO3 (utils.h:80-88) of the quaternion of SE(3) state s: double atan2, returned as `Scalar` = float. On the host
+// atan2 is libm's, on the device CUDA's.
+__host__ __device__ __forceinline__ float so3_yaw(const double* s) {
+  return (float)atan2(2 * (s[6] * s[5] + s[3] * s[4]), 1 - 2 * (s[4] * s[4] + s[5] * s[5]));
+}
+
 // Box pose in heightfield space + AABB + zone.
 struct BoxCtx {
   float R1[9];   // rows: -R.row0, R.row2, R.row1 of the orthogonalised box rotation (3x3, row-major)

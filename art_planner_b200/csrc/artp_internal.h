@@ -1,0 +1,271 @@
+// art_planner_b200/csrc/artp_internal.h -- what the three units of the C ABI share (not installed):
+//   artp_capi.cu      handle lifecycle, errors, stats and timing, map upload, the validity pipeline, pose / motion / edge
+//                     checks, compaction and bit packing
+//   artp_sampling.cu  normals and the CDF, the sampler, start / goal search, poseFrom2D, Basic, the sample distribution
+//   artp_cost.cu      path length, the edge matrix, the learned motion cost, cost weights and features
+// the handle and its lock, launch and call bookkeeping, scratch regions, argument checks, and the few functions one unit
+// calls in another. It includes no kernel header: each of those defines kernels and is compiled into exactly one unit.
+#pragma once
+
+#include <cuda.h>
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cstdint>
+#include <initializer_list>
+#include <mutex>
+#include <string>
+#include <utility>
+
+#include "../../include/artp.h"
+#include "artp_cnn.h"
+#include "artp_device.cuh"
+
+namespace artp { struct BoxRec; }
+
+namespace artp_api {
+
+constexpr int kMaxSlices = 9;   // H2D slices per host-fed round: at most 8 scheduled fractions and the remainder
+
+// One box queue: the classify stage appends records up to `end`, the queue's box kernel claims them from `claim`.
+struct QueueCtr { uint32_t end, claim; };
+// The three box queues of a round (Handle::d_ctr), or the entries one slice of a host-fed round appended (Handle::d_slices).
+// One 32-byte sector each: the box kernels of consecutive slices claim from their records at the same time.
+struct alignas(32) BoxQueues { QueueCtr big, reach, group; };
+// Per-handle device counters: the round's queues, the boxes deferred to the grouping stage, and the sampler's CDF check.
+struct Counters { BoxQueues q; uint32_t defer, scratch; };
+
+// What belongs to the current map: artp_set_map_window resets all of it.
+struct MapState {
+  bool has_sampler = false;
+  bool has_device_normals = false;  // artp_estimate_normals filled normal_x/y/z/std_dev of d_samp_layers for this map
+  bool has_device_cdf = false;      // artp_compute_sample_cdf filled cum_prob / cum_row of d_samp_layers for this map
+  bool has_normals = false;         // normal_x/y/z of d_samp_layers hold this map's normals (device-estimated or the caller's)
+  bool has_sample_filter = false;   // d_dist_layers holds this map's traversability_sample_filter ...
+  bool has_dist_observed = false;   // ... and observed layer
+};
+
+struct Handle {
+  artp_params p;
+  int device = 0;
+  int sm_count = 0;
+  artp::Checker chk;
+  float* d_H[2] = {nullptr, nullptr};
+  float2* d_T[2][artp::kMaxLevel + 1] = {};
+  uint32_t* d_C[2][artp::kMaxLevel + 1] = {};    // compact conservative copies of d_T (Field::C)
+  int pitch = 0;
+  int rows = 0, cols = 0;           // full map
+  int win_row0 = 0, win_rows = 0;   // rows held by this handle (artp_set_map_window); whole map: 0, rows
+  bool has_map = false;
+  MapState map;
+  Counters* d_ctr = nullptr;
+  uint32_t* d_defer = nullptr;      // deferred record list (bit 31: reach-box queue)
+  artp::BoxRec* d_recs = nullptr;   // classify -> warp-stage box queue (torso boxes, reach boxes of unusual size)
+  artp::BoxRec* d_recs_f = nullptr; // classify -> reach-box queue (one warp per box: zones with -inf or mergeable planes)
+  artp::BoxRec* d_recs_g = nullptr; // classify -> reach-box queue of the 8-lane-group kernel (all-finite, merge-free zones)
+  int group_grid = 0, group_smem = 0;
+  size_t recs_cap = 0;
+  uint32_t* d_block_counts = nullptr;
+  size_t block_counts_cap = 0;
+  char* d_stage = nullptr;          // device staging for the host-buffer API
+  size_t stage_cap = 0;
+  cudaStream_t stream = nullptr;    // internal compute stream for the host-buffer API
+  cudaStream_t copy_stream = nullptr;   // H2D slices of the host-buffer API
+  cudaStream_t group_stream = nullptr;  // the 8-lane-group kernel of slice i (host-fed rounds), beside the other box kernels
+  cudaEvent_t group_ev = nullptr;
+  cudaStream_t box_stream = nullptr;    // box stages of slice i, concurrent with the copy + classify of slice i + 1
+  cudaEvent_t copy_ev[kMaxSlices] = {};    // H2D of slice i landed (the call's stream waits on it)
+  cudaEvent_t slice_ev[kMaxSlices] = {};   // classify of slice i done (box_stream waits on it)
+  cudaEvent_t box_ev = nullptr;            // box stages of a round done (stream waits on it)
+  BoxQueues* d_slices = nullptr;           // per slice of a host-fed round: its share of the three queues
+  int k2_grid = 0, k2_smem = 0, k2_tcap = 0;
+  // stage B (artp_tiles.cuh): [0] big tiles (torso queue, 4 warps per CTA), [1] small tiles (reach-box queue, 8 warps)
+  artp::TileCfg tile_cfg[2] = {};
+  int tile_grid[2] = {0, 0}, tile_smem[2] = {0, 0}, tile_warps[2] = {8, 8};
+  CUtensorMap tile_map[2][2];       // [cfg][layer]: 2-D tile maps over elevation / elevation_masked
+  int mode = 0;
+  artp_cnn::State* cnn = nullptr;
+  int cnn_mode = 0;
+  // sampler (artp_set_sampler): device copies of the per-cell layers, scratch of the fused sample->check->compact path
+  artp::SamplerDev samp{};
+  float* d_samp_layers = nullptr;   // normal_x | normal_y | normal_z | std_dev | cum_prob | cum_row
+  size_t samp_layers_cap = 0;       // floats
+  char* d_samp_scratch = nullptr;
+  size_t samp_scratch_cap = 0;
+  double res = 0.0;                 // map resolution as artp_set_map received it
+  // sampling distribution (artp_distribution.cuh): the layers artp_set_sample_filter keeps for this map ...
+  float* d_dist_layers = nullptr;   // traversability_sample_filter | observed
+  size_t dist_layers_cap = 0;       // floats
+  char* d_dist_scratch = nullptr;   // n_samples | blur pass | sample_probability | cap row sums | words (artp_update_sample_distribution)
+  size_t dist_scratch_cap = 0;
+  // ... and the layers of the last artp_process_basic, its NULL-layer inputs
+  float* d_basic_keep = nullptr;    // observed | traversability_thresholded
+  size_t basic_keep_cap = 0;        // floats
+  int basic_rows = 0, basic_cols = 0;
+  bool has_basic_layers = false, has_basic_observed = false;
+  uint8_t* h_small_out = nullptr;   // mapped pinned host bytes the latency-path kernel writes its verdicts to
+  int timing = 0;
+  cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // classify | warp | reach vertex | reach plane | group
+  bool ev_valid = false;
+  bool deferred_unread = false;
+  // Cross-stream ordering of the per-handle scratch (ADVICE r1): calls may come on different streams; every call that
+  // uses a scratch group first makes its stream wait for the previous user of that group, and records an event after.
+  // group 0: d_ctr / d_recs / d_defer / d_stage / d_samp_scratch / d_dist_scratch (check, sampler, distribution);
+  // group 1: d_block_counts (compaction)
+  cudaEvent_t chain_ev[2] = {nullptr, nullptr};
+  cudaStream_t chain_stream[2] = {nullptr, nullptr};
+  bool chain_busy[2] = {false, false};
+  // Sticky error word in mapped pinned host memory: the plane-grouping stage sets it when a zone does not fit its
+  // shared-memory store (the item is then marked INVALID -- fail closed). Host-buffer calls return ARTP_E_LIMIT from the
+  // call that caused it; device-buffer (asynchronous) calls surface it through artp_poll_error().
+  uint32_t* h_err = nullptr;        // host view
+  uint32_t* d_err = nullptr;        // device view of the same word
+  int tcap_override = 0;            // test hook (artp_debug_set_group_capacity)
+  artp_stats stats{};
+  std::string err;
+  std::mutex mtx;
+};
+
+#define CU_TRY(h, expr)                                                                          \
+  do {                                                                                           \
+    cudaError_t _e = (expr);                                                                     \
+    if (_e != cudaSuccess) {                                                                     \
+      (h)->err = std::string(#expr) + ": " + cudaGetErrorString(_e);                             \
+      return ARTP_E_CUDA;                                                                        \
+    }                                                                                            \
+  } while (0)
+
+// Returns the error of a step that failed (ARTP_OK is 0).
+#define TRY(expr)                                                                                \
+  do {                                                                                           \
+    if (const int _rc = (expr)) return _rc;                                                      \
+  } while (0)
+
+// Opens an entry point that takes a handle: a null handle is ARTP_E_INVALID; otherwise `h` is the handle, and its lock is
+// held until the entry point returns. Entry points never call one another, so no call takes the lock twice.
+#define LOCK_HANDLE(h, hh)                                                                       \
+  if (!(hh)) return ARTP_E_INVALID;                                                              \
+  Handle* h = reinterpret_cast<Handle*>(hh);                                                     \
+  std::lock_guard<std::mutex> h##_lock(h->mtx)
+
+// Set up by LOCK_CALL: on every return path of the call it sets stats.last_launches to the number of kernels the call
+// launched.
+struct CallScope {
+  Handle* h;
+  uint64_t launches0;
+  explicit CallScope(Handle* h_) : h(h_), launches0(h_->stats.kernel_launches) {}
+  ~CallScope() { h->stats.last_launches = (uint32_t)(h->stats.kernel_launches - launches0); }
+};
+// LOCK_HANDLE for the entry points that launch kernels.
+#define LOCK_CALL(h, hh)                                                                         \
+  LOCK_HANDLE(h, hh);                                                                            \
+  CallScope h##_call(h)
+
+// Checks the kernel launch just issued and counts it in stats.kernel_launches.
+inline int count_launch(Handle* h) {
+  CU_TRY(h, cudaGetLastError());
+  h->stats.kernel_launches += 1;
+  return ARTP_OK;
+}
+
+// kernel<<<grid, block, smem, s>>>(args...), checked and counted.
+template <typename... P, typename... A>
+int launch(Handle* h, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, A&&... args) {
+  kernel<<<grid, block, smem, s>>>(std::forward<A>(args)...);
+  return count_launch(h);
+}
+
+// Grid-stride launches: enough blocks for n items, at most `per_sm` blocks per SM.
+inline unsigned grid_for(const Handle* h, size_t n, int block, size_t per_sm = 16) {
+  return (unsigned)std::min<size_t>((n + block - 1) / block, (size_t)h->sm_count * per_sm);
+}
+
+inline int require_map(Handle* h) {
+  if (!h->has_map) { h->err = "no map set"; return ARTP_E_NOMAP; }
+  return ARTP_OK;
+}
+// The calls over whole-map layers (sampler, normals, distribution, features) refuse a map window.
+inline int require_whole_map(Handle* h) {
+  TRY(require_map(h));
+  if (h->win_rows != h->rows) { h->err = "not available on a map window (artp_set_map_window)"; return ARTP_E_INVALID; }
+  return ARTP_OK;
+}
+inline int null_buffer(Handle* h) {
+  h->err = "null buffer";
+  return ARTP_E_INVALID;
+}
+
+// Grow a per-handle device buffer to hold `count` elements (cap counts them too); the contents are not kept. Rare (growth
+// only): the device is synchronised before the free, because a call on any stream may still read the old buffer.
+template <typename T>
+int grow(Handle* h, T*& buf, size_t& cap, size_t count) {
+  if (cap >= count) return ARTP_OK;
+  CU_TRY(h, cudaDeviceSynchronize());
+  cudaFree(buf);
+  buf = nullptr;
+  cap = 0;
+  CU_TRY(h, cudaMalloc(&buf, count * sizeof(T)));
+  cap = count;
+  return ARTP_OK;
+}
+
+// Scratch regions: grows `buf` (contents not kept) to hold region[i] = bytes[i] bytes, each at a 256-byte boundary.
+inline int carve(Handle* h, char*& buf, size_t& cap, std::initializer_list<size_t> bytes, char** region) {
+  size_t end = 0;
+  for (size_t b : bytes) end = ((end + 255) & ~(size_t)255) + b;
+  TRY(grow(h, buf, cap, end));
+  end = 0;
+  for (size_t b : bytes) {
+    end = (end + 255) & ~(size_t)255;
+    *region++ = buf + end;
+    end += b;
+  }
+  return ARTP_OK;
+}
+
+// Scratch-group ordering across streams (see Handle::chain_ev): a call on stream s that uses group g waits for the
+// group's previous user, and records itself as the next one when it ends.
+inline int chain_begin(Handle* h, int g, cudaStream_t s) {
+  if (h->chain_busy[g] && h->chain_stream[g] != s) CU_TRY(h, cudaStreamWaitEvent(s, h->chain_ev[g], 0));
+  return ARTP_OK;
+}
+inline int chain_end(Handle* h, int g, cudaStream_t s) {
+  CU_TRY(h, cudaEventRecord(h->chain_ev[g], s));
+  h->chain_stream[g] = s;
+  h->chain_busy[g] = true;
+  return ARTP_OK;
+}
+struct ChainScope {   // begin on construction, end on destruction (every return path)
+  Handle* h; int g; cudaStream_t s; int rc;
+  ChainScope(Handle* h_, int g_, cudaStream_t s_) : h(h_), g(g_), s(s_), rc(chain_begin(h_, g_, s_)) {}
+  ~ChainScope() { if (rc == ARTP_OK) chain_end(h, g, s); }
+};
+
+// Sticky plane-grouping overflow (set by the device, see Handle::h_err): read and clear.
+int take_sticky_error(Handle* h);
+
+// Host-buffer calls run on h->stream as users of scratch group 0. host_call_begin waits for the group's previous user and
+// hands out region[i] = bytes[i] bytes of d_stage (carve). host_call_end waits for the call's work, after which the group
+// is idle. For a call that ran the validity pipeline (`pipeline`) it then returns the sticky device error (Handle::h_err)
+// of the call; the verdicts are complete (fail closed) then, so only ARTP_E_CUDA from host_call_end means the call's
+// outputs are not there.
+inline int host_call_begin(Handle* h, std::initializer_list<size_t> bytes = {}, char** region = nullptr) {
+  CU_TRY(h, cudaSetDevice(h->device));
+  TRY(chain_begin(h, 0, h->stream));
+  return carve(h, h->d_stage, h->stage_cap, bytes, region);
+}
+inline int host_call_end(Handle* h, bool pipeline = false) {
+  CU_TRY(h, cudaStreamSynchronize(h->stream));
+  h->chain_busy[0] = false;
+  return pipeline ? take_sticky_error(h) : ARTP_OK;
+}
+
+// artp_capi.cu, for the sampler and the start / goal search:
+// The validity pipeline over n float states on the device (Pose3FromSE3's cast already applied) into d_valid, on s.
+int check_states_f32(Handle* h, const float* d_states, size_t n, uint8_t* d_valid, cudaStream_t s);
+// Ordered compaction of the n flags d_valid (bit-packed with `bits`) into the indices base + i of the set ones and their
+// count, int64_t indices or, with `u32`, uint32_t ones. Uses scratch group 1.
+int compact_valid(Handle* h, const uint8_t* d_valid, size_t n, int64_t base, void* d_indices, uint32_t* d_count, cudaStream_t s,
+                  bool bits = false, bool u32 = false);
+
+}  // namespace artp_api

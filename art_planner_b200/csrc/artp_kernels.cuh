@@ -40,14 +40,14 @@ struct WarpScratch {
 // Work description shared by K1/K2. EDGE mode: item w -> edge e = w / (steps+1), j = w % (steps+1);
 // j == 0 checks s2, j >= 1 checks interp(s1, s2, j/(steps+1)) (OMPL SE3 interpolation, SURVEY 8a-a14).
 struct Work {
-  const double* s1;     // EDGE: start states; POSE: unused
-  const double* s2;     // EDGE: end states;   POSE: the states
-  const float* s2f;     // POSE only: states already cast to float (exactly what Pose3FromSE3 does first); else null
-  uint8_t* valid;       // per pose / per edge
-  uint32_t item_base;   // first work item of this launch (chunked calls)
-  uint32_t n_items;     // one past the last work item of this launch
-  int steps;            // EDGE: interior steps; POSE: 0
-  int edge_mode;
+  const double* s1 = nullptr;    // EDGE: start states; POSE: unused
+  const double* s2 = nullptr;    // EDGE: end states;   POSE: the states
+  const float* s2f = nullptr;    // POSE only: states already cast to float (exactly what Pose3FromSE3 does first); else null
+  uint8_t* valid = nullptr;      // per pose / per edge
+  uint32_t item_base = 0;        // first work item of this launch (chunked calls)
+  uint32_t n_items = 0;          // one past the last work item of this launch
+  int steps = 0;                 // EDGE: interior steps; POSE: 0
+  int edge_mode = 0;
   // INTERIOR mode (edge_mode == 0, item_off != null): item i is interior state j = i - item_off[e] + 1 of edge e at
   // t = j * (1.0 / (n_e + 1)), n_e = item_off[e+1] - item_off[e]  (prm_motion_cost.cpp:345-353); valid[] is per item.
   const uint32_t* item_off = nullptr;   // n_edges + 1 exclusive prefix sums of the per-edge interior-state counts
@@ -74,26 +74,6 @@ __device__ __forceinline__ uint32_t magic_for(int n) {
 
 constexpr float kKeyScale = 16384.0f;   // bucket width 2^-14 on n0, n2 in [-1, 1]
 constexpr float kKeyMargin = 4e-6f;     // > eps + rsqrt.approx error + quantisation error (see DESIGN.md)
-
-// OMPL 1.4.2 SE3StateSpace::interpolate (RealVector lerp + SO3 slerp), double.
-__device__ __forceinline__ void se3_interpolate(const double* a, const double* b, double t, double* out) {
-  for (int i = 0; i < 3; ++i) out[i] = a[i] + (b[i] - a[i]) * t;
-  const double dq = a[3] * b[3] + a[4] * b[4] + a[5] * b[5] + a[6] * b[6];
-  const double dqa = fabs(dq);
-  const double theta = (dqa > 1.0 - 1e-9) ? 0.0 : acos(dqa);
-  if (theta > 2.220446049250313e-16) {
-    const double d = 1.0 / sin(theta);
-    const double s0 = sin((1.0 - t) * theta);
-    double s1 = sin(t * theta);
-    if (dq < 0) s1 = -s1;
-    out[3] = (a[3] * s0 + b[3] * s1) * d;
-    out[4] = (a[4] * s0 + b[4] * s1) * d;
-    out[5] = (a[5] * s0 + b[5] * s1) * d;
-    out[6] = (a[6] * s0 + b[6] * s1) * d;
-  } else {
-    out[3] = a[3]; out[4] = a[4]; out[5] = a[5]; out[6] = a[6];
-  }
-}
 
 __device__ __forceinline__ void load_item_state(const Work& w, uint32_t item, double s[7]) {
   if (w.item_off) {

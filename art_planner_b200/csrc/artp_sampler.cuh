@@ -13,24 +13,9 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
-namespace artp {
+#include "artp_device.cuh"
 
-struct SamplerDev {
-  const float* elevation_rev;   // Field::H of the elevation layer: H[x + z*pitch] = layer(x, cols-1-z)
-  int pitch;
-  const float* normal_x;        // grid_map layout: (row, col) at row + col*rows
-  const float* normal_y;
-  const float* normal_z;
-  const float* std_dev;
-  const float* cum_prob;        // may be null (uniform mode)
-  const float* cum_row;         // rows floats
-  int rows, cols;
-  double res, cx, cy;
-  double max_roll_pert, max_pitch_pert;
-  int from_distribution;
-  double low[2], high[2];
-  double reach_z;
-};
+namespace artp {
 
 // ---- Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC'11) -------------------------
 __host__ __device__ __forceinline__ void philox4x32_10(uint32_t c[4], uint32_t k0, uint32_t k1) {
@@ -173,7 +158,7 @@ __device__ __forceinline__ bool pose_from_2d(const SamplerDev& m, const double i
   if (!map_cell(m, in[0], in[1], row, col)) return false;
   const size_t at = (size_t)row + (size_t)col * m.rows;
   const double nw[3] = {(double)__ldg(m.normal_x + at), (double)__ldg(m.normal_y + at), (double)__ldg(m.normal_z + at)};
-  const double yaw = (double)(float)atan2(2 * (in[6] * in[5] + in[3] * in[4]), 1 - 2 * (in[4] * in[4] + in[5] * in[5]));
+  const double yaw = (double)so3_yaw(in);
   double nb[3];
   normal_in_yaw_frame(yaw, nw, nb);
   out[2] = cell_height(m, row, col);

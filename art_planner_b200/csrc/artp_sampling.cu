@@ -1,0 +1,670 @@
+// art_planner_b200/csrc/artp_sampling.cu -- the sampling half of the C ABI (include/artp.h): normals and the CDF, the
+// sampler (SE3FromSE2Sampler::sampleUniform) with its fused sample -> check -> compact path, the start / goal search,
+// poseFrom2D, Basic's masking and the sampler's distribution. It reaches the validity pipeline through check_states_f32
+// (artp_internal.h).
+#include <cmath>
+#include <cstdlib>
+#include <cstring>
+#include <vector>
+
+#include "artp_internal.h"
+#include "artp_sampler.cuh"
+#include "artp_basic.cuh"
+#include "artp_distribution.cuh"
+
+using namespace artp_api;
+
+namespace {
+
+// ---------------------------------------------------------------------------------------------------------------
+// Sampler: SE3FromSE2Sampler::sampleUniform on the device (artp_sampler.cuh)
+// ---------------------------------------------------------------------------------------------------------------
+int ensure_sampler_layers(Handle* h) {
+  const size_t need = 5 * (size_t)h->rows * h->cols + (size_t)h->rows + 64;
+  if (h->samp_layers_cap < need) {   // the layers computed on the device go with the old buffer
+    h->map.has_device_normals = false;
+    h->map.has_device_cdf = false;
+    h->map.has_normals = false;
+  }
+  return grow(h, h->d_samp_layers, h->samp_layers_cap, need);
+}
+
+// The map fields of the sampler's view (geometry, elevation, normal and plane-fit layers of d_samp_layers).
+void sampler_map_view(Handle* h, artp::SamplerDev& m) {
+  const size_t ncell = (size_t)h->rows * h->cols;
+  float* base = h->d_samp_layers;
+  m.elevation_rev = h->d_H[0]; m.pitch = h->pitch;
+  m.normal_x = base; m.normal_y = base + ncell; m.normal_z = base + 2 * ncell; m.std_dev = base + 3 * ncell;
+  m.rows = h->rows; m.cols = h->cols;
+  m.res = h->chk.Lx / h->rows; m.cx = h->chk.cx; m.cy = h->chk.cy;
+}
+
+// computeCumulativeProbabilityDistribution of a device-resident probability layer into cum_prob / cum_row of
+// d_samp_layers (ensure_sampler_layers first). Two launches on s.
+int launch_sample_cdf(Handle* h, const float* d_prob, cudaStream_t s) {
+  const size_t ncell = (size_t)h->rows * h->cols;
+  float* d_cum = h->d_samp_layers + 4 * ncell;
+  float* d_row = h->d_samp_layers + 5 * ncell;
+  TRY(launch(h, artp::cdf_rows_kernel, (h->rows + 63) / 64, 64, 0, s, d_prob, h->rows, h->cols, d_cum, d_row));
+  return launch(h, artp::cdf_rowwise_kernel, 1, 32, 0, s, d_row, h->rows);
+}
+
+int sampler_ready(Handle* h) {
+  TRY(require_map(h));
+  if (!h->map.has_sampler) { h->err = "no sampler layers set (artp_set_sampler after artp_set_map)"; return ARTP_E_NOMAP; }
+  return ARTP_OK;
+}
+
+// running total += chunk count (device-side, stream ordered)
+__global__ void add_count_kernel(uint32_t* total, const uint32_t* chunk) { *total += *chunk; }
+
+// out + 7 * (*total) .. : ordered gather of this chunk's valid candidates behind the previous chunks'
+__global__ void gather_chunk_kernel(const double* __restrict__ states, const int64_t* __restrict__ idx,
+                                    const uint32_t* __restrict__ chunk_count, const uint32_t* __restrict__ total_before,
+                                    size_t capacity, double* __restrict__ out) {
+  const size_t before = *total_before;
+  const size_t room = capacity > before ? capacity - before : 0;
+  const size_t cc = *chunk_count;
+  const size_t keep = cc < room ? cc : room;
+  const size_t n = keep * 7;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t k = i / 7, c = i - k * 7;
+    out[before * 7 + i] = states[(size_t)idx[k] * 7 + c];
+  }
+}
+
+constexpr size_t kSampleChunk = (size_t)1 << 21;
+
+// Sample -> check -> compact on s, in chunks of kSampleChunk draws: the valid states of draws first_sample ..
+// first_sample + n_draw - 1 in draw order into d_states_out (at most `capacity` of them), their number into *d_count.
+int sample_valid(Handle* h, uint64_t seed, uint64_t first_sample, size_t n_draw, double* d_states_out, size_t capacity,
+                 uint32_t* d_count, cudaStream_t s) {
+  CU_TRY(h, cudaMemsetAsync(d_count, 0, sizeof(uint32_t), s));
+  if (n_draw == 0) return ARTP_OK;
+  const size_t chunk = std::min(n_draw, kSampleChunk);
+  char* r[5];   // states f64 | states f32 | indices | valid | chunk count
+  TRY(carve(h, h->d_samp_scratch, h->samp_scratch_cap,
+             {chunk * 7 * sizeof(double), chunk * 7 * sizeof(float), chunk * sizeof(int64_t), chunk, sizeof(uint32_t)}, r));
+  double* d_st = (double*)r[0];
+  float* d_sf = (float*)r[1];
+  int64_t* d_idx = (int64_t*)r[2];
+  uint8_t* d_val = (uint8_t*)r[3];
+  uint32_t* d_cnt = (uint32_t*)r[4];
+  for (size_t done = 0; done < n_draw; done += chunk) {
+    const size_t m = std::min(chunk, n_draw - done);
+    TRY(launch(h, artp::sample_states_kernel, grid_for(h, m, 128), 128, 0, s, h->samp, nullptr, seed, first_sample + done, m,
+        d_st, d_sf, nullptr));
+    TRY(check_states_f32(h, d_sf, m, d_val, s));
+    // rejected (outside-map) candidates carry NaN states
+    if (!h->samp.from_distribution) TRY(launch(h, artp::reject_nan_kernel, grid_for(h, m, 256), 256, 0, s, d_st, m, d_val));
+    TRY(compact_valid(h, d_val, m, 0, d_idx, d_cnt, s));
+    TRY(launch(h, gather_chunk_kernel, grid_for(h, m * 7, 256), 256, 0, s, d_st, d_idx, d_cnt, d_count, capacity,
+        d_states_out));
+    TRY(launch(h, add_count_kernel, 1, 1, 0, s, d_count, d_cnt));
+  }
+  return ARTP_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Start / goal repair: StartState / GoalStateRegion::sampleGoal (start.cpp:7-41, goal.cpp:11-41), and the goal's
+// projection onto the map (planner.cpp:223-237, map.cpp:77-90)
+// ---------------------------------------------------------------------------------------------------------------
+// Argument checks shared by both forms; `radius` only when it is a host buffer.
+int ball_search_args(Handle* h, size_t n, uint32_t n_iter, const double* radius) {
+  TRY(require_map(h));
+  if ((uint64_t)n >= (1ull << 32) || n * ((uint64_t)n_iter + 1) >= (1ull << 32)) {
+    h->err = "n * (n_iter + 1) candidates must be < 2^32"; return ARTP_E_INVALID;
+  }
+  if (radius)
+    for (size_t q = 0; q < n; ++q)
+      if (!(radius[q] >= 0.0 && std::isfinite(radius[q]))) { h->err = "radius must be finite and >= 0"; return ARTP_E_INVALID; }
+  return ARTP_OK;
+}
+
+// The search of n > 0 queries on s, in chunks of kSampleChunk candidates; arguments checked by ball_search_args.
+int find_valid_near(Handle* h, const double* d_centres, size_t n, const double* d_radius, uint32_t n_iter, const double* d_offsets,
+                    uint64_t seed, uint64_t first_draw, double* d_states_out, int32_t* d_index, cudaStream_t s) {
+  const uint64_t total = n * ((uint64_t)n_iter + 1);
+  const size_t chunk = (size_t)std::min<uint64_t>(total, kSampleChunk);
+  char* r[3];   // candidate states f32 | verdicts | first valid candidate per query
+  TRY(carve(h, h->d_samp_scratch, h->samp_scratch_cap, {chunk * 7 * sizeof(float), chunk, n * sizeof(uint32_t)}, r));
+  float* d_sf = (float*)r[0];
+  uint8_t* d_val = (uint8_t*)r[1];
+  uint32_t* d_best = (uint32_t*)r[2];
+  artp::BallSearch b{d_centres, d_radius, d_offsets, seed, first_draw, n_iter};
+  CU_TRY(h, cudaMemsetAsync(d_best, 0xFF, n * sizeof(uint32_t), s));
+  for (uint64_t c0 = 0; c0 < total; c0 += chunk) {
+    const size_t m = (size_t)std::min<uint64_t>(chunk, total - c0);
+    TRY(launch(h, artp::ball_candidates_kernel, grid_for(h, m, 128), 128, 0, s, b, c0, m, d_sf));
+    TRY(check_states_f32(h, d_sf, m, d_val, s));
+    TRY(launch(h, artp::ball_first_valid_kernel, grid_for(h, m, 256), 256, 0, s, d_val, c0, m, n_iter, d_best));
+  }
+  return launch(h, artp::ball_result_kernel, grid_for(h, n, 128), 128, 0, s, b, n, d_best, d_states_out, d_index);
+}
+
+// cv::circle(kernel, (r, r), r, 255, FILLED) on a size x size zero image, r = size / 2 (utils.cpp:106-111): OpenCV's
+// integer midpoint circle (imgproc/src/drawing.cpp, Circle()): for every step (dx, dy) of the octant walk the rows
+// cy -+ dy get the span cx -+ dx and the rows cy -+ dx the span cx -+ dy, everything clipped to the image.
+artp::MorphKernel make_circular_kernel(int size) {
+  artp::MorphKernel k;
+  std::memset(&k, 0, sizeof(k));
+  if (size <= 0) {   // empty element: cv::erode / cv::dilate fall back to the 3 x 3 box, anchor (1, 1)
+    k.size = 3; k.anchor = 1;
+    for (int r = 0; r < 3; ++r) { k.lo[r] = 0; k.hi[r] = 2; }
+    return k;
+  }
+  k.size = size; k.anchor = size / 2;
+  for (int r = 0; r < size; ++r) { k.lo[r] = 127; k.hi[r] = -1; }
+  const int radius = size / 2, cx = radius, cy = radius;
+  auto span = [&](int y, int x0, int x1) {
+    if (y < 0 || y >= size) return;
+    x0 = std::max(x0, 0); x1 = std::min(x1, size - 1);
+    if (x0 > x1) return;
+    k.lo[y] = (int8_t)std::min<int>(k.lo[y], x0); k.hi[y] = (int8_t)std::max<int>(k.hi[y], x1);
+  };
+  int err = 0, dx = radius, dy = 0, plus = 1, minus = (radius << 1) - 1;
+  while (dx >= dy) {
+    span(cy - dy, cx - dx, cx + dx); span(cy + dy, cx - dx, cx + dx);
+    span(cy - dx, cx - dy, cx + dy); span(cy + dx, cx - dy, cx + dy);
+    dy++; err += plus; plus += 2;
+    const int mask = (err <= 0) - 1;
+    err -= minus & mask; dx += mask; minus -= mask & 2;
+  }
+  return k;
+}
+
+// cv::dilate / cv::erode of a rows x cols layer with getCircularKernel(size), one launch on s.
+int launch_morph(Handle* h, bool dilate, const float* src, float* dst, int rows, int cols, int size, unsigned grid, cudaStream_t s) {
+  const artp::MorphKernel k = make_circular_kernel(size);
+  if (dilate) return launch(h, artp::morph_kernel<true>, grid, 256, 0, s, src, dst, rows, cols, k);
+  return launch(h, artp::morph_kernel<false>, grid, 256, 0, s, src, dst, rows, cols, k);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// The sampler's distribution (artp_distribution.cuh): Basic::setTraversabilityFilter, then computeInverseSampleDensity ->
+// applyBaseSampleDistribution -> applyMaxUnknownProbability -> computeCumulativeProbabilityDistribution
+// (planner.cpp:39-58), the chain sampleGraph re-applies every recompute_density_after_n_samples vertices.
+// ---------------------------------------------------------------------------------------------------------------
+// getGaussianKernel(ksize, sigma, CV_32F) for sigma > 0: exp(-x^2 / (2 sigma^2)) at x = i - (ksize - 1) / 2, normalised
+// by the double sum, then cast to float -- equal to OpenCV's coefficients (tests/test_sample_distribution_cpu.py).
+artp::GaussTaps gauss_taps(int ksize, double sigma) {
+  artp::GaussTaps k;
+  std::memset(&k, 0, sizeof(k));
+  std::vector<double> v(ksize);
+  const double scale2X = -0.5 / (sigma * sigma);
+  double sum = 0.0;
+  for (int i = 0; i < ksize; ++i) {
+    const double x = i - (ksize - 1) * 0.5;
+    v[i] = std::exp(scale2X * (x * x));
+    sum += v[i];
+  }
+  const double inv = 1.0 / sum;
+  k.half = ksize / 2;
+  for (int t = 0; t <= k.half; ++t) k.w[t] = (float)(v[k.half + t] * inv);
+  return k;
+}
+
+// Argument checks shared by both forms; the blur's kernel size and sigma in cells (sample_density.cpp:33-35).
+int distribution_args(Handle* h, const artp_sample_distribution_params* dp, int* ksize, double* sigma) {
+  TRY(require_whole_map(h));
+  if (!dp) { h->err = "null distribution params"; return ARTP_E_INVALID; }
+  *ksize = 0; *sigma = 0.0;
+  if (dp->use_inverse_vertex_density) {
+    if (!(dp->density_blur_radius > 0.0 && std::isfinite(dp->density_blur_radius))) {
+      h->err = "density_blur_radius must be finite and > 0"; return ARTP_E_INVALID;
+    }
+    const double cells = 6 * dp->density_blur_radius / h->res;
+    if (!(cells < artp::kMaxGaussTaps + 1)) { h->err = "Gaussian kernel larger than 1023 cells"; return ARTP_E_LIMIT; }
+    int k = (int)cells;
+    if (k % 2 == 0) k += 1;
+    if (k > artp::kMaxGaussTaps) { h->err = "Gaussian kernel larger than 1023 cells"; return ARTP_E_LIMIT; }
+    *ksize = k;
+    *sigma = dp->density_blur_radius / h->res;
+  }
+  if (dp->use_max_prob_unknown_samples) {
+    if (!(dp->max_prob_unknown_samples >= 0.0 && dp->max_prob_unknown_samples <= 1.0)) {
+      h->err = "max_prob_unknown_samples must lie in [0, 1]"; return ARTP_E_INVALID;
+    }
+    if (!h->map.has_dist_observed) {
+      h->err = "the unknown-space cap needs the observed layer (artp_set_sample_filter after artp_set_map)"; return ARTP_E_INVALID;
+    }
+  }
+  return ARTP_OK;
+}
+
+// The chain on s into sample_probability (*d_prob, in d_dist_scratch) and the sampler's CDF layers; arguments checked by
+// distribution_args.
+int update_distribution(Handle* h, const artp_sample_distribution_params* dp, int ksize, double sigma, const double* d_states,
+                        size_t n, cudaStream_t s, float** d_prob) {
+  TRY(ensure_sampler_layers(h));
+  const int rows = h->rows, cols = h->cols;
+  const size_t ncell = (size_t)rows * cols, lb = ncell * sizeof(float), rb = (size_t)rows * sizeof(double);
+  char* r[7];   // n_samples | blur pass | sample_probability | known row sums | unknown row sums | max bits | cap multipliers
+  TRY(carve(h, h->d_dist_scratch, h->dist_scratch_cap, {lb, lb, lb, rb, rb, sizeof(unsigned int), 2 * sizeof(float)}, r));
+  float *n_samples = (float*)r[0], *pass = (float*)r[1], *prob = (float*)r[2], *mult = (float*)r[6];
+  double *known = (double*)r[3], *unknown = (double*)r[4];
+  unsigned int* max_bits = (unsigned int*)r[5];
+  const unsigned grid = grid_for(h, ncell, 256);
+  const float* n_blur = nullptr;
+  if (dp->use_inverse_vertex_density) {                                          // sample_density.cpp:21-42
+    CU_TRY(h, cudaMemsetAsync(n_samples, 0, ncell * sizeof(float), s));
+    CU_TRY(h, cudaMemsetAsync(max_bits, 0, sizeof(unsigned int), s));
+    if (n) {
+      artp::SamplerDev m{};
+      sampler_map_view(h, m);
+      TRY(launch(h, artp::vertex_histogram_kernel, grid_for(h, n, 256), 256, 0, s, m, d_states, n, n_samples));
+    }
+    const artp::GaussTaps k = gauss_taps(ksize, sigma);
+    TRY(launch(h, artp::gauss_pass_kernel<0>, grid, 256, 0, s, n_samples, pass, rows, cols, k));
+    TRY(launch(h, artp::gauss_pass_kernel<1>, grid, 256, 0, s, pass, n_samples, rows, cols, k));
+    TRY(launch(h, artp::abs_max_kernel, grid, 256, 0, s, n_samples, ncell, max_bits));
+    n_blur = n_samples;
+  }
+  TRY(launch(h, artp::combine_kernel, grid, 256, 0, s, n_blur, max_bits, h->map.has_sample_filter ? h->d_dist_layers : nullptr,
+      ncell, prob));
+  if (dp->use_max_prob_unknown_samples) {                                        // probability_distribution.cpp:50-91
+    const float* obs = h->d_dist_layers + ncell;
+    TRY(launch(h, artp::cap_rows_kernel, (rows + 63) / 64, 64, 0, s, prob, obs, rows, cols, known, unknown));
+    TRY(launch(h, artp::cap_mult_kernel, 1, 32, 0, s, known, unknown, rows, dp->max_prob_unknown_samples, mult));
+    TRY(launch(h, artp::cap_apply_kernel, grid, 256, 0, s, prob, obs, mult, ncell));
+  }
+  TRY(launch_sample_cdf(h, prob, s));
+  h->map.has_device_cdf = true;
+  h->map.has_sampler = false;      // the sampler must be (re)armed with artp_set_sampler
+  *d_prob = prob;
+  return ARTP_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int artp_estimate_normals(artp_handle* hh, double estimation_radius, float* normal_x, float* normal_y, float* normal_z,
+                          float* plane_fit_std_dev) {
+  LOCK_CALL(h, hh);
+  TRY(require_whole_map(h));
+  if (!(estimation_radius >= 0.0)) { h->err = "estimation_radius < 0"; return ARTP_E_INVALID; }
+  TRY(host_call_begin(h));
+  TRY(ensure_sampler_layers(h));
+  const size_t ncell = (size_t)h->rows * h->cols;
+  const double res = h->chk.Lx / h->rows;
+  float* base = h->d_samp_layers;
+  const int r_cells = (int)(estimation_radius / res), r_diag = (int)(estimation_radius * 0.70710678118 / res);   // utils.cpp:226-227
+  TRY(launch(h, artp::estimate_normals_kernel, grid_for(h, ncell, 128, 32), 128, 0, h->stream, h->d_H[0], h->pitch, h->rows,
+      h->cols, res, h->chk.cx, h->chk.cy, r_cells, r_diag, base, base + ncell, base + 2 * ncell, base + 3 * ncell));
+  float* dst[4] = {normal_x, normal_y, normal_z, plane_fit_std_dev};
+  for (int k = 0; k < 4; ++k)
+    if (dst[k]) CU_TRY(h, cudaMemcpyAsync(dst[k], base + k * ncell, ncell * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  TRY(host_call_end(h));
+  h->map.has_device_normals = true;
+  h->map.has_normals = true;
+  h->map.has_sampler = false;      // the sampler must be (re)armed with artp_set_sampler
+  return ARTP_OK;
+}
+
+int artp_compute_sample_cdf(artp_handle* hh, const float* sample_probability, float* cum_prob, float* cum_prob_rowwise) {
+  LOCK_CALL(h, hh);
+  TRY(require_whole_map(h));
+  if (!sample_probability) return null_buffer(h);
+  const size_t ncell = (size_t)h->rows * h->cols;
+  char* d_prob;
+  TRY(host_call_begin(h, {ncell * sizeof(float)}, &d_prob));
+  TRY(ensure_sampler_layers(h));
+  float* d_cum = h->d_samp_layers + 4 * ncell;
+  float* d_row = h->d_samp_layers + 5 * ncell;
+  CU_TRY(h, cudaMemcpyAsync(d_prob, sample_probability, ncell * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  TRY(launch_sample_cdf(h, (const float*)d_prob, h->stream));
+  if (cum_prob) CU_TRY(h, cudaMemcpyAsync(cum_prob, d_cum, ncell * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  if (cum_prob_rowwise)
+    CU_TRY(h, cudaMemcpyAsync(cum_prob_rowwise, d_row, (size_t)h->rows * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  TRY(host_call_end(h));
+  h->map.has_device_cdf = true;
+  h->map.has_sampler = false;      // the sampler must be (re)armed with artp_set_sampler
+  return ARTP_OK;
+}
+
+int artp_set_sampler(artp_handle* hh, const artp_sampler_params* sp, const float* normal_x, const float* normal_y,
+                     const float* normal_z, const float* plane_fit_std_dev, const float* cum_prob,
+                     const float* cum_prob_rowwise) {
+  LOCK_CALL(h, hh);
+  TRY(require_whole_map(h));
+  const bool host_normals = normal_x && normal_y && normal_z && plane_fit_std_dev;
+  if (!sp) { h->err = "null sampler params"; return ARTP_E_INVALID; }
+  if (!host_normals && (normal_x || normal_y || normal_z || plane_fit_std_dev)) {
+    h->err = "pass all four normal / plane-fit layers or none"; return ARTP_E_INVALID;
+  }
+  if (!host_normals && !h->map.has_device_normals) {
+    h->err = "no normal layers: pass them or call artp_estimate_normals after artp_set_map"; return ARTP_E_INVALID;
+  }
+  const bool host_cdf = cum_prob && cum_prob_rowwise;
+  if (sp->sample_from_distribution && !host_cdf && !(h->map.has_device_cdf && !cum_prob && !cum_prob_rowwise)) {
+    h->err = "sample_from_distribution needs the cum_prob layers (pass both, or call artp_compute_sample_cdf first)";
+    return ARTP_E_INVALID;
+  }
+  if (!sp->sample_from_distribution && !(sp->high[0] > sp->low[0] && sp->high[1] > sp->low[1])) {
+    h->err = "empty sampling bounds"; return ARTP_E_INVALID;
+  }
+  const size_t ncell = (size_t)h->rows * h->cols;
+  TRY(host_call_begin(h));
+  TRY(ensure_sampler_layers(h));
+  float* base = h->d_samp_layers;
+  if (host_normals) {
+    const float* src[4] = {normal_x, normal_y, normal_z, plane_fit_std_dev};
+    for (int k = 0; k < 4; ++k)
+      CU_TRY(h, cudaMemcpyAsync(base + k * ncell, src[k], ncell * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+    h->map.has_device_normals = false;   // overwritten by the caller's layers
+    h->map.has_normals = true;
+  }
+  artp::SamplerDev& m = h->samp;
+  sampler_map_view(h, m);
+  m.cum_prob = nullptr; m.cum_row = nullptr;
+  m.max_roll_pert = sp->max_roll_pert; m.max_pitch_pert = sp->max_pitch_pert;
+  m.from_distribution = sp->sample_from_distribution ? 1 : 0;
+  m.low[0] = sp->low[0]; m.low[1] = sp->low[1]; m.high[0] = sp->high[0]; m.high[1] = sp->high[1];
+  m.reach_z = h->p.reach_z;
+  uint32_t bad = 0;
+  if (m.from_distribution) {
+    if (host_cdf) {
+      CU_TRY(h, cudaMemcpyAsync(base + 4 * ncell, cum_prob, ncell * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+      CU_TRY(h, cudaMemcpyAsync(base + 5 * ncell, cum_prob_rowwise, (size_t)h->rows * sizeof(float), cudaMemcpyHostToDevice,
+                                h->stream));
+      h->map.has_device_cdf = false;   // overwritten by the caller's layers
+    }
+    m.cum_prob = base + 4 * ncell; m.cum_row = base + 5 * ncell;
+    // the binary searches need monotone (or all-NaN) CDF rows: refuse anything else
+    uint32_t* d_bad = &h->d_ctr->scratch;
+    CU_TRY(h, cudaMemsetAsync(d_bad, 0, sizeof(uint32_t), h->stream));
+    TRY(launch(h, artp::validate_cdf_kernel, (h->rows + 127) / 128, 128, 0, h->stream, m.cum_prob, h->rows, h->cols,
+        (size_t)h->rows, 1, d_bad));
+    TRY(launch(h, artp::validate_cdf_kernel, 1, 32, 0, h->stream, m.cum_row, 1, h->rows, 1, 0, d_bad));
+    CU_TRY(h, cudaMemcpyAsync(&bad, d_bad, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+  }
+  TRY(host_call_end(h));
+  if (bad) { h->err = "cum_prob layers are not cumulative distributions (rows must be non-decreasing or all NaN)"; return ARTP_E_INVALID; }
+  h->map.has_sampler = true;
+  return ARTP_OK;
+}
+
+int artp_sampler_uniforms(artp_handle* hh, uint64_t seed, uint64_t first_sample, size_t n, double* u) {
+  LOCK_CALL(h, hh);
+  if (n == 0) return ARTP_OK;
+  if (!u) return null_buffer(h);
+  char* d_u;
+  TRY(host_call_begin(h, {n * 6 * sizeof(double)}, &d_u));
+  TRY(launch(h, artp::sampler_uniforms_kernel, grid_for(h, n, 256), 256, 0, h->stream, seed, first_sample, n, (double*)d_u));
+  CU_TRY(h, cudaMemcpyAsync(u, d_u, n * 6 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  return host_call_end(h);
+}
+
+int artp_sample_states_device(artp_handle* hh, const double* d_u, uint64_t seed, uint64_t first_sample, size_t n,
+                              double* d_states, int32_t* d_rowcol, void* stream) {
+  LOCK_CALL(h, hh);
+  TRY(sampler_ready(h));
+  if (n == 0) return ARTP_OK;
+  if (!d_states) return null_buffer(h);
+  CU_TRY(h, cudaSetDevice(h->device));
+  return launch(h, artp::sample_states_kernel, grid_for(h, n, 128), 128, 0, (cudaStream_t)stream, h->samp, d_u, seed, first_sample, n,
+                d_states, nullptr, d_rowcol);
+}
+
+int artp_sample_states(artp_handle* hh, const double* u, uint64_t seed, uint64_t first_sample, size_t n, double* states,
+                       int32_t* rowcol) {
+  LOCK_CALL(h, hh);
+  TRY(sampler_ready(h));
+  if (n == 0) return ARTP_OK;
+  if (!states) return null_buffer(h);
+  char* r[3];   // u | states | rowcol
+  TRY(host_call_begin(h, {n * 6 * sizeof(double), n * 7 * sizeof(double), n * 2 * sizeof(int32_t)}, r));
+  if (u) CU_TRY(h, cudaMemcpyAsync(r[0], u, n * 6 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  TRY(launch(h, artp::sample_states_kernel, grid_for(h, n, 128), 128, 0, h->stream, h->samp, u ? (const double*)r[0] : nullptr,
+      seed, first_sample, n, (double*)r[1], nullptr, rowcol ? (int32_t*)r[2] : nullptr));
+  CU_TRY(h, cudaMemcpyAsync(states, r[1], n * 7 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (rowcol) CU_TRY(h, cudaMemcpyAsync(rowcol, r[2], n * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+  return host_call_end(h);
+}
+
+int artp_sample_valid_device(artp_handle* hh, uint64_t seed, uint64_t first_sample, size_t n_draw, double* d_states_out,
+                             size_t capacity, uint32_t* d_count, void* stream) {
+  LOCK_CALL(h, hh);
+  TRY(sampler_ready(h));
+  if (!d_count || (capacity && !d_states_out)) return null_buffer(h);
+  CU_TRY(h, cudaSetDevice(h->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  ChainScope cs(h, 0, s);
+  if (cs.rc) return cs.rc;
+  return sample_valid(h, seed, first_sample, n_draw, d_states_out, capacity, d_count, s);
+}
+
+int artp_sample_valid(artp_handle* hh, uint64_t seed, uint64_t first_sample, size_t n_draw, double* states, size_t capacity,
+                      size_t* n_valid) {
+  LOCK_CALL(h, hh);
+  const size_t cap = std::min(capacity, n_draw);
+  TRY(sampler_ready(h));
+  if (!n_valid || (cap && !states)) return null_buffer(h);
+  char* r[2];   // states | count
+  TRY(host_call_begin(h, {cap * 7 * sizeof(double), sizeof(uint32_t)}, r));
+  TRY(sample_valid(h, seed, first_sample, n_draw, (double*)r[0], cap, (uint32_t*)r[1], h->stream));
+  uint32_t cnt = 0;
+  CU_TRY(h, cudaMemcpyAsync(&cnt, r[1], sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+  const int rc = host_call_end(h, true);
+  if (rc == ARTP_E_CUDA) return rc;
+  const size_t keep = std::min<size_t>(cnt, cap);
+  if (keep) {   // the copy's size is the count: it follows the call's end (d_stage is still ours: the lock is held)
+    CU_TRY(h, cudaMemcpyAsync(states, r[0], keep * 7 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(h, cudaStreamSynchronize(h->stream));
+  }
+  *n_valid = cnt;      // > capacity means the output was truncated to `capacity` states
+  return rc;
+}
+
+int artp_find_valid_near_device(artp_handle* hh, const double* d_centres, size_t n, const double* d_radius, uint32_t n_iter,
+                                const double* d_offsets, uint64_t seed, uint64_t first_draw, double* d_states_out,
+                                int32_t* d_index, void* stream) {
+  LOCK_CALL(h, hh);
+  TRY(ball_search_args(h, n, n_iter, nullptr));
+  if (n == 0) return ARTP_OK;
+  if (!d_centres || !d_radius || !d_states_out || !d_index) return null_buffer(h);
+  CU_TRY(h, cudaSetDevice(h->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  ChainScope cs(h, 0, s);
+  if (cs.rc) return cs.rc;
+  return find_valid_near(h, d_centres, n, d_radius, n_iter, d_offsets, seed, first_draw, d_states_out, d_index, s);
+}
+
+int artp_find_valid_near(artp_handle* hh, const double* centres, size_t n, const double* radius, uint32_t n_iter,
+                         const double* offsets, uint64_t seed, uint64_t first_draw, double* states_out, int32_t* index) {
+  LOCK_CALL(h, hh);
+  if (n && (!centres || !radius || !states_out || !index)) return null_buffer(h);
+  TRY(ball_search_args(h, n, n_iter, radius));
+  if (n == 0) return ARTP_OK;
+  const size_t sb = n * 7 * sizeof(double), ob = offsets ? n * (size_t)n_iter * 2 * sizeof(double) : 0;
+  char* r[5];   // centres | radius | offsets | states | index
+  TRY(host_call_begin(h, {sb, n * sizeof(double), ob, sb, n * sizeof(int32_t)}, r));
+  CU_TRY(h, cudaMemcpyAsync(r[0], centres, sb, cudaMemcpyHostToDevice, h->stream));
+  CU_TRY(h, cudaMemcpyAsync(r[1], radius, n * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  if (ob) CU_TRY(h, cudaMemcpyAsync(r[2], offsets, ob, cudaMemcpyHostToDevice, h->stream));
+  TRY(find_valid_near(h, (const double*)r[0], n, (const double*)r[1], n_iter, offsets ? (const double*)r[2] : nullptr, seed,
+      first_draw, (double*)r[3], (int32_t*)r[4], h->stream));
+  CU_TRY(h, cudaMemcpyAsync(states_out, r[3], sb, cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(h, cudaMemcpyAsync(index, r[4], n * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
+  return host_call_end(h, true);
+}
+
+int artp_ball_offsets(artp_handle* hh, uint64_t seed, uint64_t first_draw, size_t n, uint32_t n_iter, const double* radius,
+                      double* offsets) {
+  LOCK_CALL(h, hh);
+  const size_t total = n * (size_t)n_iter;
+  if (total == 0) return ARTP_OK;
+  if (!radius || !offsets) return null_buffer(h);
+  if ((uint64_t)n >= (1ull << 32)) { h->err = "n must be < 2^32"; return ARTP_E_INVALID; }
+  char* r[2];   // radius | offsets
+  TRY(host_call_begin(h, {n * sizeof(double), total * 2 * sizeof(double)}, r));
+  CU_TRY(h, cudaMemcpyAsync(r[0], radius, n * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  TRY(launch(h, artp::ball_offsets_kernel, grid_for(h, total, 256), 256, 0, h->stream, seed, first_draw, n, n_iter,
+      (const double*)r[0], (double*)r[1]));
+  CU_TRY(h, cudaMemcpyAsync(offsets, r[1], total * 2 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  return host_call_end(h);
+}
+
+int artp_pose_from_2d(artp_handle* hh, const double* states_in, size_t n, double* states_out, uint8_t* inside) {
+  LOCK_CALL(h, hh);
+  TRY(require_whole_map(h));
+  if (!h->map.has_normals) {
+    h->err = "no normal layers for this map (artp_estimate_normals or artp_set_sampler after artp_set_map)"; return ARTP_E_INVALID;
+  }
+  if (n == 0) return ARTP_OK;
+  if (!states_in || !states_out) return null_buffer(h);
+  char* r[3];   // states in | states out | inside
+  TRY(host_call_begin(h, {n * 7 * sizeof(double), n * 7 * sizeof(double), n}, r));
+  artp::SamplerDev m{};
+  sampler_map_view(h, m);
+  CU_TRY(h, cudaMemcpyAsync(r[0], states_in, n * 7 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  TRY(launch(h, artp::pose_from_2d_kernel, grid_for(h, n, 128), 128, 0, h->stream, m, (const double*)r[0], n, (double*)r[1],
+      (uint8_t*)r[2]));
+  CU_TRY(h, cudaMemcpyAsync(states_out, r[1], n * 7 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (inside) CU_TRY(h, cudaMemcpyAsync(inside, r[2], n, cudaMemcpyDeviceToHost, h->stream));
+  return host_call_end(h);
+}
+
+int artp_debug_circular_kernel(int size, uint8_t* out) {   // test hook: the size x size element as 0 / 1 bytes (row-major)
+  if (size > artp::kMaxMorph || !out) return ARTP_E_INVALID;
+  const artp::MorphKernel k = make_circular_kernel(size);
+  for (int r = 0; r < k.size; ++r) for (int c = 0; c < k.size; ++c) out[r * k.size + c] = (c >= k.lo[r] && c <= k.hi[r]) ? 1 : 0;
+  return k.size;
+}
+
+int artp_process_basic(artp_handle* hh, const float* elevation, const float* traversability, const float* observed, int rows,
+                       int cols, double res, const artp_basic_params* bp, float* elevation_masked, float* traversability_thresholded) {
+  LOCK_CALL(h, hh);
+  if (!elevation || !traversability || !bp || !elevation_masked || rows < 1 || cols < 1 || !(res > 0)) {
+    h->err = "bad arguments"; return ARTP_E_INVALID;
+  }
+  if (bp->unknown_space_untraversable && !observed) { h->err = "unknown_space_untraversable needs the observed layer"; return ARTP_E_INVALID; }
+  // basic.cpp:65-74: cell counts of the structuring elements
+  const int foothold = (int)std::ceil(bp->foothold_size / res), margin = (int)std::ceil(2 * bp->foothold_margin / res),
+            hole = (int)std::floor(bp->foothold_margin_max_hole_size / res),
+            search = (int)std::ceil(2 * bp->foothold_margin_max_drop_search_radius / res);
+  if (std::max(std::max(foothold, margin), std::max(hole, search)) > artp::kMaxMorph) {
+    h->err = "structuring element larger than 64 cells"; return ARTP_E_LIMIT;
+  }
+  const size_t n = (size_t)rows * cols, lb = n * sizeof(float);
+  char* stage;
+  TRY(host_call_begin(h, {9 * lb}, &stage));
+  h->has_basic_layers = false;
+  TRY(grow(h, h->d_basic_keep, h->basic_keep_cap, 2 * n));
+  float* L = (float*)stage;   // 0 elev, 1 trav, 2 observed, 3 T0, 4 A, 5 B, 6 elev eroded, 7 elev dilated, 8 out
+  cudaStream_t s = h->stream;
+  CU_TRY(h, cudaMemcpyAsync(L, elevation, lb, cudaMemcpyHostToDevice, s));
+  CU_TRY(h, cudaMemcpyAsync(L + n, traversability, lb, cudaMemcpyHostToDevice, s));
+  if (observed) CU_TRY(h, cudaMemcpyAsync(L + 2 * n, observed, lb, cudaMemcpyHostToDevice, s));
+  const unsigned grid = grid_for(h, n, 256);
+  auto morph = [&](bool dil, const float* src, float* dst, int size) { return launch_morph(h, dil, src, dst, rows, cols, size, grid, s); };
+  float *E = L, *T0 = L + 3 * n, *A = L + 4 * n, *B = L + 5 * n, *Elo = L + 6 * n, *Ehi = L + 7 * n, *O = L + 8 * n;
+  const float drop = (float)bp->foothold_margin_max_drop, step = (float)bp->foothold_margin_min_step;
+  TRY(launch(h, artp::basic_threshold_kernel, grid, 256, 0, s, L + n, L + 2 * n, bp->unknown_space_untraversable ? 1 : 0,
+             bp->traversability_thres, n, T0));
+  TRY(morph(true, T0, A, hole)); TRY(morph(false, A, B, hole));           // dilateAndErode: close holes (:72)
+  TRY(morph(false, E, Elo, search));                                      // elevation - erode(elevation) (:75-77)
+  TRY(morph(true, E, Ehi, margin));                                       // dilate(elevation) - elevation (:84)
+  TRY(launch(h, artp::basic_select_kernel, grid, 256, 0, s, 0, E, Elo, Ehi, T0, B, drop, step, n, A));
+  TRY(morph(false, A, B, margin));                                        // erode by the safety margin (:90)
+  TRY(launch(h, artp::basic_select_kernel, grid, 256, 0, s, 1, E, Elo, Ehi, T0, B, drop, step, n, A));
+  TRY(morph(false, A, B, foothold)); TRY(morph(true, B, A, foothold));    // erodeAndDilate: remove small patches (:95)
+  TRY(launch(h, artp::basic_final_kernel, grid, 256, 0, s, E, T0, A, n, B, O));
+  CU_TRY(h, cudaMemcpyAsync(elevation_masked, O, lb, cudaMemcpyDeviceToHost, s));
+  if (traversability_thresholded) CU_TRY(h, cudaMemcpyAsync(traversability_thresholded, B, lb, cudaMemcpyDeviceToHost, s));
+  // kept for artp_set_sample_filter(h, NULL, NULL, ...)
+  if (observed) CU_TRY(h, cudaMemcpyAsync(h->d_basic_keep, L + 2 * n, lb, cudaMemcpyDeviceToDevice, s));
+  CU_TRY(h, cudaMemcpyAsync(h->d_basic_keep + n, B, lb, cudaMemcpyDeviceToDevice, s));
+  TRY(host_call_end(h));
+  h->basic_rows = rows; h->basic_cols = cols;
+  h->has_basic_layers = true;
+  h->has_basic_observed = observed != nullptr;
+  return ARTP_OK;
+}
+
+int artp_set_sample_filter(artp_handle* hh, const float* traversability_thresholded, const float* observed,
+                           float* traversability_sample_filter) {
+  LOCK_CALL(h, hh);
+  TRY(require_whole_map(h));
+  const int rows = h->rows, cols = h->cols;
+  const bool basic_fits = h->has_basic_layers && h->basic_rows == rows && h->basic_cols == cols;
+  if (!traversability_thresholded && !basic_fits) {
+    h->err = "no traversability_thresholded layer: pass it, or run artp_process_basic on a map of this size first";
+    return ARTP_E_INVALID;
+  }
+  const bool basic_observed = !observed && basic_fits && h->has_basic_observed;
+  // basic.cpp:116-122, with the implicit double -> int conversions of the int size parameters
+  const artp_params& p = h->p;
+  const int reach = (int)(std::sqrt(p.reach_x * p.reach_x + p.reach_y * p.reach_y) / h->res);
+  const int wall = (int)(std::min((p.torso_length - p.reach_x) * 0.5, (p.torso_width - p.reach_y) * 0.5) / h->res);
+  if (std::max(reach, wall) > artp::kMaxMorph) { h->err = "structuring element larger than 64 cells"; return ARTP_E_LIMIT; }
+  const size_t n = (size_t)rows * cols, lb = n * sizeof(float);
+  char* r[3];   // caller's traversability_thresholded | dilated | closed
+  TRY(host_call_begin(h, {lb, lb, lb}, r));
+  h->map.has_sample_filter = h->map.has_dist_observed = false;
+  TRY(grow(h, h->d_dist_layers, h->dist_layers_cap, 2 * n));
+  cudaStream_t s = h->stream;
+  float *filter = h->d_dist_layers, *obs = h->d_dist_layers + n;
+  const float* thr = traversability_thresholded ? (const float*)r[0] : h->d_basic_keep + n;
+  if (traversability_thresholded) CU_TRY(h, cudaMemcpyAsync(r[0], traversability_thresholded, lb, cudaMemcpyHostToDevice, s));
+  if (observed) CU_TRY(h, cudaMemcpyAsync(obs, observed, lb, cudaMemcpyHostToDevice, s));
+  if (basic_observed) CU_TRY(h, cudaMemcpyAsync(obs, h->d_basic_keep, lb, cudaMemcpyDeviceToDevice, s));
+  const unsigned grid = grid_for(h, n, 256);
+  TRY(launch_morph(h, true, thr, (float*)r[1], rows, cols, reach, grid, s));            // dilateAndErode: step over small obstacles
+  TRY(launch_morph(h, false, (float*)r[1], (float*)r[2], rows, cols, reach, grid, s));
+  TRY(launch_morph(h, false, (float*)r[2], filter, rows, cols, wall, grid, s));           // erode: keep away from walls
+  if (traversability_sample_filter)
+    CU_TRY(h, cudaMemcpyAsync(traversability_sample_filter, filter, lb, cudaMemcpyDeviceToHost, s));
+  TRY(host_call_end(h));
+  h->map.has_sample_filter = true;
+  h->map.has_dist_observed = observed || basic_observed;
+  return ARTP_OK;
+}
+
+int artp_debug_gaussian_kernel(int ksize, double sigma, float* out) {   // test hook: the ksize coefficients
+  if (ksize < 1 || ksize > artp::kMaxGaussTaps || !(ksize & 1) || !(sigma > 0) || !out) return ARTP_E_INVALID;
+  const artp::GaussTaps k = gauss_taps(ksize, sigma);
+  for (int i = 0; i < ksize; ++i) out[i] = k.w[std::abs(i - k.half)];
+  return ksize;
+}
+
+int artp_update_sample_distribution_device(artp_handle* hh, const artp_sample_distribution_params* dp,
+                                           const double* d_vertex_states, size_t n, void* stream) {
+  LOCK_CALL(h, hh);
+  int ksize;
+  double sigma;
+  TRY(distribution_args(h, dp, &ksize, &sigma));
+  if (n && !d_vertex_states) return null_buffer(h);
+  CU_TRY(h, cudaSetDevice(h->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  ChainScope cs(h, 0, s);
+  if (cs.rc) return cs.rc;
+  float* d_prob;
+  return update_distribution(h, dp, ksize, sigma, d_vertex_states, n, s, &d_prob);
+}
+
+int artp_update_sample_distribution(artp_handle* hh, const artp_sample_distribution_params* dp, const double* vertex_states,
+                                    size_t n, float* sample_probability, float* cum_prob, float* cum_prob_rowwise) {
+  LOCK_CALL(h, hh);
+  int ksize;
+  double sigma;
+  TRY(distribution_args(h, dp, &ksize, &sigma));
+  if (n && !vertex_states) return null_buffer(h);
+  const size_t sb = n * 7 * sizeof(double), ncell = (size_t)h->rows * h->cols;
+  char* r[1];
+  TRY(host_call_begin(h, {sb}, r));
+  if (n) CU_TRY(h, cudaMemcpyAsync(r[0], vertex_states, sb, cudaMemcpyHostToDevice, h->stream));
+  float* d_prob;
+  TRY(update_distribution(h, dp, ksize, sigma, (const double*)r[0], n, h->stream, &d_prob));
+  if (sample_probability)
+    CU_TRY(h, cudaMemcpyAsync(sample_probability, d_prob, ncell * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  if (cum_prob)
+    CU_TRY(h, cudaMemcpyAsync(cum_prob, h->d_samp_layers + 4 * ncell, ncell * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  if (cum_prob_rowwise)
+    CU_TRY(h, cudaMemcpyAsync(cum_prob_rowwise, h->d_samp_layers + 5 * ncell, (size_t)h->rows * sizeof(float),
+                              cudaMemcpyDeviceToHost, h->stream));
+  return host_call_end(h);
+}
+
+}  // extern "C"

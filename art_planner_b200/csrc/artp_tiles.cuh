@@ -54,12 +54,6 @@ __device__ __forceinline__ void tma_tile_2d(void* dst, const CUtensorMap* map, u
       : "memory");
 }
 
-struct TileCfg {
-  int tw, th;              // tile extent in floats (tw a multiple of 4; a zone may be at most tw - 3 wide, th high)
-  uint32_t bytes, stride;  // tw * th * 4, and that rounded up to 128 bytes
-  int x_off;               // first stored vertex column of the layer (map window), a multiple of 4
-  int slots;               // tile slots per warp: 2 = the next box's tile is prefetched while this one is decided, 1 = none
-};
 constexpr int kMaxTileWarps = 8;
 
 // map0 / map1: tiles of `elevation` / `elevation_masked` (same tile extent). queue_bit tags defer-list entries.

@@ -3,6 +3,7 @@ import ctypes
 import os
 import re
 import shutil
+import subprocess
 
 import pytest
 
@@ -35,6 +36,17 @@ def test_header_declares_the_expected_entry_points():
 def test_library_exports_every_declared_symbol(lib):
     for s in declared_symbols():
         assert hasattr(lib, s), f"libartp.so does not export {s}"
+
+
+def test_library_exports_only_the_declared_functions(lib):
+    """Kernels, C++ helpers and template instantiations stay inside libartp.so: its dynamic symbol table holds exactly
+    the functions include/artp.h declares."""
+    from art_planner_b200 import capi
+    nm = shutil.which("nm")
+    assert nm is not None, "nm (binutils) is needed to read the library's symbol table"
+    out = subprocess.run([nm, "-D", "--defined-only", capi.LIB_PATH], capture_output=True, text=True, check=True).stdout
+    exported = {line.split()[-1] for line in out.splitlines() if line.strip()}
+    assert exported == set(declared_symbols())
 
 
 def test_product_path_fails_loudly_without_gpu(lib):
