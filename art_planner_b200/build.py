@@ -9,12 +9,12 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libartp.so")
 # (source, extra flags): the geometric kernels need bit-exact fp32 (no FMA contraction, SURVEY.md section 7);
 # the motion-cost network does not.
-# The three units of the C ABI all build rows, costs and states that must equal the host's bit for bit.
+# The four units of the C ABI all build rows, costs and states that must equal the host's bit for bit.
 GEOMETRY_FLAGS = ["-fmad=false", "-Xcompiler", "-fPIC,-ffp-contract=off"]
 SOURCES = [("artp_capi.cu", GEOMETRY_FLAGS), ("artp_sampling.cu", GEOMETRY_FLAGS), ("artp_cost.cu", GEOMETRY_FLAGS),
-           ("artp_cnn.cu", ["-Xcompiler", "-fPIC"])]
+           ("artp_roadmap.cu", GEOMETRY_FLAGS), ("artp_cnn.cu", ["-Xcompiler", "-fPIC"])]
 HEADERS = ["artp_internal.h", "artp_device.cuh", "artp_kernels.cuh", "artp_sampler.cuh", "artp_tiles.cuh", "artp_basic.cuh",
-           "artp_distribution.cuh", "artp_cnn.h", "artp.map", os.path.join("..", "..", "include", "artp.h")]
+           "artp_distribution.cuh", "artp_roadmap.cuh", "artp_cnn.h", "artp.map", os.path.join("..", "..", "include", "artp.h")]
 # The library exports the C ABI (artp_*) and nothing else.
 VERSION_SCRIPT = os.path.join(CSRC, "artp.map")
 

@@ -49,6 +49,14 @@ class ArtpSampleDistributionParams(C.Structure):
                 ("use_max_prob_unknown_samples", C.c_int), ("max_prob_unknown_samples", C.c_double)]
 
 
+class ArtpRoadmapParams(C.Structure):
+    _fields_ = [("max_n_vertices", C.c_size_t), ("max_n_edges", C.c_size_t),
+                ("recompute_density_after_n_samples", C.c_size_t), ("max_draws", C.c_uint64)]
+
+
+ARTP_ROADMAP_MILESTONE, ARTP_ROADMAP_INTERPOLATED, ARTP_ROADMAP_QUERY = 1, 2, 4
+
+
 class ArtpStats(C.Structure):
     _fields_ = [("poses_checked", C.c_uint64), ("poses_deferred", C.c_uint64), ("kernel_launches", C.c_uint64),
                 ("last_deferred", C.c_uint32), ("last_launches", C.c_uint32), ("last_queued_boxes", C.c_uint32),
@@ -118,6 +126,11 @@ def load():
     lib.artp_update_sample_distribution.argtypes = [vp, C.POINTER(ArtpSampleDistributionParams), vp, sz, vp, vp, vp]
     lib.artp_update_sample_distribution_device.argtypes = [vp, C.POINTER(ArtpSampleDistributionParams), vp, sz, vp]
     lib.artp_debug_gaussian_kernel.argtypes = [i32, dbl, vp]
+    lib.artp_roadmap_clear.argtypes = [vp, sz, sz]
+    lib.artp_roadmap_add_milestones.argtypes = [vp, vp, sz]
+    lib.artp_roadmap_sample_graph.argtypes = [vp, C.POINTER(ArtpRoadmapParams), C.POINTER(ArtpSampleDistributionParams), u64, u64,
+                                              C.POINTER(u64)]
+    lib.artp_roadmap_get.argtypes = [vp, sz, vp, vp, sz, vp, C.POINTER(sz), C.POINTER(sz)]
     lib.artp_host_alloc.restype = C.c_void_p
     lib.artp_host_alloc.argtypes = [sz]
     lib.artp_host_free.argtypes = [vp]

@@ -470,6 +470,71 @@ class SE3FromSE2Sampler:
                                              C.c_void_p(count.data_ptr()), _stream_ptr()))
 
 
+class PRMRoadmap:
+    """PRMMotionCost's roadmap built on the device (prm_motion_cost.cpp:145-219, 236-247, 325-390): addValidMilestone with
+    KStarStrategy's k nearest, the interior states of every connection at <= 0.5 m lateral spacing, and the valid prefixes
+    as chains of vertices and edges. vertices() / edges() copy the store out in the order the reference's Boost graph
+    numbers them; edges carry no cost (price them with MotionCostObjective.updateEdgesBatch)."""
+
+    MILESTONE, INTERPOLATED, QUERY = capi.ARTP_ROADMAP_MILESTONE, capi.ARTP_ROADMAP_INTERPOLATED, capi.ARTP_ROADMAP_QUERY
+
+    def __init__(self, checker: StateValidityChecker, vertex_capacity: int = 60000, edge_capacity: int = 60000):
+        self._c = checker
+        self.vertex_capacity, self.edge_capacity = int(vertex_capacity), int(edge_capacity)
+        self.clear()
+
+    def clear(self) -> None:                             # PRMMotionCost::clear (:236-247)
+        h = self._c.handle
+        h.check(h.lib.artp_roadmap_clear(h.h, self.vertex_capacity, self.edge_capacity))
+
+    def addValidMilestones(self, states) -> None:
+        """addValidMilestone for each state in order: baseSolve's start / goal milestones (:451-479)."""
+        h = self._c.handle
+        s = np.ascontiguousarray(states, dtype=np.float64).reshape(-1, 7)
+        h.check(h.lib.artp_roadmap_add_milestones(h.h, s.ctypes.data, s.shape[0]))
+
+    def sampleGraph(self, sampler: SE3FromSE2Sampler, max_n_vertices: int = 10000, max_n_edges: int = 50000,
+                    recompute_density_after_n_samples: int = 1000, max_draws: int = 1 << 26, first_sample: int = 0,
+                    distribution: bool = True) -> int:
+        """PRMMotionCostMaintainer::sampleGraph's loop with `sampler`'s Philox stream from first_sample; the distribution is
+        re-applied from `sampler`'s parameters (SE3FromSE2Sampler.updateDistribution) unless distribution=False. A draw
+        budget replaces max_sample_time. Returns the draws used."""
+        h = self._c.handle
+        p = capi.ArtpRoadmapParams(int(max_n_vertices), int(max_n_edges), int(recompute_density_after_n_samples), int(max_draws))
+        dp = None
+        if distribution:
+            sp, rp = sampler._sp, h.params
+            dp = capi.ArtpSampleDistributionParams(int(sp.use_inverse_vertex_density), (rp.torso_length + rp.torso_width) * 0.25,
+                                                   int(sp.use_max_prob_unknown_samples), float(sp.max_prob_unknown_samples))
+        used = C.c_uint64(0)
+        h.check(h.lib.artp_roadmap_sample_graph(h.h, C.byref(p), None if dp is None else C.byref(dp), sampler.seed,
+                                                int(first_sample), C.byref(used)))
+        return used.value
+
+    def counts(self):
+        h = self._c.handle
+        nv, ne = C.c_size_t(0), C.c_size_t(0)
+        h.check(h.lib.artp_roadmap_get(h.h, 0, None, None, 0, None, C.byref(nv), C.byref(ne)))
+        return nv.value, ne.value
+
+    def vertices(self, first: int = 0):
+        """(states [V - first, 7] float64, kinds [V - first] uint8) of the vertices first .. V-1."""
+        h = self._c.handle
+        nv, _ = self.counts()
+        n = max(nv - int(first), 0)
+        states, kinds = np.empty((n, 7), np.float64), np.empty(n, np.uint8)
+        h.check(h.lib.artp_roadmap_get(h.h, int(first), states.ctypes.data, kinds.ctypes.data, 0, None, None, None))
+        return states, kinds
+
+    def edges(self, first: int = 0):
+        """[E - first, 2] uint32 (u, v) of the edges first .. E-1."""
+        h = self._c.handle
+        _, ne = self.counts()
+        e = np.empty((max(ne - int(first), 0), 2), np.uint32)
+        h.check(h.lib.artp_roadmap_get(h.h, 0, None, None, int(first), e.ctypes.data, None, None))
+        return e
+
+
 class StartState:
     """art_planner::StartState (start.h, start.cpp:7-41): the start pose repaired by a disc search around it, one device
     call per sampleGoal. Offsets come from the Philox "ARTB" stream of `seed`; the draw position advances by what the

@@ -644,6 +644,19 @@ int artp_api::check_states_f32(Handle* h, const float* d_states, size_t n, uint8
   return check_states(h, d_states, n, d_valid, s);
 }
 
+int artp_api::check_states_cta(Handle* h, const double* d_states, const uint32_t* d_count, const uint32_t* d_stop, size_t max_n,
+                               uint8_t* d_valid, cudaStream_t s) {
+  if (max_n == 0) return ARTP_OK;
+  if (!h->pose_states_smem) {
+    CU_TRY(h, cudaFuncSetAttribute(artp::pose_states_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    h->pose_states_smem = true;
+  }
+  TRY(launch(h, artp::pose_states_kernel, (unsigned)max_n, 256, h->k2_smem, s, h->chk, d_states, d_count, d_stop, d_valid,
+             h->k2_tcap, h->d_err));
+  h->ev_valid = false;
+  return ARTP_OK;
+}
+
 int artp_api::compact_valid(Handle* h, const uint8_t* d_valid, size_t n, int64_t base, void* d_indices, uint32_t* d_count,
                             cudaStream_t s, bool bits, bool u32) {
   if (n == 0) { CU_TRY(h, cudaMemsetAsync(d_count, 0, sizeof(uint32_t), s)); return ARTP_OK; }
@@ -751,6 +764,7 @@ void artp_destroy(artp_handle* hh) {
   cudaFree(h->d_H[0]); cudaFree(h->d_H[1]); cudaFree(h->d_ctr); cudaFree(h->d_defer); cudaFree(h->d_stage);
   cudaFree(h->d_block_counts); cudaFree(h->d_recs); cudaFree(h->d_recs_f); cudaFree(h->d_recs_g); cudaFree(h->d_samp_layers); cudaFree(h->d_samp_scratch);
   cudaFree(h->d_dist_layers); cudaFree(h->d_dist_scratch); cudaFree(h->d_basic_keep);
+  roadmap_free(h);
   if (h->h_small_out) cudaFreeHost(h->h_small_out);
   if (h->h_err) cudaFreeHost(h->h_err);
   for (int g = 0; g < 2; ++g) if (h->chain_ev[g]) cudaEventDestroy(h->chain_ev[g]);

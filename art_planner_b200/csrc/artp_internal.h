@@ -36,6 +36,8 @@ struct alignas(32) BoxQueues { QueueCtr big, reach, group; };
 struct Counters { BoxQueues q; uint32_t defer, scratch; };
 
 // What belongs to the current map: artp_set_map_window resets all of it.
+struct Roadmap;
+
 struct MapState {
   bool has_sampler = false;
   bool has_device_normals = false;  // artp_estimate_normals filled normal_x/y/z/std_dev of d_samp_layers for this map
@@ -103,6 +105,8 @@ struct Handle {
   size_t basic_keep_cap = 0;        // floats
   int basic_rows = 0, basic_cols = 0;
   bool has_basic_layers = false, has_basic_observed = false;
+  Roadmap* roadmap = nullptr;       // the PRM roadmap store (artp_roadmap.cu), from the first artp_roadmap_clear
+  bool pose_states_smem = false;    // pose_states_kernel may use the latency path's dynamic shared memory
   uint8_t* h_small_out = nullptr;   // mapped pinned host bytes the latency-path kernel writes its verdicts to
   int timing = 0;
   cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // classify | warp | reach vertex | reach plane | group
@@ -267,5 +271,24 @@ int check_states_f32(Handle* h, const float* d_states, size_t n, uint8_t* d_vali
 // count, int64_t indices or, with `u32`, uint32_t ones. Uses scratch group 1.
 int compact_valid(Handle* h, const uint8_t* d_valid, size_t n, int64_t base, void* d_indices, uint32_t* d_count, cudaStream_t s,
                   bool bits = false, bool u32 = false);
+// The latency path's per-pose routine, one CTA per state, over the device states 0 .. *d_count - 1 (at most max_n, which
+// sizes the grid) into d_valid, on s; nothing once *d_stop is set (the roadmap's interior states).
+int check_states_cta(Handle* h, const double* d_states, const uint32_t* d_count, const uint32_t* d_stop, size_t max_n,
+                     uint8_t* d_valid, cudaStream_t s);
+
+// artp_sampling.cu, for the roadmap:
+// A map and an armed sampler (ARTP_E_NOMAP otherwise).
+int sampler_armed(Handle* h);
+// artp_sample_valid_device's work on s, with the draw index of every kept state into d_draws (capacity entries).
+int sample_valid_draws(Handle* h, uint64_t seed, uint64_t first_sample, size_t n_draw, double* d_states_out, uint64_t* d_draws,
+                       size_t capacity, uint32_t* d_count, cudaStream_t s);
+// artp_update_sample_distribution_device's argument checks and work (n vertex states on the device, NaN ones not
+// counted) on s; the sampler is re-armed on the new CDF.
+int check_distribution_args(Handle* h, const artp_sample_distribution_params* dp);
+int update_distribution_rearm(Handle* h, const artp_sample_distribution_params* dp, const double* d_states, size_t n,
+                              cudaStream_t s);
+
+// artp_roadmap.cu: releases the roadmap store (artp_destroy).
+void roadmap_free(Handle* h);
 
 }  // namespace artp_api

@@ -73,12 +73,25 @@ __global__ void gather_chunk_kernel(const double* __restrict__ states, const int
   }
 }
 
+// draws + (*total) .. : the draw index of each state gather_chunk_kernel keeps, first_draw + its index in the chunk
+__global__ void gather_draws_kernel(const int64_t* __restrict__ idx, const uint32_t* __restrict__ chunk_count,
+                                    const uint32_t* __restrict__ total_before, size_t capacity, uint64_t first_draw,
+                                    uint64_t* __restrict__ draws) {
+  const size_t before = *total_before;
+  const size_t room = capacity > before ? capacity - before : 0;
+  const size_t cc = *chunk_count;
+  const size_t keep = cc < room ? cc : room;
+  for (size_t k = blockIdx.x * (size_t)blockDim.x + threadIdx.x; k < keep; k += (size_t)gridDim.x * blockDim.x)
+    draws[before + k] = first_draw + (uint64_t)idx[k];
+}
+
 constexpr size_t kSampleChunk = (size_t)1 << 21;
 
 // Sample -> check -> compact on s, in chunks of kSampleChunk draws: the valid states of draws first_sample ..
-// first_sample + n_draw - 1 in draw order into d_states_out (at most `capacity` of them), their number into *d_count.
+// first_sample + n_draw - 1 in draw order into d_states_out (at most `capacity` of them), their number into *d_count;
+// with d_draws, the draw index of each kept state too.
 int sample_valid(Handle* h, uint64_t seed, uint64_t first_sample, size_t n_draw, double* d_states_out, size_t capacity,
-                 uint32_t* d_count, cudaStream_t s) {
+                 uint32_t* d_count, cudaStream_t s, uint64_t* d_draws = nullptr) {
   CU_TRY(h, cudaMemsetAsync(d_count, 0, sizeof(uint32_t), s));
   if (n_draw == 0) return ARTP_OK;
   const size_t chunk = std::min(n_draw, kSampleChunk);
@@ -100,6 +113,9 @@ int sample_valid(Handle* h, uint64_t seed, uint64_t first_sample, size_t n_draw,
     TRY(compact_valid(h, d_val, m, 0, d_idx, d_cnt, s));
     TRY(launch(h, gather_chunk_kernel, grid_for(h, m * 7, 256), 256, 0, s, d_st, d_idx, d_cnt, d_count, capacity,
         d_states_out));
+    if (d_draws)
+      TRY(launch(h, gather_draws_kernel, grid_for(h, m, 256), 256, 0, s, d_idx, d_cnt, d_count, capacity, first_sample + done,
+          d_draws));
     TRY(launch(h, add_count_kernel, 1, 1, 0, s, d_count, d_cnt));
   }
   return ARTP_OK;
@@ -276,6 +292,36 @@ int update_distribution(Handle* h, const artp_sample_distribution_params* dp, in
 }
 
 }  // namespace
+
+int artp_api::sampler_armed(Handle* h) { return sampler_ready(h); }
+
+int artp_api::sample_valid_draws(Handle* h, uint64_t seed, uint64_t first_sample, size_t n_draw, double* d_states_out,
+                                 uint64_t* d_draws, size_t capacity, uint32_t* d_count, cudaStream_t s) {
+  return sample_valid(h, seed, first_sample, n_draw, d_states_out, capacity, d_count, s, d_draws);
+}
+
+int artp_api::check_distribution_args(Handle* h, const artp_sample_distribution_params* dp) {
+  int ksize;
+  double sigma;
+  return distribution_args(h, dp, &ksize, &sigma);
+}
+
+int artp_api::update_distribution_rearm(Handle* h, const artp_sample_distribution_params* dp, const double* d_states, size_t n,
+                                        cudaStream_t s) {
+  int ksize;
+  double sigma;
+  TRY(distribution_args(h, dp, &ksize, &sigma));
+  float* d_prob;
+  TRY(update_distribution(h, dp, ksize, sigma, d_states, n, s, &d_prob));
+  // artp_set_sampler(h, sp, ..., NULL, NULL) on the resident layers: the CDF rows just computed are cumulative
+  if (h->samp.from_distribution) {
+    const size_t ncell = (size_t)h->rows * h->cols;
+    h->samp.cum_prob = h->d_samp_layers + 4 * ncell;
+    h->samp.cum_row = h->d_samp_layers + 5 * ncell;
+  }
+  h->map.has_sampler = true;
+  return ARTP_OK;
+}
 
 extern "C" {
 

@@ -370,6 +370,53 @@ int artp_update_sample_distribution_device(artp_handle* h, const artp_sample_dis
 /* Test hook: getGaussianKernel(ksize, sigma, CV_32F) as the blur uses it (odd ksize <= 1023, sigma > 0); returns ksize. */
 int artp_debug_gaussian_kernel(int ksize, double sigma, float* out);
 
+/* ---- PRM roadmap on the device (PRMMotionCost, art_planner/src/planners/prm_motion_cost.cpp) ----------------------
+ * The handle owns an append-only roadmap: vertex states (7 doubles) with a kind byte each, and undirected edges (u, v),
+ * both in the order PRMMotionCost::addValidMilestone (:325-390) inserts them into its Boost graph, so vertex i here is
+ * vertex i of g_. Every milestone is added on the device with three kernels and no host synchronisation:
+ *   neighbours  KStarStrategy (OMPL 1.4.2 ConnectionStrategy.h): k = ceil((e + e/6) ln V), V = num_vertices(g_) with the
+ *               new milestone counted (LazyPRM::milestoneCount), over the vertices already in the roadmap, exact
+ *               (GNAT nearestK is exact) in ascending SE3StateSpace::distance (R3 Euclidean + acos(|q1.q2|), 0 above
+ *               1 - 1e-9); exact ties go to the lower vertex index (GNAT leaves them unspecified). Per neighbour
+ *               n_interp = (unsigned)(lateralDistance / 0.5) interior states at step * (1.0 / (n_interp + 1)).
+ *   check       every interior state through the validity pipeline's per-pose routine.
+ *   commit      :335-387: the valid prefix of each connection becomes a chain of interpolated vertices and edges, the
+ *               final edge only when the whole connection is valid, a direct edge when n_interp == 0.
+ * Edges carry no cost: price them with artp_motion_cost_states on the copied-out edges (updateEdges, :27-73).
+ * The map must be the whole map (a map window is ARTP_E_INVALID). A milestone that would overflow the store's capacity
+ * is not added and the call returns ARTP_E_LIMIT (the roadmap keeps every earlier milestone). */
+#define ARTP_ROADMAP_MILESTONE     1   /* a milestone (sampled, or added with artp_roadmap_add_milestones) */
+#define ARTP_ROADMAP_INTERPOLATED  2   /* an interior state of a connection (prm_motion_cost.cpp:358-365) */
+#define ARTP_ROADMAP_QUERY         4   /* with MILESTONE: added by artp_roadmap_add_milestones (start / goal, startM_ / goalM_) */
+typedef struct artp_roadmap_params {
+  size_t   max_n_vertices;                     /* params.h:51, 10000 */
+  size_t   max_n_edges;                        /* params.h:52, 50000 */
+  size_t   recompute_density_after_n_samples;  /* params.h:53, 1000; 0 = never */
+  uint64_t max_draws;                          /* sampler draws the call may use: replaces max_sample_time (:177-184) */
+} artp_roadmap_params;
+/* PRMMotionCost::clear (:236-247): empties the roadmap and sizes its store for vertex_capacity vertices and
+ * edge_capacity edges (> 0 and < 2^31; ARTP_E_INVALID otherwise). The store outlives artp_set_map. */
+int artp_roadmap_clear(artp_handle* h, size_t vertex_capacity, size_t edge_capacity);
+/* addValidMilestone for the n HOST states, in order (baseSolve's start and goal milestones, :451-479). Kind
+ * MILESTONE | QUERY: these count in the sampling density like startM_ / goalM_ (LazyPRM::getPlannerData). No roadmap
+ * (artp_roadmap_clear never called): ARTP_E_INVALID. */
+int artp_roadmap_add_milestones(artp_handle* h, const double* states, size_t n);
+/* PRMMotionCostMaintainer::sampleGraph's loop (:171-194): while V < max_n_vertices and E < max_n_edges (checked before
+ * each milestone), the next valid draw of the sampler (artp_set_sampler; Philox draws first_sample, first_sample + 1, ...)
+ * becomes a milestone; after it, when V / recompute_density_after_n_samples exceeds the number of recomputes so far
+ * (once per milestone), the distribution is recomputed as artp_update_sample_distribution(h, dp, ...) over the vertices
+ * LazyPRM::getPlannerData returns -- QUERY milestones and the endpoints of edges; an isolated milestone is not counted --
+ * and the sampler is re-armed on it; sampling goes on at the draw after the last milestone. dp NULL: no recompute.
+ * The loop also ends when max_draws draws are used. *draws_used (nullable): draws consumed, up to and including the last
+ * milestone's, or max_draws. Needs a map and an armed sampler (ARTP_E_NOMAP). */
+int artp_roadmap_sample_graph(artp_handle* h, const artp_roadmap_params* rp, const artp_sample_distribution_params* dp,
+                              uint64_t seed, uint64_t first_sample, uint64_t* draws_used);
+/* The roadmap's tail to HOST buffers: vertices first_vertex .. V-1 (states: 7 doubles each, kinds: 1 byte each; both
+ * nullable) and edges first_edge .. E-1 (edges: 2 uint32 each, nullable). *nv = V, *ne = E (nullable). A cursor past
+ * the end: ARTP_E_INVALID. */
+int artp_roadmap_get(artp_handle* h, size_t first_vertex, double* states, uint8_t* kinds, size_t first_edge,
+                     uint32_t* edges, size_t* nv, size_t* ne);
+
 /* ---- learned motion cost (MotionCostFunc, objectives/motion_cost_objective.h:22-23) ------------------------------
  * Weights: ONE flat fp32 blob in the layer order of the reference's `network` module: init_conv1..5, init_flatten,
  * tar0_conv1, out0_conv1, out1_conv1..3 -- each conv.weight [Cout][Cin][kh][kw] followed by its BatchNorm weight, bias,

@@ -35,6 +35,9 @@ struct Params {
       float max_query_edge_length{0.5f};
       float risk_threshold{0.1f};
       struct { float energy{0.0f}; float time{1.0f}; float risk{5.0f}; } cost_weights;
+      unsigned int max_n_vertices{10000u};                    // params.h:51
+      unsigned int max_n_edges{50000u};                       // params.h:52
+      unsigned int recompute_density_after_n_samples{1000u};  // params.h:53
     } prm_motion_cost;
   } planner;
   struct {
@@ -354,12 +357,78 @@ class SE3FromSE2Sampler {
     valid->resize(n_valid);
   }
   uint64_t nextIndex() const { return next_; }
+  uint64_t seed() const { return seed_; }
+  void skip(uint64_t n) { next_ += n; }   // draws another caller consumed from this stream (PRMRoadmap::sampleGraph)
  private:
   StateValidityCheckerPtr checker_;
   std::shared_ptr<Map> map_;
   artp_sampler_params sp_{};
   uint64_t seed_;
   uint64_t next_{0};
+};
+
+// PRMMotionCost's roadmap built on the device (prm_motion_cost.cpp:145-219, 236-247, 325-390; include/artp.h): the store
+// keeps g_'s insertion order, so vertex i of vertices() is the i-th vertex the reference's addValidMilestone adds.
+// Edges carry no cost: price them with MotionCostObjective::updateEdgesBatch.
+class PRMRoadmap {
+ public:
+  explicit PRMRoadmap(const StateValidityCheckerPtr& checker, size_t vertex_capacity = 60000, size_t edge_capacity = 60000)
+      : checker_(checker), vertex_capacity_(vertex_capacity), edge_capacity_(edge_capacity) { clear(); }
+  void clear() {                                                                  // PRMMotionCost::clear (:236-247)
+    const auto& h = checker_->handle();
+    h->check(artp_roadmap_clear(h->get(), vertex_capacity_, edge_capacity_), "artp_roadmap_clear");
+  }
+  // addValidMilestone for each state in order: baseSolve's start / goal milestones (:451-479).
+  void addValidMilestones(const std::vector<State>& states) {
+    const auto& h = checker_->handle();
+    h->check(artp_roadmap_add_milestones(h->get(), states.empty() ? nullptr : &states[0].x, states.size()),
+             "artp_roadmap_add_milestones");
+  }
+  // PRMMotionCostMaintainer::sampleGraph's loop (:171-194) on `sampler`'s stream, continuing at its next draw; the caps
+  // and the recompute interval from Params, the distribution re-applied as SE3FromSE2Sampler::updateDistribution does.
+  // max_draws replaces max_sample_time. Returns the draws used (the sampler's stream moves past them).
+  uint64_t sampleGraph(SE3FromSE2Sampler& sampler, uint64_t max_draws = 1ull << 26, bool distribution = true) {
+    const auto& h = checker_->handle();
+    const Params& p = h->params();
+    const artp_roadmap_params rp{p.planner.prm_motion_cost.max_n_vertices, p.planner.prm_motion_cost.max_n_edges,
+                                 p.planner.prm_motion_cost.recompute_density_after_n_samples, max_draws};
+    artp_sample_distribution_params dp{};
+    dp.use_inverse_vertex_density = p.sampler.use_inverse_vertex_density ? 1 : 0;
+    dp.density_blur_radius = (p.robot.torso.length + p.robot.torso.width) * 0.25;   // planner.cpp:48
+    dp.use_max_prob_unknown_samples = p.sampler.use_max_prob_unknown_samples ? 1 : 0;
+    dp.max_prob_unknown_samples = p.sampler.max_prob_unknown_samples;
+    uint64_t used = 0;
+    h->check(artp_roadmap_sample_graph(h->get(), &rp, distribution ? &dp : nullptr, sampler.seed(), sampler.nextIndex(), &used),
+             "artp_roadmap_sample_graph");
+    sampler.skip(used);
+    return used;
+  }
+  // The vertices first .. V-1 (states and ARTP_ROADMAP_* kinds) and the edges first .. E-1 as (u, v) pairs.
+  void vertices(size_t first, std::vector<State>* states, std::vector<uint8_t>* kinds) const {
+    size_t nv = 0, ne = 0;
+    counts(&nv, &ne);
+    const size_t n = nv > first ? nv - first : 0;
+    states->resize(n);
+    kinds->resize(n);
+    const auto& h = checker_->handle();
+    h->check(artp_roadmap_get(h->get(), first, n ? &(*states)[0].x : nullptr, n ? kinds->data() : nullptr, 0, nullptr, nullptr,
+                              nullptr), "artp_roadmap_get");
+  }
+  void edges(size_t first, std::vector<uint32_t>* uv) const {
+    size_t nv = 0, ne = 0;
+    counts(&nv, &ne);
+    const size_t n = ne > first ? ne - first : 0;
+    uv->resize(2 * n);
+    const auto& h = checker_->handle();
+    h->check(artp_roadmap_get(h->get(), 0, nullptr, nullptr, first, n ? uv->data() : nullptr, nullptr, nullptr), "artp_roadmap_get");
+  }
+  void counts(size_t* nv, size_t* ne) const {
+    const auto& h = checker_->handle();
+    h->check(artp_roadmap_get(h->get(), 0, nullptr, nullptr, 0, nullptr, nv, ne), "artp_roadmap_get");
+  }
+ private:
+  StateValidityCheckerPtr checker_;
+  size_t vertex_capacity_, edge_capacity_;
 };
 
 // ompl::base::MotionValidator as the reference uses it: discrete validation over isValid with nd segments.
