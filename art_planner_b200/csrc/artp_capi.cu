@@ -147,8 +147,7 @@ __global__ void plane_table_insert_kernel(const artp::Field f, int x_off, PlaneS
     float pl[4];
     if (!cell_tri_plane(f, x, x_off, z, u, pl)) continue;
     const uint32_t id = (uint32_t)(((size_t)z * f.pitch + x) * 2 + u);
-    const unsigned long long key = plane_key((int)floorf((pl[0] + 1.0f) * artp::kKeyScale), (int)floorf((pl[2] + 1.0f) * artp::kKeyScale),
-                                             artp::dkey(pl[3]));
+    const unsigned long long key = plane_key(artp::nkey(pl[0]), artp::nkey(pl[2]), artp::dkey(pl[3]));
     uint32_t s = plane_slot_hash(key) & mask;
     for (;;) {
       const unsigned long long old = atomicCAS(&tab[s].key, kEmptyKey, key);
@@ -171,8 +170,8 @@ __global__ void plane_table_query_kernel(const artp::Field f, int x_off, const P
     if (!cell_tri_plane(f, x, x_off, z, u, pl)) continue;
     const uint32_t id = (uint32_t)(((size_t)z * f.pitch + x) * 2 + u);
     const float e2 = 2.0f * ARTP_EPS;
-    const int kx0 = (int)floorf((pl[0] - e2 + 1.0f) * artp::kKeyScale), kx1 = (int)floorf((pl[0] + e2 + 1.0f) * artp::kKeyScale);
-    const int kz0 = (int)floorf((pl[2] - e2 + 1.0f) * artp::kKeyScale), kz1 = (int)floorf((pl[2] + e2 + 1.0f) * artp::kKeyScale);
+    const int kx0 = artp::nkey(pl[0] - e2), kx1 = artp::nkey(pl[0] + e2);
+    const int kz0 = artp::nkey(pl[2] - e2), kz1 = artp::nkey(pl[2] + e2);
     const int kd0 = artp::dkey(pl[3] - e2), kd1 = artp::dkey(pl[3] + e2);
     bool dup = false;
     for (int kx = kx0; kx <= kx1 && !dup; ++kx)

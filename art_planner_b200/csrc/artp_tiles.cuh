@@ -56,6 +56,18 @@ __device__ __forceinline__ void tma_tile_2d(void* dst, const CUtensorMap* map, u
 
 constexpr int kMaxTileWarps = 8;
 
+// This warp's `n` tile slots of tc.stride bytes in the dynamic shared memory (TMA destinations: 128-byte aligned), with
+// its two mbarriers (one per slot parity) initialised.
+__device__ __forceinline__ unsigned char* warp_tile_slots(unsigned char* smem, const TileCfg& tc, int n, uint64_t bars[2]) {
+  const int wid = threadIdx.x >> 5;
+  unsigned char* slots = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem) + 127) & ~(uintptr_t)127) +
+                         (size_t)wid * n * tc.stride;
+  if ((threadIdx.x & 31) == 0) { mbar_init(&bars[0], 1); mbar_init(&bars[1], 1); }
+  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  __syncwarp();
+  return slots;
+}
+
 // map0 / map1: tiles of `elevation` / `elevation_masked` (same tile extent). queue_bit tags defer-list entries.
 __global__ void __launch_bounds__(kMaxTileWarps * 32, 3)
 box_tiles_warp_kernel(const Checker c, const __grid_constant__ CUtensorMap map0, const __grid_constant__ CUtensorMap map1,
@@ -67,19 +79,13 @@ box_tiles_warp_kernel(const Checker c, const __grid_constant__ CUtensorMap map0,
   __shared__ uint64_t bars[kMaxTileWarps][2];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   WarpScratch& ws = ws_all[wid];
-  unsigned char* slots = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(tile_smem) + 127) & ~(uintptr_t)127) +
-                         (size_t)wid * tc.slots * tc.stride;   // TMA destinations: 128-byte aligned
-  if (lane == 0) { mbar_init(&bars[wid][0], 1); mbar_init(&bars[wid][1], 1); }
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  __syncwarp();
+  unsigned char* slots = warp_tile_slots(tile_smem, tc, tc.slots, bars[wid]);
   uint32_t phase[2] = {0u, 0u};
   const uint32_t total = *rec_count;
   // lane 0 starts the copy of record ri's zone into tile slot `slot`
   auto prefetch = [&](uint32_t ri, int slot) {
-    const uint4 zr = __ldg(reinterpret_cast<const uint4*>(recs + ri) + 3);        // R.., minB, maxB | x0 x1 z0 z1 -> words 14..17
-    const uint4 zr2 = __ldg(reinterpret_cast<const uint4*>(recs + ri) + 4);
-    const int x0 = (int)zr.z, z0 = (int)zr2.x;                                    // BoxRec words: 14 x0, 15 x1, 16 z0, 17 z1
-    const uint32_t fl = zr2.w;                                                    // word 19: flags
+    const int x0 = rec_x0(recs + ri), z0 = rec_z0(recs + ri);
+    const uint32_t fl = rec_flags(recs + ri);
     if (lane == 0) {
       mbar_expect_tx(&bars[wid][slot], tc.bytes);
       tma_tile_2d(slots + (size_t)slot * tc.stride, (fl & 7u) ? &map1 : &map0, &bars[wid][slot], (x0 & ~3) - tc.x_off, z0);
@@ -120,14 +126,7 @@ box_tiles_warp_kernel(const Checker c, const __grid_constant__ CUtensorMap map0,
     for (uint32_t ri = r0; ri < r1; ++ri) {
       const int slot = (int)(ri - r0) & (tc.slots - 1);
       if (tc.slots == 1 || ri == r0) { __syncwarp(); prefetch(ri, slot); }   // every lane is done with the slot
-      // every lane reads the whole 80-byte record itself: five 16-byte loads from one address per warp (broadcasts)
-      BoxRec r;
-      {
-        const uint4* rp = reinterpret_cast<const uint4*>(recs + ri);
-        uint4* dst = reinterpret_cast<uint4*>(&r);
-#pragma unroll
-        for (int i = 0; i < 5; ++i) dst[i] = __ldg(rp + i);
-      }
+      const BoxRec r = load_rec(recs + ri);   // every lane reads the whole record itself (broadcast loads)
       if (tc.slots == 2 && ri + 1 < r1) { __syncwarp(); prefetch(ri + 1, slot ^ 1); }   // the other slot's box (ri - 1) is finished
       const uint32_t slot_item = r.item;
       const bool foot = (r.flags & 7) != 0;
@@ -150,7 +149,7 @@ box_tiles_warp_kernel(const Checker c, const __grid_constant__ CUtensorMap map0,
       }
       if (lane == 0) {
         if (res == R_DEFER) defer_list[atomicAdd(defer_count, 1u)] = ri | queue_bit;
-        else if ((!foot && res == R_HIT) || (foot && res == R_FREE)) w.valid[slot_item] = 0;
+        else if (box_fails(foot, res)) w.valid[slot_item] = 0;
       }
     }
   }
@@ -179,12 +178,8 @@ reach_groups_kernel(const Checker c, const __grid_constant__ CUtensorMap map1, c
   __shared__ __align__(16) float ctx_all[kMaxTileWarps][4][16];   // per box of the round: R1[9], P[3], minB, x0, z0 (task stage)
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, g = lane >> 3, gl = lane & 7;
   const Field& f = c.f[1];
-  unsigned char* slots = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(tile_smem) + 127) & ~(uintptr_t)127) +
-                         (size_t)wid * 8 * tc.stride;   // [slot 0/1][group 0..3]
+  unsigned char* slots = warp_tile_slots(tile_smem, tc, 8, bars[wid]);   // [slot 0/1][group 0..3]
   uint16_t* tasks = tasks_all[wid][g];
-  if (lane == 0) { mbar_init(&bars[wid][0], 1); mbar_init(&bars[wid][1], 1); }
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  __syncwarp();
   uint32_t phase[2] = {0u, 0u};
   const uint32_t total = *rec_count;
   const unsigned gshift = (unsigned)g * 8u;
@@ -193,10 +188,7 @@ reach_groups_kernel(const Checker c, const __grid_constant__ CUtensorMap map1, c
     const uint32_t ri = first + (uint32_t)g;
     int x0 = 0, z0 = 0;
     const bool act = ri < total;
-    if (act && gl == 0) {
-      x0 = (int)__ldg(reinterpret_cast<const uint4*>(recs + ri) + 3).z;
-      z0 = (int)__ldg(reinterpret_cast<const uint4*>(recs + ri) + 4).x;
-    }
+    if (act && gl == 0) { x0 = rec_x0(recs + ri); z0 = rec_z0(recs + ri); }
     const int nact = (int)min(4u, total - first);
     if (lane == 0) mbar_expect_tx(&bars[wid][slot], (uint32_t)nact * tc.bytes);
 #pragma unroll 1
@@ -228,18 +220,8 @@ reach_groups_kernel(const Checker c, const __grid_constant__ CUtensorMap map1, c
       const int slot = round & 1;
       const uint32_t ri = r0 + 4u * (uint32_t)round + (uint32_t)g;
       const bool act = ri < total;
-      BoxRec r;
-      {
-        uint4* dst = reinterpret_cast<uint4*>(&r);
-#pragma unroll
-        for (int i = 0; i < 5; ++i) dst[i] = make_uint4(0u, 0u, 0u, 0u);
-      }
-      if (act) {
-        const uint4* rp = reinterpret_cast<const uint4*>(recs + ri);
-        uint4* dst = reinterpret_cast<uint4*>(&r);
-#pragma unroll
-        for (int i = 0; i < 5; ++i) dst[i] = __ldg(rp + i);
-      }
+      BoxRec r = {};
+      if (act) r = load_rec(recs + ri);
       if (round + 1 < nrounds) { __syncwarp(); prefetch(r0 + 4u * (uint32_t)(round + 1), slot ^ 1); }
       int alive = 0;
       if (act && gl == 0) alive = (*(volatile const uint8_t*)(w.valid + r.item) != 0);
@@ -259,7 +241,6 @@ reach_groups_kernel(const Checker c, const __grid_constant__ CUtensorMap map1, c
         cx[13] = __int_as_float(b.x0); cx[14] = __int_as_float(b.z0);
       }
       const float* tile = reinterpret_cast<const float*>(slots + (size_t)(slot * 4 + g) * tc.stride) + (b.x0 & 3);
-      const int nX = b.x1 - b.x0 + 1, nZ = b.z1 - b.z0 + 1, nV = nX * nZ, nCZ = nZ - 1;
       const float top = b.maxB + (1e-4f + 4e-6f * fabsf(b.maxB));
       bool ghit = false;
       // vertex stage, lane = vertex. Only the vertices inside the box's own xz extent are scanned: a point inside the box
@@ -267,8 +248,7 @@ reach_groups_kernel(const Checker c, const __grid_constant__ CUtensorMap map1, c
       // cells on every side (heightfield.cpp:1880-1892) -- its outer ring, 81 -> ~49 vertices for a reach box, cannot hold
       // one (margin 1e-4 m, far above the rounding of the fp32 inside test).
       {
-        const float xr = 0.5f * (fabsf(b.R1[0] * b.side[0]) + fabsf(b.R1[1] * b.side[1]) + fabsf(b.R1[2] * b.side[2])) + 1e-4f;
-        const float zr = 0.5f * (fabsf(b.R1[6] * b.side[0]) + fabsf(b.R1[7] * b.side[1]) + fabsf(b.R1[8] * b.side[2])) + 1e-4f;
+        const float xr = box_half_extent(b.R1, b.side, 0) + 1e-4f, zr = box_half_extent(b.R1, b.side, 2) + 1e-4f;
         const int vx0 = max(b.x0, (int)ceilf((b.P[0] - xr) * f.iW)), vx1 = min(b.x1, (int)floorf((b.P[0] + xr) * f.iW));
         const int vz0 = max(b.z0, (int)ceilf((b.P[2] - zr) * f.iD)), vz1 = min(b.z1, (int)floorf((b.P[2] + zr) * f.iD));
         const int nXi = max(vx1 - vx0 + 1, 0), nZi = max(vz1 - vz0 + 1, 0), nVi = nXi * nZi;
@@ -293,12 +273,9 @@ reach_groups_kernel(const Checker c, const __grid_constant__ CUtensorMap map1, c
       // plane stage: collect the candidate (cell, triangle) tasks, lane = corner
       int nt = 0;
       {
-        float px = b.P[0], pz = b.P[2];
-        const float h0 = 0.5f * b.side[0], h1 = 0.5f * b.side[1], h2 = 0.5f * b.side[2];
-        if (gl & 1) { px += h0 * b.R1[0]; pz += h0 * b.R1[6]; } else { px -= h0 * b.R1[0]; pz -= h0 * b.R1[6]; }
-        if (gl & 2) { px += h1 * b.R1[1]; pz += h1 * b.R1[7]; } else { px -= h1 * b.R1[1]; pz -= h1 * b.R1[7]; }
-        if (gl & 4) { px += h2 * b.R1[2]; pz += h2 * b.R1[8]; } else { px -= h2 * b.R1[2]; pz -= h2 * b.R1[8]; }
-        const float gx = px * f.iW, gz = pz * f.iD;
+        float pc[3];
+        box_corner(b, gl, pc);
+        const float gx = pc[0] * f.iW, gz = pc[2] * f.iD;
         const int cxl = (int)floorf(gx - c.cell_margin), cxh = (int)floorf(gx + c.cell_margin);
         const int czl = (int)floorf(gz - c.cell_margin), czh = (int)floorf(gz + c.cell_margin);
         // an upright box projects its top corners into the cells of the bottom corners: the same cells twice
@@ -373,9 +350,7 @@ reach_groups_kernel(const Checker c, const __grid_constant__ CUtensorMap map1, c
         hit_groups = __reduce_or_sync(kFull, hit_groups);
         if ((hit_groups >> g) & 1u) ghit = true;
       }
-      // a reach box that does not touch: pose invalid
-      if (gl == 0 && act && alive && !ghit) w.valid[r.item] = 0;
-      (void)nCZ;
+      if (gl == 0 && act && alive && box_fails(true, ghit ? R_HIT : R_FREE)) w.valid[r.item] = 0;
       __syncwarp();
     }
   }
