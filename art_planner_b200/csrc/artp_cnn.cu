@@ -71,7 +71,9 @@ static LayerDef layer_def(int net, int l) {
   return {1, d.b[l - 11], 1, false};
 }
 static const float kBnEps = 1e-5f;
-__device__ constexpr float kWScale = 1024.0f;   // undone exactly in the 15x15 epilogue
+// Trunk layers whose output the tensor-core path stores as an fp16 hi/lo split (directly, or after a max-pool), in the
+// bit order of the overflow flag the split kernels raise.
+static const char* const kSplitLayerNames[5] = {"init_conv1", "init_conv2", "init_conv3", "init_conv4", "init_conv5"};
 
 size_t blob_floats(int net) {
   if (net < 0 || net >= kNumNetworks) return 0;
@@ -305,13 +307,16 @@ struct ConvCfg {
 // Implicit-GEMM convolution on wgmma (see the file header). KS x KS taps, KSTEPS x 16 input channels multiplied per
 // tap (channels are stored padded to 64 = one 128-byte swizzle row per pixel), NOUT = wgmma N, NMAIN fp32 accumulators
 // for the a_hi*w_hi products (tap t -> t % NMAIN) + 1 for the two correction terms.
-// SPLIT_OUT: write the activation as fp16 hi/lo NHWC-64 (the next layer's TMA source) instead of fp32 NHWC.
+// SPLIT_OUT: write the activation as fp16 hi/lo NHWC-64 (the next layer's TMA source) instead of fp32 NHWC; an
+// activation beyond the fp16 range sets `split_bit` in *overflow.
+// inv_scale[n]: the power of two that undoes output channel n's weight scale (fold_tc_kernel).
 template <int KS, int KSTEPS, int NOUT, int NMAIN, bool SPLIT_OUT>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_constant__ CUtensorMap map_alo,
                   const __grid_constant__ CUtensorMap map_whi, const __grid_constant__ CUtensorMap map_wlo,
-                  const float* __restrict__ bias, float* __restrict__ out, __half* __restrict__ out_hi,
-                  __half* __restrict__ out_lo, int OH, int OW, int cout) {
+                  const float* __restrict__ bias, const float* __restrict__ inv_scale, float* __restrict__ out,
+                  __half* __restrict__ out_hi, __half* __restrict__ out_lo, int OH, int OW, int cout,
+                  unsigned* __restrict__ overflow, unsigned split_bit) {
   using Cfg = ConvCfg<KS, NOUT>;
   constexpr int kTaps = KS * KS, kNA = NOUT / 2, kWStages = Cfg::kWStages;
   extern __shared__ unsigned char smem_raw[];
@@ -423,11 +428,15 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         float x = 0.0f;
-        if (n + e < cout) { x = v[4 * c8 + 2 * h + e] * (1.0f / kWScale) + __ldg(bias + n + e); x = x > 0.0f ? x : 0.3f * x; }
+        if (n + e < cout) {
+          x = v[4 * c8 + 2 * h + e] * __ldg(inv_scale + n + e) + __ldg(bias + n + e);
+          x = x > 0.0f ? x : 0.3f * x;
+        }
         f[e] = x;
       }
       if (SPLIT_OUT) {
         const __half h0 = __float2half_rn(f[0]), h1 = __float2half_rn(f[1]);
+        if (__hisinf(h0) | __hisinf(h1)) atomicOr(overflow, split_bit);
         reinterpret_cast<__half2*>(out_hi + pix * 64)[n / 2] = __halves2half2(h0, h1);
         reinterpret_cast<__half2*>(out_lo + pix * 64)[n / 2] =
             __halves2half2(__float2half_rn(f[0] - __half2float(h0)), __float2half_rn(f[1] - __half2float(h1)));
@@ -448,11 +457,13 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_ahi, const __grid_cons
 
 // First layer (Cin = 1, no activation after its BN) on CUDA cores, reading the map layer directly and writing the
 // fp16 hi/lo NHWC-64 input of the second layer. One thread per (pixel, group of 8 output channels): the eight threads of
-// a pixel write its two 128-byte rows as sixteen 16-byte stores; channels C1..63 are zero.
+// a pixel write its two 128-byte rows as sixteen 16-byte stores; channels C1..63 are zero. An output beyond the fp16
+// range sets bit 0 of *overflow.
 template <int C1>
 __global__ void __launch_bounds__(256) conv1_split_kernel(const float* __restrict__ layer, int H, int W, int pitch,
                                                           const float* __restrict__ wf /*[9][1][C1]*/, const float* __restrict__ bias,
-                                                          __half* __restrict__ hi, __half* __restrict__ lo) {
+                                                          __half* __restrict__ hi, __half* __restrict__ lo,
+                                                          unsigned* __restrict__ overflow) {
   static_assert(C1 % 8 == 0 && C1 <= 64, "C1 output channels fill whole 8-channel groups of a 64-channel pixel row");
   __shared__ float sw[9 * C1 + C1];
   for (int i = threadIdx.x; i < 9 * C1 + C1; i += blockDim.x) sw[i] = i < 9 * C1 ? wf[i] : bias[i - 9 * C1];
@@ -482,6 +493,7 @@ __global__ void __launch_bounds__(256) conv1_split_kernel(const float* __restric
           f[e] = a;
         }
         const __half h0 = __float2half_rn(f[0]), h1 = __float2half_rn(f[1]);
+        if (__hisinf(h0) | __hisinf(h1)) atomicOr(overflow, 1u);
         hh[e2] = __halves2half2(h0, h1);
         ll[e2] = __halves2half2(__float2half_rn(f[0] - __half2float(h0)), __float2half_rn(f[1] - __half2float(h1)));
       }
@@ -495,9 +507,11 @@ __global__ void __launch_bounds__(256) conv1_split_kernel(const float* __restric
 }
 
 // max pooling (K x K, stride S) of an fp32 NHWC [H][W][C] activation (C a multiple of 8) into fp16 hi/lo NHWC-64.
-// One thread per (pixel, 8 channels): two 16-byte loads per tap, one 16-byte store per output array.
+// One thread per (pixel, 8 channels): two 16-byte loads per tap, one 16-byte store per output array. An output beyond
+// the fp16 range sets `split_bit` in *overflow.
 __global__ void maxpool_split_kernel(const float* __restrict__ in, int H, int W, int C, int K, int S, __half* __restrict__ hi,
-                                     __half* __restrict__ lo, int OH, int OW) {
+                                     __half* __restrict__ lo, int OH, int OW, unsigned* __restrict__ overflow,
+                                     unsigned split_bit) {
   const size_t total = (size_t)OH * OW * 8;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const int v8 = (int)(i & 7);
@@ -521,6 +535,7 @@ __global__ void maxpool_split_kernel(const float* __restrict__ in, int H, int W,
 #pragma unroll
     for (int e2 = 0; e2 < 4; ++e2) {
       const __half h0 = __float2half_rn(m[2 * e2]), h1 = __float2half_rn(m[2 * e2 + 1]);
+      if (__hisinf(h0) | __hisinf(h1)) atomicOr(overflow, split_bit);
       hh[e2] = __halves2half2(h0, h1);
       ll[e2] = __halves2half2(__float2half_rn(m[2 * e2] - __half2float(h0)), __float2half_rn(m[2 * e2 + 1] - __half2float(h1)));
     }
@@ -529,17 +544,43 @@ __global__ void maxpool_split_kernel(const float* __restrict__ in, int H, int W,
   }
 }
 
+// Weight scale of a tensor-core layer, one block per output channel n: the power of two 2^k that brings the channel's
+// largest folded |w| into [2^14, 2^15), so that w_hi stays below the fp16 maximum (65504) and w_lo above the fp16
+// subnormals wherever the weight matters; inv_scale[n] = 2^-k, which undoes it exactly in the epilogue.
+__global__ void __launch_bounds__(256) tc_scale_kernel(const float* __restrict__ w /*[cout][cin][taps]*/,
+                                                       const float* __restrict__ bn, int cout, int cin, int taps,
+                                                       float* __restrict__ inv_scale) {
+  __shared__ float red[256];
+  const int n = blockIdx.x;
+  const float s = bn[n] / sqrtf(bn[3 * cout + n] + kBnEps);
+  float m = 0.0f;
+  for (int i = threadIdx.x; i < cin * taps; i += blockDim.x) m = fmaxf(m, fabsf(w[(size_t)n * cin * taps + i] * s));
+  red[threadIdx.x] = m;
+  __syncthreads();
+  for (int k = blockDim.x / 2; k > 0; k >>= 1) {
+    if (threadIdx.x < k) red[threadIdx.x] = fmaxf(red[threadIdx.x], red[threadIdx.x + k]);
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    int e = 0;
+    frexpf(red[0], &e);                          // max|w| < 2^e (e = 0 for an all-zero channel)
+    const int k = min(max(15 - e, -100), 100);   // both 2^k and 2^-k stay normal fp32 numbers
+    inv_scale[n] = ldexpf(1.0f, -k);
+  }
+}
+
 // Tensor-core weights of one layer: [taps][NOUT][64] fp16 hi/lo (K-major rows of 128 B; pad rows / channels zero),
-// BN scale and kWScale folded; bias = beta - mean*scale.
+// BN scale and the channel's power-of-two weight scale folded; bias = beta - mean*scale.
 __global__ void fold_tc_kernel(const float* __restrict__ w /*[cout][cin][taps]*/, const float* __restrict__ bn, int cout, int cin,
-                               int taps, int nout, __half* __restrict__ whi, __half* __restrict__ wlo, float* __restrict__ bias) {
+                               int taps, int nout, const float* __restrict__ inv_scale, __half* __restrict__ whi,
+                               __half* __restrict__ wlo, float* __restrict__ bias) {
   const int total = taps * nout * 64;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const int c = i & 63, r = i >> 6, n = r % nout, tap = r / nout;
     float v = 0.0f;
     if (c < cin && n < cout) {
       const float s = bn[n] / sqrtf(bn[3 * cout + n] + kBnEps);
-      v = w[((size_t)n * cin + c) * taps + tap] * s * kWScale;   // power-of-two scale keeps w_lo out of fp16 subnormals
+      v = w[((size_t)n * cin + c) * taps + tap] * s * (1.0f / inv_scale[n]);
     }
     const __half h = __float2half_rn(v);
     whi[i] = h;
@@ -696,7 +737,7 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 // One tensor-core layer: weights (hi/lo), bias, and its launch geometry.
-struct TcLayer { __half *whi = nullptr, *wlo = nullptr; int nout = 0; };
+struct TcLayer { __half *whi = nullptr, *wlo = nullptr; float* inv_scale = nullptr; int nout = 0; };
 
 struct State {
   int device = 0, sm_count = 0;
@@ -726,6 +767,9 @@ struct State {
   bool attrs_set = false;
   float last_ms[3] = {0, 0, 0};
   cudaEvent_t ev[4] = {};
+  // fp16 range overflow of the tensor-core path's activation splits: bit i = output of trunk layer i (kSplitLayerNames)
+  unsigned* d_overflow = nullptr;
+  unsigned* h_overflow = nullptr;   // pinned
 };
 
 State* create(int device, int sm_count) {
@@ -747,7 +791,7 @@ static void free_weights(State* s) {
   cudaFree(s->d_blob);
   for (auto& p : s->d_wf) { cudaFree(p); p = nullptr; }
   for (auto& p : s->d_bias) { cudaFree(p); p = nullptr; }
-  for (auto& t : s->tc) { cudaFree(t.whi); cudaFree(t.wlo); t = TcLayer(); }
+  for (auto& t : s->tc) { cudaFree(t.whi); cudaFree(t.wlo); cudaFree(t.inv_scale); t = TcLayer(); }
   cudaFree(s->d_wf6); cudaFree(s->d_head); cudaFree(s->d_offs);
   s->d_blob = s->d_wf6 = s->d_head = nullptr;
   s->d_offs = nullptr;
@@ -758,6 +802,8 @@ void destroy(State* s) {
   free_acts(s);
   free_weights(s);
   for (auto e : s->ev) if (e) cudaEventDestroy(e);
+  cudaFree(s->d_overflow);
+  cudaFreeHost(s->h_overflow);
   delete s;
 }
 
@@ -802,6 +848,7 @@ int set_weights(State* s, const float* blob, size_t n, cudaStream_t st, std::str
       const size_t cnt = (size_t)L[l].k * L[l].k * s->tc[l].nout * 64;
       CNN_TRY(cudaMalloc(&s->tc[l].whi, cnt * sizeof(__half)));
       CNN_TRY(cudaMalloc(&s->tc[l].wlo, cnt * sizeof(__half)));
+      CNN_TRY(cudaMalloc(&s->tc[l].inv_scale, L[l].cout * sizeof(float)));
     }
     CNN_TRY(cudaMalloc(&s->d_head, head_floats(net) * sizeof(float)));
     CNN_TRY(cudaMalloc(&s->d_offs, 8 * sizeof(size_t)));
@@ -819,9 +866,11 @@ int set_weights(State* s, const float* blob, size_t n, cudaStream_t st, std::str
     const float* bn = w + (size_t)L[l].cout * L[l].cin * kk;
     // fp32 folded weights (first layer + the CUDA-core check path) and biases
     fold_conv_kernel<<<256, 256, 0, st>>>(w, bn, L[l].cout, L[l].cin, kk, l < 5 ? s->d_wf[l] : s->d_wf6, s->d_bias[l]);
-    if (l >= 1)
-      fold_tc_kernel<<<256, 256, 0, st>>>(w, bn, L[l].cout, L[l].cin, kk, s->tc[l].nout, s->tc[l].whi, s->tc[l].wlo,
-                                          s->d_bias[l]);
+    if (l >= 1) {
+      tc_scale_kernel<<<L[l].cout, 256, 0, st>>>(w, bn, L[l].cout, L[l].cin, kk, s->tc[l].inv_scale);
+      fold_tc_kernel<<<256, 256, 0, st>>>(w, bn, L[l].cout, L[l].cin, kk, s->tc[l].nout, s->tc[l].inv_scale, s->tc[l].whi,
+                                          s->tc[l].wlo, s->d_bias[l]);
+    }
   }
   HeadDims hd;
   for (int l = 0; l < 8; ++l) { hd.cin[l] = L[6 + l].cin; hd.cout[l] = L[6 + l].cout; }
@@ -884,8 +933,8 @@ static int launch_tc(State* s, int layer, __half* ahi, __half* alo, int H, int W
   if (!s->attrs_set) CNN_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
   const int OH = H - KS + 1, OW = W - KS + 1;
   const dim3 grid((OW + kTileX - 1) / kTileX, (OH + kTileY - 1) / kTileY);
-  kern<<<grid, kConvThreads, Cfg::kSmem, st>>>(maps[0], maps[1], maps[2], maps[3], s->d_bias[layer], out, ohi, olo, OH, OW,
-                                               s->layers[layer].cout);
+  kern<<<grid, kConvThreads, Cfg::kSmem, st>>>(maps[0], maps[1], maps[2], maps[3], s->d_bias[layer], s->tc[layer].inv_scale, out,
+                                               ohi, olo, OH, OW, s->layers[layer].cout, s->d_overflow, 1u << layer);
   CNN_TRY(cudaGetLastError());
   return 0;
 }
@@ -926,12 +975,13 @@ static int run_trunk(State* s, const float* d_layer, int pitch, const TrunkDims&
     CNN_TRY(cudaGetLastError());
   } else {
     int rc;
-    conv1_split_kernel<C1><<<g1, 256, 0, st>>>(d_layer, d.H0, d.W0, pitch, s->d_wf[0], s->d_bias[0], s->h1, s->l1);
+    conv1_split_kernel<C1><<<g1, 256, 0, st>>>(d_layer, d.H0, d.W0, pitch, s->d_wf[0], s->d_bias[0], s->h1, s->l1,
+                                               s->d_overflow);
     if ((rc = launch_tc<3, K2, N2, 1, false>(s, 1, s->h1, s->l1, d.H1, d.W1, s->f2, nullptr, nullptr, st, err))) return rc;
-    maxpool_split_kernel<<<g1, 256, 0, st>>>(s->f2, d.H2, d.W2, C1, 2, 2, s->hp2, s->lp2, d.HP2, d.WP2);
+    maxpool_split_kernel<<<g1, 256, 0, st>>>(s->f2, d.H2, d.W2, C1, 2, 2, s->hp2, s->lp2, d.HP2, d.WP2, s->d_overflow, 1u << 1);
     if ((rc = launch_tc<3, K2, C3, 1, true>(s, 2, s->hp2, s->lp2, d.HP2, d.WP2, nullptr, s->h3, s->l3, st, err))) return rc;
     if ((rc = launch_tc<3, K4, C3, 1, false>(s, 3, s->h3, s->l3, d.H3, d.W3, s->f4, nullptr, nullptr, st, err))) return rc;
-    maxpool_split_kernel<<<g1, 256, 0, st>>>(s->f4, d.H4, d.W4, C3, 3, 1, s->hp4, s->lp4, d.HP4, d.WP4);
+    maxpool_split_kernel<<<g1, 256, 0, st>>>(s->f4, d.H4, d.W4, C3, 3, 1, s->hp4, s->lp4, d.HP4, d.WP4, s->d_overflow, 1u << 3);
     if ((rc = launch_tc<3, K4, C3, 1, true>(s, 4, s->hp4, s->lp4, d.HP4, d.WP4, nullptr, s->h5, s->l5, st, err))) return rc;
     CNN_TRY(cudaGetLastError());
     CNN_TRY(cudaEventRecord(s->ev[1], st));
@@ -975,11 +1025,28 @@ int update_features(State* s, const float* d_layer, int rows, int cols, int pitc
     s->maps_valid = false;
   }
   if (!s->ev[0]) for (auto& e : s->ev) CNN_TRY(cudaEventCreate(&e));
+  if (!s->d_overflow) {
+    CNN_TRY(cudaMalloc(&s->d_overflow, sizeof(unsigned)));
+    CNN_TRY(cudaMallocHost(&s->h_overflow, sizeof(unsigned)));
+  }
+  s->has_features = false;
+  CNN_TRY(cudaMemsetAsync(s->d_overflow, 0, sizeof(unsigned), st));
   const int rc = s->net == kNetFull ? run_trunk<kNetFull>(s, d_layer, pitch, d, st, use_cuda_core_path, err)
                                     : run_trunk<kNetLight>(s, d_layer, pitch, d, st, use_cuda_core_path, err);
   if (rc) return rc;
   CNN_TRY(cudaEventRecord(s->ev[3], st));
+  CNN_TRY(cudaMemcpyAsync(s->h_overflow, s->d_overflow, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
   CNN_TRY(cudaStreamSynchronize(st));
+  if (*s->h_overflow) {
+    // The tensor-core path holds activations as fp16 hi + lo: beyond 65504 the split has no representation, and the
+    // features would silently be inf / NaN. The CUDA-core path (artp_set_cnn_mode bit 0) has fp32 range throughout.
+    int l = 0;
+    while (!(*s->h_overflow & (1u << l))) ++l;
+    err = std::string("motion-cost trunk: an activation of ") + kSplitLayerNames[l] +
+          " exceeds the fp16 range (65504) of the tensor-core path's hi/lo split; the elevation or weight scale is out of "
+          "range for it (the CUDA-core path, artp_set_cnn_mode bit 0, has fp32 range)";
+    return -4;
+  }
   cudaEventElapsedTime(&s->last_ms[0], s->ev[0], s->ev[1]);   // layers 1..5
   cudaEventElapsedTime(&s->last_ms[1], s->ev[2], s->ev[3]);   // 15x15 layer
   cudaEventElapsedTime(&s->last_ms[2], s->ev[0], s->ev[3]);   // whole trunk

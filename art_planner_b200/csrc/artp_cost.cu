@@ -227,7 +227,9 @@ int artp_set_cost_weights(artp_handle* hh, const float* blob, size_t n_floats) {
 int artp_update_features(artp_handle* hh) {
   LOCK_HANDLE(h, hh);
   TRY(require_whole_map(h));
-  return artp_cnn::update_features(h->cnn, h->d_H[0], h->rows, h->cols, h->pitch, h->chk.Lx / h->rows, h->chk.cx, h->chk.cy,
+  // The resolution as artp_set_map received it: the head's row / column bias truncates (rows * res) / res like the
+  // reference, and Lx / rows may differ from res in the last bit, which moves that truncation (e.g. 116 rows at 0.04).
+  return artp_cnn::update_features(h->cnn, h->d_H[0], h->rows, h->cols, h->pitch, h->res, h->chk.cx, h->chk.cy,
                                    h->stream, h->cnn_mode & 1, h->err);
 }
 

@@ -437,7 +437,12 @@ int artp_set_cost_weights(artp_handle* h, const float* blob, size_t n_floats);
 /* The architecture of the loaded weights (ARTP_COST_NET_*); ARTP_E_NOWEIGHTS before any artp_set_cost_weights. */
 int artp_get_cost_network(artp_handle* h, int* network);
 /* CostPredictor.updateFeatures (predictor.py:28-36): run the CNN trunk over the `elevation` layer of the current map
- * (orientation as cost_query_server.py:74). Call after artp_set_map whenever the map changed. */
+ * (orientation as cost_query_server.py:74). Call after artp_set_map whenever the map changed.
+ * The tensor-core path (the default artp_set_cnn_mode) stores the activations of init_conv1..5 as fp16 hi + lo pairs.
+ * If one of them exceeds the fp16 range (|a| > 65504, e.g. raw elevations thousands of metres from the frame's origin
+ * with weights calibrated near zero height), the call returns ARTP_E_LIMIT, artp_last_error() names the layer, and
+ * the handle holds no features (cost queries return ARTP_E_NOWEIGHTS until an update succeeds). The CUDA-core path
+ * (artp_set_cnn_mode bit 0) has fp32 range and never raises it. DESIGN.md section 4.3 gives the supported ranges. */
 int artp_update_features(artp_handle* h);
 /* GPUCostQueryServer.handle_cost_query_no_update (cost_query_server.py:120-141) = CostQuery.__call__: edges n x 6 floats
  * [target_x, target_y, target_yaw, start_x, start_y, start_yaw] in the map frame -> cost3 n x 3 floats
