@@ -55,6 +55,15 @@ class ArtpRoadmapParams(C.Structure):
 
 
 ARTP_ROADMAP_MILESTONE, ARTP_ROADMAP_INTERPOLATED, ARTP_ROADMAP_QUERY = 1, 2, 4
+ARTP_ROADMAP_EDGE_VALID, ARTP_ROADMAP_EDGE_REMOVED = 1, 2
+(ARTP_SOLVE_SOLVED, ARTP_SOLVE_NOT_CONNECTED, ARTP_SOLVE_NO_FEASIBLE_PATH, ARTP_SOLVE_INVALID_START,
+ ARTP_SOLVE_INVALID_GOAL) = 1, 2, 3, 4, 5
+
+
+class ArtpRoadmapSolveInfo(C.Structure):
+    _fields_ = [("status", C.c_int32), ("searches", C.c_uint32), ("sweeps", C.c_uint32), ("edges_checked", C.c_uint32),
+                ("edges_removed", C.c_uint32), ("start_vertex", C.c_uint32), ("goal_vertex", C.c_uint32),
+                ("path_vertices", C.c_void_p)]
 
 
 class ArtpStats(C.Structure):
@@ -131,6 +140,10 @@ def load():
     lib.artp_roadmap_sample_graph.argtypes = [vp, C.POINTER(ArtpRoadmapParams), C.POINTER(ArtpSampleDistributionParams), u64, u64,
                                               C.POINTER(u64)]
     lib.artp_roadmap_get.argtypes = [vp, sz, vp, vp, sz, vp, C.POINTER(sz), C.POINTER(sz)]
+    lib.artp_roadmap_update_edges.argtypes = [vp]
+    lib.artp_roadmap_solve.argtypes = [vp, vp, vp, C.POINTER(ArtpSe3Space), vp, sz, C.POINTER(sz), C.POINTER(dbl),
+                                       C.POINTER(ArtpRoadmapSolveInfo)]
+    lib.artp_roadmap_get_edge_costs.argtypes = [vp, sz, vp, vp, C.POINTER(sz)]
     lib.artp_host_alloc.restype = C.c_void_p
     lib.artp_host_alloc.argtypes = [sz]
     lib.artp_host_free.argtypes = [vp]

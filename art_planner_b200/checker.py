@@ -474,7 +474,12 @@ class PRMRoadmap:
     """PRMMotionCost's roadmap built on the device (prm_motion_cost.cpp:145-219, 236-247, 325-390): addValidMilestone with
     KStarStrategy's k nearest, the interior states of every connection at <= 0.5 m lateral spacing, and the valid prefixes
     as chains of vertices and edges. vertices() / edges() copy the store out in the order the reference's Boost graph
-    numbers them; edges carry no cost (price them with MotionCostObjective.updateEdgesBatch)."""
+    numbers them. updateEdges() prices the edges in place with the loaded motion-cost network, solve() answers a query
+    on the device, edgeCosts() copies the weights and flags out."""
+
+    EDGE_VALID, EDGE_REMOVED = capi.ARTP_ROADMAP_EDGE_VALID, capi.ARTP_ROADMAP_EDGE_REMOVED
+    SOLVED, NOT_CONNECTED, NO_FEASIBLE_PATH = capi.ARTP_SOLVE_SOLVED, capi.ARTP_SOLVE_NOT_CONNECTED, capi.ARTP_SOLVE_NO_FEASIBLE_PATH
+    INVALID_START, INVALID_GOAL = capi.ARTP_SOLVE_INVALID_START, capi.ARTP_SOLVE_INVALID_GOAL
 
     MILESTONE, INTERPOLATED, QUERY = capi.ARTP_ROADMAP_MILESTONE, capi.ARTP_ROADMAP_INTERPOLATED, capi.ARTP_ROADMAP_QUERY
 
@@ -533,6 +538,37 @@ class PRMRoadmap:
         e = np.empty((max(ne - int(first), 0), 2), np.uint32)
         h.check(h.lib.artp_roadmap_get(h.h, 0, None, None, int(first), e.ctypes.data, None, None))
         return e
+
+    def updateEdges(self) -> None:
+        """PRMMotionCostMaintainer::updateEdges (:27-73) over the whole store, on the device."""
+        h = self._c.handle
+        h.check(h.lib.artp_roadmap_update_edges(h.h))
+
+    def solve(self, start, goal, space, path_capacity: int = 4096):
+        """One query (clearQuery + PRMMotionCost::baseSolve) on the device. space: MotionValidator.se3Space(...).
+        Returns (status, path states [n, 7] from start to goal, their vertex indices [n], cost, info); the path is empty
+        unless status == SOLVED. info: searches, sweeps, edges_checked, edges_removed, start_vertex, goal_vertex."""
+        h = self._c.handle
+        a = np.ascontiguousarray(start, dtype=np.float64).reshape(7)
+        b = np.ascontiguousarray(goal, dtype=np.float64).reshape(7)
+        states, idx = np.empty((int(path_capacity), 7), np.float64), np.empty(int(path_capacity), np.uint32)
+        n, cost = C.c_size_t(0), C.c_double(0.0)
+        info = capi.ArtpRoadmapSolveInfo()
+        info.path_vertices = idx.ctypes.data
+        h.check(h.lib.artp_roadmap_solve(h.h, a.ctypes.data, b.ctypes.data, C.byref(space), states.ctypes.data, int(path_capacity),
+                                         C.byref(n), C.byref(cost), C.byref(info)))
+        out = {k: int(getattr(info, k)) for k in ("searches", "sweeps", "edges_checked", "edges_removed", "start_vertex", "goal_vertex")}
+        return int(info.status), states[:n.value].copy(), idx[:n.value].copy(), float(cost.value), out
+
+    def edgeCosts(self, first: int = 0):
+        """(cost float64 [E - first], flags uint8 [E - first] of EDGE_VALID / EDGE_REMOVED, live edges in the store)."""
+        h = self._c.handle
+        _, ne = self.counts()
+        m = max(ne - int(first), 0)
+        cost, flags = np.empty(m, np.float64), np.empty(m, np.uint8)
+        live = C.c_size_t(0)
+        h.check(h.lib.artp_roadmap_get_edge_costs(h.h, int(first), cost.ctypes.data, flags.ctypes.data, C.byref(live)))
+        return cost, flags, live.value
 
 
 class StartState:

@@ -67,6 +67,39 @@ __global__ void combine_cost_kernel(const float* __restrict__ cost3, size_t n, f
   }
 }
 
+// Rows of roadmap edges straight from the store (updateEdges :35-48, computeCostForVertexEdges :85-118). Without a list,
+// row i is edge i from its stored source u to its target v. With one, row i < *count is edge (list[i] & 0x7FFFFFFF),
+// reversed (from v to u) when bit 31 is set; rows from *count on are zero (the head prices them, nothing reads the result).
+__global__ void store_rows_kernel(const double* __restrict__ states, const uint32_t* __restrict__ edges,
+                                  const uint32_t* __restrict__ list, const uint32_t* __restrict__ count, size_t n,
+                                  float* __restrict__ rows) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    if (list && i >= *count) {
+      for (int k = 0; k < 6; ++k) rows[6 * i + k] = 0.0f;
+      continue;
+    }
+    const uint32_t e = list ? list[i] & 0x7FFFFFFFu : (uint32_t)i;
+    const bool flip = list && (list[i] >> 31);
+    const uint32_t u = edges[2 * (size_t)e], v = edges[2 * (size_t)e + 1];
+    knot_row(states + 7 * (size_t)(flip ? u : v), rows + 6 * i);
+    knot_row(states + 7 * (size_t)(flip ? v : u), rows + 6 * i + 3);
+  }
+}
+// The weights of those edges: getCost, or +inf above the risk threshold. updateEdges (no list) also marks the feasible
+// edges valid (:51-55); computeCostForVertexEdges (a list) leaves validity alone (:121-125).
+__global__ void store_cost_kernel(const float* __restrict__ cost3, const uint32_t* __restrict__ list,
+                                  const uint32_t* __restrict__ count, size_t n, float we, float wt, float wr, float thr,
+                                  double* __restrict__ ecost, uint8_t* __restrict__ eflag) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    if (list && i >= *count) continue;
+    const uint32_t e = list ? list[i] & 0x7FFFFFFFu : (uint32_t)i;
+    const float ce = cost3[3 * i], ct = cost3[3 * i + 1], cr = cost3[3 * i + 2];
+    const bool ok = (double)cr <= (double)thr;
+    ecost[e] = ok ? get_cost(ce, ct, cr, we, wt, wr) : CUDART_INF;
+    if (!list && ok) eflag[e] |= ARTP_ROADMAP_EDGE_VALID;
+  }
+}
+
 // MotionCostObjective::motionCost (motion_cost_objective.cpp:36-95) splits edge e into the pieces piece_off[e] ..
 // piece_off[e+1] - 1 (n_interp + 1 of them). Knot j of the edge is s1 for j = 0, s2 for j = n_interp + 1 (copied, not
 // interpolated) and interpolate(s1, s2, j * (1.0 / (n_interp + 1))) in between (:49, :67); piece i's row is
@@ -145,6 +178,18 @@ int motion_cost_split(Handle* h, const double* d_s1, const double* d_s2, size_t 
 }
 
 }  // namespace
+
+int artp_api::price_store_edges(Handle* h, const double* d_states, const uint32_t* d_edges, const uint32_t* d_list,
+                                const uint32_t* d_count, size_t n, float* d_rows, float* d_cost3, double* d_ecost,
+                                uint8_t* d_eflag, cudaStream_t s) {
+  TRY(check_cost_net(h));
+  if (n == 0) return ARTP_OK;
+  const unsigned grid = grid_for(h, n, 256, 8);
+  TRY(launch(h, store_rows_kernel, grid, 256, 0, s, d_states, d_edges, d_list, d_count, n, d_rows));
+  TRY(launch_cost_head(h, d_rows, n, d_cost3, s));
+  return launch(h, store_cost_kernel, grid, 256, 0, s, (const float*)d_cost3, d_list, d_count, n, h->p.cost_w_energy,
+                h->p.cost_w_time, h->p.cost_w_risk, h->p.risk_threshold, d_ecost, d_eflag);
+}
 
 static_assert(ARTP_COST_NET_LIGHT == artp_cnn::kNetLight && ARTP_COST_NET_FULL == artp_cnn::kNetFull,
               "the ABI's network numbers are the library's");

@@ -288,6 +288,15 @@ int check_distribution_args(Handle* h, const artp_sample_distribution_params* dp
 int update_distribution_rearm(Handle* h, const artp_sample_distribution_params* dp, const double* d_states, size_t n,
                               cudaStream_t s);
 
+// artp_cost.cu, for the roadmap:
+// The loaded network's weights of roadmap edges on s, from the store's states and (u, v) pairs into d_ecost / d_eflag:
+// edges 0 .. n-1 in their stored direction, feasible ones marked valid (updateEdges), or, with d_list, the first *d_count
+// (at most n) listed edges in the listed direction, validity untouched (computeCostForVertexEdges). d_rows: n x 6 floats,
+// d_cost3: n x 3 floats of scratch. ARTP_E_NOWEIGHTS without weights and features.
+int price_store_edges(Handle* h, const double* d_states, const uint32_t* d_edges, const uint32_t* d_list,
+                      const uint32_t* d_count, size_t n, float* d_rows, float* d_cost3, double* d_ecost, uint8_t* d_eflag,
+                      cudaStream_t s);
+
 // artp_roadmap.cu: releases the roadmap store (artp_destroy).
 void roadmap_free(Handle* h);
 

@@ -1,12 +1,14 @@
 // art_planner_b200/csrc/artp_roadmap.cu -- the PRM roadmap of the C ABI (include/artp.h): PRMMotionCost's graph
 // construction (art_planner/src/planners/prm_motion_cost.cpp) on the device. The store and the per-milestone kernels are
 // in artp_roadmap.cuh; the interior states go through the latency path's per-pose routine (check_states_cta) and the
-// sampler and the distribution through artp_sampling.cu (artp_internal.h).
+// sampler and the distribution through artp_sampling.cu (artp_internal.h). Queries (artp_roadmap_query.cuh) price the
+// edges through artp_cost.cu and search and validate paths without leaving the device.
 #include <cmath>
 #include <vector>
 
 #include "artp_internal.h"
 #include "artp_roadmap.cuh"
+#include "artp_roadmap_query.cuh"
 
 using namespace artp_api;
 
@@ -24,6 +26,10 @@ struct Roadmap {
   size_t icap = 0;                     // interior-state buffer, in states
   double lo[2] = {0, 0}, hi[2] = {0, 0};   // (x, y) box of every milestone so far: bounds n_interp
   bool has_box = false;
+  artp::QueryDev q{};                  // adjacency, path and validation round of artp_roadmap_solve
+  artp::QueryCtl* h_q = nullptr;       // pinned: the query's control block as the last solve left it
+  uint32_t* d_path_idx = nullptr;      // vcap: the solution's vertex indices from start to goal
+  bool search_smem = false;            // roadmap_search_kernel may use its dynamic shared memory
 };
 
 }  // namespace artp_api
@@ -45,8 +51,12 @@ void free_store(Roadmap* r) {
   artp::RoadmapDev& d = r->dev;
   for (void* p : {(void*)d.ctl, (void*)d.states, (void*)d.kind, (void*)d.edges, (void*)d.dens, (void*)d.k_of_v, (void*)d.dist,
                   (void*)d.nbr, (void*)d.n_interp, (void*)d.off, (void*)d.interior, (void*)d.valid, (void*)d.milestone,
-                  (void*)r->d_cand, (void*)r->d_draws, (void*)r->d_count, (void*)r->d_dens_states})
+                  (void*)r->d_cand, (void*)r->d_draws, (void*)r->d_count, (void*)r->d_dens_states, (void*)d.ecost, (void*)d.eflag,
+                  (void*)r->q.ctl, (void*)r->q.csr_off, (void*)r->q.csr_len, (void*)r->q.csr_nbr, (void*)r->q.csr_eid,
+                  (void*)r->q.path, (void*)r->q.path_e, (void*)r->q.plist, (void*)r->q.chk_e, (void*)r->q.chk_s1,
+                  (void*)r->q.chk_s2, (void*)r->q.chk_off, (void*)r->d_path_idx})
     cudaFree(p);
+  if (r->h_q) cudaFreeHost(r->h_q);
   if (r->h_ctl) cudaFreeHost(r->h_ctl);
   if (r->h_count) cudaFreeHost(r->h_count);
   if (r->h_draws) cudaFreeHost(r->h_draws);
@@ -163,6 +173,23 @@ int artp_roadmap_clear(artp_handle* hh, size_t vertex_capacity, size_t edge_capa
     TRY(dev_alloc(h, r->d_draws, kMaxRound));
     TRY(dev_alloc(h, r->d_count, 1));
     TRY(dev_alloc(h, r->d_dens_states, vertex_capacity * 7));
+    TRY(dev_alloc(h, d.ecost, edge_capacity));
+    TRY(dev_alloc(h, d.eflag, edge_capacity));
+    artp::QueryDev& q = r->q;
+    TRY(dev_alloc(h, q.ctl, 1));
+    TRY(dev_alloc(h, q.csr_off, vertex_capacity + 1));
+    TRY(dev_alloc(h, q.csr_len, vertex_capacity));
+    TRY(dev_alloc(h, q.csr_nbr, edge_capacity * 2));
+    TRY(dev_alloc(h, q.csr_eid, edge_capacity * 2));
+    TRY(dev_alloc(h, q.path, vertex_capacity));
+    TRY(dev_alloc(h, q.path_e, vertex_capacity));
+    TRY(dev_alloc(h, q.plist, (size_t)kcap + 2));
+    TRY(dev_alloc(h, q.chk_e, (size_t)artp::kQueryBatch));
+    TRY(dev_alloc(h, q.chk_s1, (size_t)artp::kQueryBatch));
+    TRY(dev_alloc(h, q.chk_s2, (size_t)artp::kQueryBatch));
+    TRY(dev_alloc(h, q.chk_off, (size_t)artp::kQueryBatch + 1));
+    TRY(dev_alloc(h, r->d_path_idx, vertex_capacity));
+    CU_TRY(h, cudaHostAlloc((void**)&r->h_q, sizeof(artp::QueryCtl), cudaHostAllocDefault));
     CU_TRY(h, cudaHostAlloc((void**)&r->h_ctl, sizeof(artp::RoadmapCtl), cudaHostAllocDefault));
     CU_TRY(h, cudaHostAlloc((void**)&r->h_count, sizeof(uint32_t), cudaHostAllocDefault));
     CU_TRY(h, cudaHostAlloc((void**)&r->h_draws, kMaxRound * sizeof(uint64_t), cudaHostAllocDefault));
@@ -177,6 +204,9 @@ int artp_roadmap_clear(artp_handle* hh, size_t vertex_capacity, size_t edge_capa
   r->has_box = false;
   TRY(put_ctl(h, r, h->stream));
   CU_TRY(h, cudaMemsetAsync(d.dens, 0, vertex_capacity, h->stream));
+  // a new edge weighs ob::Cost() = 0.0 with validity unknown until it is priced
+  CU_TRY(h, cudaMemsetAsync(d.ecost, 0, edge_capacity * sizeof(double), h->stream));
+  CU_TRY(h, cudaMemsetAsync(d.eflag, 0, edge_capacity, h->stream));
   return host_call_end(h);
 }
 
@@ -229,12 +259,12 @@ int artp_roadmap_sample_graph(artp_handle* hh, const artp_roadmap_params* rp, co
   uint64_t draw = first_sample;
   double accept = 0.5, v_per = 1.0, e_per = 1.0;   // running estimates: they size a round, never change its result
   int rc = ARTP_OK;
-  while (rc == ARTP_OK && c.V < max_v && c.E < max_e && draw < end) {
+  while (rc == ARTP_OK && c.V < max_v && c.E - c.n_removed < max_e && draw < end) {   // num_edges(g_): live edges
     // at most this many milestones before a stop rule fires: each adds >= 1 vertex
     uint64_t room = max_v - c.V;
     if (recompute_n) room = std::min<uint64_t>(room, (uint64_t)recompute_n * (c.n_proc + 1) > c.V
                                                          ? (uint64_t)recompute_n * (c.n_proc + 1) - c.V : 1);
-    const double guess = std::min((double)room / v_per, (double)(max_e - c.E) / e_per);
+    const double guess = std::min((double)room / v_per, (double)(max_e - (c.E - c.n_removed)) / e_per);
     const size_t B = (size_t)std::max<double>(1.0, std::min<double>({std::ceil(guess) + 4.0, (double)room, (double)kMaxRound}));
     const uint64_t n_draw = std::min<uint64_t>(end - draw, (uint64_t)std::max(4096.0, 1.25 * (double)B / accept));
     if ((rc = sample_valid_draws(h, seed, draw, (size_t)n_draw, r->d_cand, r->d_draws, B, r->d_count, s))) break;
@@ -290,6 +320,156 @@ int artp_roadmap_get(artp_handle* hh, size_t first_vertex, double* states, uint8
     CU_TRY(h, cudaMemcpyAsync(edges, r->dev.edges + first_edge * 2, te * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
   if (nv) *nv = V;
   if (ne) *ne = E;
+  return host_call_end(h);
+}
+
+int artp_roadmap_update_edges(artp_handle* hh) {
+  LOCK_CALL(h, hh);
+  TRY(require_roadmap(h));
+  Roadmap* r = h->roadmap;
+  const size_t E = r->h_ctl->E;
+  char* reg[2];   // edge rows | cost3
+  TRY(host_call_begin(h, {E * 6 * sizeof(float), E * 3 * sizeof(float)}, reg));
+  TRY(price_store_edges(h, r->dev.states, r->dev.edges, nullptr, nullptr, E, (float*)reg[0], (float*)reg[1], r->dev.ecost,
+                        r->dev.eflag, h->stream));
+  return host_call_end(h);
+}
+
+int artp_roadmap_solve(artp_handle* hh, const double* start, const double* goal, const artp_se3_space* space,
+                       double* path_states, size_t path_capacity, size_t* n_path, double* cost,
+                       artp_roadmap_solve_info* info) {
+  LOCK_CALL(h, hh);
+  TRY(require_roadmap(h));
+  TRY(require_whole_map(h));
+  if (!start || !goal || !space) return null_buffer(h);
+  Roadmap* r = h->roadmap;
+  artp::QueryDev& q = r->q;
+  for (int i = 0; i < 7; ++i)
+    if (!std::isfinite(start[i]) || !std::isfinite(goal[i])) { h->err = "non-finite start or goal"; return ARTP_E_INVALID; }
+  // the segment lengths of artp_valid_segment_count
+  const double frac = space->longest_valid_segment_fraction > 0 ? space->longest_valid_segment_fraction : 0.01;
+  double e2 = 0;
+  for (int i = 0; i < 3; ++i) e2 += (space->high[i] - space->low[i]) * (space->high[i] - space->low[i]);
+  q.seg_r3 = std::sqrt(e2) * frac;
+  q.seg_so3 = 0.5 * 3.14159265358979323846 * frac;
+  if (!(q.seg_r3 > 0)) { h->err = "bad SE3 space parameters"; return ARTP_E_INVALID; }
+  if (r->dev.vcap > artp::kSearchCtas * artp::kSearchSliceMax) {
+    h->err = "roadmap too large for the on-chip search (vertex capacity above 77440)"; return ARTP_E_LIMIT;
+  }
+  // A cost query without weights fails before the roadmap changes (the check artp_roadmap_update_edges makes).
+  TRY(price_store_edges(h, nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr, h->stream));
+  if (n_path) *n_path = 0;
+  artp_roadmap_solve_info out{};
+  out.path_vertices = info ? info->path_vertices : nullptr;
+  // SE3StateSpace::satisfiesBounds: the position inside the RealVectorBounds
+  for (int w = 0; w < 2; ++w)
+    for (int i = 0; i < 3; ++i) {
+      const double x = (w ? goal : start)[i];
+      if (x < space->low[i] || x > space->high[i]) {
+        out.status = w ? ARTP_SOLVE_INVALID_GOAL : ARTP_SOLVE_INVALID_START;
+        if (info) *info = out;
+        return ARTP_OK;
+      }
+    }
+  grow_box(r, start[0], start[1], start[0], start[1]);
+  grow_box(r, goal[0], goal[1], goal[0], goal[1]);
+  TRY(fit_interior(h, r));
+  q.qcap = (uint32_t)std::min<size_t>(r->icap, artp::kQueryBatch);
+  const uint32_t slice_cap = (r->dev.vcap + artp::kSearchCtas - 1) / artp::kSearchCtas;
+  const size_t search_smem = ((size_t)slice_cap * artp::kSearchVertexBytes + 7) & ~(size_t)7;
+  if (!r->search_smem) {
+    CU_TRY(h, cudaFuncSetAttribute(artp::roadmap_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)(artp::kSearchSliceMax * artp::kSearchVertexBytes)));
+    r->search_smem = true;
+  }
+  const size_t n_price = (size_t)r->dev.kcap + 2, out_cap = std::min<size_t>(path_capacity, r->dev.vcap);
+  char* reg[4];   // start, goal | edge rows | cost3 | path states
+  TRY(host_call_begin(h, {14 * sizeof(double), n_price * 6 * sizeof(float), n_price * 3 * sizeof(float),
+                          out_cap * 7 * sizeof(double)}, reg));
+  cudaStream_t s = h->stream;
+  const double* d_sg = (const double*)reg[0];
+  CU_TRY(h, cudaMemcpyAsync(reg[0], start, 7 * sizeof(double), cudaMemcpyHostToDevice, s));
+  CU_TRY(h, cudaMemcpyAsync(reg[0] + 7 * sizeof(double), goal, 7 * sizeof(double), cudaMemcpyHostToDevice, s));
+  TRY(put_ctl(h, r, s));
+  *r->h_q = artp::QueryCtl{};
+  r->h_q->two = 2;
+  CU_TRY(h, cudaMemcpyAsync(q.ctl, r->h_q, sizeof(artp::QueryCtl), cudaMemcpyHostToDevice, s));
+  CU_TRY(h, cudaMemsetAsync(q.csr_len, 0, (size_t)r->dev.vcap * sizeof(uint32_t), s));
+  const unsigned vgrid = grid_for(h, r->dev.vcap, 256, 4), egrid = grid_for(h, r->dev.ecap, 256, 4);
+  int rc = ARTP_OK;
+  auto step = [&](int x) { if (rc == ARTP_OK) rc = x; };
+  // the pose check of both ends, clearQuery, the two milestones
+  step(check_states_cta(h, d_sg, &q.ctl->two, &r->dev.ctl->stop, 2, q.ctl->pose_ok, s));
+  step(launch(h, artp::query_begin_kernel, vgrid, 256, 0, s, r->dev, q));
+  for (int w = 0; w < 2 && rc == ARTP_OK; ++w) {
+    step(launch(h, artp::query_mark_kernel, 1, 1, 0, s, r->dev, q, w));
+    step(queue_milestone(h, r, d_sg, (uint32_t)w, ARTP_ROADMAP_MILESTONE | ARTP_ROADMAP_QUERY, s));
+  }
+  // the adjacency, then the edges at the start and at the goal, in that order (:484-485)
+  step(launch(h, artp::csr_count_kernel, egrid, 256, 0, s, r->dev, q));
+  step(launch(h, artp::csr_scan_kernel, 1, 1024, 0, s, r->dev, q));
+  step(launch(h, artp::csr_fill_kernel, egrid, 256, 0, s, r->dev, q));
+  step(launch(h, artp::csr_sort_kernel, vgrid, 256, 0, s, r->dev, q));
+  for (int w = 0; w < 2 && rc == ARTP_OK; ++w) {
+    step(launch(h, artp::query_price_list_kernel, 1, 256, 0, s, r->dev, q, w));
+    step(price_store_edges(h, r->dev.states, r->dev.edges, q.plist, &q.ctl->n_price, n_price, (float*)reg[1], (float*)reg[2],
+                           r->dev.ecost, r->dev.eflag, s));
+  }
+  // do constructSolution while (!solution && sameComponent(start, goal)) (:508-512): rounds of search and validation,
+  // queued four at a time; the kernels of a round that is not due return at once.
+  const uint64_t max_rounds = (uint64_t)r->dev.ecap + r->dev.vcap + 8;   // a round removes an edge, validates one or ends
+  for (uint64_t round = 0; rc == ARTP_OK;) {
+    for (int k = 0; k < 4 && rc == ARTP_OK; ++k, ++round) {
+      step(launch(h, artp::roadmap_search_kernel, artp::kSearchCtas, artp::kSearchThreads, search_smem, s, r->dev, q, slice_cap));
+      step(launch(h, artp::query_gather_kernel, 1, 256, 0, s, r->dev, q));
+      step(check_states_cta(h, r->dev.interior, &q.ctl->n_check, &q.ctl->idle, q.qcap, r->dev.valid, s));
+      step(launch(h, artp::query_apply_kernel, 1, 256, 0, s, r->dev, q));
+    }
+    if (rc != ARTP_OK) break;
+    step(get_ctl(h, r, s));
+    CU_TRY(h, cudaMemcpyAsync(r->h_q, q.ctl, sizeof(artp::QueryCtl), cudaMemcpyDeviceToHost, s));
+    CU_TRY(h, cudaStreamSynchronize(s));
+    if (r->h_q->status != artp::Q_RUNNING || r->h_ctl->stop) break;
+    if (round > max_rounds) { h->err = "query did not end"; rc = ARTP_E_LIMIT; }
+  }
+  const artp::QueryCtl& c = *r->h_q;
+  if (rc == ARTP_OK && c.status == ARTP_SOLVE_SOLVED) {
+    step(launch(h, artp::query_finish_kernel, 1, 256, 0, s, r->dev, q, r->d_path_idx, (double*)reg[3], (uint32_t)out_cap));
+    if (rc == ARTP_OK) {
+      CU_TRY(h, cudaMemcpyAsync(r->h_q, q.ctl, sizeof(artp::QueryCtl), cudaMemcpyDeviceToHost, s));
+      const size_t n = c.path_n;   // read by the rounds' copy: the finish kernel does not change it
+      if (n <= path_capacity) {
+        if (path_states) CU_TRY(h, cudaMemcpyAsync(path_states, reg[3], n * 7 * sizeof(double), cudaMemcpyDeviceToHost, s));
+        if (out.path_vertices)
+          CU_TRY(h, cudaMemcpyAsync(out.path_vertices, r->d_path_idx, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+      }
+    }
+  }
+  rc = finish(h, r, rc);
+  if (rc != ARTP_OK) return rc;
+  if (c.status == artp::Q_LIMIT) { h->err = "query exceeded a search or validation bound"; return ARTP_E_LIMIT; }
+  out.status = c.status; out.searches = c.searches; out.sweeps = c.sweeps; out.edges_checked = c.checked;
+  out.edges_removed = c.removed; out.start_vertex = c.start; out.goal_vertex = c.goal;
+  if (info) *info = out;
+  if (c.status != ARTP_SOLVE_SOLVED) return ARTP_OK;
+  if (n_path) *n_path = c.path_n;
+  if (cost) *cost = c.cost;
+  if (c.path_n > path_capacity) { h->err = "path_capacity too small"; return ARTP_E_LIMIT; }
+  return ARTP_OK;
+}
+
+int artp_roadmap_get_edge_costs(artp_handle* hh, size_t first_edge, double* cost, uint8_t* flags, size_t* n_live) {
+  LOCK_CALL(h, hh);
+  TRY(require_roadmap(h));
+  Roadmap* r = h->roadmap;
+  const size_t E = r->h_ctl->E;
+  if (first_edge > E) { h->err = "roadmap cursor past the end"; return ARTP_E_INVALID; }
+  TRY(host_call_begin(h));
+  const size_t te = E - first_edge;
+  if (cost && te)
+    CU_TRY(h, cudaMemcpyAsync(cost, r->dev.ecost + first_edge, te * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (flags && te) CU_TRY(h, cudaMemcpyAsync(flags, r->dev.eflag + first_edge, te, cudaMemcpyDeviceToHost, h->stream));
+  if (n_live) *n_live = E - r->h_ctl->n_removed;
   return host_call_end(h);
 }
 

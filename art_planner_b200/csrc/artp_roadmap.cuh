@@ -22,6 +22,7 @@ enum : uint32_t {
   RM_STOP_RECOMPUTE = 2u,   // V / recompute_density_after_n_samples > n_proc after a milestone (:190-193)
   RM_STOP_FULL = 4u,        // the milestone did not fit the store: not added
   RM_STOP_INTERIOR = 8u,    // the interior states did not fit their buffer: not added
+  RM_STOP_QUERY = 16u,      // artp_roadmap_solve found its start or goal invalid: neither is added
 };
 
 // The roadmap's device control block: counters, the current milestone's connections and the stop rules.
@@ -34,6 +35,7 @@ struct RoadmapCtl {
   uint32_t n_proc;          // recomputes so far (sampleGraph's n_proc)
   uint32_t max_v, max_e;    // stop rules, 0 = off
   uint32_t recompute_n;     // 0 = off
+  uint32_t n_removed;       // edges a query removed (artp_roadmap_query.cuh): E - n_removed are live
 };
 
 struct RoadmapDev {
@@ -53,6 +55,8 @@ struct RoadmapDev {
   uint8_t* valid;           // icap
   uint32_t icap;
   double* milestone;        // 7: the current milestone
+  double* ecost;            // ecap: edge weights (updateEdges / computeCostForVertexEdges); 0.0 until priced
+  uint8_t* eflag;           // ecap: ARTP_ROADMAP_EDGE_* bits
 };
 
 // OMPL 1.4.2 SE3StateSpace::distance = RealVectorStateSpace::distance (sqrt of the running sum of squares) + 1.0 *
@@ -206,7 +210,7 @@ __global__ void __launch_bounds__(kCommitThreads) roadmap_commit_kernel(RoadmapD
         ctl->n_proc += 1;
         stop |= RM_STOP_RECOMPUTE;
       }
-      if (ctl->max_v && !(V1 < ctl->max_v && E1 < ctl->max_e)) stop |= RM_STOP_CAPS;
+      if (ctl->max_v && !(V1 < ctl->max_v && E1 - ctl->n_removed < ctl->max_e)) stop |= RM_STOP_CAPS;   // num_edges(g_): live edges
       ctl->stop = stop;
     }
   }

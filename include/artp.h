@@ -382,7 +382,7 @@ int artp_debug_gaussian_kernel(int ksize, double sigma, float* out);
  *   check       every interior state through the validity pipeline's per-pose routine.
  *   commit      :335-387: the valid prefix of each connection becomes a chain of interpolated vertices and edges, the
  *               final edge only when the whole connection is valid, a direct edge when n_interp == 0.
- * Edges carry no cost: price them with artp_motion_cost_states on the copied-out edges (updateEdges, :27-73).
+ * Edges are priced and searched in place by the query calls below.
  * The map must be the whole map (a map window is ARTP_E_INVALID). A milestone that would overflow the store's capacity
  * is not added and the call returns ARTP_E_LIMIT (the roadmap keeps every earlier milestone). */
 #define ARTP_ROADMAP_MILESTONE     1   /* a milestone (sampled, or added with artp_roadmap_add_milestones) */
@@ -416,6 +416,52 @@ int artp_roadmap_sample_graph(artp_handle* h, const artp_roadmap_params* rp, con
  * the end: ARTP_E_INVALID. */
 int artp_roadmap_get(artp_handle* h, size_t first_vertex, double* states, uint8_t* kinds, size_t first_edge,
                      uint32_t* edges, size_t* nv, size_t* ne);
+
+/* ---- queries on the device roadmap (updateEdges :27-73, computeCostForVertexEdges :77-128, baseSolve :440-532,
+ * constructSolution :536-673) ------------------------------------------------------------------------------------------
+ * Every edge carries a double weight and a flag byte. A never-priced edge weighs 0.0 with no flag (ob::Cost(),
+ * VALIDITY_UNKNOWN). The store stays append-only: an edge a query removes keeps its slot, with the REMOVED flag. */
+#define ARTP_ROADMAP_EDGE_VALID    1   /* VALIDITY_TRUE: priced feasible by artp_roadmap_update_edges, or motion-checked */
+#define ARTP_ROADMAP_EDGE_REMOVED  2   /* removed by constructSolution's failed motion check; not part of the graph */
+/* updateEdges over the whole store: every edge (u, v) is priced by the loaded network from u towards v (row
+ * [v.x v.y yaw(v) u.x u.y yaw(u)], artp_edge_matrix_from_states' arithmetic on the device); weight = getCost and the
+ * VALID flag when the risk is within the threshold, else +inf and the flag untouched. Equal bit for bit to
+ * artp_motion_cost_states on the copied-out edges. No weights or features: ARTP_E_NOWEIGHTS; no roadmap: ARTP_E_INVALID. */
+int artp_roadmap_update_edges(artp_handle* h);
+#define ARTP_SOLVE_SOLVED            1
+#define ARTP_SOLVE_NOT_CONNECTED     2   /* start and goal in different components (baseSolve returns TIMEOUT) */
+#define ARTP_SOLVE_NO_FEASIBLE_PATH  3   /* connected, but not over edges of finite weight ("Could not find solution path") */
+#define ARTP_SOLVE_INVALID_START     4
+#define ARTP_SOLVE_INVALID_GOAL      5
+typedef struct artp_roadmap_solve_info {
+  int32_t  status;                     /* ARTP_SOLVE_* */
+  uint32_t searches;                   /* constructSolution calls (shortest-path searches) */
+  uint32_t sweeps;                     /* relaxation sweeps of all searches */
+  uint32_t edges_checked;              /* edges motion-checked */
+  uint32_t edges_removed;              /* edges removed (failed motion checks) */
+  uint32_t start_vertex, goal_vertex;  /* their vertex indices */
+  uint32_t* path_vertices;             /* in: nullable HOST buffer of path_capacity entries; the path's vertex indices */
+} artp_roadmap_solve_info;
+/* One query, Planner::plan's clearQuery + PRMMotionCost::baseSolve. start, goal: 7 HOST doubles each. A state outside
+ * space's bounds or failing the pose check: status INVALID_START / INVALID_GOAL, the roadmap unchanged. Otherwise the
+ * earlier QUERY vertices lose their QUERY bit, start and goal are added like artp_roadmap_add_milestones, and the edges
+ * at the start, then at the goal, are priced from the query vertex towards its neighbour, validity untouched (an edge
+ * joining the two ends with the goal's direction; the edges between the interpolated vertices of their connections stay
+ * at 0.0). Then, on the device, until a path stands or start and goal are disconnected: distances from the start over
+ * the live edges of finite weight (d[v] = min fl(d[u] + w): what Dijkstra with a zero heuristic computes); the path is
+ * the optimal one with the fewest edges, the lowest predecessor index on ties (Boost leaves ties to its heap); its edges
+ * without the VALID flag are motion-checked from the start-side to the goal-side vertex as artp_check_motions_segments
+ * does (nd from *space), the passing ones become VALID, the first failing one from the goal's side is REMOVED.
+ * path_states: nullable HOST buffer of path_capacity x 7 doubles, start to goal. *n_path: its length; above
+ * path_capacity nothing is written and the call returns ARTP_E_LIMIT. *cost: the sum of the path's weights from the
+ * start, left to right. info: nullable. A vertex capacity above what the search holds on chip (77 440): ARTP_E_LIMIT.
+ * ARTP_E_NOWEIGHTS / ARTP_E_INVALID / ARTP_E_NOMAP as artp_roadmap_update_edges and artp_roadmap_add_milestones. */
+int artp_roadmap_solve(artp_handle* h, const double* start, const double* goal, const artp_se3_space* space,
+                       double* path_states, size_t path_capacity, size_t* n_path, double* cost,
+                       artp_roadmap_solve_info* info);
+/* The weights (doubles) and flags (bytes) of the edges first_edge .. E-1 to HOST buffers (both nullable), like
+ * artp_roadmap_get. *n_live (nullable): edges without the REMOVED flag in the whole store. */
+int artp_roadmap_get_edge_costs(artp_handle* h, size_t first_edge, double* cost, uint8_t* flags, size_t* n_live);
 
 /* ---- learned motion cost (MotionCostFunc, objectives/motion_cost_objective.h:22-23) ------------------------------
  * Weights: ONE flat fp32 blob in the layer order of the reference's `network` module: init_conv1..5, init_flatten,

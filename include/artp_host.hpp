@@ -369,7 +369,9 @@ class SE3FromSE2Sampler {
 
 // PRMMotionCost's roadmap built on the device (prm_motion_cost.cpp:145-219, 236-247, 325-390; include/artp.h): the store
 // keeps g_'s insertion order, so vertex i of vertices() is the i-th vertex the reference's addValidMilestone adds.
-// Edges carry no cost: price them with MotionCostObjective::updateEdgesBatch.
+// updateEdges / solve / edgeCosts price, search and validate in place. With -DARTP_WITH_OMPL, PRMMotionCost::solve maps onto
+// them as: sampleGraph (which ends in updateEdges, :209) -> sampleGraph(); updateEdges(), and baseSolve after
+// Planner::plan's clearQuery -> solve(start, goal, space); the PathGeometric is built from the returned states.
 class PRMRoadmap {
  public:
   explicit PRMRoadmap(const StateValidityCheckerPtr& checker, size_t vertex_capacity = 60000, size_t edge_capacity = 60000)
@@ -425,6 +427,45 @@ class PRMRoadmap {
   void counts(size_t* nv, size_t* ne) const {
     const auto& h = checker_->handle();
     h->check(artp_roadmap_get(h->get(), 0, nullptr, nullptr, 0, nullptr, nv, ne), "artp_roadmap_get");
+  }
+  // PRMMotionCostMaintainer::updateEdges (:27-73) over the whole store, on the device.
+  void updateEdges() {
+    const auto& h = checker_->handle();
+    h->check(artp_roadmap_update_edges(h->get()), "artp_roadmap_update_edges");
+  }
+  // One query (clearQuery + PRMMotionCost::baseSolve) on the device. Returns info.status (ARTP_SOLVE_*); path and
+  // path_vertices hold the solution from start to goal when it is ARTP_SOLVE_SOLVED, and are empty otherwise.
+  struct Solution {
+    std::vector<State> path;
+    std::vector<uint32_t> path_vertices;
+    double cost = 0.0;
+    artp_roadmap_solve_info info{};
+  };
+  int solve(const State& start, const State& goal, const artp_se3_space& space, Solution* out, size_t path_capacity = 4096) {
+    const auto& h = checker_->handle();
+    out->path.resize(path_capacity);
+    out->path_vertices.resize(path_capacity);
+    out->info = artp_roadmap_solve_info{};
+    out->info.path_vertices = out->path_vertices.data();
+    size_t n = 0;
+    h->check(artp_roadmap_solve(h->get(), &start.x, &goal.x, &space, &out->path[0].x, path_capacity, &n, &out->cost, &out->info),
+             "artp_roadmap_solve");
+    out->path.resize(n);
+    out->path_vertices.resize(n);
+    out->info.path_vertices = nullptr;
+    return out->info.status;
+  }
+  // The weights and ARTP_ROADMAP_EDGE_* flags of the edges first .. E-1; returns the live edges of the whole store.
+  size_t edgeCosts(size_t first, std::vector<double>* cost, std::vector<uint8_t>* flags) const {
+    size_t nv = 0, ne = 0, live = 0;
+    counts(&nv, &ne);
+    const size_t n = ne > first ? ne - first : 0;
+    cost->resize(n);
+    flags->resize(n);
+    const auto& h = checker_->handle();
+    h->check(artp_roadmap_get_edge_costs(h->get(), first, n ? cost->data() : nullptr, n ? flags->data() : nullptr, &live),
+             "artp_roadmap_get_edge_costs");
+    return live;
   }
  private:
   StateValidityCheckerPtr checker_;
