@@ -194,67 +194,101 @@ __global__ void fill_u8_kernel(uint8_t* p, size_t n, uint8_t v) {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] = v;
 }
 
-// Ordered compaction: (A) per-block counts, (B) single-block exclusive scan, (C) scatter.
-constexpr int kCompactBlock = 1024;
+// Ordered compaction in one pass: a single-pass scan with decoupled look-back (Merrill & Garland 2016). Each CTA takes the
+// next tile of kCompactTile items from a counter, so a tile only ever waits on tiles whose CTAs are already running. Warp w of
+// a tile owns kCompactRounds consecutive runs of 32 items; a run's 32 flags are one ballot (one word of a bit-packed mask),
+// which gives the in-tile ranks. The CTA publishes its tile's count (AGGREGATE), then warp 0 sums the statuses of the
+// preceding tiles back to the nearest INCLUSIVE one and publishes the tile's inclusive prefix; the scatter then writes the
+// indices in item order. Status word of a tile: epoch (bits 34-63) | flag (bits 32-33) | value (bits 0-31). A status of
+// another epoch (an earlier call) reads as not yet published, so the states need no reset between calls. Word 0 of the
+// state array is the tile counter; the CTA that draws the last tile sets it back to 0 and writes the count.
+constexpr int kCompactThreads = 256, kCompactRounds = 16;
+constexpr int kCompactTile = kCompactThreads * kCompactRounds;   // 4096 items
+constexpr unsigned long long kTileAggregate = 1ull << 32, kTileInclusive = 2ull << 32, kTileFlags = 3ull << 32;
+constexpr uint32_t kCompactEpochs = 1u << 30;
 // BITS: the mask is bit-packed (item i = bit i&31 of word i>>5, artp_pack_valid_bits_device), else one byte per item.
-template <bool BITS>
-__device__ __forceinline__ int mask_at(const uint8_t* __restrict__ valid, size_t i) {
-  if (BITS) return (int)((reinterpret_cast<const uint32_t*>(valid)[i >> 5] >> (i & 31)) & 1u);
-  return valid[i] != 0;
-}
-template <bool BITS>
-__global__ void compact_count_kernel(const uint8_t* __restrict__ valid, size_t n, uint32_t* __restrict__ counts) {
-  const size_t i = (size_t)blockIdx.x * kCompactBlock + threadIdx.x;
-  const int v = (i < n) && mask_at<BITS>(valid, i);
-  const int c = __syncthreads_count(v);
-  if (threadIdx.x == 0) counts[blockIdx.x] = (uint32_t)c;
-}
-__global__ void compact_scan_kernel(uint32_t* counts, size_t nb, uint32_t* total) {
-  __shared__ uint32_t carry;
-  __shared__ uint32_t wsum[32];
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  for (size_t b0 = 0; b0 < nb; b0 += blockDim.x) {
-    const size_t i = b0 + threadIdx.x;
-    const uint32_t v = i < nb ? counts[i] : 0u;
-    uint32_t x = v;
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-    if (lane == 31) wsum[wid] = x;
-    __syncthreads();
-    if (wid == 0) {
-      uint32_t s = lane < (int)(blockDim.x >> 5) ? wsum[lane] : 0u;
-      for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, s, o); if (lane >= o) s += y; }
-      wsum[lane] = s;
-    }
-    __syncthreads();
-    const uint32_t before = carry + (wid ? wsum[wid - 1] : 0u) + x - v;
-    if (i < nb) counts[i] = before;
-    __syncthreads();
-    if (threadIdx.x == blockDim.x - 1) carry = before + v;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *total = carry;
-}
 template <bool BITS, typename IndexT>
-__global__ void compact_scatter_kernel(const uint8_t* __restrict__ valid, size_t n, int64_t base,
-                                       const uint32_t* __restrict__ offsets, IndexT* __restrict__ out) {
-  __shared__ uint32_t wsum[32];
-  const size_t i = (size_t)blockIdx.x * kCompactBlock + threadIdx.x;
-  const int v = (i < n) && mask_at<BITS>(valid, i);
-  const unsigned bal = __ballot_sync(0xffffffffu, v);
+__global__ void __launch_bounds__(kCompactThreads)
+compact_kernel(const uint8_t* __restrict__ valid, size_t n, int64_t base, unsigned long long* __restrict__ state, uint32_t epoch,
+               IndexT* __restrict__ out, uint32_t* __restrict__ count) {
+  __shared__ uint32_t s_tile, s_before;
+  __shared__ uint32_t wsum[kCompactThreads / 32];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (lane == 0) wsum[wid] = __popc(bal);
-  __syncthreads();
-  if (wid == 0) {
-    uint32_t s = wsum[lane];
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, s, o); if (lane >= o) s += y; }
-    wsum[lane] = s;
+  const size_t ntiles = (n + kCompactTile - 1) / kCompactTile;
+  if (threadIdx.x == 0) {
+    s_tile = (uint32_t)atomicAdd(state, 1ull);
+    if (s_tile == ntiles - 1) *state = 0ull;   // every other CTA has drawn its tile: ready for the next call
   }
   __syncthreads();
-  if (v) {
-    const uint32_t pos = offsets[blockIdx.x] + (wid ? wsum[wid - 1] : 0u) + __popc(bal & ((1u << lane) - 1u));
-    out[pos] = (IndexT)(base + (int64_t)i);
+  const uint32_t tile = s_tile;
+  const size_t run0 = (size_t)tile * kCompactTile + (size_t)wid * 32 * kCompactRounds;   // first item of this warp's runs
+  uint32_t bal[kCompactRounds];
+  if (BITS) {
+    const uint32_t* words = reinterpret_cast<const uint32_t*>(valid);
+    const size_t wi = (run0 >> 5) + lane;
+    uint32_t mine = 0;
+    if (lane < kCompactRounds && wi < (n + 31) / 32) {
+      mine = words[wi];
+      if (n - 32 * wi < 32) mine &= (1u << (n - 32 * wi)) - 1u;   // bits past n are not items
+    }
+#pragma unroll
+    for (int r = 0; r < kCompactRounds; ++r) bal[r] = __shfl_sync(0xffffffffu, mine, r);
+  } else {
+    uint8_t v[kCompactRounds];
+#pragma unroll
+    for (int r = 0; r < kCompactRounds; ++r) {
+      const size_t i = run0 + 32 * r + lane;
+      v[r] = i < n ? valid[i] : 0;
+    }
+#pragma unroll
+    for (int r = 0; r < kCompactRounds; ++r) bal[r] = __ballot_sync(0xffffffffu, v[r] != 0);
+  }
+  uint32_t wtot = 0;
+#pragma unroll
+  for (int r = 0; r < kCompactRounds; ++r) wtot += __popc(bal[r]);
+  if (lane == 0) wsum[wid] = wtot;
+  __syncthreads();
+  const unsigned long long tag = (unsigned long long)epoch << 34;
+  volatile unsigned long long* st = state + 1;
+  if (wid == 0) {
+    uint32_t x = lane < kCompactThreads / 32 ? wsum[lane] : 0u;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+    if (lane < kCompactThreads / 32) wsum[lane] = x;   // inclusive prefix over the warps
+    const uint32_t agg = __shfl_sync(0xffffffffu, x, kCompactThreads / 32 - 1);
+    uint32_t before = 0;
+    if (tile == 0) {
+      if (lane == 0) st[0] = tag | kTileInclusive | agg;
+    } else {
+      if (lane == 0) st[tile] = tag | kTileAggregate | agg;
+      for (long long j = (long long)tile - 1;; j -= 32) {   // lane k reads tile j - k
+        const long long t = j - lane;
+        unsigned long long s;
+        do {
+          s = t >= 0 ? st[t] : (tag | kTileInclusive);
+        } while (__any_sync(0xffffffffu, (s >> 34) != epoch || !(s & kTileFlags)));
+        const unsigned inc = __ballot_sync(0xffffffffu, (s & kTileFlags) == kTileInclusive);
+        const int stop = inc ? __ffs(inc) - 1 : 31;   // the nearest inclusive prefix ends the look-back
+        uint32_t v = lane <= stop ? (uint32_t)s : 0u;
+#pragma unroll
+        for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        before += v;
+        if (inc) break;
+      }
+      if (lane == 0) st[tile] = tag | kTileInclusive | (uint32_t)(before + agg);
+    }
+    if (lane == 0) {
+      s_before = before;
+      if (tile == ntiles - 1) *count = before + agg;
+    }
+  }
+  __syncthreads();
+  uint32_t pos = s_before + (wid ? wsum[wid - 1] : 0u);
+  const unsigned lt = (1u << lane) - 1u;
+#pragma unroll
+  for (int r = 0; r < kCompactRounds; ++r) {
+    if ((bal[r] >> lane) & 1u) out[pos + __popc(bal[r] & lt)] = (IndexT)(base + (int64_t)(run0 + 32 * r + lane));
+    pos += __popc(bal[r]);
   }
 }
 
@@ -362,8 +396,11 @@ int launch_grouping(Handle* h, artp::Work w, size_t lo, size_t hi, cudaStream_t 
 
 // Device round: the items [base, end) are on the device. Classify, the three box kernels, then the grouping stage. The box
 // kernels only ever clear verdicts of different boxes, so the two reach kernels fork onto box_stream / group_stream after
-// the classify stage and join before the grouping stage (each kernel has a latency floor of 20-30 us). With stage timing
-// on, everything runs in order on s, and a timed round records the per-stage events.
+// the classify stage (each kernel has a latency floor of 20-30 us), and the big-tile kernel onto tile_stream, whose greatest
+// priority gets its CTAs onto the SMs before the 8-lane kernel fills them (on the default priority it started after the
+// 8-lane kernel in about half of the steps and ended last). The grouping stage waits for tile_stream and box_stream only;
+// group_stream joins s after it. With stage timing on, everything runs in order on s, and a timed round records the
+// per-stage events.
 int run_round_device(Handle* h, const artp::Work& w, cudaStream_t s, size_t base, size_t end, bool timed) {
   CU_TRY(h, cudaMemsetAsync(h->d_ctr, 0, sizeof(Counters), s));
   if (timed) CU_TRY(h, cudaEventRecord(h->ev[0], s));
@@ -372,26 +409,32 @@ int run_round_device(Handle* h, const artp::Work& w, cudaStream_t s, size_t base
   const bool fork = !h->timing && h->chk.reach_tw;
   if (fork) {
     CU_TRY(h, cudaEventRecord(h->slice_ev[0], s));
+    CU_TRY(h, cudaStreamWaitEvent(h->tile_stream, h->slice_ev[0], 0));
     CU_TRY(h, cudaStreamWaitEvent(h->box_stream, h->slice_ev[0], 0));
     if (h->group_grid) CU_TRY(h, cudaStreamWaitEvent(h->group_stream, h->slice_ev[0], 0));
   }
   BoxQueues* q = &h->d_ctr->q;
-  TRY(launch_big_tile(h, w, base, end, q, s));
+  TRY(launch_big_tile(h, w, base, end, q, fork ? h->tile_stream : s));
   if (timed) CU_TRY(h, cudaEventRecord(h->ev[2], s));
   TRY(launch_reach_warp(h, w, base, end, q, fork ? h->box_stream : s, UINT_MAX));
   if (timed) CU_TRY(h, cudaEventRecord(h->ev[3], s));
   TRY(launch_reach_groups(h, w, base, end, q, fork ? h->group_stream : s, UINT_MAX));
   if (fork) {
+    // The grouping stage reads the defer list, which only the two box_tiles_warp_kernel launches (tile_stream,
+    // box_stream) write. reach_groups_kernel defers nothing, and it and the grouping stage only ever clear verdict bytes
+    // of different boxes, so the grouping stage need not wait for it: group_stream joins s after the grouping launch.
+    CU_TRY(h, cudaEventRecord(h->tile_ev, h->tile_stream));
+    CU_TRY(h, cudaStreamWaitEvent(s, h->tile_ev, 0));
     CU_TRY(h, cudaEventRecord(h->box_ev, h->box_stream));
     CU_TRY(h, cudaStreamWaitEvent(s, h->box_ev, 0));
-    if (h->group_grid) {
-      CU_TRY(h, cudaEventRecord(h->group_ev, h->group_stream));
-      CU_TRY(h, cudaStreamWaitEvent(s, h->group_ev, 0));
-    }
   }
   if (timed) CU_TRY(h, cudaEventRecord(h->ev[4], s));
   TRY(launch_grouping(h, w, base, end, s));
   if (timed) { CU_TRY(h, cudaEventRecord(h->ev[5], s)); h->ev_valid = true; }
+  if (fork && h->group_grid) {
+    CU_TRY(h, cudaEventRecord(h->group_ev, h->group_stream));
+    CU_TRY(h, cudaStreamWaitEvent(s, h->group_ev, 0));
+  }
   return ARTP_OK;
 }
 
@@ -661,19 +704,23 @@ int artp_api::compact_valid(Handle* h, const uint8_t* d_valid, size_t n, int64_t
   if (n == 0) { CU_TRY(h, cudaMemsetAsync(d_count, 0, sizeof(uint32_t), s)); return ARTP_OK; }
   ChainScope cs(h, 1, s);
   if (cs.rc) return cs.rc;
-  const size_t nb = (n + kCompactBlock - 1) / kCompactBlock;
-  TRY(grow(h, h->d_block_counts, h->block_counts_cap, nb));
-  TRY(bits ? launch(h, compact_count_kernel<true>, (unsigned)nb, kCompactBlock, 0, s, d_valid, n, h->d_block_counts)
-           : launch(h, compact_count_kernel<false>, (unsigned)nb, kCompactBlock, 0, s, d_valid, n, h->d_block_counts));
-  TRY(launch(h, compact_scan_kernel, 1, 1024, 0, s, h->d_block_counts, nb, d_count));
+  const size_t nt = (n + kCompactTile - 1) / kCompactTile;
+  if (h->compact_state_cap < nt + 1 || h->compact_epoch + 1 >= kCompactEpochs) {
+    // a new array, or the epochs wrapped: clear it once (word 0, the tile counter, included)
+    TRY(grow(h, h->d_compact_state, h->compact_state_cap, nt + 1));
+    CU_TRY(h, cudaMemsetAsync(h->d_compact_state, 0, h->compact_state_cap * sizeof(unsigned long long), s));
+    h->compact_epoch = 0;
+  }
+  const uint32_t epoch = ++h->compact_epoch;
+  unsigned long long* st = h->d_compact_state;
   if (bits)
-    return launch(h, compact_scatter_kernel<true, int64_t>, (unsigned)nb, kCompactBlock, 0, s, d_valid, n, base, h->d_block_counts,
-                  (int64_t*)d_indices);
+    return launch(h, compact_kernel<true, int64_t>, (unsigned)nt, kCompactThreads, 0, s, d_valid, n, base, st, epoch,
+                  (int64_t*)d_indices, d_count);
   if (u32)
-    return launch(h, compact_scatter_kernel<false, uint32_t>, (unsigned)nb, kCompactBlock, 0, s, d_valid, n, base,
-                  h->d_block_counts, (uint32_t*)d_indices);
-  return launch(h, compact_scatter_kernel<false, int64_t>, (unsigned)nb, kCompactBlock, 0, s, d_valid, n, base, h->d_block_counts,
-                (int64_t*)d_indices);
+    return launch(h, compact_kernel<false, uint32_t>, (unsigned)nt, kCompactThreads, 0, s, d_valid, n, base, st, epoch,
+                  (uint32_t*)d_indices, d_count);
+  return launch(h, compact_kernel<false, int64_t>, (unsigned)nt, kCompactThreads, 0, s, d_valid, n, base, st, epoch,
+                (int64_t*)d_indices, d_count);
 }
 
 extern "C" {
@@ -717,7 +764,12 @@ int artp_create(const artp_params* params, artp_handle** out) {
     return fail("no usable kernel image (built for sm_90a)", e);
   for (cudaStream_t* st : {&h->stream, &h->copy_stream, &h->box_stream, &h->group_stream})
     if ((e = cudaStreamCreateWithFlags(st, cudaStreamNonBlocking)) != cudaSuccess) return fail("cudaStreamCreate", e);
+  int prio_least = 0, prio_greatest = 0;
+  if ((e = cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest)) != cudaSuccess) return fail("cudaDeviceGetStreamPriorityRange", e);
+  if ((e = cudaStreamCreateWithPriority(&h->tile_stream, cudaStreamNonBlocking, prio_greatest)) != cudaSuccess)
+    return fail("cudaStreamCreateWithPriority", e);
   if ((e = cudaEventCreateWithFlags(&h->group_ev, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
+  if ((e = cudaEventCreateWithFlags(&h->tile_ev, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
   for (int i = 0; i < kMaxSlices; ++i) {
     if ((e = cudaEventCreateWithFlags(&h->copy_ev[i], cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
     if ((e = cudaEventCreateWithFlags(&h->slice_ev[i], cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
@@ -752,7 +804,9 @@ void artp_destroy(artp_handle* hh) {
   if (h->copy_stream) { cudaStreamSynchronize(h->copy_stream); cudaStreamDestroy(h->copy_stream); }
   if (h->box_stream) { cudaStreamSynchronize(h->box_stream); cudaStreamDestroy(h->box_stream); }
   if (h->group_stream) { cudaStreamSynchronize(h->group_stream); cudaStreamDestroy(h->group_stream); }
+  if (h->tile_stream) { cudaStreamSynchronize(h->tile_stream); cudaStreamDestroy(h->tile_stream); }
   if (h->group_ev) cudaEventDestroy(h->group_ev);
+  if (h->tile_ev) cudaEventDestroy(h->tile_ev);
   for (int i = 0; i < kMaxSlices; ++i) {
     if (h->copy_ev[i]) cudaEventDestroy(h->copy_ev[i]);
     if (h->slice_ev[i]) cudaEventDestroy(h->slice_ev[i]);
@@ -761,7 +815,7 @@ void artp_destroy(artp_handle* hh) {
   cudaFree(h->d_slices);
   for (int k = 0; k < 2; ++k) for (int l = 0; l <= artp::kMaxLevel; ++l) { cudaFree(h->d_T[k][l]); cudaFree(h->d_C[k][l]); }
   cudaFree(h->d_H[0]); cudaFree(h->d_H[1]); cudaFree(h->d_ctr); cudaFree(h->d_defer); cudaFree(h->d_stage);
-  cudaFree(h->d_block_counts); cudaFree(h->d_recs); cudaFree(h->d_recs_f); cudaFree(h->d_recs_g); cudaFree(h->d_samp_layers); cudaFree(h->d_samp_scratch);
+  cudaFree(h->d_compact_state); cudaFree(h->d_recs); cudaFree(h->d_recs_f); cudaFree(h->d_recs_g); cudaFree(h->d_samp_layers); cudaFree(h->d_samp_scratch);
   cudaFree(h->d_dist_layers); cudaFree(h->d_dist_scratch); cudaFree(h->d_basic_keep);
   roadmap_free(h);
   if (h->h_small_out) cudaFreeHost(h->h_small_out);

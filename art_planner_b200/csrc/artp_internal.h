@@ -67,14 +67,17 @@ struct Handle {
   artp::BoxRec* d_recs_g = nullptr; // classify -> reach-box queue of the 8-lane-group kernel (all-finite, merge-free zones)
   int group_grid = 0, group_smem = 0;
   size_t recs_cap = 0;
-  uint32_t* d_block_counts = nullptr;
-  size_t block_counts_cap = 0;
+  unsigned long long* d_compact_state = nullptr;   // compaction: tile counter, then one status word per tile (compact_kernel)
+  size_t compact_state_cap = 0;
+  uint32_t compact_epoch = 0;       // epoch of the last compaction's tile statuses
   char* d_stage = nullptr;          // device staging for the host-buffer API
   size_t stage_cap = 0;
   cudaStream_t stream = nullptr;    // internal compute stream for the host-buffer API
   cudaStream_t copy_stream = nullptr;   // H2D slices of the host-buffer API
   cudaStream_t group_stream = nullptr;  // the 8-lane-group kernel of slice i (host-fed rounds), beside the other box kernels
   cudaEvent_t group_ev = nullptr;
+  cudaStream_t tile_stream = nullptr;   // device rounds: the big-tile kernel, at the greatest stream priority
+  cudaEvent_t tile_ev = nullptr;
   cudaStream_t box_stream = nullptr;    // box stages of slice i, concurrent with the copy + classify of slice i + 1
   cudaEvent_t copy_ev[kMaxSlices] = {};    // H2D of slice i landed (the call's stream waits on it)
   cudaEvent_t slice_ev[kMaxSlices] = {};   // classify of slice i done (box_stream waits on it)
@@ -115,7 +118,7 @@ struct Handle {
   // Cross-stream ordering of the per-handle scratch (ADVICE r1): calls may come on different streams; every call that
   // uses a scratch group first makes its stream wait for the previous user of that group, and records an event after.
   // group 0: d_ctr / d_recs / d_defer / d_stage / d_samp_scratch / d_dist_scratch (check, sampler, distribution);
-  // group 1: d_block_counts (compaction)
+  // group 1: d_compact_state (compaction)
   cudaEvent_t chain_ev[2] = {nullptr, nullptr};
   cudaStream_t chain_stream[2] = {nullptr, nullptr};
   bool chain_busy[2] = {false, false};
