@@ -66,6 +66,18 @@ class ArtpRoadmapSolveInfo(C.Structure):
                 ("path_vertices", C.c_void_p)]
 
 
+ARTP_OBJ_LEARNED, ARTP_OBJ_PATH_LENGTH, ARTP_OBJ_NONE = 0, 1, 2
+ARTP_SIMPLIFY_MAX_STATES = 4096
+
+
+class ArtpSimplifyInfo(C.Structure):
+    _fields_ = [(n, C.c_uint32) for n in (
+        "n_in", "n_simplified", "n_out", "reduce_edits", "collapse_edits", "shortcut_edits", "bspline_edits",
+        "motion_checks", "state_checks", "rounds", "discarded")] + [
+        ("check_passed", C.c_int32), ("returned_simplified", C.c_int32), ("cost_original", C.c_double),
+        ("cost_simplified", C.c_double)]
+
+
 class ArtpStats(C.Structure):
     _fields_ = [("poses_checked", C.c_uint64), ("poses_deferred", C.c_uint64), ("kernel_launches", C.c_uint64),
                 ("last_deferred", C.c_uint32), ("last_launches", C.c_uint32), ("last_queued_boxes", C.c_uint32),
@@ -144,6 +156,9 @@ def load():
     lib.artp_roadmap_solve.argtypes = [vp, vp, vp, C.POINTER(ArtpSe3Space), vp, sz, C.POINTER(sz), C.POINTER(dbl),
                                        C.POINTER(ArtpRoadmapSolveInfo)]
     lib.artp_roadmap_get_edge_costs.argtypes = [vp, sz, vp, vp, C.POINTER(sz)]
+    lib.artp_debug_se3_ops.argtypes = [vp, vp, vp, vp, sz, vp, vp]
+    lib.artp_simplify_path.argtypes = [vp, vp, sz, C.POINTER(ArtpSe3Space), i32, dbl, u64, vp, sz, C.POINTER(sz),
+                                       C.POINTER(ArtpSimplifyInfo)]
     lib.artp_host_alloc.restype = C.c_void_p
     lib.artp_host_alloc.argtypes = [sz]
     lib.artp_host_free.argtypes = [vp]

@@ -571,6 +571,49 @@ class PRMRoadmap:
         return cost, flags, live.value
 
 
+class PathSimplifier:
+    """OMPL 1.4.2's PathSimplifier::simplifyMax and Planner::getSolutionPath(true) (planner.cpp:266-298) on the device
+    (artp_simplify_path; the rules are oracle/path_simplify_oracle.py's). space: MotionValidator.se3Space(...) -- the
+    motion checks' segment counts. objective: "learned" (MotionCostObjective, needs weights and features) or
+    "path_length" (getObjective's PathLengthObjective): the final comparison's cost. seed: the Philox "ARTS" stream
+    that replaces OMPL's RNG."""
+
+    OBJECTIVES = {"learned": capi.ARTP_OBJ_LEARNED, "path_length": capi.ARTP_OBJ_PATH_LENGTH}
+
+    def __init__(self, checker: StateValidityChecker, space, objective: str = "learned", seed: int = 0,
+                 max_query_edge_length: float = 0.5):
+        self._c = checker
+        self.space = space
+        self.objective = objective
+        self.seed = int(seed)
+        self.max_query_edge_length = float(max_query_edge_length)   # the learned objective's piece length
+
+    def _run(self, path, objective=None):
+        h = self._c.handle
+        p = np.ascontiguousarray(path, dtype=np.float64).reshape(-1, 7)
+        cap = 256 * p.shape[0] + 64      # the longest path the schedule can leave
+        out = np.empty((cap, 7), np.float64)
+        n = C.c_size_t(0)
+        info = capi.ArtpSimplifyInfo()
+        h.check(h.lib.artp_simplify_path(h.h, p.ctypes.data, p.shape[0], C.byref(self.space),
+                                         self.OBJECTIVES[self.objective] if objective is None else objective,
+                                         self.max_query_edge_length, self.seed, out.ctypes.data, cap, C.byref(n), C.byref(info)))
+        d = {k: getattr(info, k) for k, _ in capi.ArtpSimplifyInfo._fields_}
+        return out[:n.value].copy(), {k: (float(v) if isinstance(v, float) else int(v)) for k, v in d.items()}
+
+    def getSolutionPath(self, path, simplify: bool = True):
+        """(states [n, 7], info): the simplified path unless its check fails or the original is strictly cheaper.
+        simplify=False returns the path unchanged (and info None), like the reference's flag."""
+        if not simplify:
+            return np.array(path, dtype=np.float64).reshape(-1, 7), None
+        return self._run(path)
+
+    def simplifyMax(self, path):
+        """(states [n, 7], info): the simplified path whenever it passes the check (no cost comparison), else the
+        original."""
+        return self._run(path, capi.ARTP_OBJ_NONE)
+
+
 class StartState:
     """art_planner::StartState (start.h, start.cpp:7-41): the start pose repaired by a disc search around it, one device
     call per sampleGoal. Offsets come from the Philox "ARTB" stream of `seed`; the draw position advances by what the

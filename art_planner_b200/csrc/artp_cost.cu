@@ -153,12 +153,14 @@ int launch_cost_head(Handle* h, const float* d_edges, size_t n, float* d_cost3, 
   return rc || n == 0 ? rc : count_launch(h);
 }
 
-int path_length_cost(Handle* h, const double* d_s1, const double* d_s2, size_t n, double* d_cost, cudaStream_t s) {
+}  // namespace
+
+int artp_api::path_length_cost(Handle* h, const double* d_s1, const double* d_s2, size_t n, double* d_cost, cudaStream_t s) {
   return launch(h, path_length_kernel, grid_for(h, n, 256, 8), 256, 0, s, d_s1, d_s2, n, d_cost, h->p.use_directional_cost,
                 h->p.max_lon_vel, h->p.max_lat_vel, h->p.max_ang_vel);
 }
 
-int check_cost_net(Handle* h) {
+int artp_api::check_cost_net(Handle* h) {
   if (!artp_cnn::has_weights(h->cnn)) { h->err = "motion-cost weights not set"; return ARTP_E_NOWEIGHTS; }
   if (!artp_cnn::has_features(h->cnn)) {
     h->err = "features not computed (call artp_update_features after artp_set_map)";
@@ -167,17 +169,14 @@ int check_cost_net(Handle* h) {
   return ARTP_OK;
 }
 
-// The split cost of n edges with total_pieces pieces on s: piece rows, the head, the per-edge reduction.
-int motion_cost_split(Handle* h, const double* d_s1, const double* d_s2, size_t n, const uint32_t* d_piece_off, size_t total_pieces,
-                      float* d_rows, float* d_cost3, double* d_cost, cudaStream_t s) {
+int artp_api::motion_cost_split(Handle* h, const double* d_s1, const double* d_s2, size_t n, const uint32_t* d_piece_off, size_t total_pieces,
+                                 float* d_rows, float* d_cost3, double* d_cost, cudaStream_t s) {
   TRY(launch(h, split_rows_kernel, grid_for(h, total_pieces, 256, 8), 256, 0, s, d_s1, d_s2, (uint32_t)n, d_piece_off,
              total_pieces, d_rows));
   TRY(launch_cost_head(h, d_rows, total_pieces, d_cost3, s));
   return launch(h, split_reduce_kernel, grid_for(h, n, 256, 8), 256, 0, s, d_cost3, d_piece_off, n, h->p.cost_w_energy,
                 h->p.cost_w_time, h->p.cost_w_risk, h->p.risk_threshold, d_cost);
 }
-
-}  // namespace
 
 int artp_api::price_store_edges(Handle* h, const double* d_states, const uint32_t* d_edges, const uint32_t* d_list,
                                 const uint32_t* d_count, size_t n, float* d_rows, float* d_cost3, double* d_ecost,

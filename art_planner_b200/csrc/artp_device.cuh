@@ -100,6 +100,42 @@ __device__ __forceinline__ void se3_interpolate(const double* a, const double* b
   }
 }
 
+// OMPL 1.4.2 SE3StateSpace::distance = RealVectorStateSpace::distance (sqrt of the running sum of squares) + 1.0 *
+// SO3StateSpace::distance (arcLength: acos(|q1.q2|), 0 above 1 - MAX_QUATERNION_NORM_ERROR = 1 - 1e-9), in double.
+__device__ __forceinline__ double se3_distance(const double* a, const double* b) {
+  double r = 0.0;
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    const double d = a[i] - b[i];
+    r += d * d;
+  }
+  const double dq = fabs(a[3] * b[3] + a[4] * b[4] + a[5] * b[5] + a[6] * b[6]);
+  const double so3 = dq > 1.0 - 1e-9 ? 0.0 : acos(dq);
+  return sqrt(r) + so3;
+}
+
+// SE3StateSpace::validSegmentCount as artp_valid_segment_count computes it on the host.
+__device__ __forceinline__ uint32_t segment_count(const double* a, const double* b, double seg_r3, double seg_so3) {
+  const double dx = a[0] - b[0], dy = a[1] - b[1], dz = a[2] - b[2];
+  const double d3 = sqrt(dx * dx + dy * dy + dz * dz);
+  const double dq = fabs(a[3] * b[3] + a[4] * b[4] + a[5] * b[5] + a[6] * b[6]);
+  const double ds = dq > 1.0 - 1e-9 ? 0.0 : acos(dq);
+  const unsigned n3 = (unsigned)ceil(d3 / seg_r3), ns = (unsigned)ceil(ds / seg_so3);
+  return max(max(n3, ns), 1u);   // identical states: only s2 is checked
+}
+
+// ---- Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC'11) -------------------------
+__host__ __device__ __forceinline__ void philox4x32_10(uint32_t c[4], uint32_t k0, uint32_t k1) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const uint64_t p0 = (uint64_t)0xD2511F53u * c[0], p1 = (uint64_t)0xCD9E8D57u * c[2];
+    const uint32_t n0 = (uint32_t)(p1 >> 32) ^ c[1] ^ k0, n1 = (uint32_t)p1;
+    const uint32_t n2 = (uint32_t)(p0 >> 32) ^ c[3] ^ k1, n3 = (uint32_t)p0;
+    c[0] = n0; c[1] = n1; c[2] = n2; c[3] = n3;
+    k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
+  }
+}
+
 // getYawFromSO3 (utils.h:80-88) of the quaternion of SE(3) state s: double atan2, returned as `Scalar` = float. On the host
 // atan2 is libm's, on the device CUDA's.
 __host__ __device__ __forceinline__ float so3_yaw(const double* s) {

@@ -109,6 +109,8 @@ struct Handle {
   int basic_rows = 0, basic_cols = 0;
   bool has_basic_layers = false, has_basic_observed = false;
   Roadmap* roadmap = nullptr;       // the PRM roadmap store (artp_roadmap.cu), from the first artp_roadmap_clear
+  char* d_simplify = nullptr;       // artp_simplify_path: state pool, path, round buffers (artp_path_simplify.cu)
+  size_t simplify_cap = 0;
   bool pose_states_smem = false;    // pose_states_kernel may use the latency path's dynamic shared memory
   uint8_t* h_small_out = nullptr;   // mapped pinned host bytes the latency-path kernel writes its verdicts to
   int timing = 0;
@@ -299,6 +301,16 @@ int update_distribution_rearm(Handle* h, const artp_sample_distribution_params* 
 int price_store_edges(Handle* h, const double* d_states, const uint32_t* d_edges, const uint32_t* d_list,
                       const uint32_t* d_count, size_t n, float* d_rows, float* d_cost3, double* d_ecost, uint8_t* d_eflag,
                       cudaStream_t s);
+
+// artp_cost.cu, for the path simplifier:
+// PathLengthObjective::motionCost of n edges (d_s1[i] -> d_s2[i]) into d_cost on s.
+int path_length_cost(Handle* h, const double* d_s1, const double* d_s2, size_t n, double* d_cost, cudaStream_t s);
+// ARTP_E_NOWEIGHTS unless the network has weights and features.
+int check_cost_net(Handle* h);
+// MotionCostObjective::motionCost of n edges with the piece offsets d_piece_off (n + 1, total_pieces in all) on s: piece
+// rows, the head, the per-edge reduction (artp_motion_cost_split_device's work).
+int motion_cost_split(Handle* h, const double* d_s1, const double* d_s2, size_t n, const uint32_t* d_piece_off,
+                      size_t total_pieces, float* d_rows, float* d_cost3, double* d_cost, cudaStream_t s);
 
 // artp_roadmap.cu: releases the roadmap store (artp_destroy).
 void roadmap_free(Handle* h);

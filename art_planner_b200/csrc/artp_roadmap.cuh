@@ -59,20 +59,6 @@ struct RoadmapDev {
   uint8_t* eflag;           // ecap: ARTP_ROADMAP_EDGE_* bits
 };
 
-// OMPL 1.4.2 SE3StateSpace::distance = RealVectorStateSpace::distance (sqrt of the running sum of squares) + 1.0 *
-// SO3StateSpace::distance (arcLength: acos(|q1.q2|), 0 above 1 - MAX_QUATERNION_NORM_ERROR = 1 - 1e-9), in double.
-__device__ __forceinline__ double se3_distance(const double* a, const double* b) {
-  double r = 0.0;
-#pragma unroll
-  for (int i = 0; i < 3; ++i) {
-    const double d = a[i] - b[i];
-    r += d * d;
-  }
-  const double dq = fabs(a[3] * b[3] + a[4] * b[4] + a[5] * b[5] + a[6] * b[6]);
-  const double so3 = dq > 1.0 - 1e-9 ? 0.0 : acos(dq);
-  return sqrt(r) + so3;
-}
-
 // (d, j) orders before (e, k): ascending distance, exact ties by vertex index.
 __device__ __forceinline__ bool nn_before(double d, uint32_t j, double e, uint32_t k) { return d < e || (d == e && j < k); }
 

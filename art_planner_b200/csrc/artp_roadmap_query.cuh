@@ -353,16 +353,6 @@ roadmap_search_kernel(RoadmapDev r, QueryDev q, uint32_t cap) {
 }
 
 // ---- validation ------------------------------------------------------------------------------------------------------
-// SE3StateSpace::validSegmentCount as artp_valid_segment_count computes it on the host.
-__device__ __forceinline__ uint32_t segment_count(const double* a, const double* b, double seg_r3, double seg_so3) {
-  const double dx = a[0] - b[0], dy = a[1] - b[1], dz = a[2] - b[2];
-  const double d3 = sqrt(dx * dx + dy * dy + dz * dz);
-  const double dq = fabs(a[3] * b[3] + a[4] * b[4] + a[5] * b[5] + a[6] * b[6]);
-  const double ds = dq > 1.0 - 1e-9 ? 0.0 : acos(dq);
-  const unsigned n3 = (unsigned)ceil(d3 / seg_r3), ns = (unsigned)ceil(ds / seg_so3);
-  return max(max(n3, ns), 1u);   // identical states: only s2 is checked
-}
-
 // The path's edges without the VALID flag, from the goal's side, as many as fit a round, and the states
 // DiscreteMotionValidator::checkMotion(start-side vertex, goal-side vertex) visits: interpolate(j / nd), j = 1 .. nd - 1,
 // then the goal-side vertex itself.

@@ -17,18 +17,6 @@
 
 namespace artp {
 
-// ---- Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC'11) -------------------------
-__host__ __device__ __forceinline__ void philox4x32_10(uint32_t c[4], uint32_t k0, uint32_t k1) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    const uint64_t p0 = (uint64_t)0xD2511F53u * c[0], p1 = (uint64_t)0xCD9E8D57u * c[2];
-    const uint32_t n0 = (uint32_t)(p1 >> 32) ^ c[1] ^ k0, n1 = (uint32_t)p1;
-    const uint32_t n2 = (uint32_t)(p0 >> 32) ^ c[3] ^ k1, n3 = (uint32_t)p0;
-    c[0] = n0; c[1] = n1; c[2] = n2; c[3] = n3;
-    k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-  }
-}
-
 constexpr uint32_t kSamplerTag = 0x41525450u;   // "ARTP": separates this stream from any other use of the key
 
 // The six uniform01 doubles of sample `idx` under `seed`: words of Philox blocks (idx, b), b = 0..2; each double is

@@ -463,6 +463,80 @@ int artp_roadmap_solve(artp_handle* h, const double* start, const double* goal, 
  * artp_roadmap_get. *n_live (nullable): edges without the REMOVED flag in the whole store. */
 int artp_roadmap_get_edge_costs(artp_handle* h, size_t first_edge, double* cost, uint8_t* flags, size_t* n_live);
 
+/* ---- the solution path simplified on the device (Planner::getSolutionPath(true), planner.cpp:266-298) -------------
+ * OMPL 1.4.2's PathSimplifier::simplifyMax as the simplifier SimpleSetup::simplifySolution builds from the space
+ * information (objective PathLengthOptimizationObjective: cost = SE3StateSpace::distance, combined by +, a < b better; no
+ * goal region, so no findBetterGoal), then getSolutionPath's check and cost comparison. Restated in
+ * oracle/path_simplify_oracle.py, which is the definition; the rules:
+ *   schedule        fewer than 3 states: unchanged. Else reduceVertices; collapseCloseVertices; reduceVertices again
+ *                   while the previous call changed the path, at most 5 more times; shortcutPath while the previous call
+ *                   changed the path, at most 5 times; smoothBSpline(path, 3, length / 100); checkAndRepair's check.
+ *                   Every call of these takes a maxSteps and maxEmptySteps of its entry state count.
+ *   reduceVertices  checkMotion(front, back) first (success: the two states). Else attempts p1 = uniformInt(0, maxN),
+ *                   p2 = uniformInt(max(p1 - range, 0), min(maxN, p1 + range)), range = 1 + floor(0.5 + count * 0.33);
+ *                   |p1 - p2| < 2: p2 = p1 + 2 if p1 < maxN - 1, else p1 - 2 if p1 > 1, else no attempt; a passing
+ *                   checkMotion(states[p1], states[p2]) erases the states between and resets the empty-step count.
+ *   collapseCloseVertices  each step the pair (i, j >= i + 2) of least SE3 distance (first in (i, j) order on ties) not
+ *                   marked: checkMotion passes -> the states between are erased; fails -> the pair is marked for good (the
+ *                   mark belongs to the two states, not their positions).
+ *   shortcutPath    points p0 = uniformReal(0, L), p1 = uniformReal(max(0, p0 - 0.33 L), min(p0 + 0.33 L, L)) along the
+ *                   cumulative distances, each snapped to the next / previous waypoint within L * 0.005, else interpolated
+ *                   on its segment; same or adjacent segments or waypoints: no attempt (OMPL 1.4.2's three tests and the
+ *                   three of later releases, without which 1.4.2 erases a reversed range); checkMotion(s0, s1), then the shortcut is kept
+ *                   unless the cost along the path (partial first segment, whole segments, partial last segment, left to
+ *                   right) is strictly lower than distance(s0, s1); the four edits of OMPL 1.4.2's shortcutPath.
+ *   smoothBSpline   up to 3 steps of: subdivide (the midpoint after every state but the last), then for every even i in
+ *                   [2, n - 1): if isValid(states[i-1]), m = mid(mid(states[i-1], states[i]), mid(states[i], states[i+1]));
+ *                   checkMotion(states[i-1], m) and then checkMotion(m, states[i+1]) pass and distance(states[i], m) >
+ *                   length / 100 (fixed before the first step) -> states[i] = m. A step that replaces nothing ends it.
+ *   check           checkAndRepair's check (both end states valid, then every motion in order) without its repair
+ *                   sampling, then PathGeometric::check (first state valid, every motion in order). Either failing
+ *                   returns the original path (OMPL would try to repair first).
+ *   comparison      PathGeometric::cost of both paths under `objective` (left-to-right sum of motion costs from 0.0); the
+ *                   original is returned only when its cost is strictly lower.
+ *   checkMotion     DiscreteMotionValidator: interpolate(s1, s2, j / nd), j = 1 .. nd - 1, then s2, nd from *space as
+ *                   artp_check_motions_segments computes it; isValid is the pose check.
+ * Randomness: attempt i of the c-th simplifier call of the schedule (from 0, one per call of the five functions above)
+ * takes the two doubles of Philox4x32-10(key = seed, counter = (i, c, 0, "ARTS")), formed as artp_sampler_uniforms forms
+ * them; uniformInt(a, b) = a + min(floor(u * (b - a + 1)), b - a), uniformReal(a, b) = a + u * (b - a). This is not
+ * OMPL's mt19937 stream: same rules, other draws.
+ * The path stays on the device for the whole call; the host reads its control block once per batch of rounds. */
+#define ARTP_OBJ_LEARNED       0   /* MotionCostObjective (planner_ros.cpp:313-317): artp_motion_cost_split's cost at the
+                                      call's max_query_edge_length (params.h:54, 0.5; > 0), +inf above the risk threshold;
+                                      needs weights and features. The argument is read for this objective only. */
+#define ARTP_OBJ_PATH_LENGTH   1   /* getObjective (planner.cpp:27-35): PathLengthObjective at weight 1.0
+                                      (artp_path_length_cost) */
+#define ARTP_OBJ_NONE          2   /* no comparison: the simplified path whenever it passes the check (simplifyMax) */
+#define ARTP_SIMPLIFY_MAX_STATES 4096   /* input states at most (ARTP_E_LIMIT above) */
+typedef struct artp_simplify_info {
+  uint32_t n_in, n_simplified, n_out;   /* states in, after the simplifier, returned */
+  uint32_t reduce_edits;                /* reduceVertices erasures (front-back success included) */
+  uint32_t collapse_edits;              /* collapseCloseVertices erasures */
+  uint32_t shortcut_edits;              /* shortcutPath edits kept */
+  uint32_t bspline_edits;               /* smoothBSpline replacements */
+  uint32_t motion_checks, state_checks; /* checkMotion and isValid calls of the restated schedule and check */
+  uint32_t rounds;                      /* device rounds (gather, pose check, apply) that checked states */
+  uint32_t discarded;                   /* speculative attempts checked in a round after the attempt it applied */
+  int32_t  check_passed;                /* the simplified path passed both checks */
+  int32_t  returned_simplified;         /* 1: the output is the simplified path, 0: the original */
+  double   cost_original, cost_simplified;   /* under `objective`; NaN when the check failed (not compared) */
+} artp_simplify_info;
+/* path: n HOST states (7 doubles each, finite), start to goal. max_query_edge_length: the learned objective's piece
+ * length (MotionCostObjective's, params.h:54), read for ARTP_OBJ_LEARNED only. out: HOST buffer of capacity states; *n_out (nullable) =
+ * the returned path's length; above capacity nothing is written and the call returns ARTP_E_LIMIT. info: nullable.
+ * n == 0, a non-finite state, a bad space or objective, or a map window: ARTP_E_INVALID; no map: ARTP_E_NOMAP;
+ * n > ARTP_SIMPLIFY_MAX_STATES, or one motion of more than 1024 states: ARTP_E_LIMIT (the state pool, 512 n + 64 states,
+ * holds the worst case of the schedule); ARTP_OBJ_LEARNED without weights or features: ARTP_E_NOWEIGHTS (before any work). */
+int artp_simplify_path(artp_handle* h, const double* path, size_t n, const artp_se3_space* space, int objective,
+                       double max_query_edge_length, uint64_t seed, double* out, size_t capacity, size_t* n_out,
+                       artp_simplify_info* info);
+/* TEST HOOK, not part of the planner interface (like the other artp_debug_* entry points): dist[i] = SE3StateSpace::distance(a[i], b[i]) and interp[i] = interpolate(a[i], b[i], t[i]) (HOST buffers)
+ * with the device arithmetic artp_simplify_path uses. Its decisions turn on exact ties (evenly spaced states give equal
+ * distances) that CUDA's acos / sin and libm's may break differently, so a restatement compared with it bit for bit
+ * takes these two functions from here. */
+int artp_debug_se3_ops(artp_handle* h, const double* a, const double* b, const double* t, size_t n, double* dist,
+                       double* interp);
+
 /* ---- learned motion cost (MotionCostFunc, objectives/motion_cost_objective.h:22-23) ------------------------------
  * Weights: ONE flat fp32 blob in the layer order of the reference's `network` module: init_conv1..5, init_flatten,
  * tar0_conv1, out0_conv1, out1_conv1..3 -- each conv.weight [Cout][Cin][kh][kw] followed by its BatchNorm weight, bias,

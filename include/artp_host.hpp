@@ -472,6 +472,47 @@ class PRMRoadmap {
   size_t vertex_capacity_, edge_capacity_;
 };
 
+// Planner::getSolutionPath (planner.cpp:266-298) on the device (artp_simplify_path; the rules are in include/artp.h):
+// OMPL 1.4.2's PathSimplifier::simplifyMax, the check of the simplified path and the strict cost comparison under the
+// planner's objective -- LEARNED (MotionCostObjective, pieces of params().planner.prm_motion_cost.max_query_edge_length;
+// needs weights and features) or PATH_LENGTH (getObjective's PathLengthObjective). The random stream is Philox under
+// `seed`, not OMPL's mt19937. With -DARTP_WITH_OMPL, getSolutionPath(og::PathGeometric) builds the returned path.
+class PathSimplifier {
+ public:
+  enum Objective { LEARNED = ARTP_OBJ_LEARNED, PATH_LENGTH = ARTP_OBJ_PATH_LENGTH };
+  struct Result {
+    std::vector<State> path;    // the returned path: the simplified one, or the original
+    artp_simplify_info info{};  // state counts, edits per stage, checkMotion / isValid counts, check, both costs
+  };
+  PathSimplifier(const StateValidityCheckerPtr& checker, const artp_se3_space& space, Objective objective = LEARNED,
+                 uint64_t seed = 0)
+      : checker_(checker), space_(space), objective_(objective), seed_(seed) {}
+  // getSolutionPath(simplify): without simplify the path comes back unchanged (info zeroed).
+  Result getSolutionPath(const std::vector<State>& path, bool simplify = true) const {
+    if (!simplify) return Result{path, artp_simplify_info{}};
+    return run(path, objective_);
+  }
+  // simplifySolution + the check, without the cost comparison: the simplified path whenever it passes the check.
+  Result simplifyMax(const std::vector<State>& path) const { return run(path, ARTP_OBJ_NONE); }
+  void setSeed(uint64_t seed) { seed_ = seed; }
+ private:
+  Result run(const std::vector<State>& path, int objective) const {
+    const auto& h = checker_->handle();
+    Result r;
+    r.path.resize(256 * path.size() + 64);   // the longest path the schedule can leave
+    size_t n = 0;
+    h->check(artp_simplify_path(h->get(), path.empty() ? nullptr : &path[0].x, path.size(), &space_, objective,
+                                h->params().planner.prm_motion_cost.max_query_edge_length, seed_, &r.path[0].x, r.path.size(),
+                                &n, &r.info), "artp_simplify_path");
+    r.path.resize(n);
+    return r;
+  }
+  StateValidityCheckerPtr checker_;
+  artp_se3_space space_;
+  Objective objective_;
+  uint64_t seed_;
+};
+
 // ompl::base::MotionValidator as the reference uses it: discrete validation over isValid with nd segments.
 class MotionValidator {
  public:
@@ -740,8 +781,10 @@ class MotionCostObjective {
 #include <ompl/base/objectives/PathLengthOptimizationObjective.h>
 #include <ompl/util/RandomNumbers.h>
 #include <ompl/base/spaces/SE3StateSpace.h>
+#include <ompl/geometric/PathGeometric.h>
 namespace artp_host {
 namespace ob = ompl::base;
+namespace og = ompl::geometric;
 inline State fromOmpl(const ob::State* s) {
   const auto* se3 = s->as<ob::SE3StateSpace::StateType>();
   State o;
@@ -806,6 +849,24 @@ class OmplDiscSearchGoal : public ob::GoalState {
 };
 class OmplStartState : public OmplDiscSearchGoal { public: using OmplDiscSearchGoal::OmplDiscSearchGoal; };
 class OmplGoalStateRegion : public OmplDiscSearchGoal { public: using OmplDiscSearchGoal::OmplDiscSearchGoal; };
+
+// Planner::getSolutionPath(simplify) over an og::PathGeometric: the device call, then the returned states as a new path.
+inline og::PathGeometric getSolutionPath(const PathSimplifier& simplifier, const og::PathGeometric& path, bool simplify) {
+  if (!simplify) return path;
+  std::vector<State> in(path.getStateCount());
+  for (size_t i = 0; i < in.size(); ++i) in[i] = fromOmpl(path.getState(i));
+  const PathSimplifier::Result r = simplifier.getSolutionPath(in);
+  og::PathGeometric out(path.getSpaceInformation());
+  ob::State* s = out.getSpaceInformation()->allocState();
+  for (const State& t : r.path) {
+    auto* se3 = s->as<ob::SE3StateSpace::StateType>();
+    se3->setXYZ(t.x, t.y, t.z);
+    se3->rotation().x = t.qx; se3->rotation().y = t.qy; se3->rotation().z = t.qz; se3->rotation().w = t.qw;
+    out.append(s);
+  }
+  out.getSpaceInformation()->freeState(s);
+  return out;
+}
 
 class OmplPathLengthObjective : public ob::PathLengthOptimizationObjective {
  public:
