@@ -4,7 +4,7 @@ edge cost, behind a C ABI (include/artp.h) and a host-side mirror of the referen
 from . import synth  # noqa: F401
 from .capi import ArtpError  # noqa: F401
 from .checker import (GoalStateRegion, MotionCostObjective, MotionValidator, PathLengthObjective,  # noqa: F401
-                      PathSimplifier, PRMRoadmap, SE3FromSE2Sampler, StartState, StateValidityChecker)
+                      PathSimplifier, Planner, PRMRoadmap, SE3FromSE2Sampler, StartState, StateValidityChecker)
 
 __all__ = ["synth", "ArtpError", "StateValidityChecker", "MotionValidator", "PathLengthObjective", "MotionCostObjective", "SE3FromSE2Sampler",
-           "StartState", "GoalStateRegion", "PRMRoadmap", "PathSimplifier"]
+           "StartState", "GoalStateRegion", "PRMRoadmap", "PathSimplifier", "Planner"]

@@ -9,10 +9,11 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libartp.so")
 # (source, extra flags): the geometric kernels need bit-exact fp32 (no FMA contraction, SURVEY.md section 7);
 # the motion-cost network does not.
-# The five units of the C ABI all build rows, costs and states that must equal the host's bit for bit.
+# The six units of the C ABI all build rows, costs and states that must equal the host's bit for bit.
 GEOMETRY_FLAGS = ["-fmad=false", "-Xcompiler", "-fPIC,-ffp-contract=off"]
 SOURCES = [("artp_capi.cu", GEOMETRY_FLAGS), ("artp_sampling.cu", GEOMETRY_FLAGS), ("artp_cost.cu", GEOMETRY_FLAGS),
-           ("artp_roadmap.cu", GEOMETRY_FLAGS), ("artp_path_simplify.cu", GEOMETRY_FLAGS), ("artp_cnn.cu", ["-Xcompiler", "-fPIC"])]
+           ("artp_roadmap.cu", GEOMETRY_FLAGS), ("artp_path_simplify.cu", GEOMETRY_FLAGS),
+           ("artp_planner.cu", GEOMETRY_FLAGS), ("artp_cnn.cu", ["-Xcompiler", "-fPIC"])]
 HEADERS = ["artp_internal.h", "artp_device.cuh", "artp_kernels.cuh", "artp_sampler.cuh", "artp_tiles.cuh", "artp_basic.cuh",
            "artp_distribution.cuh", "artp_roadmap.cuh", "artp_roadmap_query.cuh", "artp_cnn.h", "artp.map", os.path.join("..", "..", "include", "artp.h")]
 # The library exports the C ABI (artp_*) and nothing else.

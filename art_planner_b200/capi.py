@@ -78,6 +78,34 @@ class ArtpSimplifyInfo(C.Structure):
         ("cost_simplified", C.c_double)]
 
 
+ARTP_PLANNER_UNKNOWN, ARTP_PLANNER_INVALID_START, ARTP_PLANNER_INVALID_GOAL, ARTP_PLANNER_NO_MAP, ARTP_PLANNER_NOT_SOLVED, \
+    ARTP_PLANNER_SOLVED = 0, 1, 2, 3, 4, 5
+
+
+class ArtpPlannerParams(C.Structure):
+    _fields_ = [("start_radius", C.c_double), ("goal_radius", C.c_double), ("n_iter", C.c_uint32),
+                ("max_n_vertices", C.c_size_t), ("max_n_edges", C.c_size_t), ("recompute_density_after_n_samples", C.c_size_t),
+                ("max_query_edge_length", C.c_double), ("max_draws", C.c_uint64), ("vertex_capacity", C.c_size_t),
+                ("edge_capacity", C.c_size_t), ("max_roll_pert", C.c_double), ("max_pitch_pert", C.c_double),
+                ("sample_from_distribution", C.c_int), ("use_inverse_vertex_density", C.c_int),
+                ("use_max_prob_unknown_samples", C.c_int), ("max_prob_unknown_samples", C.c_double), ("basic", ArtpBasicParams),
+                ("simplify", C.c_int), ("clear_roadmap", C.c_int), ("seed", C.c_uint64)]
+
+
+class ArtpPlanInfo(C.Structure):
+    _fields_ = [("status", C.c_int32), ("sampled", C.c_int32)] + [(n, C.c_uint64) for n in (
+        "first_sample", "draws_used", "start_draw", "goal_draw", "simplify_seed", "n_vertices", "n_edges")] + [
+        ("solve", ArtpRoadmapSolveInfo), ("path_cost", C.c_double), ("simplify", ArtpSimplifyInfo)] + [
+        (n, C.c_int32) for n in ("goal_clipped", "goal_inside", "start_index", "goal_index")] + [
+        (n, C.c_double * 7) for n in ("goal_clipped_state", "goal_projected", "start_repaired", "goal_repaired")] + [
+        (n, C.c_float) for n in ("ms_sample_graph", "ms_update_edges", "ms_endpoints", "ms_solve", "ms_simplify")] + [
+        ("host_syncs", C.c_uint32), ("bytes_h2d", C.c_uint64), ("bytes_d2h", C.c_uint64)]
+
+
+class ArtpPlannerMapInfo(C.Structure):
+    _fields_ = [("host_syncs", C.c_uint32), ("bytes_h2d", C.c_uint64), ("bytes_d2h", C.c_uint64)]
+
+
 class ArtpStats(C.Structure):
     _fields_ = [("poses_checked", C.c_uint64), ("poses_deferred", C.c_uint64), ("kernel_launches", C.c_uint64),
                 ("last_deferred", C.c_uint32), ("last_launches", C.c_uint32), ("last_queued_boxes", C.c_uint32),
@@ -159,6 +187,10 @@ def load():
     lib.artp_debug_se3_ops.argtypes = [vp, vp, vp, vp, sz, vp, vp]
     lib.artp_simplify_path.argtypes = [vp, vp, sz, C.POINTER(ArtpSe3Space), i32, dbl, u64, vp, sz, C.POINTER(sz),
                                        C.POINTER(ArtpSimplifyInfo)]
+    lib.artp_planner_set_map.argtypes = [vp, C.POINTER(ArtpPlannerParams), vp, vp, vp, vp, i32, i32, dbl, dbl, dbl,
+                                         C.POINTER(ArtpPlannerMapInfo)]
+    lib.artp_planner_get_space.argtypes = [vp, C.POINTER(ArtpSe3Space)]
+    lib.artp_plan.argtypes = [vp, C.POINTER(ArtpPlannerParams), vp, vp, vp, sz, C.POINTER(sz), C.POINTER(ArtpPlanInfo)]
     lib.artp_host_alloc.restype = C.c_void_p
     lib.artp_host_alloc.argtypes = [sz]
     lib.artp_host_free.argtypes = [vp]

@@ -614,6 +614,103 @@ class PathSimplifier:
         return self._run(path, capi.ARTP_OBJ_NONE)
 
 
+class Planner:
+    """art_planner::Planner for planner.name prm_motion_cost (planner.cpp:135-298) on the device: setMap is
+    artp_planner_set_map, plan is artp_plan (with getSolutionPath's simplification when params.simplify), and every stage
+    hands its data to the next in device memory. params: a capi.ArtpPlannerParams (Planner.params() builds one from the
+    shipped values). The learned objective needs MotionCostObjective(checker).setWeights first."""
+
+    UNKNOWN, INVALID_START, INVALID_GOAL, NO_MAP, NOT_SOLVED, SOLVED = range(6)   # PlannerStatus (planner_status.h)
+
+    def __init__(self, checker: StateValidityChecker, params):
+        self._c = checker
+        self.parameters = params
+        self._path, self._solved, self._info = None, False, None
+
+    @staticmethod
+    def params(seed: int = 0, **kw):
+        """An ArtpPlannerParams with the shipped values (params.yaml, params.h) and `kw` overrides; the Basic fields may be
+        given as basic=BasicParams-like object."""
+        p = capi.ArtpPlannerParams()
+        d = dict(start_radius=0.2, goal_radius=0.5, n_iter=1000, max_n_vertices=10000, max_n_edges=50000,
+                 recompute_density_after_n_samples=1000, max_query_edge_length=0.5, max_draws=1 << 26, vertex_capacity=20000,
+                 edge_capacity=60000, max_roll_pert=3.33 / 180 * np.pi, max_pitch_pert=10.0 / 180 * np.pi,
+                 sample_from_distribution=1, use_inverse_vertex_density=1, use_max_prob_unknown_samples=1,
+                 max_prob_unknown_samples=0.1, simplify=1, clear_roadmap=0, seed=int(seed))
+        basic = kw.pop("basic", None)
+        d.update(kw)
+        for k, v in d.items():
+            setattr(p, k, v)
+        b = basic if basic is not None else type("B", (), dict(traversability_thres=0.15, unknown_space_untraversable=1,
+                                                                 foothold_margin=0.3, foothold_margin_max_hole_size=0.3,
+                                                                 foothold_margin_max_drop=0.3,
+                                                                 foothold_margin_max_drop_search_radius=0.16,
+                                                                 foothold_margin_min_step=0.3, foothold_size=0.1))
+        p.basic = capi.ArtpBasicParams(float(b.traversability_thres), int(b.unknown_space_untraversable), float(b.foothold_margin),
+                                       float(b.foothold_margin_max_hole_size), float(b.foothold_margin_max_drop),
+                                       float(b.foothold_margin_max_drop_search_radius), float(b.foothold_margin_min_step),
+                                       float(b.foothold_size))
+        return p
+
+    def setMap(self, elevation, traversability, elevation_inpainted, traversability_inpainted, res: float, cx: float,
+               cy: float) -> dict:
+        """Planner::setMap + the new-map chain. elevation / traversability: the RAW layers (NaN = unknown; traversability
+        may be None); *_inpainted: what inpaintMatrix returned for them (None with a None traversability). Returns the
+        call's host_syncs, bytes_h2d and bytes_d2h."""
+        f = lambda a: None if a is None else np.asfortranarray(a, dtype=np.float32)
+        e, t, ei, ti = f(elevation), f(traversability), f(elevation_inpainted), f(traversability_inpainted)
+        h = self._c.handle
+        mi = capi.ArtpPlannerMapInfo()
+        h.check(h.lib.artp_planner_set_map(h.h, C.byref(self.parameters), *[None if a is None else a.ctypes.data for a in (e, t, ei, ti)],
+                                           e.shape[0], e.shape[1], float(res), float(cx), float(cy), C.byref(mi)))
+        return {k: int(getattr(mi, k)) for k, _ in capi.ArtpPlannerMapInfo._fields_}
+
+    def space(self):
+        """The artp_se3_space setMap installed (capi.ArtpSe3Space)."""
+        sp = capi.ArtpSe3Space()
+        self._c.handle.check(self._c.handle.lib.artp_planner_get_space(self._c.handle.h, C.byref(sp)))
+        return sp
+
+    def plan(self, start, goal, capacity: int = 1 << 16) -> int:
+        """Planner::plan (+ getSolutionPath's simplification when the params say so): returns the PlannerStatus."""
+        h = self._c.handle
+        a = np.ascontiguousarray(start, dtype=np.float64).reshape(7)
+        b = np.ascontiguousarray(goal, dtype=np.float64).reshape(7)
+        self._solved, self._path, self._info = False, None, None   # a failing call leaves no solution behind
+        out = np.empty((int(capacity), 7), np.float64)
+        n = C.c_size_t(0)
+        info = capi.ArtpPlanInfo()
+        h.check(h.lib.artp_plan(h.h, C.byref(self.parameters), a.ctypes.data, b.ctypes.data, out.ctypes.data, int(capacity),
+                                C.byref(n), C.byref(info)))
+        self._info = info
+        self._solved = info.status == self.SOLVED
+        self._path = out[:n.value].copy()
+        return int(info.status)
+
+    def getSolutionPath(self):
+        """The last plan's path [n, 7] (simplified when the params said so); raises like planner.cpp:268-270 when the
+        plan did not solve."""
+        if not self._solved:
+            raise RuntimeError("Requested failed solution path.")
+        return self._path
+
+    def info(self) -> dict:
+        """The last plan's artp_plan_info as a dict (nested solve / simplify dicts, 7-vectors as arrays)."""
+        def conv(s):
+            out = {}
+            for k, _ in s._fields_:
+                v = getattr(s, k)
+                if isinstance(v, C.Structure):
+                    v = conv(v)
+                elif isinstance(v, C.Array):
+                    v = np.array(v[:])
+                out[k] = v
+            return out
+        d = conv(self._info)
+        d["solve"].pop("path_vertices", None)
+        return d
+
+
 class StartState:
     """art_planner::StartState (start.h, start.cpp:7-41): the start pose repaired by a disc search around it, one device
     call per sampleGoal. Offsets come from the Philox "ARTB" stream of `seed`; the draw position advances by what the

@@ -96,16 +96,19 @@ __global__ void build_codes_kernel(const float2* __restrict__ T, const unsigned 
 
 // Encoding of the compact tables of one layer: base = the smallest finite height, step = the smallest power of two
 // with dec(kCodeMax) >= the largest finite height (checked with the device's own dec()).
+void code_scale_of(float lo, float hi, float& base, float& step) {
+  base = lo <= hi ? lo : 0.0f;
+  int e = -126;
+  while (e < 127 && artp::code_dec(base, std::ldexp(1.0f, e), artp::kCodeMax) < hi) ++e;
+  step = std::ldexp(1.0f, e);
+}
 void code_scale(const float* layer, size_t n, float& base, float& step) {
   float lo = HUGE_VALF, hi = -HUGE_VALF;
   for (size_t i = 0; i < n; ++i) {
     const float v = layer[i] * 1.0f + 0.0f;   // the stored height (reverse_columns_kernel)
     if (std::fabs(v) < HUGE_VALF) { lo = std::min(lo, v); hi = std::max(hi, v); }
   }
-  base = lo <= hi ? lo : 0.0f;
-  int e = -126;
-  while (e < 127 && artp::code_dec(base, std::ldexp(1.0f, e), artp::kCodeMax) < hi) ++e;
-  step = std::ldexp(1.0f, e);
+  code_scale_of(lo, hi, base, step);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -818,6 +821,7 @@ void artp_destroy(artp_handle* hh) {
   cudaFree(h->d_compact_state); cudaFree(h->d_recs); cudaFree(h->d_recs_f); cudaFree(h->d_recs_g); cudaFree(h->d_samp_layers); cudaFree(h->d_samp_scratch);
   cudaFree(h->d_dist_layers); cudaFree(h->d_dist_scratch); cudaFree(h->d_basic_keep); cudaFree(h->d_simplify);
   roadmap_free(h);
+  planner_free(h);
   if (h->h_small_out) cudaFreeHost(h->h_small_out);
   if (h->h_err) cudaFreeHost(h->h_err);
   for (int g = 0; g < 2; ++g) if (h->chain_ev[g]) cudaEventDestroy(h->chain_ev[g]);
@@ -921,6 +925,14 @@ int artp_set_map(artp_handle* hh, const float* elevation, const float* elevation
 int artp_set_map_window(artp_handle* hh, const float* elevation, const float* elevation_masked, int rows, int cols, double res,
                         double cx, double cy, int row0, int nrows) {
   LOCK_CALL(h, hh);
+  h->planner_map = false;
+  return upload_map(h, elevation, elevation_masked, false, rows, cols, res, cx, cy, row0, nrows);
+}
+
+}  // extern "C"
+
+int artp_api::upload_map(Handle* h, const float* elevation, const float* elevation_masked, bool device_src, int rows, int cols,
+                         double res, double cx, double cy, int row0, int nrows) {
   if (!elevation || !elevation_masked || rows < 2 || cols < 2 || !(res > 0)) { h->err = "bad map arguments"; return ARTP_E_INVALID; }
   if (row0 < 0 || nrows < 2 || row0 + nrows > rows || (row0 & 3)) {
     h->err = "bad map window (row0 must be a multiple of 4, 0 <= row0, row0 + nrows <= rows, nrows >= 2)"; return ARTP_E_INVALID;
@@ -985,7 +997,18 @@ int artp_set_map_window(artp_handle* hh, const float* elevation, const float* el
   TRY(grow(h, h->d_stage, h->stage_cap, ncell * sizeof(float)));
   const float* src[2] = {elevation, elevation_masked};
   float cbase[2], cstep[2];
-  for (int k = 0; k < 2; ++k) code_scale(src[k], ncell, cbase[k], cstep[k]);
+  if (device_src) {   // the finite range of each layer from the device: the only bytes that come back
+    uint32_t* d_mm = (uint32_t*)h->d_stage;
+    uint32_t mm[6];
+    for (int k = 0; k < 2; ++k) TRY(finite_min_max(h, src[k], ncell, d_mm + 3 * k, h->stream));
+    TRY(copy_async(h, mm, d_mm, sizeof(mm), cudaMemcpyDeviceToHost, h->stream));
+    TRY(sync_stream(h, h->stream));
+    for (int k = 0; k < 2; ++k)
+      code_scale_of(mm[3 * k + 2] ? key_float(mm[3 * k]) : HUGE_VALF, mm[3 * k + 2] ? key_float(mm[3 * k + 1]) : -HUGE_VALF,
+                    cbase[k], cstep[k]);
+  } else {
+    for (int k = 0; k < 2; ++k) code_scale(src[k], ncell, cbase[k], cstep[k]);
+  }
   // plane tables (temporary): 4 slots per cell = load factor 0.5 for the 2 triangles of a cell
   size_t cap = 1;
   while (cap < 4 * ncell) cap <<= 1;
@@ -994,9 +1017,10 @@ int artp_set_map_window(artp_handle* hh, const float* elevation, const float* el
   CU_TRY(h, cudaMalloc(&d_tab, cap * sizeof(PlaneSlot)));
   if (cudaMalloc(&d_merge, 3 * npad) != cudaSuccess) { cudaFree(d_tab); h->err = "cudaMalloc (plane tables)"; return ARTP_E_CUDA; }
   for (int k = 0; k < 2; ++k) {
-    CU_TRY(h, cudaMemcpyAsync(h->d_stage, src[k], ncell * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+    if (!device_src) TRY(copy_async(h, h->d_stage, src[k], ncell * sizeof(float), cudaMemcpyHostToDevice, h->stream));
     const unsigned g4 = (unsigned)h->sm_count * 4, g8 = (unsigned)h->sm_count * 8;
-    TRY(launch(h, reverse_columns_kernel, g4, 256, 0, h->stream, (const float*)h->d_stage, h->d_H[k], nrows, cols, pitch));
+    TRY(launch(h, reverse_columns_kernel, g4, 256, 0, h->stream, device_src ? src[k] : (const float*)h->d_stage, h->d_H[k], nrows,
+               cols, pitch));
     artp::Field fk = f;                     // local storage, global geometry: cell x of the window is global cell x + row0
     fk.H = h->d_H[k]; fk.pitch = pitch; fk.nx = nrows;
     TRY(launch(h, plane_table_clear_kernel, g8, 256, 0, h->stream, d_tab, cap));
@@ -1097,6 +1121,8 @@ int artp_set_map_window(artp_handle* hh, const float* elevation, const float* el
   h->res = res;
   return ARTP_OK;
 }
+
+extern "C" {
 
 int artp_check_poses(artp_handle* hh, const double* states, size_t n, uint8_t* valid) {
   LOCK_CALL(h, hh);

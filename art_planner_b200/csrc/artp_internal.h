@@ -3,6 +3,7 @@
 //                     checks, compaction and bit packing
 //   artp_sampling.cu  normals and the CDF, the sampler, start / goal search, poseFrom2D, Basic, the sample distribution
 //   artp_cost.cu      path length, the edge matrix, the learned motion cost, cost weights and features
+//   artp_planner.cu   artp_planner_set_map / artp_plan: the replan, over the lock-free bodies declared at the end
 // the handle and its lock, launch and call bookkeeping, scratch regions, argument checks, and the few functions one unit
 // calls in another. It includes no kernel header: each of those defines kernels and is compiled into exactly one unit.
 #pragma once
@@ -46,6 +47,10 @@ struct MapState {
   bool has_sample_filter = false;   // d_dist_layers holds this map's traversability_sample_filter ...
   bool has_dist_observed = false;   // ... and observed layer
 };
+
+// Host <-> device traffic and host synchronisations of the calls that count them (artp_plan reports its own).
+struct Traffic { uint64_t h2d = 0, d2h = 0; uint32_t syncs = 0; };
+struct PlannerState;   // artp_planner_set_map / artp_plan (artp_planner.cu)
 
 struct Handle {
   artp_params p;
@@ -130,6 +135,9 @@ struct Handle {
   uint32_t* h_err = nullptr;        // host view
   uint32_t* d_err = nullptr;        // device view of the same word
   int tcap_override = 0;            // test hook (artp_debug_set_group_capacity)
+  PlannerState* planner = nullptr;  // from the first artp_planner_set_map
+  bool planner_map = false;         // the current map was installed by artp_planner_set_map
+  Traffic traffic;
   artp_stats stats{};
   std::string err;
   std::mutex mtx;
@@ -253,6 +261,19 @@ struct ChainScope {   // begin on construction, end on destruction (every return
 // Sticky plane-grouping overflow (set by the device, see Handle::h_err): read and clear.
 int take_sticky_error(Handle* h);
 
+// Copies and synchronisations counted in Handle::traffic (the paths artp_plan takes use these).
+inline int copy_async(Handle* h, void* dst, const void* src, size_t bytes, cudaMemcpyKind kind, cudaStream_t s) {
+  CU_TRY(h, cudaMemcpyAsync(dst, src, bytes, kind, s));
+  if (kind == cudaMemcpyHostToDevice) h->traffic.h2d += bytes;
+  if (kind == cudaMemcpyDeviceToHost) h->traffic.d2h += bytes;
+  return ARTP_OK;
+}
+inline int sync_stream(Handle* h, cudaStream_t s) {
+  CU_TRY(h, cudaStreamSynchronize(s));
+  h->traffic.syncs += 1;
+  return ARTP_OK;
+}
+
 // Host-buffer calls run on h->stream as users of scratch group 0. host_call_begin waits for the group's previous user and
 // hands out region[i] = bytes[i] bytes of d_stage (carve). host_call_end waits for the call's work, after which the group
 // is idle. For a call that ran the validity pipeline (`pipeline`) it then returns the sticky device error (Handle::h_err)
@@ -264,7 +285,7 @@ inline int host_call_begin(Handle* h, std::initializer_list<size_t> bytes = {}, 
   return carve(h, h->d_stage, h->stage_cap, bytes, region);
 }
 inline int host_call_end(Handle* h, bool pipeline = false) {
-  CU_TRY(h, cudaStreamSynchronize(h->stream));
+  TRY(sync_stream(h, h->stream));
   h->chain_busy[0] = false;
   return pipeline ? take_sticky_error(h) : ARTP_OK;
 }
@@ -314,5 +335,58 @@ int motion_cost_split(Handle* h, const double* d_s1, const double* d_s2, size_t 
 
 // artp_roadmap.cu: releases the roadmap store (artp_destroy).
 void roadmap_free(Handle* h);
+
+// ---- the bodies of public entry points, without the lock, for artp_plan / artp_planner_set_map (artp_planner.cu) ----
+// artp_capi.cu: artp_set_map_window's work. device_src: the two layers are DEVICE pointers (rows x cols, grid_map layout)
+// and the compact-code scales come from a device reduction instead of a host pass.
+int upload_map(Handle* h, const float* elevation, const float* elevation_masked, bool device_src, int rows, int cols,
+               double res, double cx, double cy, int row0, int nrows);
+// artp_sampling.cu:
+// Basic over the device layers L[0, n) elevation, L[n, 2n) traversability, L[2n, 3n) observed (read when has_observed)
+// with 6 more layers of scratch behind them; elevation_masked ends at L + 8n, traversability_thresholded at L + 5n, and
+// both Basic layers are kept for set_sample_filter_basic. Structuring elements above 64 cells: ARTP_E_LIMIT.
+int process_basic(Handle* h, float* L, int rows, int cols, double res, const artp_basic_params* bp, bool has_observed,
+                  cudaStream_t s);
+// The size limits the map chain would hit at resolution res (ARTP_E_LIMIT): Basic's structuring elements, and with
+// `distribution` the sample filter's and (inverse_density) the density blur's.
+int map_chain_limits(Handle* h, const artp_basic_params* bp, double res, bool distribution, bool inverse_density);
+int estimate_normals(Handle* h, double estimation_radius, cudaStream_t s);
+int set_sample_filter_basic(Handle* h, cudaStream_t s);   // artp_set_sample_filter(h, NULL, NULL, NULL)
+// artp_set_sampler(h, sp, NULL x 6) on the layers the device computed for this map (no CDF validation: they are cumulative).
+int arm_sampler_device(Handle* h, const artp_sampler_params* sp);
+int ball_search(Handle* h, const double* d_centres, size_t n, const double* d_radius, uint32_t n_iter, uint64_t seed,
+                uint64_t first_draw, double* d_states_out, int32_t* d_index, cudaStream_t s);
+int pose_from_2d(Handle* h, const double* d_in, size_t n, double* d_out, uint8_t* d_inside, cudaStream_t s);
+// artp_roadmap.cu:
+int roadmap_clear(Handle* h, size_t vertex_capacity, size_t edge_capacity);
+bool has_roadmap(const Handle* h);
+int roadmap_sample_graph(Handle* h, const artp_roadmap_params* rp, const artp_sample_distribution_params* dp, uint64_t seed,
+                         uint64_t first_sample, uint64_t* draws_used);
+int roadmap_update_edges(Handle* h);
+void roadmap_counts(const Handle* h, size_t* nv, size_t* ne);
+// artp_roadmap_solve's work; with d_sg (DEVICE: start then goal, 14 doubles) the endpoints are not read on the host: a
+// device check gives their bounds verdict and (x, y), and d_path_out (DEVICE, path_capacity x 7) receives the path instead
+// of path_states.
+int roadmap_solve(Handle* h, const double* start, const double* goal, const double* d_sg, const artp_se3_space* space,
+                  double* path_states, double* d_path_out, size_t path_capacity, size_t* n_path, double* cost,
+                  artp_roadmap_solve_info* info);
+// artp_path_simplify.cu: artp_simplify_path's work; with d_path (DEVICE, n states) the pool is seeded on the device and the
+// learned cost's piece offsets are computed there.
+int simplify_path(Handle* h, const double* path, const double* d_path, size_t n, const artp_se3_space* space, int objective,
+                  double max_query_edge_length, uint64_t seed, double* out, size_t capacity, size_t* n_out,
+                  artp_simplify_info* info);
+// artp_planner.cu:
+// Finite minimum and maximum of n floats (-0 counted as +0) on s: d_out = {key(min), key(max), finite count} with the
+// order-preserving keys of float_key.
+int finite_min_max(Handle* h, const float* d_layer, size_t n, uint32_t* d_out, cudaStream_t s);
+float key_float(uint32_t key);
+// MotionCostObjective::motionCost's piece offsets of the n - 1 edges of the DEVICE path d_states (n + 0 entries, exclusive,
+// then the total) on s; *total is read back (one synchronisation). ARTP_E_INVALID for an edge of 2^32 pieces or more.
+// Planner::plan's checks of the endpoints of a device solve (start then goal, 14 doubles at d_sg) into d_out[5]: 0, -1
+// (a non-finite state), ARTP_SOLVE_INVALID_START or ARTP_SOLVE_INVALID_GOAL (outside space's bounds), then both (x, y).
+int endpoint_check(Handle* h, const double* d_sg, const artp_se3_space* space, double* d_out, cudaStream_t s);
+int piece_offsets(Handle* h, const double* d_states, size_t n, double max_query_edge_length, uint32_t* d_off, size_t* total,
+                  cudaStream_t s);
+void planner_free(Handle* h);
 
 }  // namespace artp_api

@@ -670,15 +670,18 @@ __global__ void se3_ops_kernel(const double* __restrict__ a, const double* __res
   }
 }
 
-// PathGeometric::cost under the objective: the per-edge costs on the device, summed left to right from 0.0.
+// PathGeometric::cost under the objective: the per-edge costs on the device, summed left to right from 0.0. states: the
+// HOST copy of the path, or NULL: the learned cost's piece offsets are then computed on the device into d_off (n entries).
 int path_cost(Handle* h, const double* d_states, const double* states, size_t n, int objective, double max_query_edge_length,
-              double* cost) {
+              uint32_t* d_off, double* cost) {
   *cost = 0.0;
   if (n < 2) return ARTP_OK;
   const size_t ne = n - 1;
   std::vector<uint32_t> off;
   size_t total = 0;
-  if (objective == ARTP_OBJ_LEARNED) {
+  if (objective == ARTP_OBJ_LEARNED && !states) {
+    TRY(piece_offsets(h, d_states, n, max_query_edge_length, d_off, &total, h->stream));
+  } else if (objective == ARTP_OBJ_LEARNED) {
     off.resize(ne + 1);
     for (size_t e = 0; e < ne; ++e) {   // n_interp as artp_motion_cost_split computes it
       off[e] = (uint32_t)total;
@@ -695,15 +698,15 @@ int path_cost(Handle* h, const double* d_states, const double* states, size_t n,
                                           total * 3 * sizeof(float)}, r));
   cudaStream_t s = h->stream;
   if (objective == ARTP_OBJ_LEARNED) {
-    CU_TRY(h, cudaMemcpyAsync(r[1], off.data(), (ne + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-    TRY(motion_cost_split(h, d_states, d_states + 7, ne, (const uint32_t*)r[1], total, (float*)r[2], (float*)r[3],
-                          (double*)r[0], s));
+    if (states) TRY(copy_async(h, r[1], off.data(), (ne + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+    TRY(motion_cost_split(h, d_states, d_states + 7, ne, states ? (const uint32_t*)r[1] : d_off, total, (float*)r[2],
+                          (float*)r[3], (double*)r[0], s));
   } else {
     TRY(path_length_cost(h, d_states, d_states + 7, ne, (double*)r[0], s));
   }
   std::vector<double> c(ne);
-  CU_TRY(h, cudaMemcpyAsync(c.data(), r[0], ne * sizeof(double), cudaMemcpyDeviceToHost, s));
-  CU_TRY(h, cudaStreamSynchronize(s));   // `off` outlives its copy
+  TRY(copy_async(h, c.data(), r[0], ne * sizeof(double), cudaMemcpyDeviceToHost, s));
+  TRY(sync_stream(h, s));   // `off` outlives its copy
   double sum = 0.0;
   for (double v : c) sum += v;
   *cost = sum;
@@ -718,14 +721,24 @@ int artp_simplify_path(artp_handle* hh, const double* path, size_t n, const artp
                        double max_query_edge_length, uint64_t seed, double* out, size_t capacity, size_t* n_out,
                        artp_simplify_info* info) {
   LOCK_CALL(h, hh);
-  if (!space || (n && !path)) return null_buffer(h);
+  if (n && !path) return null_buffer(h);
+  return simplify_path(h, path, nullptr, n, space, objective, max_query_edge_length, seed, out, capacity, n_out, info);
+}
+
+}  // extern "C"
+
+int artp_api::simplify_path(Handle* h, const double* path, const double* d_path, size_t n, const artp_se3_space* space,
+                            int objective, double max_query_edge_length, uint64_t seed, double* out, size_t capacity,
+                            size_t* n_out, artp_simplify_info* info) {
+  if (!space) return null_buffer(h);
   if (n == 0) { h->err = "empty path"; return ARTP_E_INVALID; }
   if (objective != ARTP_OBJ_LEARNED && objective != ARTP_OBJ_PATH_LENGTH && objective != ARTP_OBJ_NONE) {
     h->err = "objective must be ARTP_OBJ_LEARNED, ARTP_OBJ_PATH_LENGTH or ARTP_OBJ_NONE"; return ARTP_E_INVALID;
   }
   TRY(require_whole_map(h));
-  for (size_t i = 0; i < n * 7; ++i)
-    if (!std::isfinite(path[i])) { h->err = "non-finite path state"; return ARTP_E_INVALID; }
+  if (!d_path)
+    for (size_t i = 0; i < n * 7; ++i)
+      if (!std::isfinite(path[i])) { h->err = "non-finite path state"; return ARTP_E_INVALID; }
   if (n > ARTP_SIMPLIFY_MAX_STATES) { h->err = "path longer than ARTP_SIMPLIFY_MAX_STATES"; return ARTP_E_LIMIT; }
   if (objective == ARTP_OBJ_LEARNED) {
     if (!(max_query_edge_length > 0.0)) { h->err = "max_query_edge_length must be > 0"; return ARTP_E_INVALID; }
@@ -746,17 +759,19 @@ int artp_simplify_path(artp_handle* hh, const double* path, size_t n, const artp
   d.ncap = (uint32_t)(256 * n + 64);
   d.pcap = (uint32_t)(512 * n + 64);
   const size_t pairs = n * (n - 1) / 2 + 1;
-  char* r[13];
+  char* r[14];
   TRY(carve(h, h->d_simplify, h->simplify_cap,
             {sizeof(SimpCtl), (size_t)d.pcap * 7 * sizeof(double), (size_t)d.ncap * sizeof(uint32_t),
              (size_t)d.ncap * sizeof(uint32_t), (size_t)d.ncap * sizeof(uint32_t), pairs * sizeof(double),
              (size_t)d.ncap * sizeof(double), kAttempts * sizeof(Att), kBatch * 14 * sizeof(double),
-             (kBatch + 1) * sizeof(uint32_t), kBatch * 2, kBatch * 7 * sizeof(double), (size_t)d.ncap * 7 * sizeof(double)},
+             (kBatch + 1) * sizeof(uint32_t), kBatch * 2, kBatch * 7 * sizeof(double), (size_t)d.ncap * 7 * sizeof(double),
+             d_path ? (size_t)d.ncap * sizeof(uint32_t) : 0},
             r));
   d.ctl = (SimpCtl*)r[0]; d.pool = (double*)r[1]; d.path = (uint32_t*)r[2]; d.tmp = (uint32_t*)r[3]; d.cid = (uint32_t*)r[4];
   d.pair = (double*)r[5]; d.dists = (double*)r[6]; d.att = (Att*)r[7]; d.mot = (double*)r[8]; d.mot_off = (uint32_t*)r[9];
   d.mot_ok = (uint8_t*)r[10]; d.valid = (uint8_t*)r[10] + kBatch; d.chk = (double*)r[11];
   double* d_simp = (double*)r[12];   // the simplified path, in order
+  uint32_t* d_off = (uint32_t*)r[13];  // device piece offsets of the learned cost (device path only)
   TRY(host_call_begin(h));
   cudaStream_t s = h->stream;
   // the input path is pool states 0 .. n-1
@@ -769,9 +784,10 @@ int artp_simplify_path(artp_handle* hh, const double* path, size_t n, const artp
   c.fresh = 1;
   c.n = c.np = c.n_in = (uint32_t)n;
   c.n_simplified = (uint32_t)n;
-  CU_TRY(h, cudaMemcpyAsync(d.pool, path, n * 7 * sizeof(double), cudaMemcpyHostToDevice, s));
-  CU_TRY(h, cudaMemcpyAsync(d.path, ids.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-  CU_TRY(h, cudaMemcpyAsync(d.ctl, &c, sizeof(SimpCtl), cudaMemcpyHostToDevice, s));
+  if (d_path) CU_TRY(h, cudaMemcpyAsync(d.pool, d_path, n * 7 * sizeof(double), cudaMemcpyDeviceToDevice, s));
+  else TRY(copy_async(h, d.pool, path, n * 7 * sizeof(double), cudaMemcpyHostToDevice, s));
+  TRY(copy_async(h, d.path, ids.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+  TRY(copy_async(h, d.ctl, &c, sizeof(SimpCtl), cudaMemcpyHostToDevice, s));
   // rounds, kRoundsPerSync at a time; the check grid follows what the rounds asked for
   uint32_t cap = 256;
   const uint64_t max_batches = 64 * (uint64_t)n + 1024;   // far above any schedule: every round advances an attempt
@@ -783,8 +799,8 @@ int artp_simplify_path(artp_handle* hh, const double* path, size_t n, const artp
       if (rc == ARTP_OK) rc = launch(h, simplify_apply_kernel, 1, kThreads, 0, s, d);
     }
     if (rc != ARTP_OK) break;
-    CU_TRY(h, cudaMemcpyAsync(&c, d.ctl, sizeof(SimpCtl), cudaMemcpyDeviceToHost, s));
-    CU_TRY(h, cudaStreamSynchronize(s));
+    TRY(copy_async(h, &c, d.ctl, sizeof(SimpCtl), cudaMemcpyDeviceToHost, s));
+    TRY(sync_stream(h, s));
     if (c.status != S_RUNNING) break;
     cap = std::min<uint32_t>(kBatch, std::max<uint32_t>(64, (c.want + 63) & ~63u));
     if (b > max_batches) { h->err = "path simplification did not end"; rc = ARTP_E_LIMIT; }
@@ -794,16 +810,16 @@ int artp_simplify_path(artp_handle* hh, const double* path, size_t n, const artp
     rc = ARTP_E_LIMIT;
   }
   // the simplified path, and the comparison
-  std::vector<double> simp((size_t)c.n * 7);
+  std::vector<double> simp(d_path ? 0 : (size_t)c.n * 7);   // a device path: the costs' piece offsets come from the device
   if (rc == ARTP_OK) rc = launch(h, simplify_out_kernel, grid_for(h, (size_t)c.n * 7, 256, 4), 256, 0, s, d, d_simp);
-  if (rc == ARTP_OK) {
-    CU_TRY(h, cudaMemcpyAsync(simp.data(), d_simp, simp.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
-    CU_TRY(h, cudaStreamSynchronize(s));
+  if (rc == ARTP_OK && !d_path) {
+    TRY(copy_async(h, simp.data(), d_simp, simp.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+    TRY(sync_stream(h, s));
   }
   double cost_o = std::nan(""), cost_s = std::nan("");
   if (rc == ARTP_OK && c.check_passed && objective != ARTP_OBJ_NONE) {
-    rc = path_cost(h, d_simp, simp.data(), c.n, objective, max_query_edge_length, &cost_s);
-    if (rc == ARTP_OK) rc = path_cost(h, d.pool, path, n, objective, max_query_edge_length, &cost_o);
+    rc = path_cost(h, d_simp, d_path ? nullptr : simp.data(), c.n, objective, max_query_edge_length, d_off, &cost_s);
+    if (rc == ARTP_OK) rc = path_cost(h, d.pool, path, n, objective, max_query_edge_length, d_off, &cost_o);
   }
   const int rc_end = host_call_end(h, true);
   if (rc != ARTP_OK) return rc;
@@ -821,9 +837,16 @@ int artp_simplify_path(artp_handle* hh, const double* path, size_t n, const artp
   }
   if (n_out) *n_out = nr;
   if (nr > capacity) { h->err = "capacity too small"; return ARTP_E_LIMIT; }
-  if (out) std::copy_n(simplified ? simp.data() : path, nr * 7, out);
+  if (out && d_path) {   // the returned path's one trip to the host
+    TRY(copy_async(h, out, simplified ? d_simp : d.pool, nr * 7 * sizeof(double), cudaMemcpyDeviceToHost, s));
+    TRY(sync_stream(h, s));
+  } else if (out) {
+    std::copy_n(simplified ? simp.data() : path, nr * 7, out);
+  }
   return ARTP_OK;
 }
+
+extern "C" {
 
 int artp_debug_se3_ops(artp_handle* hh, const double* a, const double* b, const double* t, size_t n, double* dist,
                        double* interp) {

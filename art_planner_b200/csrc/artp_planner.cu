@@ -1,0 +1,459 @@
+// art_planner_b200/csrc/artp_planner.cu -- Planner::setMap and Planner::plan + getSolutionPath for prm_motion_cost
+// (art_planner/src/planner.cpp:135-298) as two calls of the C ABI (include/artp.h): artp_planner_set_map and artp_plan.
+// The stages are the ones the public entry points run (their bodies without the lock, artp_internal.h); between them every
+// layer, state and path stays in device memory. The kernels here are the pieces no entry point had: the finite range of a
+// layer, the "observed" layer, the goal's bounds clip, the endpoints' check and the learned cost's piece offsets.
+#include <cfloat>
+#include <cmath>
+#include <cstring>
+
+#include "artp_internal.h"
+
+using namespace artp_api;
+
+namespace artp_api {
+
+struct PlannerState {
+  float* d_layers = nullptr;         // raw elevation | raw traversability | Basic's 9 layers (artp_api::process_basic)
+  size_t layers_cap = 0;             // floats
+  double* d_q = nullptr;             // query block (QB_* offsets)
+  double* d_path = nullptr;          // the solved path (vertex capacity x 7)
+  size_t path_cap = 0;               // states
+  artp_se3_space space{};
+  uint64_t generation = 0;           // map generation: stands in for the grid_map timestamp sampleGraph compares
+  uint64_t sampled_generation = 0;   // the generation the last sampleGraph saw
+  bool seeded = false;
+  uint64_t seed = 0, next_sample = 0, start_draw = 0, goal_draw = 0, simplify_calls = 0;
+  cudaEvent_t ev[6] = {};
+};
+
+}  // namespace artp_api
+
+namespace {
+
+// Offsets (in doubles) of the query block d_q.
+enum : size_t {
+  QB_START = 0, QB_GOAL = 7, QB_CLIPPED = 14, QB_PROJECTED = 21, QB_REPAIRED = 28 /* start, goal: 14 */, QB_RADIUS = 42,
+  QB_FLAGS = 44 /* inside byte, clipped byte, two int32 ball indices */, QB_MINMAX = 46, QB_SIZE = 64
+};
+
+__device__ __forceinline__ uint32_t float_key(float f) {   // order-preserving: a < b <=> key(a) < key(b)
+  const uint32_t u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// minCoeffOfFinites / maxCoeffOfFinites: min and max over the finite cells, -0 taken as +0 (the two compare equal).
+__global__ void finite_min_max_kernel(const float* __restrict__ a, size_t n, uint32_t* __restrict__ out) {
+  uint32_t lo = 0xFFFFFFFFu, hi = 0u, cnt = 0u;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float v = a[i] + 0.0f;
+    if (fabsf(v) < CUDART_INF_F) { const uint32_t k = float_key(v); lo = min(lo, k); hi = max(hi, k); ++cnt; }
+  }
+  lo = __reduce_min_sync(0xFFFFFFFFu, lo);
+  hi = __reduce_max_sync(0xFFFFFFFFu, hi);
+  cnt = __reduce_add_sync(0xFFFFFFFFu, cnt);
+  if ((threadIdx.x & 31) == 0 && cnt) { atomicMin(out, lo); atomicMax(out + 1, hi); atomicAdd(out + 2, cnt); }
+}
+
+// addKnownCells (basic.cpp:25-38): observed = 1 where every basic layer ({elevation, traversability}, map.cpp:16) is finite
+// (grid_map's isValid). A missing traversability layer is checkTraversability's 1.0 (basic.cpp:13-21), written to trav_fill.
+__global__ void observed_kernel(const float* __restrict__ elevation, const float* __restrict__ traversability, size_t n,
+                                float* __restrict__ observed, float* __restrict__ trav_fill) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    bool ok = fabsf(elevation[i]) < CUDART_INF_F;
+    if (traversability) ok = ok && fabsf(traversability[i]) < CUDART_INF_F;
+    else trav_fill[i] = 1.0f;
+    observed[i] = ok ? 1.0f : 0.0f;
+  }
+}
+
+constexpr double kQuatNormError = 1e-9;   // SO3StateSpace's MAX_QUATERNION_NORM_ERROR
+
+// Planner::plan :207-221: satisfiesBounds, else enforceBounds, of the SE(3) goal. R3: RealVectorStateSpace's test with the
+// DBL_EPSILON slack, then the clamp. SO3: satisfiesBounds is |norm - 1| < 1e-9; enforceBounds normalises when the SQUARED
+// norm differs from 1 by more than DBL_EPSILON, to the identity when the norm is below DBL_EPSILON.
+__global__ void goal_clip_kernel(const double* __restrict__ in, artp_se3_space sp, double* __restrict__ out,
+                                 uint8_t* __restrict__ clipped) {
+  double s[7];
+  for (int k = 0; k < 7; ++k) s[k] = in[k];
+  bool ok = true;
+  for (int i = 0; i < 3; ++i)
+    if (s[i] - DBL_EPSILON > sp.high[i] || s[i] + DBL_EPSILON < sp.low[i]) ok = false;
+  const double nrm_sq = s[3] * s[3] + s[4] * s[4] + s[5] * s[5] + s[6] * s[6];
+  const double norm = sqrt(nrm_sq);
+  if (!(fabs(norm - 1.0) < kQuatNormError)) ok = false;
+  if (!ok) {
+    for (int i = 0; i < 3; ++i) {
+      if (s[i] > sp.high[i]) s[i] = sp.high[i];
+      else if (s[i] < sp.low[i]) s[i] = sp.low[i];
+    }
+    if (fabs(nrm_sq - 1.0) > DBL_EPSILON) {
+      if (norm < DBL_EPSILON) { s[3] = s[4] = s[5] = 0.0; s[6] = 1.0; }
+      else for (int k = 3; k < 7; ++k) s[k] /= norm;
+    }
+  }
+  for (int k = 0; k < 7; ++k) out[k] = s[k];
+  *clipped = ok ? 0 : 1;
+}
+
+// artp_roadmap_solve's checks of its endpoints, on the device: any non-finite state (-1), then start, then goal outside
+// the bounds (no slack: the position inside the RealVectorBounds); then both (x, y).
+__global__ void endpoint_check_kernel(const double* __restrict__ sg, artp_se3_space sp, double* __restrict__ out) {
+  double verdict = 0.0;
+  for (int k = 0; k < 14; ++k)
+    if (!isfinite(sg[k])) verdict = -1.0;
+  if (verdict == 0.0)
+    for (int w = 0; w < 2 && verdict == 0.0; ++w)
+      for (int i = 0; i < 3; ++i)
+        if (sg[7 * w + i] < sp.low[i] || sg[7 * w + i] > sp.high[i]) { verdict = w ? ARTP_SOLVE_INVALID_GOAL : ARTP_SOLVE_INVALID_START; break; }
+  out[0] = verdict;
+  out[1] = sg[0]; out[2] = sg[1]; out[3] = sg[7]; out[4] = sg[8];
+}
+
+// MotionCostObjective::motionCost's split of the n - 1 edges of a path (artp_motion_cost_split's rule): pieces =
+// (unsigned)(lateralDistance / max_query_edge_length) + 1; off = their exclusive prefix sums (n entries, the last = total).
+// res[0] = the total (64 bits), res[1] = 1 when an edge has 2^32 pieces or more. One CTA.
+constexpr int kOffThreads = 1024;
+__global__ void __launch_bounds__(kOffThreads)
+piece_offsets_kernel(const double* __restrict__ st, size_t n, double mql, uint32_t* __restrict__ off,
+                     unsigned long long* __restrict__ res) {
+  __shared__ unsigned long long part[kOffThreads];
+  __shared__ int bad;
+  const size_t ne = n - 1, per = (ne + kOffThreads - 1) / kOffThreads;
+  const size_t e0 = threadIdx.x * per, e1 = min(ne, e0 + per);
+  if (threadIdx.x == 0) bad = 0;
+  __syncthreads();
+  auto pieces = [&](size_t e) -> unsigned long long {
+    const double dx = st[7 * (e + 1)] - st[7 * e], dy = st[7 * (e + 1) + 1] - st[7 * e + 1];
+    const double q = sqrt(dx * dx + dy * dy) / mql;
+    if (!(q < 4294967296.0)) { bad = 1; return 0ull; }
+    return (unsigned long long)(unsigned int)q + 1ull;
+  };
+  unsigned long long sum = 0;
+  for (size_t e = e0; e < e1; ++e) sum += pieces(e);
+  part[threadIdx.x] = sum;
+  __syncthreads();
+  if (threadIdx.x == 0) {   // exclusive scan of the 1024 chunk sums
+    unsigned long long run = 0;
+    for (int t = 0; t < kOffThreads; ++t) { const unsigned long long v = part[t]; part[t] = run; run += v; }
+    res[0] = run;
+    off[ne] = (uint32_t)run;
+  }
+  __syncthreads();
+  unsigned long long run = part[threadIdx.x];
+  for (size_t e = e0; e < e1; ++e) { off[e] = (uint32_t)run; run += pieces(e); }
+  __syncthreads();
+  if (threadIdx.x == 0) res[1] = bad;
+}
+
+int planner_status(int32_t solve_status) {   // planner.cpp:254-261
+  switch (solve_status) {
+    case ARTP_SOLVE_SOLVED: return ARTP_PLANNER_SOLVED;
+    case ARTP_SOLVE_NOT_CONNECTED: case ARTP_SOLVE_NO_FEASIBLE_PATH: return ARTP_PLANNER_NOT_SOLVED;
+    case ARTP_SOLVE_INVALID_START: return ARTP_PLANNER_INVALID_START;
+    case ARTP_SOLVE_INVALID_GOAL: return ARTP_PLANNER_INVALID_GOAL;
+    default: return ARTP_PLANNER_UNKNOWN;
+  }
+}
+
+PlannerState* planner_of(Handle* h) {
+  if (!h->planner) h->planner = new PlannerState();
+  return h->planner;
+}
+
+artp_sample_distribution_params dist_params(const Handle* h, const artp_planner_params* pp) {
+  artp_sample_distribution_params dp{};
+  dp.use_inverse_vertex_density = pp->use_inverse_vertex_density;
+  dp.density_blur_radius = (h->p.torso_length + h->p.torso_width) * 0.25;   // planner.cpp:48
+  dp.use_max_prob_unknown_samples = pp->use_max_prob_unknown_samples;
+  dp.max_prob_unknown_samples = pp->max_prob_unknown_samples;
+  return dp;
+}
+
+int plan_args(Handle* h, const artp_planner_params* pp) {
+  if (!pp) return null_buffer(h);
+  if (!(pp->start_radius >= 0.0 && std::isfinite(pp->start_radius) && pp->goal_radius >= 0.0 && std::isfinite(pp->goal_radius))) {
+    h->err = "start_radius and goal_radius must be finite and >= 0"; return ARTP_E_INVALID;
+  }
+  if (pp->max_n_vertices >= 0xFFFFFFFFull || pp->max_n_edges >= 0xFFFFFFFFull ||
+      pp->recompute_density_after_n_samples >= 0xFFFFFFFFull) {
+    h->err = "roadmap caps must be < 2^32"; return ARTP_E_INVALID;
+  }
+  if (pp->vertex_capacity == 0 || pp->edge_capacity == 0 || pp->vertex_capacity >= 0x7FFFFFFFull || pp->edge_capacity >= 0x7FFFFFFFull) {
+    h->err = "roadmap capacities must be > 0 and < 2^31"; return ARTP_E_INVALID;
+  }
+  if (pp->n_iter >= 0xFFFFFFFFu) { h->err = "n_iter must be < 2^32 - 1"; return ARTP_E_INVALID; }
+  if (pp->simplify && !(pp->max_query_edge_length > 0.0)) { h->err = "max_query_edge_length must be > 0"; return ARTP_E_INVALID; }
+  if (pp->use_max_prob_unknown_samples && !(pp->max_prob_unknown_samples >= 0.0 && pp->max_prob_unknown_samples <= 1.0)) {
+    h->err = "max_prob_unknown_samples must lie in [0, 1]"; return ARTP_E_INVALID;
+  }
+  return ARTP_OK;
+}
+
+int record(Handle* h, PlannerState* st, int i) {
+  CU_TRY(h, cudaEventRecord(st->ev[i], h->stream));
+  return ARTP_OK;
+}
+
+}  // namespace
+
+int artp_api::finite_min_max(Handle* h, const float* d_layer, size_t n, uint32_t* d_out, cudaStream_t s) {
+  CU_TRY(h, cudaMemsetAsync(d_out, 0xFF, sizeof(uint32_t), s));
+  CU_TRY(h, cudaMemsetAsync(d_out + 1, 0, 2 * sizeof(uint32_t), s));
+  return launch(h, finite_min_max_kernel, grid_for(h, n, 256, 8), 256, 0, s, d_layer, n, d_out);
+}
+
+float artp_api::key_float(uint32_t key) {
+  const uint32_t u = (key & 0x80000000u) ? (key & 0x7FFFFFFFu) : ~key;
+  float f;
+  std::memcpy(&f, &u, sizeof(f));
+  return f;
+}
+
+int artp_api::endpoint_check(Handle* h, const double* d_sg, const artp_se3_space* space, double* d_out, cudaStream_t s) {
+  return launch(h, endpoint_check_kernel, 1, 1, 0, s, d_sg, *space, d_out);
+}
+
+int artp_api::piece_offsets(Handle* h, const double* d_states, size_t n, double max_query_edge_length, uint32_t* d_off,
+                            size_t* total, cudaStream_t s) {
+  char* r[1];
+  TRY(carve(h, h->d_stage, h->stage_cap, {2 * sizeof(unsigned long long)}, r));
+  TRY(launch(h, piece_offsets_kernel, 1, kOffThreads, 0, s, d_states, n, max_query_edge_length, d_off, (unsigned long long*)r[0]));
+  unsigned long long res[2];
+  TRY(copy_async(h, res, r[0], sizeof(res), cudaMemcpyDeviceToHost, s));
+  TRY(sync_stream(h, s));
+  if (res[1]) { h->err = "path edge too long for the learned cost"; return ARTP_E_INVALID; }
+  if (res[0] > 0xFFFFFFFFull) { h->err = "too many cost pieces (>= 2^32)"; return ARTP_E_INVALID; }
+  *total = (size_t)res[0];
+  return ARTP_OK;
+}
+
+void artp_api::planner_free(Handle* h) {
+  PlannerState* st = h->planner;
+  if (!st) return;
+  cudaFree(st->d_layers); cudaFree(st->d_q); cudaFree(st->d_path);
+  for (cudaEvent_t e : st->ev) if (e) cudaEventDestroy(e);
+  delete st;
+  h->planner = nullptr;
+}
+
+extern "C" {
+
+int artp_planner_set_map(artp_handle* hh, const artp_planner_params* pp, const float* elevation, const float* traversability,
+                         const float* elevation_inpainted, const float* traversability_inpainted, int rows, int cols,
+                         double res, double cx, double cy, artp_planner_map_info* info) {
+  LOCK_CALL(h, hh);
+  // every check before any work: a refused map leaves the previous one installed
+  if (!pp || !elevation || !elevation_inpainted) return null_buffer(h);
+  if (!traversability != !traversability_inpainted) {
+    h->err = "pass both traversability layers (raw and inpainted) or neither"; return ARTP_E_INVALID;
+  }
+  if (rows < 2 || cols < 2 || !(res > 0) || !std::isfinite(cx) || !std::isfinite(cy)) { h->err = "bad map arguments"; return ARTP_E_INVALID; }
+  TRY(plan_args(h, pp));
+  TRY(map_chain_limits(h, &pp->basic, res, pp->sample_from_distribution != 0, pp->use_inverse_vertex_density != 0));
+  PlannerState* st = planner_of(h);
+  const size_t n = (size_t)rows * cols, lb = n * sizeof(float);
+  const Traffic t0 = h->traffic;
+  TRY(host_call_begin(h));
+  cudaStream_t s = h->stream;
+  TRY(grow(h, st->d_layers, st->layers_cap, 11 * n));
+  float *raw_e = st->d_layers, *raw_t = st->d_layers + n, *L = st->d_layers + 2 * n;
+  TRY(copy_async(h, raw_e, elevation, lb, cudaMemcpyHostToDevice, s));
+  TRY(copy_async(h, L, elevation_inpainted, lb, cudaMemcpyHostToDevice, s));
+  if (traversability) {
+    TRY(copy_async(h, raw_t, traversability, lb, cudaMemcpyHostToDevice, s));
+    TRY(copy_async(h, L + n, traversability_inpainted, lb, cudaMemcpyHostToDevice, s));
+  }
+  // observed, and the SE(3) bounds from the RAW elevation (planner.cpp:146-156)
+  TRY(launch(h, observed_kernel, grid_for(h, n, 256), 256, 0, s, raw_e, traversability ? raw_t : nullptr, n, L + 2 * n, L + n));
+  if (!st->d_q) CU_TRY(h, cudaMalloc(&st->d_q, QB_SIZE * sizeof(double)));
+  uint32_t* d_mm = reinterpret_cast<uint32_t*>(st->d_q + QB_MINMAX);
+  TRY(finite_min_max(h, raw_e, n, d_mm, s));
+  uint32_t mm[3];
+  TRY(copy_async(h, mm, d_mm, sizeof(mm), cudaMemcpyDeviceToHost, s));
+  TRY(host_call_end(h));
+  if (!mm[2]) { h->err = "the elevation layer has no finite cell"; return ARTP_E_INVALID; }
+  artp_se3_space sp{};
+  const double Lx = rows * res, Ly = cols * res;   // grid_map getLength: the FULL length, not half of it
+  sp.low[0] = cx - Lx; sp.high[0] = cx + Lx;
+  sp.low[1] = cy - Ly; sp.high[1] = cy + Ly;
+  sp.low[2] = (double)key_float(mm[0]) - h->p.reach_z / 2;
+  sp.high[2] = (double)key_float(mm[1]) + h->p.reach_z / 2;
+  sp.longest_valid_segment_fraction = 0.01;
+  // processors::Basic, then the upload of the elevation and the masked layer straight from device memory. From here on a
+  // failure (only a CUDA error can remain) leaves no planner map.
+  h->planner_map = false;
+  TRY(host_call_begin(h));
+  TRY(process_basic(h, L, rows, cols, res, &pp->basic, true, s));
+  TRY(host_call_end(h));
+  TRY(upload_map(h, L, L + 8 * n, true, rows, cols, res, cx, cy, 0, rows));
+  // the rest of the new-map chain (planner.cpp:39-58): normals, sample filter, distribution without vertices, CDF, sampler
+  TRY(host_call_begin(h));
+  TRY(estimate_normals(h, (h->p.torso_length + h->p.torso_width) * 0.25, s));
+  artp_sampler_params smp{};
+  smp.max_roll_pert = pp->max_roll_pert; smp.max_pitch_pert = pp->max_pitch_pert;
+  smp.sample_from_distribution = pp->sample_from_distribution;
+  smp.low[0] = sp.low[0]; smp.low[1] = sp.low[1]; smp.high[0] = sp.high[0]; smp.high[1] = sp.high[1];
+  if (pp->sample_from_distribution) {
+    TRY(set_sample_filter_basic(h, s));
+    const artp_sample_distribution_params dp = dist_params(h, pp);
+    TRY(check_distribution_args(h, &dp));
+    TRY(update_distribution_rearm(h, &dp, nullptr, 0, s));
+  }
+  TRY(arm_sampler_device(h, &smp));
+  TRY(host_call_end(h));
+  // CostPredictor.updateFeatures, when a network is loaded
+  if (h->cnn && artp_cnn::network(h->cnn) >= 0) {
+    CU_TRY(h, cudaSetDevice(h->device));
+    if (const int rc = artp_cnn::update_features(h->cnn, h->d_H[0], h->rows, h->cols, h->pitch, h->res, h->chk.cx, h->chk.cy,
+                                                 h->stream, h->cnn_mode & 1, h->err))
+      return rc;
+  }
+  st->space = sp;
+  st->generation += 1;
+  h->planner_map = true;
+  if (info) {
+    CU_TRY(h, cudaStreamSynchronize(h->stream));   // the features' kernels are part of the call
+    info->host_syncs = h->traffic.syncs - t0.syncs + 1;
+    info->bytes_h2d = h->traffic.h2d - t0.h2d;
+    info->bytes_d2h = h->traffic.d2h - t0.d2h;
+  }
+  return ARTP_OK;
+}
+
+int artp_planner_get_space(artp_handle* hh, artp_se3_space* out) {
+  LOCK_HANDLE(h, hh);
+  if (!out) return null_buffer(h);
+  if (!h->planner_map) { h->err = "no map set by artp_planner_set_map"; return ARTP_E_NOMAP; }
+  *out = h->planner->space;
+  return ARTP_OK;
+}
+
+int artp_plan(artp_handle* hh, const artp_planner_params* pp, const double* start, const double* goal, double* path,
+              size_t capacity, size_t* n_path, artp_plan_info* info) {
+  LOCK_CALL(h, hh);
+  if (!start || !goal) return null_buffer(h);
+  TRY(plan_args(h, pp));
+  for (int i = 0; i < 7; ++i)
+    if (!std::isfinite(start[i]) || !std::isfinite(goal[i])) { h->err = "non-finite start or goal"; return ARTP_E_INVALID; }
+  if (n_path) *n_path = 0;
+  artp_plan_info o{};
+  o.solve.path_vertices = info ? info->solve.path_vertices : nullptr;
+  o.start_index = o.goal_index = -1;
+  if (h->has_map && h->win_rows != h->rows) { h->err = "not available on a map window (artp_set_map_window)"; return ARTP_E_INVALID; }
+  if (!h->planner_map) {                                   // planner.cpp:197-200
+    o.status = ARTP_PLANNER_NO_MAP;
+    if (info) *info = o;
+    return ARTP_OK;
+  }
+  TRY(check_cost_net(h));                                  // the learned objective prices the edges
+  if (pp->sample_from_distribution) {                      // sampleGraph's recomputes: their limits before any draw
+    const artp_sample_distribution_params dp = dist_params(h, pp);
+    TRY(check_distribution_args(h, &dp));
+  }
+  PlannerState* st = h->planner;
+  const Traffic t0 = h->traffic;
+  for (auto& e : st->ev)
+    if (!e) CU_TRY(h, cudaEventCreate(&e));
+  if (!st->seeded || st->seed != pp->seed) {   // a new seed starts every stream at its beginning
+    st->seeded = true; st->seed = pp->seed;
+    st->next_sample = st->start_draw = st->goal_draw = st->simplify_calls = 0;
+  }
+  cudaStream_t s = h->stream;
+  // PRMMotionCost::clear (the ROS node's ss_->clear(), planner_ros.cpp:359,373), or the first roadmap of this handle
+  if (pp->clear_roadmap || !has_roadmap(h)) TRY(roadmap_clear(h, pp->vertex_capacity, pp->edge_capacity));
+  size_t nv = 0, ne = 0;
+  // PRMMotionCost::solve -> sampleGraph: sample and updateEdges only when the map changed (prm_motion_cost.cpp:146-153)
+  TRY(record(h, st, 0));
+  o.first_sample = st->next_sample;
+  if (st->sampled_generation != st->generation) {
+    artp_roadmap_params rp{pp->max_n_vertices, pp->max_n_edges, pp->recompute_density_after_n_samples, pp->max_draws};
+    const artp_sample_distribution_params dp = dist_params(h, pp);
+    uint64_t used = 0;
+    TRY(roadmap_sample_graph(h, &rp, pp->sample_from_distribution ? &dp : nullptr, pp->seed, st->next_sample, &used));
+    TRY(record(h, st, 1));
+    TRY(roadmap_update_edges(h));
+    st->sampled_generation = st->generation;
+    st->next_sample += used;
+    o.sampled = 1;
+    o.draws_used = used;
+  } else {
+    TRY(record(h, st, 1));
+  }
+  TRY(host_call_begin(h));
+  TRY(record(h, st, 2));
+  // the goal: clip (:207-221), projection when on the map (:223-237); then setStartAndGoal's two searches (:167-189)
+  double* q = st->d_q;
+  uint8_t* flags = reinterpret_cast<uint8_t*>(q + QB_FLAGS);
+  int32_t* idx = reinterpret_cast<int32_t*>(q + QB_FLAGS) + 1;
+  double hq[14 + 2];
+  std::copy_n(start, 7, hq); std::copy_n(goal, 7, hq + 7);
+  hq[14] = pp->start_radius; hq[15] = pp->goal_radius;
+  TRY(copy_async(h, q + QB_START, hq, 14 * sizeof(double), cudaMemcpyHostToDevice, s));
+  TRY(copy_async(h, q + QB_RADIUS, hq + 14, 2 * sizeof(double), cudaMemcpyHostToDevice, s));
+  TRY(launch(h, goal_clip_kernel, 1, 1, 0, s, (const double*)(q + QB_GOAL), st->space, q + QB_CLIPPED, flags + 1));
+  TRY(pose_from_2d(h, q + QB_CLIPPED, 1, q + QB_PROJECTED, flags, s));
+  o.start_draw = st->start_draw; o.goal_draw = st->goal_draw;
+  TRY(ball_search(h, q + QB_START, 1, q + QB_RADIUS, pp->n_iter, pp->seed, st->start_draw, q + QB_REPAIRED, idx, s));
+  TRY(ball_search(h, q + QB_PROJECTED, 1, q + QB_RADIUS + 1, pp->n_iter, ~pp->seed, st->goal_draw, q + QB_REPAIRED + 7, idx + 1, s));
+  TRY(record(h, st, 3));
+  TRY(host_call_end(h, true));
+  // baseSolve on the device roadmap with the device endpoints
+  if (st->path_cap < pp->vertex_capacity) {
+    cudaFree(st->d_path); st->d_path = nullptr; st->path_cap = 0;
+    CU_TRY(h, cudaMalloc(&st->d_path, pp->vertex_capacity * 7 * sizeof(double)));
+    st->path_cap = pp->vertex_capacity;
+  }
+  size_t n_solved = 0;
+  double cost = 0.0;
+  TRY(roadmap_solve(h, nullptr, nullptr, q + QB_REPAIRED, &st->space, nullptr, st->d_path, st->path_cap, &n_solved, &cost, &o.solve));
+  TRY(record(h, st, 4));
+  o.status = planner_status(o.solve.status);
+  o.path_cost = cost;
+  size_t n_out = 0;
+  int rc = ARTP_OK;
+  if (o.status == ARTP_PLANNER_SOLVED && pp->simplify) {   // getSolutionPath(true) under MotionCostObjective
+    o.simplify_seed = pp->seed + st->simplify_calls;
+    st->simplify_calls += 1;
+    rc = simplify_path(h, nullptr, st->d_path, n_solved, &st->space, ARTP_OBJ_LEARNED, pp->max_query_edge_length, o.simplify_seed,
+                       path, capacity, &n_out, &o.simplify);
+  } else if (o.status == ARTP_PLANNER_SOLVED) {
+    n_out = n_solved;
+    if (n_out > capacity) { h->err = "capacity too small"; rc = ARTP_E_LIMIT; }
+    else if (path) {
+      TRY(copy_async(h, path, st->d_path, n_out * 7 * sizeof(double), cudaMemcpyDeviceToHost, s));
+      TRY(sync_stream(h, s));
+    }
+  }
+  // the record of the query: endpoints, ball indices, flags (one copy at the end)
+  TRY(host_call_begin(h));
+  TRY(record(h, st, 5));
+  double qb[QB_MINMAX];
+  TRY(copy_async(h, qb, q, sizeof(qb), cudaMemcpyDeviceToHost, s));
+  TRY(host_call_end(h));
+  const uint8_t* fb = reinterpret_cast<const uint8_t*>(qb + QB_FLAGS);
+  const int32_t* ib = reinterpret_cast<const int32_t*>(qb + QB_FLAGS) + 1;
+  o.goal_inside = fb[0]; o.goal_clipped = fb[1];
+  o.start_index = ib[0]; o.goal_index = ib[1];
+  std::copy_n(qb + QB_CLIPPED, 7, o.goal_clipped_state);
+  std::copy_n(qb + QB_PROJECTED, 7, o.goal_projected);
+  std::copy_n(qb + QB_REPAIRED, 7, o.start_repaired);
+  std::copy_n(qb + QB_REPAIRED + 7, 7, o.goal_repaired);
+  // the searches' streams advance by what the reference's loops draw (StartState.sampleGoal's mirror)
+  st->start_draw += o.start_index >= 0 ? (uint64_t)o.start_index : pp->n_iter;
+  st->goal_draw += o.goal_index >= 0 ? (uint64_t)o.goal_index : pp->n_iter;
+  float* ms[5] = {&o.ms_sample_graph, &o.ms_update_edges, &o.ms_endpoints, &o.ms_solve, &o.ms_simplify};
+  const int from[5] = {0, 1, 2, 3, 4}, to[5] = {1, 2, 3, 4, 5};
+  for (int k = 0; k < 5; ++k) CU_TRY(h, cudaEventElapsedTime(ms[k], st->ev[from[k]], st->ev[to[k]]));
+  roadmap_counts(h, &nv, &ne);
+  o.n_vertices = nv; o.n_edges = ne;
+  o.host_syncs = h->traffic.syncs - t0.syncs;
+  o.bytes_h2d = h->traffic.h2d - t0.h2d;
+  o.bytes_d2h = h->traffic.d2h - t0.d2h;
+  if (info) *info = o;
+  if (rc != ARTP_OK) return rc;
+  if (n_path) *n_path = n_out;
+  return ARTP_OK;
+}
+
+}  // extern "C"

@@ -108,12 +108,10 @@ int queue_milestone(Handle* h, Roadmap* r, const double* d_cand, uint32_t i, uin
 
 // The host's control block to the device (h_ctl is current: every roadmap call ends with it copied back).
 int put_ctl(Handle* h, Roadmap* r, cudaStream_t s) {
-  CU_TRY(h, cudaMemcpyAsync(r->dev.ctl, r->h_ctl, sizeof(artp::RoadmapCtl), cudaMemcpyHostToDevice, s));
-  return ARTP_OK;
+  return copy_async(h, r->dev.ctl, r->h_ctl, sizeof(artp::RoadmapCtl), cudaMemcpyHostToDevice, s);
 }
 int get_ctl(Handle* h, Roadmap* r, cudaStream_t s) {
-  CU_TRY(h, cudaMemcpyAsync(r->h_ctl, r->dev.ctl, sizeof(artp::RoadmapCtl), cudaMemcpyDeviceToHost, s));
-  return ARTP_OK;
+  return copy_async(h, r->h_ctl, r->dev.ctl, sizeof(artp::RoadmapCtl), cudaMemcpyDeviceToHost, s);
 }
 
 int stopped_full(Handle* h, const Roadmap* r) {
@@ -141,10 +139,7 @@ void artp_api::roadmap_free(Handle* h) {
   h->roadmap = nullptr;
 }
 
-extern "C" {
-
-int artp_roadmap_clear(artp_handle* hh, size_t vertex_capacity, size_t edge_capacity) {
-  LOCK_CALL(h, hh);
+int artp_api::roadmap_clear(Handle* h, size_t vertex_capacity, size_t edge_capacity) {
   if (vertex_capacity == 0 || edge_capacity == 0 || vertex_capacity >= 0x7FFFFFFFull || edge_capacity >= 0x7FFFFFFFull) {
     h->err = "roadmap capacities must be > 0 and < 2^31"; return ARTP_E_INVALID;
   }
@@ -210,32 +205,8 @@ int artp_roadmap_clear(artp_handle* hh, size_t vertex_capacity, size_t edge_capa
   return host_call_end(h);
 }
 
-int artp_roadmap_add_milestones(artp_handle* hh, const double* states, size_t n) {
-  LOCK_CALL(h, hh);
-  TRY(require_roadmap(h));
-  TRY(require_whole_map(h));
-  if (n == 0) return ARTP_OK;
-  if (!states) return null_buffer(h);
-  Roadmap* r = h->roadmap;
-  for (size_t i = 0; i < n * 7; ++i)
-    if (!std::isfinite(states[i])) { h->err = "non-finite milestone state"; return ARTP_E_INVALID; }
-  for (size_t i = 0; i < n; ++i) grow_box(r, states[i * 7], states[i * 7 + 1], states[i * 7], states[i * 7 + 1]);
-  TRY(fit_interior(h, r));
-  char* d_states;
-  TRY(host_call_begin(h, {n * 7 * sizeof(double)}, &d_states));
-  cudaStream_t s = h->stream;
-  CU_TRY(h, cudaMemcpyAsync(d_states, states, n * 7 * sizeof(double), cudaMemcpyHostToDevice, s));
-  TRY(put_ctl(h, r, s));
-  int rc = ARTP_OK;
-  for (size_t i = 0; i < n && rc == ARTP_OK; ++i)
-    rc = queue_milestone(h, r, (const double*)d_states, (uint32_t)i, ARTP_ROADMAP_MILESTONE | ARTP_ROADMAP_QUERY, s);
-  if (rc == ARTP_OK) rc = get_ctl(h, r, s);
-  return finish(h, r, rc);
-}
-
-int artp_roadmap_sample_graph(artp_handle* hh, const artp_roadmap_params* rp, const artp_sample_distribution_params* dp,
-                              uint64_t seed, uint64_t first_sample, uint64_t* draws_used) {
-  LOCK_CALL(h, hh);
+int artp_api::roadmap_sample_graph(Handle* h, const artp_roadmap_params* rp, const artp_sample_distribution_params* dp,
+                                   uint64_t seed, uint64_t first_sample, uint64_t* draws_used) {
   if (!rp) { h->err = "null roadmap params"; return ARTP_E_INVALID; }
   TRY(sampler_armed(h));
   TRY(require_whole_map(h));
@@ -268,8 +239,8 @@ int artp_roadmap_sample_graph(artp_handle* hh, const artp_roadmap_params* rp, co
     const size_t B = (size_t)std::max<double>(1.0, std::min<double>({std::ceil(guess) + 4.0, (double)room, (double)kMaxRound}));
     const uint64_t n_draw = std::min<uint64_t>(end - draw, (uint64_t)std::max(4096.0, 1.25 * (double)B / accept));
     if ((rc = sample_valid_draws(h, seed, draw, (size_t)n_draw, r->d_cand, r->d_draws, B, r->d_count, s))) break;
-    CU_TRY(h, cudaMemcpyAsync(r->h_count, r->d_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-    CU_TRY(h, cudaStreamSynchronize(s));
+    TRY(copy_async(h, r->h_count, r->d_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    TRY(sync_stream(h, s));
     const uint32_t count = *r->h_count;
     accept = std::max(1e-4, (double)count / (double)n_draw);
     const size_t C = std::min<size_t>(count, B);
@@ -280,8 +251,8 @@ int artp_roadmap_sample_graph(artp_handle* hh, const artp_roadmap_params* rp, co
     for (size_t i = 0; i < C && rc == ARTP_OK; ++i) rc = queue_milestone(h, r, r->d_cand, (uint32_t)i, ARTP_ROADMAP_MILESTONE, s);
     if (rc) break;
     if ((rc = get_ctl(h, r, s))) break;
-    CU_TRY(h, cudaMemcpyAsync(r->h_draws, r->d_draws, C * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
-    CU_TRY(h, cudaStreamSynchronize(s));
+    TRY(copy_async(h, r->h_draws, r->d_draws, C * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+    TRY(sync_stream(h, s));
     if (c.stop & (artp::RM_STOP_FULL | artp::RM_STOP_INTERIOR)) {
       if (c.done) draw = r->h_draws[c.done - 1] + 1;
       break;
@@ -303,28 +274,7 @@ int artp_roadmap_sample_graph(artp_handle* hh, const artp_roadmap_params* rp, co
   return finish(h, r, rc);
 }
 
-int artp_roadmap_get(artp_handle* hh, size_t first_vertex, double* states, uint8_t* kinds, size_t first_edge, uint32_t* edges,
-                     size_t* nv, size_t* ne) {
-  LOCK_CALL(h, hh);
-  TRY(require_roadmap(h));
-  Roadmap* r = h->roadmap;
-  const size_t V = r->h_ctl->V, E = r->h_ctl->E;
-  if (first_vertex > V || first_edge > E) { h->err = "roadmap cursor past the end"; return ARTP_E_INVALID; }
-  TRY(host_call_begin(h));
-  cudaStream_t s = h->stream;
-  const size_t tv = V - first_vertex, te = E - first_edge;
-  if (states && tv)
-    CU_TRY(h, cudaMemcpyAsync(states, r->dev.states + first_vertex * 7, tv * 7 * sizeof(double), cudaMemcpyDeviceToHost, s));
-  if (kinds && tv) CU_TRY(h, cudaMemcpyAsync(kinds, r->dev.kind + first_vertex, tv, cudaMemcpyDeviceToHost, s));
-  if (edges && te)
-    CU_TRY(h, cudaMemcpyAsync(edges, r->dev.edges + first_edge * 2, te * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-  if (nv) *nv = V;
-  if (ne) *ne = E;
-  return host_call_end(h);
-}
-
-int artp_roadmap_update_edges(artp_handle* hh) {
-  LOCK_CALL(h, hh);
+int artp_api::roadmap_update_edges(Handle* h) {
   TRY(require_roadmap(h));
   Roadmap* r = h->roadmap;
   const size_t E = r->h_ctl->E;
@@ -335,17 +285,17 @@ int artp_roadmap_update_edges(artp_handle* hh) {
   return host_call_end(h);
 }
 
-int artp_roadmap_solve(artp_handle* hh, const double* start, const double* goal, const artp_se3_space* space,
-                       double* path_states, size_t path_capacity, size_t* n_path, double* cost,
-                       artp_roadmap_solve_info* info) {
-  LOCK_CALL(h, hh);
+int artp_api::roadmap_solve(Handle* h, const double* start, const double* goal, const double* d_sg, const artp_se3_space* space,
+                            double* path_states, double* d_path_out, size_t path_capacity, size_t* n_path, double* cost,
+                            artp_roadmap_solve_info* info) {
   TRY(require_roadmap(h));
   TRY(require_whole_map(h));
-  if (!start || !goal || !space) return null_buffer(h);
+  if (!space) return null_buffer(h);
   Roadmap* r = h->roadmap;
   artp::QueryDev& q = r->q;
-  for (int i = 0; i < 7; ++i)
-    if (!std::isfinite(start[i]) || !std::isfinite(goal[i])) { h->err = "non-finite start or goal"; return ARTP_E_INVALID; }
+  if (!d_sg)
+    for (int i = 0; i < 7; ++i)
+      if (!std::isfinite(start[i]) || !std::isfinite(goal[i])) { h->err = "non-finite start or goal"; return ARTP_E_INVALID; }
   // the segment lengths of artp_valid_segment_count
   const double frac = space->longest_valid_segment_fraction > 0 ? space->longest_valid_segment_fraction : 0.01;
   double e2 = 0;
@@ -361,18 +311,36 @@ int artp_roadmap_solve(artp_handle* hh, const double* start, const double* goal,
   if (n_path) *n_path = 0;
   artp_roadmap_solve_info out{};
   out.path_vertices = info ? info->path_vertices : nullptr;
-  // SE3StateSpace::satisfiesBounds: the position inside the RealVectorBounds
-  for (int w = 0; w < 2; ++w)
-    for (int i = 0; i < 3; ++i) {
-      const double x = (w ? goal : start)[i];
-      if (x < space->low[i] || x > space->high[i]) {
-        out.status = w ? ARTP_SOLVE_INVALID_GOAL : ARTP_SOLVE_INVALID_START;
-        if (info) *info = out;
-        return ARTP_OK;
-      }
+  double xy[4];   // (x, y) of start and goal
+  if (d_sg) {      // the device's verdict (endpoint_check) and the (x, y) that size the interior-state buffer
+    double* d_chk;
+    double chk[5];
+    TRY(host_call_begin(h, {sizeof(chk)}, (char**)&d_chk));
+    TRY(endpoint_check(h, d_sg, space, d_chk, h->stream));
+    TRY(copy_async(h, chk, d_chk, sizeof(chk), cudaMemcpyDeviceToHost, h->stream));
+    TRY(host_call_end(h));
+    if (chk[0] == -1.0) { h->err = "non-finite start or goal"; return ARTP_E_INVALID; }
+    if (chk[0] != 0.0) {
+      out.status = (int32_t)chk[0];
+      if (info) *info = out;
+      return ARTP_OK;
     }
-  grow_box(r, start[0], start[1], start[0], start[1]);
-  grow_box(r, goal[0], goal[1], goal[0], goal[1]);
+    std::copy_n(chk + 1, 4, xy);
+  } else {
+    // SE3StateSpace::satisfiesBounds: the position inside the RealVectorBounds
+    for (int w = 0; w < 2; ++w)
+      for (int i = 0; i < 3; ++i) {
+        const double x = (w ? goal : start)[i];
+        if (x < space->low[i] || x > space->high[i]) {
+          out.status = w ? ARTP_SOLVE_INVALID_GOAL : ARTP_SOLVE_INVALID_START;
+          if (info) *info = out;
+          return ARTP_OK;
+        }
+      }
+    xy[0] = start[0]; xy[1] = start[1]; xy[2] = goal[0]; xy[3] = goal[1];
+  }
+  grow_box(r, xy[0], xy[1], xy[0], xy[1]);
+  grow_box(r, xy[2], xy[3], xy[2], xy[3]);
   TRY(fit_interior(h, r));
   q.qcap = (uint32_t)std::min<size_t>(r->icap, artp::kQueryBatch);
   const uint32_t slice_cap = (r->dev.vcap + artp::kSearchCtas - 1) / artp::kSearchCtas;
@@ -387,13 +355,16 @@ int artp_roadmap_solve(artp_handle* hh, const double* start, const double* goal,
   TRY(host_call_begin(h, {14 * sizeof(double), n_price * 6 * sizeof(float), n_price * 3 * sizeof(float),
                           out_cap * 7 * sizeof(double)}, reg));
   cudaStream_t s = h->stream;
-  const double* d_sg = (const double*)reg[0];
-  CU_TRY(h, cudaMemcpyAsync(reg[0], start, 7 * sizeof(double), cudaMemcpyHostToDevice, s));
-  CU_TRY(h, cudaMemcpyAsync(reg[0] + 7 * sizeof(double), goal, 7 * sizeof(double), cudaMemcpyHostToDevice, s));
+  if (!d_sg) {
+    TRY(copy_async(h, reg[0], start, 7 * sizeof(double), cudaMemcpyHostToDevice, s));
+    TRY(copy_async(h, reg[0] + 7 * sizeof(double), goal, 7 * sizeof(double), cudaMemcpyHostToDevice, s));
+    d_sg = (const double*)reg[0];
+  }
+  double* d_path = d_path_out ? d_path_out : (double*)reg[3];
   TRY(put_ctl(h, r, s));
   *r->h_q = artp::QueryCtl{};
   r->h_q->two = 2;
-  CU_TRY(h, cudaMemcpyAsync(q.ctl, r->h_q, sizeof(artp::QueryCtl), cudaMemcpyHostToDevice, s));
+  TRY(copy_async(h, q.ctl, r->h_q, sizeof(artp::QueryCtl), cudaMemcpyHostToDevice, s));
   CU_TRY(h, cudaMemsetAsync(q.csr_len, 0, (size_t)r->dev.vcap * sizeof(uint32_t), s));
   const unsigned vgrid = grid_for(h, r->dev.vcap, 256, 4), egrid = grid_for(h, r->dev.ecap, 256, 4);
   int rc = ARTP_OK;
@@ -427,21 +398,21 @@ int artp_roadmap_solve(artp_handle* hh, const double* start, const double* goal,
     }
     if (rc != ARTP_OK) break;
     step(get_ctl(h, r, s));
-    CU_TRY(h, cudaMemcpyAsync(r->h_q, q.ctl, sizeof(artp::QueryCtl), cudaMemcpyDeviceToHost, s));
-    CU_TRY(h, cudaStreamSynchronize(s));
+    TRY(copy_async(h, r->h_q, q.ctl, sizeof(artp::QueryCtl), cudaMemcpyDeviceToHost, s));
+    TRY(sync_stream(h, s));
     if (r->h_q->status != artp::Q_RUNNING || r->h_ctl->stop) break;
     if (round > max_rounds) { h->err = "query did not end"; rc = ARTP_E_LIMIT; }
   }
   const artp::QueryCtl& c = *r->h_q;
   if (rc == ARTP_OK && c.status == ARTP_SOLVE_SOLVED) {
-    step(launch(h, artp::query_finish_kernel, 1, 256, 0, s, r->dev, q, r->d_path_idx, (double*)reg[3], (uint32_t)out_cap));
+    step(launch(h, artp::query_finish_kernel, 1, 256, 0, s, r->dev, q, r->d_path_idx, d_path, (uint32_t)out_cap));
     if (rc == ARTP_OK) {
-      CU_TRY(h, cudaMemcpyAsync(r->h_q, q.ctl, sizeof(artp::QueryCtl), cudaMemcpyDeviceToHost, s));
+      TRY(copy_async(h, r->h_q, q.ctl, sizeof(artp::QueryCtl), cudaMemcpyDeviceToHost, s));
       const size_t n = c.path_n;   // read by the rounds' copy: the finish kernel does not change it
       if (n <= path_capacity) {
-        if (path_states) CU_TRY(h, cudaMemcpyAsync(path_states, reg[3], n * 7 * sizeof(double), cudaMemcpyDeviceToHost, s));
+        if (path_states && !d_path_out) TRY(copy_async(h, path_states, d_path, n * 7 * sizeof(double), cudaMemcpyDeviceToHost, s));
         if (out.path_vertices)
-          CU_TRY(h, cudaMemcpyAsync(out.path_vertices, r->d_path_idx, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+          TRY(copy_async(h, out.path_vertices, r->d_path_idx, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
       }
     }
   }
@@ -456,6 +427,82 @@ int artp_roadmap_solve(artp_handle* hh, const double* start, const double* goal,
   if (cost) *cost = c.cost;
   if (c.path_n > path_capacity) { h->err = "path_capacity too small"; return ARTP_E_LIMIT; }
   return ARTP_OK;
+}
+
+bool artp_api::has_roadmap(const Handle* h) { return h->roadmap && h->roadmap->dev.ctl; }
+
+void artp_api::roadmap_counts(const Handle* h, size_t* nv, size_t* ne) {
+  *nv = h->roadmap->h_ctl->V;
+  *ne = h->roadmap->h_ctl->E;
+}
+
+extern "C" {
+
+int artp_roadmap_clear(artp_handle* hh, size_t vertex_capacity, size_t edge_capacity) {
+  LOCK_CALL(h, hh);
+  return roadmap_clear(h, vertex_capacity, edge_capacity);
+}
+
+int artp_roadmap_add_milestones(artp_handle* hh, const double* states, size_t n) {
+  LOCK_CALL(h, hh);
+  TRY(require_roadmap(h));
+  TRY(require_whole_map(h));
+  if (n == 0) return ARTP_OK;
+  if (!states) return null_buffer(h);
+  Roadmap* r = h->roadmap;
+  for (size_t i = 0; i < n * 7; ++i)
+    if (!std::isfinite(states[i])) { h->err = "non-finite milestone state"; return ARTP_E_INVALID; }
+  for (size_t i = 0; i < n; ++i) grow_box(r, states[i * 7], states[i * 7 + 1], states[i * 7], states[i * 7 + 1]);
+  TRY(fit_interior(h, r));
+  char* d_states;
+  TRY(host_call_begin(h, {n * 7 * sizeof(double)}, &d_states));
+  cudaStream_t s = h->stream;
+  CU_TRY(h, cudaMemcpyAsync(d_states, states, n * 7 * sizeof(double), cudaMemcpyHostToDevice, s));
+  TRY(put_ctl(h, r, s));
+  int rc = ARTP_OK;
+  for (size_t i = 0; i < n && rc == ARTP_OK; ++i)
+    rc = queue_milestone(h, r, (const double*)d_states, (uint32_t)i, ARTP_ROADMAP_MILESTONE | ARTP_ROADMAP_QUERY, s);
+  if (rc == ARTP_OK) rc = get_ctl(h, r, s);
+  return finish(h, r, rc);
+}
+
+int artp_roadmap_sample_graph(artp_handle* hh, const artp_roadmap_params* rp, const artp_sample_distribution_params* dp,
+                              uint64_t seed, uint64_t first_sample, uint64_t* draws_used) {
+  LOCK_CALL(h, hh);
+  return roadmap_sample_graph(h, rp, dp, seed, first_sample, draws_used);
+}
+
+int artp_roadmap_get(artp_handle* hh, size_t first_vertex, double* states, uint8_t* kinds, size_t first_edge, uint32_t* edges,
+                     size_t* nv, size_t* ne) {
+  LOCK_CALL(h, hh);
+  TRY(require_roadmap(h));
+  Roadmap* r = h->roadmap;
+  const size_t V = r->h_ctl->V, E = r->h_ctl->E;
+  if (first_vertex > V || first_edge > E) { h->err = "roadmap cursor past the end"; return ARTP_E_INVALID; }
+  TRY(host_call_begin(h));
+  cudaStream_t s = h->stream;
+  const size_t tv = V - first_vertex, te = E - first_edge;
+  if (states && tv)
+    CU_TRY(h, cudaMemcpyAsync(states, r->dev.states + first_vertex * 7, tv * 7 * sizeof(double), cudaMemcpyDeviceToHost, s));
+  if (kinds && tv) CU_TRY(h, cudaMemcpyAsync(kinds, r->dev.kind + first_vertex, tv, cudaMemcpyDeviceToHost, s));
+  if (edges && te)
+    CU_TRY(h, cudaMemcpyAsync(edges, r->dev.edges + first_edge * 2, te * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  if (nv) *nv = V;
+  if (ne) *ne = E;
+  return host_call_end(h);
+}
+
+int artp_roadmap_update_edges(artp_handle* hh) {
+  LOCK_CALL(h, hh);
+  return roadmap_update_edges(h);
+}
+
+int artp_roadmap_solve(artp_handle* hh, const double* start, const double* goal, const artp_se3_space* space,
+                       double* path_states, size_t path_capacity, size_t* n_path, double* cost,
+                       artp_roadmap_solve_info* info) {
+  LOCK_CALL(h, hh);
+  if (!start || !goal) return null_buffer(h);
+  return roadmap_solve(h, start, goal, nullptr, space, path_states, nullptr, path_capacity, n_path, cost, info);
 }
 
 int artp_roadmap_get_edge_costs(artp_handle* hh, size_t first_edge, double* cost, uint8_t* flags, size_t* n_live) {

@@ -537,6 +537,111 @@ int artp_simplify_path(artp_handle* h, const double* path, size_t n, const artp_
 int artp_debug_se3_ops(artp_handle* h, const double* a, const double* b, const double* t, size_t n, double* dist,
                        double* interp);
 
+/* ---- the planner: Planner::setMap and Planner::plan + getSolutionPath for prm_motion_cost (planner.cpp:135-298) ----
+ * The shipped replan (PlannerRos::updateMapAndPlanFromCurrentRobotPose, planner.name prm_motion_cost,
+ * simplify_solution true) as two calls whose stages hand data to each other in device memory: no layer, state or path
+ * goes through host memory between them. The host reads only control words: the finite range of the raw elevation, the
+ * compact-code scales of the two uploaded layers, the loops' control blocks (sampleGraph, solve, simplify), the endpoints'
+ * bounds verdict with their (x, y) (they size the roadmap's interior-state buffer), the learned cost's piece total and
+ * per-edge costs, and at the end the returned path and the info record.
+ *
+ * artp_planner_set_map   Planner::setMap (:135-163) and Map::setMap's new-map chain (setUpMapProcessors, :39-58):
+ *   observed           addKnownCells (basic.cpp:25-38): 1 where elevation and traversability (Map::setMap's basic layers,
+ *                      map.cpp:16) are finite -- grid_map's isValid, which is not in the reference tree (unpinned
+ *                      restatement). A NULL traversability is checkTraversability's 1.0 layer (basic.cpp:13-21).
+ *   SE(3) bounds       x: cx -+ rows * res (the FULL length, not half of it), y: cy -+ cols * res, z:
+ *                      (double)minCoeffOfFinites(raw elevation) - reach_z / 2 .. (double)maxCoeffOfFinites(..) + reach_z / 2,
+ *                      from the RAW layer, before any processing; -0 is taken as +0. Min and max are order-free: exact.
+ *                      A layer with no finite cell: ARTP_E_INVALID (grid_map's result there is not pinned).
+ *   Basic              artp_process_basic on the INPAINTED layers (TELEA inpainting, which also quantises finite cells to
+ *                      8 bits, stays with the caller: always pass inpaintMatrix's output), then the map upload of the
+ *                      inpainted elevation and elevation_masked straight from device memory (artp_set_map's rules).
+ *   the chain          artp_estimate_normals ((torso.length + torso.width) * 0.25); with sample_from_distribution the
+ *                      sample filter, the distribution without vertices and its CDF; the sampler armed with the bounds' x / y;
+ *                      artp_update_features when weights are loaded.
+ *   generation         a map counter, +1 per installed map: it stands in for the grid_map timestamp that
+ *                      PRMMotionCostMaintainer::sampleGraph compares (prm_motion_cost.cpp:146-153).
+ * Layers are HOST pointers in grid_map layout (artp_set_map). Every check runs before the installed map changes, and a
+ * refused map leaves the previous one installed. The checks are the arguments, the structuring elements' and the blur's
+ * size limits (ARTP_E_LIMIT, as the chained calls) and the finite cell (found by the bounds' reduction). Only a CUDA error
+ * after that leaves no planner map. info (nullable) receives the call's host synchronisations and bytes copied. artp_set_map / artp_set_map_window install a map the planner does not own: artp_plan then
+ * answers NO_MAP.
+ *
+ * artp_plan   Planner::plan (:193-262) + getSolutionPath (:266-298), in the reference's order:
+ *   1. no planner map: status NO_MAP (a map window: ARTP_E_INVALID); no weights or features: ARTP_E_NOWEIGHTS.
+ *   2. clear_roadmap: PRMMotionCost::clear (the ROS node's ss_->clear(), planner_ros.cpp:359,373); the first plan of a
+ *      handle creates the store (vertex_capacity, edge_capacity).
+ *   3. sampleGraph + updateEdges (artp_roadmap_sample_graph, artp_roadmap_update_edges) ONLY when the map generation
+ *      differs from the one the last sampleGraph saw. So clear_roadmap on an unchanged map plans on a roadmap that holds
+ *      only start and goal: the reference's behaviour, reproduced on purpose.
+ *   4. the goal: satisfiesBounds, else enforceBounds (:207-221), then the projection when (x, y) lies on the map (:223-237,
+ *      artp_pose_from_2d). OMPL 1.4.2 is not in the tree; restated (unpinned): R3 passes when no coordinate has
+ *      v - DBL_EPSILON > high or v + DBL_EPSILON < low, and enforceBounds clamps; SO3 passes when |norm - 1| < 1e-9
+ *      (MAX_QUATERNION_NORM_ERROR), and enforceBounds acts when |x^2 + y^2 + z^2 + w^2 - 1| > DBL_EPSILON: the identity
+ *      when the norm is below DBL_EPSILON, else each component divided by the norm. A failing test applies both
+ *      components' enforceBounds. The start is neither clipped nor projected.
+ *   5. setStartAndGoal (:167-189): the start search (start_radius) and the goal search (goal_radius), artp_find_valid_near.
+ *   6. baseSolve on the device roadmap, as artp_roadmap_solve defines it, from the device endpoints.
+ *   7. solved and simplify: artp_simplify_path under ARTP_OBJ_LEARNED at max_query_edge_length, from the device path.
+ * Status (planner_status.h, planner.cpp:254-261): ARTP_SOLVE_NOT_CONNECTED and NO_FEASIBLE_PATH become NOT_SOLVED,
+ * INVALID_START / INVALID_GOAL pass through. Unsolved: no path (*n_path = 0), as getSolutionPath throws.
+ * Streams, all from `seed`: the sampler's "ARTP" stream (key seed) from draw info.first_sample; the start search's "ARTB"
+ * stream (key seed) from info.start_draw and the goal search's (key ~seed) from info.goal_draw, each advanced like
+ * StartState.sampleGoal's mirror (k draws for candidate k, n_iter when none is valid); the simplifier's key seed + c for the
+ * handle's c-th simplify. A new seed restarts every position at 0. info reports the positions used, so the same replan
+ * through the chained public calls gives the same result bit for bit.
+ * path: HOST buffer of capacity states (nullable); a path above capacity: ARTP_E_LIMIT, nothing written. Bad parameters, a
+ * non-finite start / goal or an n_iter of 2^32 - 1 (ARTP_E_INVALID), and the distribution's limits for sampleGraph's
+ * recomputes (artp_update_sample_distribution's codes) are checked before any work. */
+#define ARTP_PLANNER_UNKNOWN        0   /* art_planner::PlannerStatus (planner_status.h) */
+#define ARTP_PLANNER_INVALID_START  1
+#define ARTP_PLANNER_INVALID_GOAL   2
+#define ARTP_PLANNER_NO_MAP         3
+#define ARTP_PLANNER_NOT_SOLVED     4
+#define ARTP_PLANNER_SOLVED         5
+typedef struct artp_planner_params {
+  double   start_radius, goal_radius;                 /* start_goal_search, params.h:38-40 */
+  uint32_t n_iter;
+  size_t   max_n_vertices, max_n_edges, recompute_density_after_n_samples;   /* prm_motion_cost, params.h:51-53 */
+  double   max_query_edge_length;                     /* params.h:54; > 0 when simplify */
+  uint64_t max_draws;                                 /* sampler draws per sampleGraph: replaces max_sample_time */
+  size_t   vertex_capacity, edge_capacity;            /* the roadmap store (artp_roadmap_clear) */
+  double   max_roll_pert, max_pitch_pert;             /* sampler, params.h:79-84 */
+  int      sample_from_distribution, use_inverse_vertex_density, use_max_prob_unknown_samples;
+  double   max_prob_unknown_samples;
+  artp_basic_params basic;                            /* params.h:23-35 */
+  int      simplify, clear_roadmap;                   /* simplify_solution; the ROS node's ss_->clear() */
+  uint64_t seed;
+} artp_planner_params;
+typedef struct artp_plan_info {
+  int32_t  status;                      /* ARTP_PLANNER_* */
+  int32_t  sampled;                     /* sampleGraph and updateEdges ran (the map generation changed) */
+  uint64_t first_sample, draws_used;    /* sampler draws used: first_sample .. first_sample + draws_used - 1 */
+  uint64_t start_draw, goal_draw;       /* the first draws of the two searches */
+  uint64_t simplify_seed;               /* artp_simplify_path's seed (when it ran) */
+  uint64_t n_vertices, n_edges;         /* the roadmap after the plan */
+  artp_roadmap_solve_info solve;        /* path_vertices: in, nullable */
+  double   path_cost;                   /* artp_roadmap_solve's *cost of the solved path */
+  artp_simplify_info simplify;          /* zero unless the simplifier ran */
+  int32_t  goal_clipped, goal_inside;   /* enforceBounds applied; the projection applied */
+  int32_t  start_index, goal_index;     /* the searches' candidate indices (-1: none valid) */
+  double   goal_clipped_state[7], goal_projected[7], start_repaired[7], goal_repaired[7];
+  float    ms_sample_graph, ms_update_edges, ms_endpoints, ms_solve, ms_simplify;   /* events on the call's stream */
+  uint32_t host_syncs;                  /* host synchronisations of the call */
+  uint64_t bytes_h2d, bytes_d2h;        /* bytes the call copied host -> device and device -> host */
+} artp_plan_info;
+typedef struct artp_planner_map_info {
+  uint32_t host_syncs;                  /* host synchronisations of the call */
+  uint64_t bytes_h2d, bytes_d2h;        /* bytes the call copied host -> device and device -> host */
+} artp_planner_map_info;
+int artp_planner_set_map(artp_handle* h, const artp_planner_params* pp, const float* elevation, const float* traversability,
+                         const float* elevation_inpainted, const float* traversability_inpainted, int rows, int cols,
+                         double res, double cx, double cy, artp_planner_map_info* info);
+/* The artp_se3_space artp_planner_set_map installed (ARTP_E_NOMAP before). */
+int artp_planner_get_space(artp_handle* h, artp_se3_space* out);
+int artp_plan(artp_handle* h, const artp_planner_params* pp, const double* start, const double* goal, double* path,
+              size_t capacity, size_t* n_path, artp_plan_info* info);
+
 /* ---- learned motion cost (MotionCostFunc, objectives/motion_cost_objective.h:22-23) ------------------------------
  * Weights: ONE flat fp32 blob in the layer order of the reference's `network` module: init_conv1..5, init_flatten,
  * tar0_conv1, out0_conv1, out1_conv1..3 -- each conv.weight [Cout][Cin][kh][kw] followed by its BatchNorm weight, bias,

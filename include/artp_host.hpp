@@ -513,6 +513,85 @@ class PathSimplifier {
   uint64_t seed_;
 };
 
+// art_planner::PlannerStatus (planner_status.h).
+enum PlannerStatus { UNKNOWN = ARTP_PLANNER_UNKNOWN, INVALID_START = ARTP_PLANNER_INVALID_START,
+                     INVALID_GOAL = ARTP_PLANNER_INVALID_GOAL, NO_MAP = ARTP_PLANNER_NO_MAP,
+                     NOT_SOLVED = ARTP_PLANNER_NOT_SOLVED, SOLVED = ARTP_PLANNER_SOLVED };
+
+// art_planner::Planner for planner.name prm_motion_cost (planner.cpp:135-298) on the device: setMap is
+// artp_planner_set_map, plan is artp_plan (the simplification of getSolutionPath(true) runs inside it when
+// parameters().simplify is set), and the stages hand data to each other in device memory. The parameters start from
+// Params (caps, max_query_edge_length, sampler) and the shipped values of params.yaml for the rest; change them through
+// parameters(). With -DARTP_WITH_OMPL, getSolutionPath(si) builds the returned og::PathGeometric.
+class Planner {
+ public:
+  explicit Planner(const StateValidityCheckerPtr& checker) : checker_(checker) {
+    const Params& p = checker->handle()->params();
+    pp_.start_radius = 0.2; pp_.goal_radius = 0.5; pp_.n_iter = 1000;   // params.yaml:20-22
+    pp_.max_n_vertices = p.planner.prm_motion_cost.max_n_vertices;
+    pp_.max_n_edges = p.planner.prm_motion_cost.max_n_edges;
+    pp_.recompute_density_after_n_samples = p.planner.prm_motion_cost.recompute_density_after_n_samples;
+    pp_.max_query_edge_length = p.planner.prm_motion_cost.max_query_edge_length;
+    pp_.max_draws = 1ull << 26;
+    pp_.vertex_capacity = 2 * (size_t)pp_.max_n_vertices; pp_.edge_capacity = (size_t)pp_.max_n_edges + 10000;
+    pp_.max_roll_pert = p.sampler.max_roll_pert; pp_.max_pitch_pert = p.sampler.max_pitch_pert;
+    pp_.sample_from_distribution = p.sampler.sample_from_distribution;
+    pp_.use_inverse_vertex_density = p.sampler.use_inverse_vertex_density;
+    pp_.use_max_prob_unknown_samples = p.sampler.use_max_prob_unknown_samples;
+    pp_.max_prob_unknown_samples = p.sampler.max_prob_unknown_samples;
+    pp_.basic = artp_basic_params{0.15f, p.planner.unknown_space_untraversable ? 1 : 0, 0.3, 0.3, 0.3, 0.16, 0.3, 0.1};
+    pp_.simplify = 1; pp_.clear_roadmap = 0; pp_.seed = 0;
+  }
+  artp_planner_params& parameters() { return pp_; }
+
+  // Planner::setMap: elevation / traversability are the RAW layers (NaN unknown; traversability may be empty), the
+  // inpainted ones what inpaintMatrix returned for them (empty with an empty traversability). Geometry from `map`.
+  void setMap(const Map& map, const std::vector<float>& elevation, const std::vector<float>& traversability,
+              const std::vector<float>& elevation_inpainted, const std::vector<float>& traversability_inpainted) {
+    const auto& h = checker_->handle();
+    h->check(artp_planner_set_map(h->get(), &pp_, elevation.data(), traversability.empty() ? nullptr : traversability.data(),
+                                  elevation_inpainted.data(),
+                                  traversability_inpainted.empty() ? nullptr : traversability_inpainted.data(), map.rows,
+                                  map.cols, map.resolution, map.position_x, map.position_y, &map_info_),
+             "artp_planner_set_map");
+  }
+  artp_se3_space space() const {
+    artp_se3_space sp{};
+    checker_->handle()->check(artp_planner_get_space(checker_->handle()->get(), &sp), "artp_planner_get_space");
+    return sp;
+  }
+  PlannerStatus plan(const State& start, const State& goal) {
+    const auto& h = checker_->handle();
+    solved_ = false;                    // a failing call leaves no solution behind
+    path_.assign(4 * pp_.vertex_capacity + 64, State{});
+    size_t n = 0;
+    info_ = artp_plan_info{};
+    struct ClearOnThrow {
+      std::vector<State>& p; bool armed = true;
+      ~ClearOnThrow() { if (armed) p.clear(); }
+    } guard{path_};
+    h->check(artp_plan(h->get(), &pp_, &start.x, &goal.x, &path_[0].x, path_.size(), &n, &info_), "artp_plan");
+    guard.armed = false;
+    path_.resize(n);
+    solved_ = info_.status == ARTP_PLANNER_SOLVED;
+    return static_cast<PlannerStatus>(info_.status);
+  }
+  // The last plan's path (simplified when parameters().simplify is set); throws like planner.cpp:268-270.
+  const std::vector<State>& getSolutionPath() const {
+    if (!solved_) throw std::runtime_error("Requested failed solution path.");
+    return path_;
+  }
+  const artp_plan_info& info() const { return info_; }
+  const artp_planner_map_info& mapInfo() const { return map_info_; }   // the last setMap's syncs and bytes
+ private:
+  StateValidityCheckerPtr checker_;
+  artp_planner_params pp_{};
+  std::vector<State> path_;
+  artp_plan_info info_{};
+  artp_planner_map_info map_info_{};
+  bool solved_{false};
+};
+
 // ompl::base::MotionValidator as the reference uses it: discrete validation over isValid with nd segments.
 class MotionValidator {
  public:
@@ -865,6 +944,21 @@ inline og::PathGeometric getSolutionPath(const PathSimplifier& simplifier, const
     out.append(s);
   }
   out.getSpaceInformation()->freeState(s);
+  return out;
+}
+
+// Planner::getSolutionPath(simplify) for the Planner mirror: its last plan's path (simplified as its parameters say) as an
+// og::PathGeometric; throws like planner.cpp:268-270 when the plan did not solve.
+inline og::PathGeometric getSolutionPath(const Planner& planner, const ob::SpaceInformationPtr& si) {
+  og::PathGeometric out(si);
+  ob::State* s = si->allocState();
+  for (const State& t : planner.getSolutionPath()) {
+    auto* se3 = s->as<ob::SE3StateSpace::StateType>();
+    se3->setXYZ(t.x, t.y, t.z);
+    se3->rotation().x = t.qx; se3->rotation().y = t.qy; se3->rotation().z = t.qz; se3->rotation().w = t.qw;
+    out.append(s);
+  }
+  si->freeState(s);
   return out;
 }
 
