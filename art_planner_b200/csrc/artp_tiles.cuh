@@ -180,7 +180,7 @@ reach_groups_kernel(const Checker c, const __grid_constant__ CUtensorMap map1, c
   const Field& f = c.f[1];
   unsigned char* slots = warp_tile_slots(tile_smem, tc, 8, bars[wid]);   // [slot 0/1][group 0..3]
   uint16_t* tasks = tasks_all[wid][g];
-  uint32_t phase[2] = {0u, 0u};
+  uint32_t phase = 0u;                     // bit s: parity of tile slot s's barrier (a bit mask, not an indexed array)
   const uint32_t total = *rec_count;
   const unsigned gshift = (unsigned)g * 8u;
   // lanes 0, 8, 16, 24 read the zone origins of the four records of a round, lane 0 starts their copies
@@ -226,8 +226,8 @@ reach_groups_kernel(const Checker c, const __grid_constant__ CUtensorMap map1, c
       int alive = 0;
       if (act && gl == 0) alive = (*(volatile const uint8_t*)(w.valid + r.item) != 0);
       alive = __shfl_sync(kFull, alive, 0, 8);
-      mbar_wait(&bars[wid][slot], phase[slot]);
-      phase[slot] ^= 1u;
+      mbar_wait(&bars[wid][slot], (phase >> slot) & 1u);
+      phase ^= 1u << slot;
       __syncwarp();                        // lanes leave the barrier poll at different times
       bool gdone = !(act && alive);        // group-uniform
       BoxCtx b;
@@ -340,8 +340,10 @@ reach_groups_kernel(const Checker c, const __grid_constant__ CUtensorMap map1, c
               const int nc = box_plane(tb, pl, 4, cxs, czs);
               const int tcx = isUp ? ccx : ccx + 1, tcz = isUp ? ccz : ccz + 1;
               bool hit = false;
-#pragma unroll 1
-              for (int i = 0; i < nc; ++i) hit = hit || on_tri(f, isUp, tcx, tcz, cxs[i], czs[i]);
+              // unrolled over box_plane's four contacts, the count as a predicate: with constant indices the contacts stay in
+              // registers (a loop over nc put them, and this stage's loads and stores, in local memory)
+#pragma unroll
+              for (int i = 0; i < 4; ++i) hit = hit || (i < nc && on_tri(f, isUp, tcx, tcz, cxs[i], czs[i]));
               if (hit) hit_groups |= 1u << gi;
             }
           }
