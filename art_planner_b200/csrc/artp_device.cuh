@@ -10,6 +10,10 @@
 #include <math_constants.h>
 #include <stdint.h>
 
+#include <cmath>
+
+#include "../../include/artp.h"
+
 #define ARTP_EPS 1.1920928955078125e-07f  // dEpsilon = FLT_EPSILON (ode/ode/src/common.h:42)
 
 namespace artp {
@@ -114,14 +118,94 @@ __device__ __forceinline__ double se3_distance(const double* a, const double* b)
   return sqrt(r) + so3;
 }
 
-// SE3StateSpace::validSegmentCount as artp_valid_segment_count computes it on the host.
-__device__ __forceinline__ uint32_t segment_count(const double* a, const double* b, double seg_r3, double seg_so3) {
+// ---- Edge discretisation ---------------------------------------------------------------------------------------------
+// How an edge (a, b) is cut into the states a check visits or into the pieces the learned cost prices. Every unit that
+// uses these is compiled without FMA contraction (build.py), so a __host__ __device__ body does the same arithmetic on
+// both sides.
+
+// Longest valid segment of the R^3 and SO(3) parts of an SE(3) space: maximum extent * longestValidSegmentFraction, with
+// the extents |high - low| and pi/2 (OMPL 1.4.2 StateSpace.cpp).
+struct SegLen { double r3, so3; };
+// The segment lengths of sp (fraction 0.01 when sp's is not positive); false for a space whose R^3 length is not > 0.
+inline bool segment_lengths(const artp_se3_space& sp, SegLen& out) {
+  const double frac = sp.longest_valid_segment_fraction > 0 ? sp.longest_valid_segment_fraction : 0.01;
+  double e2 = 0;
+  for (int i = 0; i < 3; ++i) e2 += (sp.high[i] - sp.low[i]) * (sp.high[i] - sp.low[i]);
+  out.r3 = std::sqrt(e2) * frac;
+  out.so3 = 0.5 * 3.14159265358979323846 * frac;
+  return out.r3 > 0;
+}
+
+// ompl::base::CompoundStateSpace::validSegmentCount for SE3: the larger of (unsigned)ceil(distance / segment length) over
+// the R^3 part (Euclidean distance) and the SO(3) part (arc length acos(|q1.q2|), 0 above 1 - 1e-9). 0 for identical states.
+__host__ __device__ __forceinline__ uint32_t valid_segment_count(const double* a, const double* b, SegLen seg) {
   const double dx = a[0] - b[0], dy = a[1] - b[1], dz = a[2] - b[2];
   const double d3 = sqrt(dx * dx + dy * dy + dz * dz);
   const double dq = fabs(a[3] * b[3] + a[4] * b[4] + a[5] * b[5] + a[6] * b[6]);
   const double ds = dq > 1.0 - 1e-9 ? 0.0 : acos(dq);
-  const unsigned n3 = (unsigned)ceil(d3 / seg_r3), ns = (unsigned)ceil(ds / seg_so3);
-  return max(max(n3, ns), 1u);   // identical states: only s2 is checked
+  const unsigned n3 = (unsigned)ceil(d3 / seg.r3), ns = (unsigned)ceil(ds / seg.so3);
+  return n3 > ns ? n3 : ns;
+}
+// The segments DiscreteMotionValidator::checkMotion walks: at least one, so identical states check s2 only.
+__host__ __device__ __forceinline__ uint32_t segment_count(const double* a, const double* b, SegLen seg) {
+  const uint32_t nd = valid_segment_count(a, b, seg);
+  return nd > 1u ? nd : 1u;
+}
+
+// lateralDistance (utils.h:52-61) from a to b over a length L.
+__host__ __device__ __forceinline__ double lateral_ratio(const double* a, const double* b, double L) {
+  const double dx = b[0] - a[0], dy = b[1] - a[1];
+  return sqrt(dx * dx + dy * dy) / L;
+}
+// Interior states of a roadmap connection: (unsigned)(lateralDistance / L), L = kMaxDist (prm_motion_cost.cpp:340-343).
+__host__ __device__ __forceinline__ uint32_t lateral_count(const double* a, const double* b, double L) {
+  return (unsigned)lateral_ratio(a, b, L);
+}
+// Pieces MotionCostObjective::motionCost splits an edge into: (unsigned)(lateralDistance / max_query_edge_length) + 1
+// (motion_cost_objective.cpp:40-45); 0 when that quotient does not fit 32 bits or is not finite.
+__host__ __device__ __forceinline__ uint64_t cost_pieces(const double* a, const double* b, double L) {
+  const double q = lateral_ratio(a, b, L);
+  if (!(q < 4294967296.0)) return 0;
+  return (uint64_t)(unsigned int)q + 1;
+}
+
+// Interior state j (1 .. n) of an edge with n interior states: interpolate(a, b, j * (1.0 / (n + 1))), the product form
+// of prm_motion_cost.cpp:345-353 and motion_cost_objective.cpp:49-67 (not OMPL's j / nd quotient).
+template <typename I>   // the caller's index type; j and n + 1 convert to double exactly either way
+__device__ __forceinline__ void interior_state(const double* a, const double* b, I j, I n, double* s) {
+  const double n_interp_div = 1.0 / (double)(n + 1);
+  se3_interpolate(a, b, (double)j * n_interp_div, s);
+}
+// State j (1 .. nd) DiscreteMotionValidator::checkMotion visits on nd segments: interpolate(a, b, j / nd), and b itself
+// for j = nd.
+template <typename I>
+__device__ __forceinline__ void segment_state(const double* a, const double* b, I j, I nd, double* s) {
+  if (j == nd) {
+#pragma unroll
+    for (int k = 0; k < 7; ++k) s[k] = b[k];
+  } else {
+    se3_interpolate(a, b, (double)j / (double)nd, s);
+  }
+}
+
+// The edge that flat index `item` belongs to, over the exclusive prefix sums off[0 .. n] of the edges' item counts: the
+// largest e < n with off[e] <= item (off is non-decreasing, off[0] = 0). Ldg reads off through the read-only cache, which
+// is only right when nothing writes off during the kernel.
+template <bool Ldg>
+__device__ __forceinline__ uint32_t edge_of_item(const uint32_t* off, uint32_t n, uint32_t item) {
+  uint32_t lo = 0, hi = n;
+  while (hi - lo > 1) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if ((Ldg ? __ldg(off + mid) : off[mid]) <= item) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+// The number of leading valid verdicts among an edge's n (n when the whole edge is valid).
+__device__ __forceinline__ uint32_t leading_valid(const uint8_t* valid, uint32_t n) {
+  uint32_t p = 0;
+  while (p < n && valid[p]) ++p;
+  return p;
 }
 
 // ---- Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC'11) -------------------------

@@ -17,6 +17,7 @@
 #include <mutex>
 #include <string>
 #include <utility>
+#include <vector>
 
 #include "../../include/artp.h"
 #include "artp_cnn.h"
@@ -332,6 +333,10 @@ int check_cost_net(Handle* h);
 // rows, the head, the per-edge reduction (artp_motion_cost_split_device's work).
 int motion_cost_split(Handle* h, const double* d_s1, const double* d_s2, size_t n, const uint32_t* d_piece_off,
                       size_t total_pieces, float* d_rows, float* d_cost3, double* d_cost, cudaStream_t s);
+// The piece offsets of motionCost's split of the n HOST edges (s1 + 7 e, s2 + 7 e) at max_query_edge_length: off (n + 1
+// entries, exclusive, then the total) and *total. ARTP_E_INVALID when an edge or the total has 2^32 pieces or more.
+int cost_piece_offsets(Handle* h, const double* s1, const double* s2, size_t n, double max_query_edge_length,
+                       std::vector<uint32_t>& off, size_t* total);
 
 // artp_roadmap.cu: releases the roadmap store (artp_destroy).
 void roadmap_free(Handle* h);

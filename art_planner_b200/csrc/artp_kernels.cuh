@@ -103,27 +103,14 @@ __device__ __forceinline__ void edge_state(const double* s1, const double* s2, u
 
 __device__ __forceinline__ void load_item_state(const Work& w, uint32_t item, double s[7]) {
   if (w.item_off) {
-    uint32_t lo = 0, hi = w.n_edges;          // largest e with item_off[e] <= item
-    while (hi - lo > 1) {
-      const uint32_t mid = (lo + hi) >> 1;
-      if (__ldg(w.item_off + mid) <= item) lo = mid; else hi = mid;
-    }
+    const uint32_t lo = edge_of_item<true>(w.item_off, w.n_edges, item);
     const uint32_t o0 = __ldg(w.item_off + lo), o1 = __ldg(w.item_off + lo + 1);
     const int n_e = (int)(o1 - o0), step = (int)(item - o0) + 1;
     double a[7], b[7];
 #pragma unroll
     for (int k = 0; k < 7; ++k) { a[k] = w.s1[(size_t)lo * 7 + k]; b[k] = w.s2[(size_t)lo * 7 + k]; }
-    if (w.quotient) {
-      if (step == n_e) {
-#pragma unroll
-        for (int k = 0; k < 7; ++k) s[k] = b[k];
-      } else {
-        se3_interpolate(a, b, (double)step / (double)n_e, s);
-      }
-      return;
-    }
-    const double n_interp_div = 1.0 / (double)(n_e + 1);
-    se3_interpolate(a, b, (double)step * n_interp_div, s);
+    if (w.quotient) segment_state(a, b, step, n_e, s);
+    else interior_state(a, b, step, n_e, s);
     return;
   }
   if (!w.edge_mode) {

@@ -84,7 +84,7 @@ struct SimpDev {
   uint8_t* mot_ok;           // kBatch
   double* chk;               // kBatch x 7: the states to check
   uint8_t* valid;            // kBatch
-  double seg_r3, seg_so3;
+  artp::SegLen seg;
   uint64_t seed;
 };
 
@@ -184,7 +184,7 @@ __device__ bool add_motion(const SimpDev& d, SimpCtl& s, const double* s1, const
 }
 
 __device__ __forceinline__ uint32_t nd_of(const SimpDev& d, const double* a, const double* b) {
-  return artp::segment_count(a, b, d.seg_r3, d.seg_so3);
+  return artp::segment_count(a, b, d.seg);
 }
 
 // The entry work of the call that starts now (the whole CTA; s in shared memory, thread 0 writes it).
@@ -463,19 +463,14 @@ __global__ void __launch_bounds__(kThreads) simplify_gather_kernel(SimpDev d, ui
     s.idle = total == 0;
   }
   __syncthreads();
-  // the states of every motion: interpolate(s1, s2, j / nd), j = 1 .. nd - 1, then s2
+  // the states of every motion (mot_off was written in this launch: plain loads)
   for (uint32_t item = tid; item < total; item += blockDim.x) {
-    uint32_t lo = 0, hi = n_mot;   // largest m with mot_off[m] <= item
-    while (hi - lo > 1) {
-      const uint32_t mid = (lo + hi) >> 1;
-      if (d.mot_off[mid] <= item) lo = mid; else hi = mid;
-    }
+    const uint32_t lo = artp::edge_of_item<false>(d.mot_off, n_mot, item);
     const uint32_t o0 = d.mot_off[lo], nd = d.mot_off[lo + 1] - o0, j = item - o0 + 1;
     double a[7], b[7], st[7];
 #pragma unroll
     for (int k = 0; k < 7; ++k) { a[k] = d.mot[14 * (size_t)lo + k]; b[k] = d.mot[14 * (size_t)lo + 7 + k]; }
-    if (j == nd) copy7(st, b);
-    else artp::se3_interpolate(a, b, (double)j / (double)nd, st);
+    artp::segment_state(a, b, j, nd, st);
     copy7(d.chk + 7 * (size_t)item, st);
   }
   if (tid == 0) *d.ctl = s;
@@ -489,9 +484,8 @@ __global__ void __launch_bounds__(kThreads) simplify_apply_kernel(SimpDev d) {
   __syncthreads();
   if (s.status != S_RUNNING || s.n_att == 0) return;   // a round cut before its first attempt does nothing
   for (uint32_t m = tid; m < s.n_mot; m += blockDim.x) {
-    uint8_t ok = 1;
-    for (uint32_t k = d.mot_off[m]; k < d.mot_off[m + 1]; ++k) ok &= d.valid[k] ? 1 : 0;
-    d.mot_ok[m] = ok;
+    const uint32_t o0 = d.mot_off[m], nd = d.mot_off[m + 1] - o0;
+    d.mot_ok[m] = artp::leading_valid(d.valid + o0, nd) == nd;
   }
   __syncthreads();
   if (tid != 0) return;
@@ -682,16 +676,7 @@ int path_cost(Handle* h, const double* d_states, const double* states, size_t n,
   if (objective == ARTP_OBJ_LEARNED && !states) {
     TRY(piece_offsets(h, d_states, n, max_query_edge_length, d_off, &total, h->stream));
   } else if (objective == ARTP_OBJ_LEARNED) {
-    off.resize(ne + 1);
-    for (size_t e = 0; e < ne; ++e) {   // n_interp as artp_motion_cost_split computes it
-      off[e] = (uint32_t)total;
-      const double dx = states[7 * (e + 1)] - states[7 * e], dy = states[7 * (e + 1) + 1] - states[7 * e + 1];
-      const double q = std::sqrt(dx * dx + dy * dy) / max_query_edge_length;
-      if (!(q < 4294967296.0)) { h->err = "path edge too long for the learned cost"; return ARTP_E_INVALID; }
-      total += (size_t)(unsigned int)q + 1;
-      if (total > 0xFFFFFFFFull) { h->err = "too many cost pieces (>= 2^32)"; return ARTP_E_INVALID; }
-    }
-    off[ne] = (uint32_t)total;
+    TRY(cost_piece_offsets(h, states, states + 7, ne, max_query_edge_length, off, &total));
   }
   char* r[4];   // costs | piece offsets | rows | cost3
   TRY(carve(h, h->d_stage, h->stage_cap, {ne * sizeof(double), (ne + 1) * sizeof(uint32_t), total * 6 * sizeof(float),
@@ -744,14 +729,8 @@ int artp_api::simplify_path(Handle* h, const double* path, const double* d_path,
     if (!(max_query_edge_length > 0.0)) { h->err = "max_query_edge_length must be > 0"; return ARTP_E_INVALID; }
     TRY(check_cost_net(h));
   }
-  // the segment lengths of artp_valid_segment_count
-  const double frac = space->longest_valid_segment_fraction > 0 ? space->longest_valid_segment_fraction : 0.01;
-  double e2 = 0;
-  for (int i = 0; i < 3; ++i) e2 += (space->high[i] - space->low[i]) * (space->high[i] - space->low[i]);
   SimpDev d{};
-  d.seg_r3 = std::sqrt(e2) * frac;
-  d.seg_so3 = 0.5 * 3.14159265358979323846 * frac;
-  if (!(d.seg_r3 > 0)) { h->err = "bad SE3 space parameters"; return ARTP_E_INVALID; }
+  if (!artp::segment_lengths(*space, d.seg)) { h->err = "bad SE3 space parameters"; return ARTP_E_INVALID; }
   d.seed = seed;
   // Worst case: a shortcutPath call adds at most one state per attempt and makes at most its entry length of attempts,
   // so five calls leave <= 32 n states, with <= 62 n new pool states; subdivide thrice -> <= 256 n states, and

@@ -110,8 +110,8 @@ __global__ void endpoint_check_kernel(const double* __restrict__ sg, artp_se3_sp
   out[1] = sg[0]; out[2] = sg[1]; out[3] = sg[7]; out[4] = sg[8];
 }
 
-// MotionCostObjective::motionCost's split of the n - 1 edges of a path (artp_motion_cost_split's rule): pieces =
-// (unsigned)(lateralDistance / max_query_edge_length) + 1; off = their exclusive prefix sums (n entries, the last = total).
+// MotionCostObjective::motionCost's split of the n - 1 edges of a path (artp::cost_pieces); off = their exclusive prefix
+// sums (n entries, the last = total).
 // res[0] = the total (64 bits), res[1] = 1 when an edge has 2^32 pieces or more. One CTA.
 constexpr int kOffThreads = 1024;
 __global__ void __launch_bounds__(kOffThreads)
@@ -124,10 +124,9 @@ piece_offsets_kernel(const double* __restrict__ st, size_t n, double mql, uint32
   if (threadIdx.x == 0) bad = 0;
   __syncthreads();
   auto pieces = [&](size_t e) -> unsigned long long {
-    const double dx = st[7 * (e + 1)] - st[7 * e], dy = st[7 * (e + 1) + 1] - st[7 * e + 1];
-    const double q = sqrt(dx * dx + dy * dy) / mql;
-    if (!(q < 4294967296.0)) { bad = 1; return 0ull; }
-    return (unsigned long long)(unsigned int)q + 1ull;
+    const uint64_t p = artp::cost_pieces(st + 7 * e, st + 7 * (e + 1), mql);
+    if (!p) bad = 1;
+    return p;
   };
   unsigned long long sum = 0;
   for (size_t e = e0; e < e1; ++e) sum += pieces(e);

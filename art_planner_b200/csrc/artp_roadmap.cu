@@ -296,13 +296,7 @@ int artp_api::roadmap_solve(Handle* h, const double* start, const double* goal, 
   if (!d_sg)
     for (int i = 0; i < 7; ++i)
       if (!std::isfinite(start[i]) || !std::isfinite(goal[i])) { h->err = "non-finite start or goal"; return ARTP_E_INVALID; }
-  // the segment lengths of artp_valid_segment_count
-  const double frac = space->longest_valid_segment_fraction > 0 ? space->longest_valid_segment_fraction : 0.01;
-  double e2 = 0;
-  for (int i = 0; i < 3; ++i) e2 += (space->high[i] - space->low[i]) * (space->high[i] - space->low[i]);
-  q.seg_r3 = std::sqrt(e2) * frac;
-  q.seg_so3 = 0.5 * 3.14159265358979323846 * frac;
-  if (!(q.seg_r3 > 0)) { h->err = "bad SE3 space parameters"; return ARTP_E_INVALID; }
+  if (!artp::segment_lengths(*space, q.seg)) { h->err = "bad SE3 space parameters"; return ARTP_E_INVALID; }
   if (r->dev.vcap > artp::kSearchCtas * artp::kSearchSliceMax) {
     h->err = "roadmap too large for the on-chip search (vertex capacity above 77440)"; return ARTP_E_LIMIT;
   }

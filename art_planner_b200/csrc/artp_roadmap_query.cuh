@@ -62,7 +62,7 @@ struct QueryDev {
   uint32_t* chk_s2;          // ... their goal-side vertex ...
   uint32_t* chk_off;         // kQueryBatch + 1: ... and their first state
   uint32_t qcap;             // states a round may hold (the interior-state buffer, at most kQueryBatch)
-  double seg_r3, seg_so3;    // longest valid segment of the R^3 and SO(3) parts (artp_valid_segment_count)
+  SegLen seg;                // the space's segment lengths (segment_count)
 };
 
 __device__ __forceinline__ bool query_off(const RoadmapDev& r, const QueryDev& q) {
@@ -369,7 +369,7 @@ __global__ void __launch_bounds__(256) query_gather_kernel(RoadmapDev r, QueryDe
       const uint32_t e = q.path_e[i];
       if (r.eflag[e] & ARTP_ROADMAP_EDGE_VALID) continue;
       const uint32_t prev = q.path[i], pos = q.path[i + 1];
-      const uint32_t nd = segment_count(r.states + (size_t)pos * 7, r.states + (size_t)prev * 7, q.seg_r3, q.seg_so3);
+      const uint32_t nd = segment_count(r.states + (size_t)pos * 7, r.states + (size_t)prev * 7, q.seg);
       if (n == kQueryBatch || total + nd > q.qcap) { more = 1; break; }
       q.chk_e[n] = e; q.chk_s1[n] = pos; q.chk_s2[n] = prev; q.chk_off[n] = total;
       total += nd;
@@ -383,21 +383,12 @@ __global__ void __launch_bounds__(256) query_gather_kernel(RoadmapDev r, QueryDe
   __syncthreads();
   const uint32_t n = s_n, total = s_total;
   for (uint32_t item = threadIdx.x; item < total; item += blockDim.x) {
-    uint32_t lo = 0, hi = n;   // largest c with chk_off[c] <= item
-    while (hi - lo > 1) {
-      const uint32_t mid = (lo + hi) >> 1;
-      if (q.chk_off[mid] <= item) lo = mid; else hi = mid;
-    }
+    const uint32_t lo = edge_of_item<false>(q.chk_off, n, item);   // chk_off was written in this launch: plain loads
     const uint32_t o0 = q.chk_off[lo], nd = q.chk_off[lo + 1] - o0, j = item - o0 + 1;
     double a[7], b[7], s[7];
 #pragma unroll
     for (int k = 0; k < 7; ++k) { a[k] = r.states[(size_t)q.chk_s1[lo] * 7 + k]; b[k] = r.states[(size_t)q.chk_s2[lo] * 7 + k]; }
-    if (j == nd) {
-#pragma unroll
-      for (int k = 0; k < 7; ++k) s[k] = b[k];
-    } else {
-      se3_interpolate(a, b, (double)j / (double)nd, s);
-    }
+    segment_state(a, b, j, nd, s);
 #pragma unroll
     for (int k = 0; k < 7; ++k) r.interior[(size_t)item * 7 + k] = s[k];
   }
@@ -420,8 +411,8 @@ __global__ void __launch_bounds__(256) query_apply_kernel(RoadmapDev r, QueryDev
   if (query_off(r, q) || qc->phase != 1) return;
   const uint32_t n = qc->n_chk;
   for (uint32_t c = threadIdx.x; c < n; c += blockDim.x) {
-    uint32_t ok = 1;
-    for (uint32_t i = q.chk_off[c]; i < q.chk_off[c + 1]; ++i) ok &= r.valid[i] ? 1u : 0u;
+    const uint32_t o0 = q.chk_off[c], nd = q.chk_off[c + 1] - o0;
+    const uint32_t ok = leading_valid(r.valid + o0, nd) == nd;
     if (ok) r.eflag[q.chk_e[c]] |= ARTP_ROADMAP_EDGE_VALID;
     q.chk_s1[c] = ok;
   }

@@ -1,6 +1,7 @@
 """CPU-only: the oracle restatement (oracle/artp_oracle.c) on the off-grid geometries of offgrid_cases.py against the
-golden verdicts of the reference's own compiled ODE (oracle/make_golden_offgrid.py), and the classify-path coverage of
-that matrix restated in numpy."""
+golden verdicts of the reference's own compiled ODE (oracle/make_golden_offgrid.py), the library's host segment count
+against the same golden, and the classify-path coverage of that matrix restated in numpy."""
+import ctypes as C
 import hashlib
 import os
 
@@ -9,7 +10,7 @@ import pytest
 
 import cases
 import offgrid_cases as oc
-from art_planner_b200 import synth
+from art_planner_b200 import capi, synth
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -103,6 +104,12 @@ def test_port_edges_match_reference_golden(mk, gold, omaps, port_lib):
     low, high = oc.se3_bounds(m, oc.PARAMS["yaml"].reach_z)
     nd = o.valid_segment_count(low, high, s1, s2)
     assert np.array_equal(nd, gold[f"segments_{mk}/nd"])
+    # the library's host count (no handle, no device) gives the same nd
+    space = capi.ArtpSe3Space((C.c_double * 3)(*low), (C.c_double * 3)(*high), 0.01)
+    a, b = np.ascontiguousarray(s1, np.float64), np.ascontiguousarray(s2, np.float64)
+    lib_nd = np.empty(n, np.int32)
+    assert capi.load().artp_valid_segment_count(C.byref(space), a.ctypes.data, b.ctypes.data, n, lib_nd.ctypes.data) == capi.ARTP_OK
+    assert np.array_equal(lib_nd, gold[f"segments_{mk}/nd"])
     sv, t = o.check_motions_segments(s1, s2, nd)
     assert np.array_equal(sv, unpack(gold, f"segments_{mk}/mask", n)) and np.array_equal(t, gold[f"segments_{mk}/last_t"])
 

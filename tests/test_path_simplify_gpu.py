@@ -171,8 +171,9 @@ def test_error_codes():
     import art_planner_b200 as ap
     env = Env(rc.make_case("rough_fbm"), weights=False)
     h, lib = env.chk.handle, env.chk.handle.lib
-    p = synth.make_terrain_poses(env.c.m, 200, seed=5)
-    p = p[env.is_valid(p)][:5]
+    p = synth.make_terrain_poses(env.c.m, 1000, seed=5)
+    p = np.ascontiguousarray(p[env.is_valid(p)][:5])
+    assert p.shape == (5, 7)   # every call below reads 5 states from p
     out = np.empty((400, 7))
 
     def call(path, n, objective=capi.ARTP_OBJ_PATH_LENGTH, cap=400, handle=h.h):
