@@ -18,7 +18,6 @@ compiled reference, or costs read back from the device.
 """
 from __future__ import annotations
 
-import heapq
 import math
 
 import numpy as np
@@ -51,24 +50,55 @@ class QueryRoadmap(ro.Roadmap):
     def live(self, e: int) -> bool:
         return not self.flag[e] & REMOVED
 
+    def _live_edges(self):
+        """(edge indices, [n, 2] endpoints) of the live edges in ascending edge index. The int64 copy of the edge list and
+        the rows of csr() are cached under (id(edges), len(edges), n_removed), which assumes two things: an edge becomes
+        REMOVED only through remove_edge, and `edges` is only appended to or replaced together with a fresh roadmap
+        (a new list of the same length under a reused id would be missed). Code that breaks either calls
+        invalidate()."""
+        key = (id(self.edges), len(self.edges), self.n_removed)
+        if getattr(self, "_live_key", None) != key:
+            ea = getattr(self, "_ea", None)
+            if ea is None or getattr(self, "_ea_of", None) != id(self.edges) or ea.shape[0] > len(self.edges):
+                ea = np.zeros((0, 2), np.int64)
+            if ea.shape[0] < len(self.edges):
+                ea = np.concatenate([ea, np.asarray(self.edges[ea.shape[0]:], np.int64).reshape(-1, 2)])
+            self._ea, self._ea_of = ea, id(self.edges)
+            ids = np.flatnonzero((np.asarray(self.flag, np.uint8).reshape(-1) & REMOVED) == 0)
+            self._live, self._live_key, self._csr = (ids, ea[ids]), key, None
+        return self._live
+
+    def invalidate(self) -> None:
+        """Drops the cached edge array and rows (after changing `edges` or REMOVED flags other than by appending or
+        remove_edge)."""
+        self._live_key, self._ea = None, None
+
     def incident(self, v: int):
         """(edge index, other endpoint) of v's live edges in ascending edge index."""
-        return [(e, b if a == v else a) for e, (a, b) in enumerate(self.edges) if self.live(e) and v in (a, b)]
+        ids, ea = self._live_edges()
+        at = (ea[:, 0] == v) | (ea[:, 1] == v)
+        return [(int(e), int(b if a == v else a)) for e, (a, b) in zip(ids[at], ea[at])]
+
+    def csr(self):
+        """The live edges as rows per vertex, neighbours in ascending edge index: (offsets [V + 1], neighbour, edge index).
+        An edge appears in both endpoints' rows (twice in one row for a loop)."""
+        ids, ea = self._live_edges()
+        if self._csr is None or self._csr[0].shape[0] != self.V + 1:
+            row = np.concatenate([ea[:, 0], ea[:, 1]])
+            nbr = np.concatenate([ea[:, 1], ea[:, 0]])
+            eid = np.concatenate([ids, ids])
+            order = np.lexsort((eid, row))
+            self._csr = np.searchsorted(row[order], np.arange(self.V + 1)), nbr[order], eid[order]
+        return self._csr
 
     def adjacency(self):
-        adj = [[] for _ in range(self.V)]
-        for e, (a, b) in enumerate(self.edges):
-            if self.live(e):
-                adj[a].append((e, b))
-                adj[b].append((e, a))
-        return adj
+        off, nbr, eid = self.csr()
+        return [list(zip(eid[off[v]:off[v + 1]].tolist(), nbr[off[v]:off[v + 1]].tolist())) for v in range(self.V)]
 
     def refresh_density(self) -> None:
         """LazyPRM::getPlannerData's vertices: startM_ / goalM_ and the endpoints of (live) edges."""
         self.dens[:] = False
-        for e, (a, b) in enumerate(self.edges):
-            if self.live(e):
-                self.dens[a] = self.dens[b] = True
+        self.dens[self._live_edges()[1].reshape(-1)] = True
         self.dens[:self.V] |= (self.kinds[:self.V] & ro.QUERY) != 0
 
     def clear_query(self) -> None:
@@ -108,61 +138,72 @@ def cost_for_vertex_edges(rm: QueryRoadmap, v: int, edge_cost) -> None:
         rm.cost[e] = float(c)
 
 
+def _rows(off, vs):
+    """The CSR positions of the rows of vertices vs, and the row vertex of each."""
+    lo, n = off[vs], off[vs + 1] - off[vs]
+    pos = np.repeat(lo - np.cumsum(n) + n, n) + np.arange(int(n.sum()))
+    return pos, np.repeat(vs, n)
+
+
 def connected(rm: QueryRoadmap, a: int, b: int) -> bool:
     """sameComponent: over live edges of any weight."""
-    adj = rm.adjacency()
-    seen, todo = {a}, [a]
-    while todo:
-        v = todo.pop()
-        for _, n in adj[v]:
-            if n not in seen:
-                seen.add(n)
-                todo.append(n)
-    return b in seen
+    off, nbr, _ = rm.csr()
+    seen = np.zeros(rm.V, bool)
+    seen[a] = True
+    frontier = np.array([a])
+    while frontier.size and not seen[b]:
+        n = nbr[_rows(off, frontier)[0]]
+        frontier = np.unique(n[~seen[n]])
+        seen[frontier] = True
+    return bool(seen[b])
 
 
 def dijkstra(rm: QueryRoadmap, start: int):
-    """d[v] over live edges of finite weight, each sum rounded as Dijkstra's combineCosts rounds it."""
-    adj = rm.adjacency()
-    d = [INF] * rm.V
+    """d[v] over live edges of finite weight, each sum rounded as Dijkstra's combineCosts rounds it: the least fixpoint of
+    d[v] = min fl(d[u] + w), reached by relaxing the rows of the vertices whose distance fell until none falls (w >= 0 and
+    fl(+) monotone: any relaxation order ends there)."""
+    off, nbr, eid = rm.csr()
+    w = np.asarray(rm.cost, np.float64).reshape(-1)[eid]
+    d = np.full(rm.V, INF)
     d[start] = 0.0
-    heap = [(0.0, start)]
-    while heap:
-        dv, v = heapq.heappop(heap)
-        if dv > d[v]:
-            continue
-        for e, n in adj[v]:
-            w = rm.cost[e]
-            if not w < INF:
-                continue
-            if dv + w < d[n]:
-                d[n] = dv + w
-                heapq.heappush(heap, (d[n], n))
-    return d
+    frontier = np.array([start])
+    while frontier.size:
+        pos, src = _rows(off, frontier)
+        ok = w[pos] < INF
+        pos, src = pos[ok], src[ok]
+        nd = d[src] + w[pos]
+        lower = d.copy()
+        np.minimum.at(lower, nbr[pos], nd)
+        frontier = np.flatnonzero(lower < d)
+        d = lower
+    return d.tolist()
 
 
 def shortest_path(rm: QueryRoadmap, d, start: int, goal: int):
     """The tie rule: edge (u, v) is tight if fl(d[u] + w) == d[v]; level = hops from the start over tight edges (a BFS);
     pred[v] = the tight neighbour one level down with the lowest index, then the lowest edge index. Returns the path's
     (vertices, edges) from the goal back to the start."""
-    adj = rm.adjacency()
-    level = {start: 0}
-    frontier = [start]
-    while frontier:
-        nxt = []
-        for v in frontier:
-            for e, n in adj[v]:
-                w = rm.cost[e]
-                if w < INF and d[v] + w == d[n] and n not in level:
-                    level[n] = level[v] + 1
-                    nxt.append(n)
-        frontier = nxt
+    off, nbr, eid = rm.csr()
+    w = np.asarray(rm.cost, np.float64).reshape(-1)[eid]
+    d = np.asarray(d, np.float64)
+    level = np.full(rm.V, -1, np.int64)
+    level[start] = 0
+    frontier, t = np.array([start]), 0
+    while frontier.size:
+        pos, src = _rows(off, frontier)
+        n = nbr[pos]
+        tight = (w[pos] < INF) & (d[src] + w[pos] == d[n]) & (level[n] < 0)
+        frontier = np.unique(n[tight])
+        t += 1
+        level[frontier] = t
     verts, edges, v = [goal], [], goal
     while v != start:
-        best = min((n, e) for e, n in adj[v]
-                   if rm.cost[e] < INF and d[n] < INF and level.get(n) == level[v] - 1 and d[n] + rm.cost[e] == d[v])
-        edges.append(best[1])
-        v = best[0]
+        sl = slice(off[v], off[v + 1])
+        n, e, we = nbr[sl], eid[sl], w[sl]
+        ok = (we < INF) & (d[n] < INF) & (level[n] == level[v] - 1) & (d[n] + we == d[v])
+        k = np.lexsort((e[ok], n[ok]))[0]
+        v = int(n[ok][k])
+        edges.append(int(e[ok][k]))
         verts.append(v)
     return verts, edges
 
