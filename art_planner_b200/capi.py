@@ -195,6 +195,7 @@ def load():
     lib.artp_host_alloc.argtypes = [sz]
     lib.artp_host_free.argtypes = [vp]
     lib.artp_debug_set_group_capacity.argtypes = [vp, i32]
+    lib.artp_debug_get_reach_queue.argtypes = [vp, vp, sz, C.POINTER(sz)]
     lib.artp_set_timing.argtypes = [vp, i32]
     lib.artp_get_last_timing.argtypes = [vp, C.POINTER(C.c_float)]
     lib.artp_get_last_stage_timing.argtypes = [vp, C.POINTER(C.c_float)]

@@ -339,6 +339,16 @@ class StateValidityChecker:
     def debugSetGroupCapacity(self, max_triangles: int) -> None:
         self._h.check(self._h.lib.artp_debug_set_group_capacity(self._h.h, int(max_triangles)))
 
+    def debugReachQueue(self):
+        """Records of the one-warp-per-box reach queue of the last call's last round: (zone [n, 4] int32 x0, x1, z0, z1;
+        flags [n] uint32), read from the device (BoxRec, artp_kernels.cuh)."""
+        import numpy as np
+        n = C.c_size_t(0)
+        self._h.check(self._h.lib.artp_debug_get_reach_queue(self._h.h, None, 0, C.byref(n)))
+        buf = np.empty((n.value, 20), dtype=np.uint32)
+        self._h.check(self._h.lib.artp_debug_get_reach_queue(self._h.h, C.c_void_p(buf.ctypes.data), n.value, C.byref(n)))
+        return buf[:, 14:18].view(np.int32).copy(), buf[:, 19].copy()
+
     def stats(self) -> dict:
         return self._h.stats()
 

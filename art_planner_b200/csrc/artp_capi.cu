@@ -895,6 +895,18 @@ int artp_debug_set_group_capacity(artp_handle* hh, int max_triangles) {
   return ARTP_OK;
 }
 
+int artp_debug_get_reach_queue(artp_handle* hh, void* recs, size_t cap, size_t* n) {
+  LOCK_HANDLE(h, hh);
+  if (!n || (cap && !recs)) return ARTP_E_INVALID;
+  CU_TRY(h, cudaSetDevice(h->device));
+  Counters ctr{};
+  CU_TRY(h, cudaMemcpy(&ctr, h->d_ctr, sizeof(ctr), cudaMemcpyDeviceToHost));   // synchronises the device
+  *n = ctr.q.reach.end;
+  const size_t k = std::min(cap, (size_t)ctr.q.reach.end);
+  if (k) CU_TRY(h, cudaMemcpy(recs, h->d_recs_f, k * sizeof(artp::BoxRec), cudaMemcpyDeviceToHost));
+  return ARTP_OK;
+}
+
 int artp_get_stats(artp_handle* hh, artp_stats* out) {
   LOCK_HANDLE(h, hh);
   if (!out) return ARTP_E_INVALID;

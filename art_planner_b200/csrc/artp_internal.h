@@ -69,8 +69,8 @@ struct Handle {
   Counters* d_ctr = nullptr;
   uint32_t* d_defer = nullptr;      // deferred record list (bit 31: reach-box queue)
   artp::BoxRec* d_recs = nullptr;   // classify -> warp-stage box queue (torso boxes, reach boxes of unusual size)
-  artp::BoxRec* d_recs_f = nullptr; // classify -> reach-box queue (one warp per box: zones with -inf or mergeable planes)
-  artp::BoxRec* d_recs_g = nullptr; // classify -> reach-box queue of the 8-lane-group kernel (all-finite, merge-free zones)
+  artp::BoxRec* d_recs_f = nullptr; // classify -> reach-box queue (one warp per box: zones with mergeable planes or not reduced by the tables)
+  artp::BoxRec* d_recs_g = nullptr; // classify -> reach-box queue of the 8-lane-group kernel (merge-free zones, with or without -inf)
   int group_grid = 0, group_smem = 0;
   size_t recs_cap = 0;
   unsigned long long* d_compact_state = nullptr;   // compaction: tile counter, then one status word per tile (compact_kernel)

@@ -152,6 +152,13 @@ __device__ __forceinline__ void cell_plane(const Field& f, bool isUp, int cx, in
 // The collider's rules for one cell (heightfield.cpp:1306-1441) against a box bottom minB: a vertex collides when it is
 // finite and above minB; the Up (A, B, C) / Down (D, B, C) triangle is kept when its vertices are finite and one of them
 // collides; vertex v (0 A, 1 B, 2 C, 3 D) is tested when it collides and belongs to a kept triangle.
+// tri_kept is the triangle rule: with no NaN (heights are finite or -inf), "all three finite and one above minB" is
+// "lowest > -inf, highest < +inf and highest > minB".
+__device__ __forceinline__ bool tri_kept(bool isUp, float hA, float hB, float hC, float hD, float minB) {
+  const float h0 = isUp ? hA : hD;
+  const float lo = fminf(h0, fminf(hB, hC)), hi = fmaxf(h0, fmaxf(hB, hC));
+  return lo > -CUDART_INF_F && hi < CUDART_INF_F && hi > minB;
+}
 struct CellKeep {
   bool up, dn, cA, cB, cC, cD;
   __device__ __forceinline__ bool tested(int v) const {
@@ -159,11 +166,11 @@ struct CellKeep {
   }
 };
 __device__ __forceinline__ CellKeep cell_keep(float hA, float hB, float hC, float hD, float minB) {
-  const bool fA = finitef(hA), fB = finitef(hB), fC = finitef(hC), fD = finitef(hD);
   CellKeep k;
-  k.cA = fA && hA > minB; k.cB = fB && hB > minB; k.cC = fC && hC > minB; k.cD = fD && hD > minB;
-  k.up = (k.cA || k.cB || k.cC) && (fA && fB && fC);
-  k.dn = (k.cB || k.cC || k.cD) && (fB && fC && fD);
+  k.cA = finitef(hA) && hA > minB; k.cB = finitef(hB) && hB > minB;
+  k.cC = finitef(hC) && hC > minB; k.cD = finitef(hD) && hD > minB;
+  k.up = tri_kept(true, hA, hB, hC, hD, minB);
+  k.dn = tri_kept(false, hA, hB, hC, hD, minB);
   return k;
 }
 
@@ -229,6 +236,23 @@ __device__ __forceinline__ void zcell(const ZoneView& v, int lx, int lz, float& 
   const float* q = v.p + lz * v.stride + lx;
   if (SMEM) { hA = q[0]; hB = q[1]; hC = q[v.stride]; hD = q[v.stride + 1]; }
   else { hA = __ldg(q); hB = __ldg(q + 1); hC = __ldg(q + v.stride); hD = __ldg(q + v.stride + 1); }
+}
+
+// cell_keep's vertex rule, per vertex: a colliding vertex (xi, zi) of an nX x nZ zone is tested when one of the up to six triangles
+// around it is kept (tri_kept: with the vertex above minB, when its three vertices are finite). Cell c of the four around
+// it holds the vertex as its D (c = 0, Down only), C (1), B (2) or A (3, Up only).
+template <bool SMEM>
+__device__ __forceinline__ bool vertex_in_kept_triangle(const ZoneView& zv, int nX, int nZ, int xi, int zi, float minB) {
+  bool kept = false;
+#pragma unroll 1
+  for (int c = 0; c < 4 && !kept; ++c) {
+    const int cxi = xi - 1 + (c & 1), czi = zi - 1 + (c >> 1);
+    if (cxi < 0 || czi < 0 || cxi >= nX - 1 || czi >= nZ - 1) continue;
+    float hA, hB, hC, hD;
+    zcell<SMEM>(zv, cxi, czi, hA, hB, hC, hD);
+    kept = (c != 0 && tri_kept(true, hA, hB, hC, hD, minB)) || (c != 3 && tri_kept(false, hA, hB, hC, hD, minB));
+  }
+  return kept;
 }
 
 // Bloom keys of the merge screen. Level 1 (cheap, every kept triangle): buckets of the APPROXIMATE normal (n0, n2);
@@ -460,12 +484,8 @@ __device__ int box_collide_warp(const Field& f, const BoxCtx& b, const ZoneView&
     if (actc) {
       float hA, hB, hC, hD;
       zcell<SMEM>(zv, ccx - b.x0, ccz - b.z0, hA, hB, hC, hD);
-      // cell_keep's rule for this lane's triangle, written out: through the helper, box_tiles_warp_kernel spills 16
-      // bytes more (96 instead of 80 bytes of stack, sm_90a, CUDA 12.9)
-      const bool fA = finitef(hA), fB = finitef(hB), fC = finitef(hC), fD = finitef(hD);
-      const bool cA = fA && hA > b.minB, cB = fB && hB > b.minB, cC = fC && hC > b.minB, cD = fD && hD > b.minB;
       const bool isUp = (u == 0);
-      bool keep = isUp ? ((cA || cB || cC) && (fA && fB && fC)) : ((cB || cC || cD) && (fB && fC && fD));
+      bool keep = tri_kept(isUp, hA, hB, hC, hD, b.minB);
       if (merge_free && keep) {
         const float hT = isUp ? fmaxf(hA, fmaxf(hB, hC)) : fmaxf(hD, fmaxf(hB, hC));
         keep = hT > py_pair - 1e-3f;
@@ -950,9 +970,9 @@ classify_items_kernel(const Checker c, const Work w, BoxRec* __restrict__ recs_w
         // reach boxes go to their own queue (small TMA tiles); the torso -- and a reach box whose zone would not fit the
         // small tile -- to the big-tile queue
         const bool thread_path = foot && (b.x1 - b.x0) + 4 <= c.reach_tw && (b.z1 - b.z0) + 1 <= c.reach_th;
-        // ... and of those, the common kind (all-finite, merge-free zone, reduced by the tables) to the 8-lane-group kernel
-        const bool group_path = thread_path && recs_g != nullptr &&
-                                (fl & (REC_ALLFINITE | REC_MERGEFREE | REC_NEEDS_REDUCE)) == (REC_ALLFINITE | REC_MERGEFREE);
+        // ... and of those, the merge-free ones reduced by the tables (no merge screen, no zone reduction; a zone with -inf
+        // heights too) to the 8-lane-group kernel
+        const bool group_path = thread_path && recs_g != nullptr && (fl & (REC_MERGEFREE | REC_NEEDS_REDUCE)) == REC_MERGEFREE;
         s.pend[k][i] = (uint8_t)(fl | (uint32_t)(group_path ? PEND_GROUP : thread_path ? PEND_REACH : PEND_BIG) << 6);
         // Vertex probes here only for reach boxes (one cell); an undecided torso is rare and its probes run lane-parallel
         // at the head of the warp stage instead. Classify without the probes measured slower: the boxes they decide

@@ -11,9 +11,9 @@
 // No address arithmetic, L1 wavefronts or registers are spent on the gather, and all later reads are shared-memory reads.
 //
 // Three queues feed three launches: box_tiles_warp_kernel once over the big-tile queue (torso boxes; one tile slot per
-// warp) and once over the reach boxes that need the merge screen or non-finite handling (small tiles, two slots), and
-// reach_groups_kernel over the common reach boxes (all-finite, merge-free: four boxes per warp, below). A box whose zone
-// does not fit its tile (cannot happen for the sizes the tiles are derived from) goes to the exact grouping stage.
+// warp) and once over the reach boxes that need the merge screen or the zone reduction (small tiles, two slots), and
+// reach_groups_kernel over the other reach boxes (merge-free, with or without -inf: four boxes per warp, below). A box
+// whose zone does not fit its tile (cannot happen for the sizes the tiles are derived from) goes to the exact grouping stage.
 // Queue records are claimed with guided chunk sizes (a share of what is left), one claim ahead of the work.
 // Round 2 also tried one THREAD per reach box over the staged tiles (no cross-lane traffic at all): SIMT divergence
 // left 8-10 of 32 lanes busy and it was slower (profiles/r02_v1_reach_*).
@@ -156,7 +156,7 @@ box_tiles_warp_kernel(const Checker c, const __grid_constant__ CUtensorMap map0,
 }
 
 // -------------------------------------------------------------------------------------------------------------------
-// Reach boxes, the common kind: all-finite, merge-free zone (no screen, no grouping), reduced by the tables. A reach
+// Reach boxes of a merge-free zone (no screen, no grouping) reduced by the tables, with or without -inf heights. A reach
 // box's 81 vertices / 8 corners do not fill a warp (the one-warp-per-box kernel above runs them at 20 of 32 lanes and pays
 // its per-box overhead 1 : 1), so here a warp decides FOUR boxes at a time, 8 lanes each: lane = vertex in the vertex
 // stage, lane = corner when the candidate cells are collected; the candidate (cell, triangle) tasks of the four boxes are
@@ -243,10 +243,12 @@ reach_groups_kernel(const Checker c, const __grid_constant__ CUtensorMap map1, c
       const float* tile = reinterpret_cast<const float*>(slots + (size_t)(slot * 4 + g) * tc.stride) + (b.x0 & 3);
       const float top = b.maxB + (1e-4f + 4e-6f * fabsf(b.maxB));
       bool ghit = false;
+      const bool allFinite = (r.flags & REC_ALLFINITE) != 0;   // group-uniform
       // vertex stage, lane = vertex. Only the vertices inside the box's own xz extent are scanned: a point inside the box
       // has |x - P.x| <= xr = sum_j |R1[0][j]| side_j / 2 (and likewise in z), while the zone is that extent padded to whole
       // cells on every side (heightfield.cpp:1880-1892) -- its outer ring, 81 -> ~49 vertices for a reach box, cannot hold
-      // one (margin 1e-4 m, far above the rounding of the fp32 inside test).
+      // one (margin 1e-4 m, far above the rounding of the fp32 inside test). In a zone with -inf heights a vertex inside the
+      // box counts only if the collider tests it (vertex_in_kept_triangle): checked for the rare hit, not for every vertex.
       {
         const float xr = box_half_extent(b.R1, b.side, 0) + 1e-4f, zr = box_half_extent(b.R1, b.side, 2) + 1e-4f;
         const int vx0 = max(b.x0, (int)ceilf((b.P[0] - xr) * f.iW)), vx1 = min(b.x1, (int)floorf((b.P[0] + xr) * f.iW));
@@ -264,6 +266,9 @@ reach_groups_kernel(const Checker c, const __grid_constant__ CUtensorMap map1, c
             const int zi = (nXi > 1) ? (int)__umulhi((uint32_t)t, magicX) : t, xi = t - zi * nXi;
             const float h = tin[zi * tc.tw + xi];
             hit = h > b.minB && h < top && vertex_inside(b, (vx0 + xi) * f.sW, h, (vz0 + zi) * f.sD);
+            if (hit && !allFinite)
+              hit = vertex_in_kept_triangle<true>(ZoneView{tile, tc.tw}, b.x1 - b.x0 + 1, b.z1 - b.z0 + 1, vx0 - b.x0 + xi,
+                                                  vz0 - b.z0 + zi, b.minB);
           }
           if ((__ballot_sync(kFull, hit) >> gshift) & 0xffu) { ghit = true; gdone = true; }
           if (__all_sync(kFull, gdone)) break;
@@ -332,9 +337,8 @@ reach_groups_kernel(const Checker c, const __grid_constant__ CUtensorMap map1, c
             const bool isUp = (tk & 1) == 0;
             const int lx = tk >> 9, lz = (tk >> 1) & 0xff, ccx = tx0 + lx, ccz = tz0 + lz;
             const float* p = reinterpret_cast<const float*>(slots + (size_t)(slot * 4 + gi) * tc.stride) + (tx0 & 3) + lz * tc.tw + lx;
-            const float hA = p[0], hB = p[1], hC = p[tc.tw], hD = p[tc.tw + 1];   // all finite (REC_ALLFINITE)
-            const bool keep = isUp ? (hA > tb.minB || hB > tb.minB || hC > tb.minB) : (hB > tb.minB || hC > tb.minB || hD > tb.minB);
-            if (keep) {
+            const float hA = p[0], hB = p[1], hC = p[tc.tw], hD = p[tc.tw + 1];
+            if (tri_kept(isUp, hA, hB, hC, hD, tb.minB)) {
               float pl[4], cxs[4], czs[4];
               cell_plane(f, isUp, ccx, ccz, hA, hB, hC, hD, pl);
               const int nc = box_plane(tb, pl, 4, cxs, czs);

@@ -93,8 +93,8 @@ typedef struct artp_stats {
   uint32_t last_launches;      /* kernels launched by the most recent call */
   uint32_t last_queued_boxes;  /* boxes the classify stage queued for the later stages in the most recent call's last round */
   uint32_t last_queued_warp_stage;   /* ... of which in the big-tile queue (torso boxes, reach boxes of unusual size) */
-  uint32_t last_queued_reach_stage;  /* ... of which in the one-warp-per-box reach queue (zones with -inf or mergeable planes) */
-  uint32_t last_reach_plane_stage;   /* ... of which in the 8-lane-group reach queue (all-finite, merge-free zones) */
+  uint32_t last_queued_reach_stage;  /* ... of which in the one-warp-per-box reach queue (zones with mergeable planes or not reduced by the tables) */
+  uint32_t last_reach_plane_stage;   /* ... of which in the 8-lane-group reach queue (merge-free zones, with or without -inf) */
 } artp_stats;
 
 int  artp_create(const artp_params* params, artp_handle** out);
@@ -290,6 +290,9 @@ int artp_get_stats(artp_handle* h, artp_stats* out);
 int artp_poll_error(artp_handle* h);
 /* Test hook: cap the plane store at max_triangles (0 = no cap) from the next artp_set_map on. */
 int artp_debug_set_group_capacity(artp_handle* h, int max_triangles);
+/* Test hook: *n = length of the one-warp-per-box reach queue of the most recent check call's last round; its first
+ * min(*n, cap) records (80 bytes each, artp_kernels.cuh BoxRec) are copied to the HOST buffer recs. Synchronises the device. */
+int artp_debug_get_reach_queue(artp_handle* h, void* recs, size_t cap, size_t* n);
 
 /* Environment switch (a test hook, never needed in production):
  *   ARTP_NO_GROUPS=1        (read at artp_set_map) every undecided reach box takes the one-warp-per-box queue instead of the
