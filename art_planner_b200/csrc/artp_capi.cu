@@ -10,12 +10,79 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <cudaTypedefs.h>
 #include <type_traits>
 #include <vector>
 
 #include "artp_internal.h"
 #include "artp_kernels.cuh"
 #include "artp_tiles.cuh"
+
+namespace artp_api {
+
+constexpr int kMaxSlices = 9;   // H2D slices per host-fed round: at most 8 scheduled fractions and the remainder
+
+struct QueueCtr { uint32_t end, claim; };   // classify appends records up to end, the queue's box kernel claims from claim
+// The three box queues of a round (Pipeline::d_ctr), or one host-fed slice's share of them (Pipeline::d_slices). One
+// 32-byte sector each: the box kernels of consecutive slices claim from their records at the same time.
+struct alignas(32) BoxQueues { QueueCtr big, reach, group; };
+struct Counters { BoxQueues q; uint32_t defer; };   // a round's queues, and its boxes deferred to the grouping stage
+
+// A kernel's launch for the current map: at most `grid` CTAs of `block` threads with `smem` bytes of dynamic shared memory.
+struct Shape { int grid = 0, block = 0, smem = 0; };
+
+// The validity pipeline of a handle: box queues, per-map launch shapes, and the streams and events of its rounds.
+struct Pipeline {
+  enum { kBig, kReach, kGroup };   // the record queues, in BoxQueues order
+  Counters* d_ctr = nullptr;
+  // classify -> [kBig] the big-tile queue (torso boxes, reach boxes of unusual size), [kReach] the one-warp-per-box
+  // reach-box queue (zones with mergeable planes or not reduced by the tables), [kGroup] the 8-lane-group kernel's queue
+  // (merge-free zones, with or without -inf)
+  artp::BoxRec* recs[3] = {};
+  uint32_t* d_defer = nullptr;     // deferred record list (bit 31: reach-box queue)
+  size_t recs_cap = 0;             // entries of each record queue and of d_defer
+  BoxQueues* d_slices = nullptr;   // per slice of a host-fed round: its share of the three queues
+  unsigned long long* d_compact_state = nullptr;   // compaction: tile counter, then one status word per tile (compact_kernel)
+  size_t compact_state_cap = 0;
+  uint32_t compact_epoch = 0;      // epoch of the last compaction's tile statuses
+  // stage B (artp_tiles.cuh): [0] big tiles (torso queue), [1] small tiles (reach-box queue)
+  artp::TileCfg tile_cfg[2] = {};
+  CUtensorMap tile_map[2][2];      // [cfg][layer]: 2-D tile maps over elevation / elevation_masked
+  Shape tile[2];                   // stage B's two queues
+  Shape groups;                    // the 8-lane-group kernel; grid 0: no 8-lane queue
+  Shape grouping;                  // the plane-grouping stage, also the dynamic shared memory of the latency-path kernels
+  int tcap = 0;                    // triangles of the grouping stage's plane store
+  int tcap_override = 0;           // test hook (artp_debug_set_group_capacity)
+  int mode = 0;                    // artp_set_mode
+  uint8_t* h_small_out = nullptr;  // mapped pinned host bytes the latency-path kernel writes its verdicts to
+  bool deferred_unread = false;    // the last round's deferred boxes are not yet counted in stats.poses_deferred
+  // artp_create creates the streams (non-blocking) and ordering events (cudaEventDisableTiming) from these two arrays.
+  cudaStream_t streams[4] = {};
+  cudaStream_t& copy_stream = streams[0];    // H2D slices of the host-buffer API
+  cudaStream_t& box_stream = streams[1];     // box stages of slice i, concurrent with the copy + classify of slice i + 1
+  cudaStream_t& group_stream = streams[2];   // the 8-lane-group kernel, beside the other box kernels
+  cudaStream_t& tile_stream = streams[3];    // device rounds: the big-tile kernel, at the greatest stream priority
+  cudaEvent_t order_ev[2 * kMaxSlices + 3] = {};
+  cudaEvent_t *const copy_ev = order_ev, *const slice_ev = order_ev + kMaxSlices;   // slice i: H2D landed, classify done
+  cudaEvent_t& box_ev = order_ev[2 * kMaxSlices];   // a round's kernels on box_stream / group_stream / tile_stream done
+  cudaEvent_t &group_ev = order_ev[2 * kMaxSlices + 1], &tile_ev = order_ev[2 * kMaxSlices + 2];
+  // artp_set_timing: a timed round records ev[0] before classify and ev[i] after stage i of classify | big tiles |
+  // reach-box warps | 8-lane groups | plane grouping
+  int timing = 0;
+  cudaEvent_t ev[6] = {};
+  bool ev_valid = false;
+  // Releases whatever artp_create and the calls created (the handle's device is current).
+  ~Pipeline() {
+    for (cudaStream_t s : streams) if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
+    for (cudaEvent_t e : order_ev) if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+    for (artp::BoxRec* r : recs) cudaFree(r);
+    cudaFree(d_ctr); cudaFree(d_defer); cudaFree(d_slices); cudaFree(d_compact_state);
+    if (h_small_out) cudaFreeHost(h_small_out);
+  }
+};
+
+}  // namespace artp_api
 
 using namespace artp_api;
 
@@ -311,16 +378,13 @@ constexpr size_t kChunkItems = 1u << 20;   // work items per internal launch rou
 
 int ensure_queues(Handle* h, size_t n_items) {
   const size_t need = 5 * std::min(n_items, kChunkItems);
-  if (h->recs_cap >= need) return ARTP_OK;
+  if (h->pipe->recs_cap >= need) return ARTP_OK;
   const size_t cap = std::max<size_t>(need, 1u << 16);
-  h->recs_cap = 0;   // the four queues share it: set once all four have grown
-  size_t had[4] = {0, 0, 0, 0};
-  int rc;
-  TRY(grow(h, h->d_recs, had[0], cap));
-  TRY(grow(h, h->d_recs_f, had[1], cap));
-  TRY(grow(h, h->d_recs_g, had[2], cap));
-  TRY(grow(h, h->d_defer, had[3], cap));
-  h->recs_cap = cap;
+  h->pipe->recs_cap = 0;   // the four buffers share it: set once all four have grown
+  for (artp::BoxRec*& r : h->pipe->recs) { size_t had = 0; TRY(grow(h, r, had, cap)); }
+  size_t had = 0;
+  TRY(grow(h, h->pipe->d_defer, had, cap));
+  h->pipe->recs_cap = cap;
   return ARTP_OK;
 }
 
@@ -349,52 +413,52 @@ __global__ void close_slice_kernel(const BoxQueues* round, BoxQueues* slices, in
   slices[i].big = {round->big.end, prev.big.end};
 }
 
-// Stage launchers shared by both rounds. Each launches its kernel over the items [lo, hi).
-int launch_classify(Handle* h, artp::Work w, size_t lo, size_t hi, cudaStream_t s) {
+// Stage launchers shared by both rounds. Each launches its kernel over the items [lo, hi) of w (items).
+artp::Work items(artp::Work w, size_t lo, size_t hi) {
   w.item_base = (uint32_t)lo;
   w.n_items = (uint32_t)hi;
-  BoxQueues* q = &h->d_ctr->q;   // every round appends to the round's queues
+  return w;
+}
+int launch_classify(Handle* h, const artp::Work& w, size_t lo, size_t hi, BoxQueues* q, cudaStream_t s) {
+  const Pipeline& p = *h->pipe;
   return launch(h, artp::classify_items_kernel, (unsigned)((hi - lo + artp::kClassifyItems - 1) / artp::kClassifyItems),
-                artp::kClassifyItems, 0, s, h->chk, w, h->d_recs, h->d_recs_f, h->group_grid ? h->d_recs_g : nullptr, &q->big.end,
-                &q->reach.end, &q->group.end, h->mode == 1);
+                artp::kClassifyItems, 0, s, h->chk, items(w, lo, hi), p.recs[p.kBig], p.recs[p.kReach],
+                p.groups.grid ? p.recs[p.kGroup] : nullptr, &q->big.end, &q->reach.end, &q->group.end, p.mode == 1);
 }
 
-// The box kernels over the queue entries q, one launcher per queue: the big-tile queue, and the two reach-box queues (one
-// warp per box; 8-lane groups), which exist only for some box sizes. reach_cap caps the grids of the two reach kernels.
-int launch_big_tile(Handle* h, artp::Work w, size_t lo, size_t hi, BoxQueues* q, cudaStream_t s) {
-  w.item_base = (uint32_t)lo;
-  w.n_items = (uint32_t)hi;
-  const int wpc = h->tile_warps[0];   // no more CTAs than there can be boxes: up to five big-tile boxes per item
-  const unsigned grid = (unsigned)std::min<size_t>((size_t)h->tile_grid[0], (5 * (hi - lo) + wpc - 1) / wpc);
-  return launch(h, artp::box_tiles_warp_kernel, grid, wpc * 32, h->tile_smem[0], s, h->chk, h->tile_map[0][0], h->tile_map[0][1],
-                h->tile_cfg[0], w, h->d_recs, &q->big.end, &q->big.claim, &h->d_ctr->defer, h->d_defer, 0u, h->mode == 1);
+// Classify appends to the queues q, each box kernel takes its queue's entries: the big-tile queue and the two reach-box
+// queues (one warp per box; 8-lane groups), which exist only for some box sizes. reach_cap caps both reach grids.
+int launch_big_tile(Handle* h, const artp::Work& w, size_t lo, size_t hi, BoxQueues* q, cudaStream_t s) {
+  Pipeline& p = *h->pipe;
+  const int wpc = p.tile[0].block / 32;   // no more CTAs than there can be boxes: up to five big-tile boxes per item
+  const unsigned grid = (unsigned)std::min<size_t>((size_t)p.tile[0].grid, (5 * (hi - lo) + wpc - 1) / wpc);
+  return launch(h, artp::box_tiles_warp_kernel, grid, p.tile[0].block, p.tile[0].smem, s, h->chk, p.tile_map[0][0],
+                p.tile_map[0][1], p.tile_cfg[0], items(w, lo, hi), p.recs[p.kBig], &q->big.end, &q->big.claim, &p.d_ctr->defer,
+                p.d_defer, 0u, p.mode == 1);
 }
-int launch_reach_warp(Handle* h, artp::Work w, size_t lo, size_t hi, BoxQueues* q, cudaStream_t s, unsigned reach_cap) {
+int launch_reach_warp(Handle* h, const artp::Work& w, size_t lo, size_t hi, BoxQueues* q, cudaStream_t s, unsigned reach_cap) {
   if (!h->chk.reach_tw) return ARTP_OK;
-  w.item_base = (uint32_t)lo;
-  w.n_items = (uint32_t)hi;
-  const int wpc = h->tile_warps[1];
-  const unsigned grid = (unsigned)std::min<size_t>({(size_t)h->tile_grid[1], (4 * (hi - lo) + wpc - 1) / wpc, reach_cap});
-  return launch(h, artp::box_tiles_warp_kernel, grid, wpc * 32, h->tile_smem[1], s, h->chk, h->tile_map[1][1], h->tile_map[1][1],
-                h->tile_cfg[1], w, h->d_recs_f, &q->reach.end, &q->reach.claim, &h->d_ctr->defer, h->d_defer, artp::kDeferReachBit,
-                h->mode == 1);
+  Pipeline& p = *h->pipe;
+  const int wpc = p.tile[1].block / 32;
+  const unsigned grid = (unsigned)std::min<size_t>({(size_t)p.tile[1].grid, (4 * (hi - lo) + wpc - 1) / wpc, reach_cap});
+  return launch(h, artp::box_tiles_warp_kernel, grid, p.tile[1].block, p.tile[1].smem, s, h->chk, p.tile_map[1][1],
+                p.tile_map[1][1], p.tile_cfg[1], items(w, lo, hi), p.recs[p.kReach], &q->reach.end, &q->reach.claim,
+                &p.d_ctr->defer, p.d_defer, artp::kDeferReachBit, p.mode == 1);
 }
-int launch_reach_groups(Handle* h, artp::Work w, size_t lo, size_t hi, BoxQueues* q, cudaStream_t s, unsigned reach_cap) {
-  if (!h->group_grid) return ARTP_OK;
-  w.item_base = (uint32_t)lo;
-  w.n_items = (uint32_t)hi;
-  const unsigned grid = (unsigned)std::min<size_t>({(size_t)h->group_grid, (hi - lo + 7) / 8, reach_cap});
-  return launch(h, artp::reach_groups_kernel, grid, artp::kMaxTileWarps * 32, h->group_smem, s, h->chk, h->tile_map[1][1],
-                h->tile_cfg[1], w, h->d_recs_g, &q->group.end, &q->group.claim);
+int launch_reach_groups(Handle* h, const artp::Work& w, size_t lo, size_t hi, BoxQueues* q, cudaStream_t s, unsigned reach_cap) {
+  const Pipeline& p = *h->pipe;
+  if (!p.groups.grid) return ARTP_OK;
+  const unsigned grid = (unsigned)std::min<size_t>({(size_t)p.groups.grid, (hi - lo + 7) / 8, reach_cap});
+  return launch(h, artp::reach_groups_kernel, grid, p.groups.block, p.groups.smem, s, h->chk, p.tile_map[1][1], p.tile_cfg[1],
+                items(w, lo, hi), p.recs[p.kGroup], &q->group.end, &q->group.claim);
 }
 
 // The plane-grouping stage over every box the round [lo, hi) deferred.
-int launch_grouping(Handle* h, artp::Work w, size_t lo, size_t hi, cudaStream_t s) {
-  w.item_base = (uint32_t)lo;
-  w.n_items = (uint32_t)hi;
-  const unsigned grid = (unsigned)std::min<size_t>((size_t)h->k2_grid, 5 * (hi - lo));
-  return launch(h, artp::box_items_block_kernel, grid, artp::kBlockStageThreads, h->k2_smem, s, h->chk, w, h->d_recs, h->d_recs_f,
-                &h->d_ctr->defer, h->d_defer, h->k2_tcap, h->d_err);
+int launch_grouping(Handle* h, const artp::Work& w, size_t lo, size_t hi, cudaStream_t s) {
+  const Pipeline& p = *h->pipe;
+  const unsigned grid = (unsigned)std::min<size_t>((size_t)p.grouping.grid, 5 * (hi - lo));
+  return launch(h, artp::box_items_block_kernel, grid, p.grouping.block, p.grouping.smem, s, h->chk, items(w, lo, hi),
+                p.recs[p.kBig], p.recs[p.kReach], &p.d_ctr->defer, p.d_defer, p.tcap, h->d_err);
 }
 
 // Device round: the items [base, end) are on the device. Classify, the three box kernels, then the grouping stage. The box
@@ -405,38 +469,39 @@ int launch_grouping(Handle* h, artp::Work w, size_t lo, size_t hi, cudaStream_t 
 // group_stream joins s after it. With stage timing on, everything runs in order on s, and a timed round records the
 // per-stage events.
 int run_round_device(Handle* h, const artp::Work& w, cudaStream_t s, size_t base, size_t end, bool timed) {
-  CU_TRY(h, cudaMemsetAsync(h->d_ctr, 0, sizeof(Counters), s));
-  if (timed) CU_TRY(h, cudaEventRecord(h->ev[0], s));
-  TRY(launch_classify(h, w, base, end, s));
-  if (timed) CU_TRY(h, cudaEventRecord(h->ev[1], s));
-  const bool fork = !h->timing && h->chk.reach_tw;
+  Pipeline& p = *h->pipe;
+  CU_TRY(h, cudaMemsetAsync(p.d_ctr, 0, sizeof(Counters), s));
+  if (timed) CU_TRY(h, cudaEventRecord(p.ev[0], s));
+  BoxQueues* q = &p.d_ctr->q;
+  TRY(launch_classify(h, w, base, end, q, s));
+  if (timed) CU_TRY(h, cudaEventRecord(p.ev[1], s));
+  const bool fork = !p.timing && h->chk.reach_tw;
   if (fork) {
-    CU_TRY(h, cudaEventRecord(h->slice_ev[0], s));
-    CU_TRY(h, cudaStreamWaitEvent(h->tile_stream, h->slice_ev[0], 0));
-    CU_TRY(h, cudaStreamWaitEvent(h->box_stream, h->slice_ev[0], 0));
-    if (h->group_grid) CU_TRY(h, cudaStreamWaitEvent(h->group_stream, h->slice_ev[0], 0));
+    CU_TRY(h, cudaEventRecord(p.slice_ev[0], s));
+    CU_TRY(h, cudaStreamWaitEvent(p.tile_stream, p.slice_ev[0], 0));
+    CU_TRY(h, cudaStreamWaitEvent(p.box_stream, p.slice_ev[0], 0));
+    if (p.groups.grid) CU_TRY(h, cudaStreamWaitEvent(p.group_stream, p.slice_ev[0], 0));
   }
-  BoxQueues* q = &h->d_ctr->q;
-  TRY(launch_big_tile(h, w, base, end, q, fork ? h->tile_stream : s));
-  if (timed) CU_TRY(h, cudaEventRecord(h->ev[2], s));
-  TRY(launch_reach_warp(h, w, base, end, q, fork ? h->box_stream : s, UINT_MAX));
-  if (timed) CU_TRY(h, cudaEventRecord(h->ev[3], s));
-  TRY(launch_reach_groups(h, w, base, end, q, fork ? h->group_stream : s, UINT_MAX));
+  TRY(launch_big_tile(h, w, base, end, q, fork ? p.tile_stream : s));
+  if (timed) CU_TRY(h, cudaEventRecord(p.ev[2], s));
+  TRY(launch_reach_warp(h, w, base, end, q, fork ? p.box_stream : s, UINT_MAX));
+  if (timed) CU_TRY(h, cudaEventRecord(p.ev[3], s));
+  TRY(launch_reach_groups(h, w, base, end, q, fork ? p.group_stream : s, UINT_MAX));
   if (fork) {
     // The grouping stage reads the defer list, which only the two box_tiles_warp_kernel launches (tile_stream,
     // box_stream) write. reach_groups_kernel defers nothing, and it and the grouping stage only ever clear verdict bytes
     // of different boxes, so the grouping stage need not wait for it: group_stream joins s after the grouping launch.
-    CU_TRY(h, cudaEventRecord(h->tile_ev, h->tile_stream));
-    CU_TRY(h, cudaStreamWaitEvent(s, h->tile_ev, 0));
-    CU_TRY(h, cudaEventRecord(h->box_ev, h->box_stream));
-    CU_TRY(h, cudaStreamWaitEvent(s, h->box_ev, 0));
+    CU_TRY(h, cudaEventRecord(p.tile_ev, p.tile_stream));
+    CU_TRY(h, cudaStreamWaitEvent(s, p.tile_ev, 0));
+    CU_TRY(h, cudaEventRecord(p.box_ev, p.box_stream));
+    CU_TRY(h, cudaStreamWaitEvent(s, p.box_ev, 0));
   }
-  if (timed) CU_TRY(h, cudaEventRecord(h->ev[4], s));
+  if (timed) CU_TRY(h, cudaEventRecord(p.ev[4], s));
   TRY(launch_grouping(h, w, base, end, s));
-  if (timed) { CU_TRY(h, cudaEventRecord(h->ev[5], s)); h->ev_valid = true; }
-  if (fork && h->group_grid) {
-    CU_TRY(h, cudaEventRecord(h->group_ev, h->group_stream));
-    CU_TRY(h, cudaStreamWaitEvent(s, h->group_ev, 0));
+  if (timed) { CU_TRY(h, cudaEventRecord(p.ev[5], s)); p.ev_valid = true; }
+  if (fork && p.groups.grid) {
+    CU_TRY(h, cudaEventRecord(p.group_ev, p.group_stream));
+    CU_TRY(h, cudaStreamWaitEvent(s, p.group_ev, 0));
   }
   return ARTP_OK;
 }
@@ -449,6 +514,7 @@ int run_round_device(Handle* h, const artp::Work& w, cudaStream_t s, size_t base
 //   group_stream   the 8-lane-group kernel of slice i, beside them
 // so the copy, the classify stage and the box stages of consecutive slices overlap; s waits for box_stream at the end.
 int run_round_piped(Handle* h, const artp::Work& w, cudaStream_t s, const HostFeed& feed, size_t base, size_t end) {
+  Pipeline& p = *h->pipe;
   size_t cut[kMaxSlices + 1];
   int ncut = 0;
   cut[0] = base;
@@ -464,54 +530,56 @@ int run_round_piped(Handle* h, const artp::Work& w, cudaStream_t s, const HostFe
     for (size_t lo = base; lo < end; lo += feed.slice_items) cut[++ncut] = std::min(end, lo + feed.slice_items);
   }
   assert(ncut <= kMaxSlices);
-  CU_TRY(h, cudaMemsetAsync(h->d_ctr, 0, sizeof(Counters), s));
+  CU_TRY(h, cudaMemsetAsync(p.d_ctr, 0, sizeof(Counters), s));
   const unsigned reach_cap = (unsigned)(kPipeReachCtasPerSm * h->sm_count);
   for (int si = 0; si < ncut; ++si) {
     const size_t lo = cut[si], hi = cut[si + 1];
     CU_TRY(h, cudaMemcpyAsync(feed.dev + lo * feed.bytes_per_item, feed.host + lo * feed.bytes_per_item,
-                              (hi - lo) * feed.bytes_per_item, cudaMemcpyHostToDevice, h->copy_stream));
-    CU_TRY(h, cudaEventRecord(h->copy_ev[si], h->copy_stream));
-    CU_TRY(h, cudaStreamWaitEvent(s, h->copy_ev[si], 0));
-    TRY(launch_classify(h, w, lo, hi, s));
-    TRY(launch(h, close_slice_kernel, 1, 1, 0, s, &h->d_ctr->q, h->d_slices, si));
-    CU_TRY(h, cudaEventRecord(h->slice_ev[si], s));
-    CU_TRY(h, cudaStreamWaitEvent(h->box_stream, h->slice_ev[si], 0));
-    if (h->group_grid) CU_TRY(h, cudaStreamWaitEvent(h->group_stream, h->slice_ev[si], 0));
+                              (hi - lo) * feed.bytes_per_item, cudaMemcpyHostToDevice, p.copy_stream));
+    CU_TRY(h, cudaEventRecord(p.copy_ev[si], p.copy_stream));
+    CU_TRY(h, cudaStreamWaitEvent(s, p.copy_ev[si], 0));
+    TRY(launch_classify(h, w, lo, hi, &p.d_ctr->q, s));
+    TRY(launch(h, close_slice_kernel, 1, 1, 0, s, &p.d_ctr->q, p.d_slices, si));
+    CU_TRY(h, cudaEventRecord(p.slice_ev[si], s));
+    CU_TRY(h, cudaStreamWaitEvent(p.box_stream, p.slice_ev[si], 0));
+    if (p.groups.grid) CU_TRY(h, cudaStreamWaitEvent(p.group_stream, p.slice_ev[si], 0));
     // the big-tile queue (torso boxes: few) of this slice behind its reach-box queue: issued ahead of the reach kernels,
     // it made host-fed calls 2-4 % slower (H100 80GB HBM3, 400 W power limit)
-    TRY(launch_reach_groups(h, w, lo, hi, h->d_slices + si, h->group_stream, reach_cap));
-    TRY(launch_reach_warp(h, w, lo, hi, h->d_slices + si, h->box_stream, reach_cap));
-    TRY(launch_big_tile(h, w, lo, hi, h->d_slices + si, h->box_stream));
+    TRY(launch_reach_groups(h, w, lo, hi, p.d_slices + si, p.group_stream, reach_cap));
+    TRY(launch_reach_warp(h, w, lo, hi, p.d_slices + si, p.box_stream, reach_cap));
+    TRY(launch_big_tile(h, w, lo, hi, p.d_slices + si, p.box_stream));
   }
-  if (h->group_grid) {
+  if (p.groups.grid) {
     // the grouping stage (box_stream) runs last: the group kernels must not clear a verdict after it has been copied out
-    CU_TRY(h, cudaEventRecord(h->group_ev, h->group_stream));
-    CU_TRY(h, cudaStreamWaitEvent(h->box_stream, h->group_ev, 0));
+    CU_TRY(h, cudaEventRecord(p.group_ev, p.group_stream));
+    CU_TRY(h, cudaStreamWaitEvent(p.box_stream, p.group_ev, 0));
   }
-  TRY(launch_grouping(h, w, base, end, h->box_stream));
-  CU_TRY(h, cudaEventRecord(h->box_ev, h->box_stream));
-  CU_TRY(h, cudaStreamWaitEvent(s, h->box_ev, 0));
+  TRY(launch_grouping(h, w, base, end, p.box_stream));
+  CU_TRY(h, cudaEventRecord(p.box_ev, p.box_stream));
+  CU_TRY(h, cudaStreamWaitEvent(s, p.box_ev, 0));
   return ARTP_OK;
 }
 
 // Launch the pipeline for a prepared Work (items 0 .. w.n_items = the whole call) on stream s, in rounds of kChunkItems
-// work items (bounds the box queues). With a host feed, a round larger than one slice is piped; any other round (and
-// every round while stage timing is on) has its states copied on s and runs as a device round.
+// work items (bounds the box queues), and count the items in stats.poses_checked. With a host feed, a round larger than
+// one slice is piped; any other round (and every round while stage timing is on) has its states copied on s and runs as
+// a device round.
 int run_items(Handle* h, artp::Work w, cudaStream_t s, const HostFeed* feed = nullptr) {
   const size_t n_total = w.n_items;
   TRY(ensure_queues(h, n_total));
   for (size_t base = 0; base < n_total; base += kChunkItems) {
     const size_t end = std::min(n_total, base + kChunkItems);
-    if (feed && feed->slice_items < end - base && !h->timing) {
+    if (feed && feed->slice_items < end - base && !h->pipe->timing) {
       TRY(run_round_piped(h, w, s, *feed, base, end));
     } else {
       if (feed)
         CU_TRY(h, cudaMemcpyAsync(feed->dev + base * feed->bytes_per_item, feed->host + base * feed->bytes_per_item,
                                   (end - base) * feed->bytes_per_item, cudaMemcpyHostToDevice, s));
-      TRY(run_round_device(h, w, s, base, end, h->timing && end == n_total));
+      TRY(run_round_device(h, w, s, base, end, h->pipe->timing && end == n_total));
     }
   }
-  h->deferred_unread = true;
+  h->pipe->deferred_unread = true;
+  h->stats.poses_checked += n_total;
   return ARTP_OK;
 }
 
@@ -523,29 +591,26 @@ int check_common(Handle* h, size_t n) {
 
 // Latency path for n <= kSmallBatch host states (doubles): one launch, verdicts through mapped host memory.
 int check_poses_small(Handle* h, const artp::SmallBatch& sb, size_t n, uint8_t* valid, int steps = -1) {
+  Pipeline& p = *h->pipe;
   TRY(host_call_begin(h));
-  if (!h->h_small_out) {
-    CU_TRY(h, cudaHostAlloc((void**)&h->h_small_out, 64, cudaHostAllocMapped));
-    CU_TRY(h, cudaFuncSetAttribute(artp::pose_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  }
   uint8_t* d_out = nullptr;
-  CU_TRY(h, cudaHostGetDevicePointer((void**)&d_out, h->h_small_out, 0));
-  TRY(launch(h, artp::pose_small_kernel, (unsigned)n, 256, h->k2_smem, h->stream, h->chk, sb, d_out, h->k2_tcap, h->d_err,
-      h->mode == 1, steps));
+  CU_TRY(h, cudaHostGetDevicePointer((void**)&d_out, p.h_small_out, 0));
+  TRY(launch(h, artp::pose_small_kernel, (unsigned)n, 256, p.grouping.smem, h->stream, h->chk, sb, d_out, p.tcap, h->d_err,
+      p.mode == 1, steps));
   const int rc = host_call_end(h, true);
   if (rc == ARTP_E_CUDA) return rc;
   if (steps < 0) {
-    std::memcpy(valid, h->h_small_out, n);
+    std::memcpy(valid, p.h_small_out, n);
   } else {   // n = edges * (steps + 1) state verdicts -> one flag per edge
     const size_t per = (size_t)steps + 1;
     for (size_t e = 0; e < n / per; ++e) {
       uint8_t ok = 1;
-      for (size_t j = 0; j < per; ++j) ok &= h->h_small_out[e * per + j];
+      for (size_t j = 0; j < per; ++j) ok &= p.h_small_out[e * per + j];
       valid[e] = ok;
     }
   }
   h->stats.poses_checked += n;
-  h->ev_valid = false;
+  p.ev_valid = false;
   return rc;
 }
 
@@ -558,9 +623,7 @@ int check_states(Handle* h, const T* d_states, size_t n, uint8_t* d_valid, cudaS
   if constexpr (std::is_same_v<T, float>) w.s2f = d_states; else w.s2 = d_states;
   w.valid = d_valid;
   w.n_items = (uint32_t)n;
-  TRY(run_items(h, w, s, feed));
-  h->stats.poses_checked += n;
-  return ARTP_OK;
+  return run_items(h, w, s, feed);
 }
 
 // The pose entry points. A float state gives the same verdict as the double one while the H2D stream is 28 B/pose
@@ -577,7 +640,7 @@ int check_poses(Handle* h, const T* states, size_t n, uint8_t* valid, bool on_de
     if (cs.rc) return cs.rc;
     return check_states(h, states, n, valid, stream);
   }
-  if (n <= (size_t)artp::kSmallBatch && !h->timing) {
+  if (n <= (size_t)artp::kSmallBatch && !h->pipe->timing) {
     artp::SmallBatch sb;
     for (size_t i = 0; i < n * 7; ++i) (&sb.s[0][0])[i] = (double)states[i];   // exact; a float state is cast back in the kernel
     return check_poses_small(h, sb, n, valid);
@@ -602,9 +665,7 @@ int check_motions_on(Handle* h, const double* d_s1, const double* d_s2, size_t n
   const size_t items = n * ((size_t)n_steps + 1);
   artp::Work w;
   w.s1 = d_s1; w.s2 = d_s2; w.valid = d_valid; w.n_items = (uint32_t)items; w.steps = n_steps; w.edge_mode = 1;
-  TRY(run_items(h, w, s));
-  h->stats.poses_checked += items;
-  return ARTP_OK;
+  return run_items(h, w, s);
 }
 
 // valid_prefix[e] = number of leading 1s in item_valid[item_off[e] .. item_off[e+1])
@@ -636,9 +697,7 @@ int check_items_prefix(Handle* h, const double* d_s1, const double* d_s2, size_t
     w.item_off = d_item_off; w.n_edges = (uint32_t)n; w.quotient = quotient;
     TRY(run_items(h, w, s));
   }
-  TRY(launch(h, edge_prefix_kernel, grid_for(h, n, 256, 8), 256, 0, s, d_item_valid, d_item_off, n, d_valid_prefix));
-  h->stats.poses_checked += total_items;
-  return ARTP_OK;
+  return launch(h, edge_prefix_kernel, grid_for(h, n, 256, 8), 256, 0, s, d_item_valid, d_item_off, n, d_valid_prefix);
 }
 
 // check_items_prefix over host buffers: the n = off.size() - 1 edges (s1[e], s2[e]) with their item offsets `off`;
@@ -663,6 +722,83 @@ int pack_valid_bits(Handle* h, const uint8_t* d_valid, size_t n, uint32_t* d_bit
   CU_TRY(h, cudaSetDevice(h->device));
   const size_t words = (n + 31) / 32;
   return launch(h, pack_bits_kernel, grid_for(h, words * 32, 256, 8), 256, 0, s, d_valid, n, d_bits);
+}
+
+// The elapsed times ev[from] -> ev[to] of each pair into ms, once the last timed round has ended.
+int timed_round_ms(Handle* h, float* ms, std::initializer_list<std::pair<int, int>> pairs) {
+  const Pipeline& p = *h->pipe;
+  if (!ms) return ARTP_E_INVALID;
+  if (!p.timing || !p.ev_valid) { h->err = "timing not enabled or no call recorded"; return ARTP_E_INVALID; }
+  CU_TRY(h, cudaSetDevice(h->device));
+  CU_TRY(h, cudaEventSynchronize(p.ev[5]));
+  for (const auto& [from, to] : pairs) CU_TRY(h, cudaEventElapsedTime(ms++, p.ev[from], p.ev[to]));
+  return ARTP_OK;
+}
+
+// Lets `kernel` take max_smem bytes of dynamic shared memory; out = its launch at block threads and smem bytes, full grid.
+template <typename... P>
+int fit_shape(Handle* h, void (*kernel)(P...), int block, int smem, int max_smem, Shape& out) {
+  CU_TRY(h, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+  int per_sm = 0;
+  CU_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, smem));
+  out = {h->sm_count * std::max(per_sm, 1), block, smem};
+  return ARTP_OK;
+}
+
+// The box kernels' launch shapes for the map just installed (h->d_H, pitch, cols, win_row0), from each box's zone bound
+// span and the grouping stage's plane store (upload_map): attributes, occupancy grids, tile maps, chk's reach tile.
+int set_shapes(Handle* h, const int span[2][2], int tcap, int store) {
+  Pipeline& p = *h->pipe;
+  TRY(fit_shape(h, artp::box_items_block_kernel, artp::kBlockStageThreads, store, store, p.grouping));
+  p.tcap = tcap;
+  // Stage B tiles (artp_tiles.cuh): a zone spans at most ceil(2 r / s) + 3 vertices per axis; + 3 columns because the
+  // tile starts at x0 & ~3; width rounded up to a multiple of 4 floats (16-byte rows).
+  PFN_cuTensorMapEncodeTiled encode = nullptr;
+  cudaDriverEntryPointQueryResult qres;
+  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void**)&encode, cudaEnableDefault, &qres) != cudaSuccess || !encode) {
+    h->err = "cuTensorMapEncodeTiled not available from the driver"; return ARTP_E_CUDA;
+  }
+  h->chk.reach_tw = 0; h->chk.reach_th = 0;
+  for (int q = 0; q < 2; ++q) {          // 0: big tiles (torso box bound), 1: small tiles (reach box bound)
+    const int tw = std::min((span[q][0] + 3 + 3 + 3) & ~3, 256), th = std::min(span[q][1] + 3, 256);
+    artp::TileCfg tc;
+    tc.tw = tw; tc.th = th; tc.bytes = (uint32_t)tw * th * 4; tc.stride = (tc.bytes + 127u) & ~127u;
+    // big tiles: one slot per warp (three 8-warp CTAs per SM hide the copy latency better than a second 7 KB slot);
+    // small tiles: two slots, the next box's tile is in flight while this one is decided
+    tc.slots = (tc.stride > 2048) ? 1 : 2;
+    int wpc = 8;
+    while (wpc > 1 && (size_t)wpc * tc.slots * tc.stride + 128 > 72 * 1024) wpc >>= 1;
+    if ((size_t)wpc * tc.slots * tc.stride + 128 > 200 * 1024) {
+      if (q == 1) { p.tile[1] = Shape{}; continue; }   // no reach-box queue: everything takes the big-tile queue
+      // boxes this large relative to the cells: tiles capped, oversized zones go to the grouping stage
+      tc.tw = 64; tc.th = 64; tc.bytes = 64 * 64 * 4; tc.stride = tc.bytes; tc.slots = 1; wpc = 4;
+    }
+    const cuuint64_t gdim[2] = {(cuuint64_t)h->pitch, (cuuint64_t)h->cols};
+    const cuuint64_t gstr[1] = {(cuuint64_t)h->pitch * sizeof(float)};
+    const cuuint32_t box[2] = {(cuuint32_t)tc.tw, (cuuint32_t)tc.th};
+    const cuuint32_t one[2] = {1, 1};
+    for (int layer = 0; layer < 2; ++layer) {
+      const CUresult cr = encode(&p.tile_map[q][layer], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, h->d_H[layer], gdim, gstr, box, one,
+                                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      if (cr != CUDA_SUCCESS) { h->err = "cuTensorMapEncodeTiled failed (" + std::to_string((int)cr) + ")"; return ARTP_E_CUDA; }
+    }
+    tc.x_off = h->win_row0;
+    p.tile_cfg[q] = tc;
+    p.tile[q] = {0, wpc * 32, (int)((size_t)wpc * tc.slots * tc.stride + 128)};
+    if (q == 1) { h->chk.reach_tw = tc.tw; h->chk.reach_th = tc.th; }
+  }
+  p.groups = Shape{};
+  if (h->chk.reach_tw && p.tile_cfg[1].tw <= 127 && p.tile_cfg[1].th <= 255) {   // task packing: 7 + 8 bits of cell coordinates
+    const int gsm = artp::kMaxTileWarps * 8 * (int)p.tile_cfg[1].stride + 128;
+    if (gsm <= 160 * 1024 && !std::getenv("ARTP_NO_GROUPS")) {   // ARTP_NO_GROUPS: every reach box takes the one-warp-per-box queue
+      TRY(fit_shape(h, artp::reach_groups_kernel, artp::kMaxTileWarps * 32, gsm, gsm, p.groups));
+    }
+  }
+  const int smax = std::max(p.tile[0].smem, p.tile[1].smem);   // one kernel runs both tile sizes
+  for (Shape& t : p.tile)
+    if (t.block) TRY(fit_shape(h, artp::box_tiles_warp_kernel, t.block, t.smem, smax, t));
+  return ARTP_OK;
 }
 
 }  // namespace
@@ -690,38 +826,32 @@ int artp_api::check_states_f32(Handle* h, const float* d_states, size_t n, uint8
 int artp_api::check_states_cta(Handle* h, const double* d_states, const uint32_t* d_count, const uint32_t* d_stop, size_t max_n,
                                uint8_t* d_valid, cudaStream_t s) {
   if (max_n == 0) return ARTP_OK;
-  if (!h->pose_states_smem) {
-    CU_TRY(h, cudaFuncSetAttribute(artp::pose_states_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    h->pose_states_smem = true;
-  }
-  TRY(launch(h, artp::pose_states_kernel, (unsigned)max_n, 256, h->k2_smem, s, h->chk, d_states, d_count, d_stop, d_valid,
-             h->k2_tcap, h->d_err));
-  h->ev_valid = false;
+  TRY(launch(h, artp::pose_states_kernel, (unsigned)max_n, 256, h->pipe->grouping.smem, s, h->chk, d_states, d_count, d_stop,
+             d_valid, h->pipe->tcap, h->d_err));
+  h->pipe->ev_valid = false;
   return ARTP_OK;
 }
 
 int artp_api::compact_valid(Handle* h, const uint8_t* d_valid, size_t n, int64_t base, void* d_indices, uint32_t* d_count,
                             cudaStream_t s, bool bits, bool u32) {
+  Pipeline& p = *h->pipe;
   if (n == 0) { CU_TRY(h, cudaMemsetAsync(d_count, 0, sizeof(uint32_t), s)); return ARTP_OK; }
   ChainScope cs(h, 1, s);
   if (cs.rc) return cs.rc;
   const size_t nt = (n + kCompactTile - 1) / kCompactTile;
-  if (h->compact_state_cap < nt + 1 || h->compact_epoch + 1 >= kCompactEpochs) {
+  if (p.compact_state_cap < nt + 1 || p.compact_epoch + 1 >= kCompactEpochs) {
     // a new array, or the epochs wrapped: clear it once (word 0, the tile counter, included)
-    TRY(grow(h, h->d_compact_state, h->compact_state_cap, nt + 1));
-    CU_TRY(h, cudaMemsetAsync(h->d_compact_state, 0, h->compact_state_cap * sizeof(unsigned long long), s));
-    h->compact_epoch = 0;
+    TRY(grow(h, p.d_compact_state, p.compact_state_cap, nt + 1));
+    CU_TRY(h, cudaMemsetAsync(p.d_compact_state, 0, p.compact_state_cap * sizeof(unsigned long long), s));
+    p.compact_epoch = 0;
   }
-  const uint32_t epoch = ++h->compact_epoch;
-  unsigned long long* st = h->d_compact_state;
-  if (bits)
-    return launch(h, compact_kernel<true, int64_t>, (unsigned)nt, kCompactThreads, 0, s, d_valid, n, base, st, epoch,
-                  (int64_t*)d_indices, d_count);
-  if (u32)
-    return launch(h, compact_kernel<false, uint32_t>, (unsigned)nt, kCompactThreads, 0, s, d_valid, n, base, st, epoch,
-                  (uint32_t*)d_indices, d_count);
-  return launch(h, compact_kernel<false, int64_t>, (unsigned)nt, kCompactThreads, 0, s, d_valid, n, base, st, epoch,
-                (int64_t*)d_indices, d_count);
+  const uint32_t epoch = ++p.compact_epoch;
+  auto run = [&](auto kernel, auto* indices) {
+    return launch(h, kernel, (unsigned)nt, kCompactThreads, 0, s, d_valid, n, base, p.d_compact_state, epoch, indices, d_count);
+  };
+  if (bits) return run(compact_kernel<true, int64_t>, (int64_t*)d_indices);
+  if (u32) return run(compact_kernel<false, uint32_t>, (uint32_t*)d_indices);
+  return run(compact_kernel<false, int64_t>, (int64_t*)d_indices);
 }
 
 extern "C" {
@@ -763,23 +893,26 @@ int artp_create(const artp_params* params, artp_handle** out) {
   cudaFuncAttributes fa;
   if ((e = cudaFuncGetAttributes(&fa, artp::box_tiles_warp_kernel)) != cudaSuccess)
     return fail("no usable kernel image (built for sm_90a)", e);
-  for (cudaStream_t* st : {&h->stream, &h->copy_stream, &h->box_stream, &h->group_stream})
-    if ((e = cudaStreamCreateWithFlags(st, cudaStreamNonBlocking)) != cudaSuccess) return fail("cudaStreamCreate", e);
   int prio_least = 0, prio_greatest = 0;
   if ((e = cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest)) != cudaSuccess) return fail("cudaDeviceGetStreamPriorityRange", e);
-  if ((e = cudaStreamCreateWithPriority(&h->tile_stream, cudaStreamNonBlocking, prio_greatest)) != cudaSuccess)
-    return fail("cudaStreamCreateWithPriority", e);
-  if ((e = cudaEventCreateWithFlags(&h->group_ev, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
-  if ((e = cudaEventCreateWithFlags(&h->tile_ev, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
-  for (int i = 0; i < kMaxSlices; ++i) {
-    if ((e = cudaEventCreateWithFlags(&h->copy_ev[i], cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
-    if ((e = cudaEventCreateWithFlags(&h->slice_ev[i], cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
+  if ((e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)) != cudaSuccess) return fail("cudaStreamCreate", e);
+  Pipeline& p = *(h->pipe = new Pipeline());
+  for (cudaStream_t& st : p.streams) {
+    e = &st == &p.tile_stream ? cudaStreamCreateWithPriority(&st, cudaStreamNonBlocking, prio_greatest)
+                              : cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
+    if (e != cudaSuccess) return fail("cudaStreamCreate", e);
   }
-  if ((e = cudaEventCreateWithFlags(&h->box_ev, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
-  if ((e = cudaMalloc(&h->d_slices, kMaxSlices * sizeof(BoxQueues))) != cudaSuccess) return fail("cudaMalloc", e);
-  if ((e = cudaMalloc(&h->d_ctr, sizeof(Counters))) != cudaSuccess) return fail("cudaMalloc", e);
-  for (int g = 0; g < 2; ++g)
-    if ((e = cudaEventCreateWithFlags(&h->chain_ev[g], cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
+  for (cudaEvent_t& ev : p.order_ev)
+    if ((e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
+  for (cudaEvent_t& ev : h->chain_ev)
+    if ((e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)) != cudaSuccess) return fail("cudaEventCreate", e);
+  if ((e = cudaMalloc(&p.d_slices, kMaxSlices * sizeof(BoxQueues))) != cudaSuccess) return fail("cudaMalloc", e);
+  if ((e = cudaMalloc(&p.d_ctr, sizeof(Counters))) != cudaSuccess) return fail("cudaMalloc", e);
+  if ((e = cudaHostAlloc((void**)&p.h_small_out, 64, cudaHostAllocMapped)) != cudaSuccess) return fail("cudaHostAlloc", e);
+  // the latency-path kernels' plane store (the grouping stage's, sized per map) may take up to 200 KB
+  for (const void* k : {(const void*)artp::pose_small_kernel, (const void*)artp::pose_states_kernel})
+    if ((e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)) != cudaSuccess)
+      return fail("cudaFuncSetAttribute", e);
   if ((e = cudaHostAlloc((void**)&h->h_err, 64, cudaHostAllocMapped)) != cudaSuccess) return fail("cudaHostAlloc", e);
   *h->h_err = 0;
   if ((e = cudaHostGetDevicePointer((void**)&h->d_err, h->h_err, 0)) != cudaSuccess) return fail("cudaHostGetDevicePointer", e);
@@ -802,29 +935,15 @@ void artp_destroy(artp_handle* hh) {
   Handle* h = reinterpret_cast<Handle*>(hh);
   cudaSetDevice(h->device);
   if (h->stream) { cudaStreamSynchronize(h->stream); cudaStreamDestroy(h->stream); }
-  if (h->copy_stream) { cudaStreamSynchronize(h->copy_stream); cudaStreamDestroy(h->copy_stream); }
-  if (h->box_stream) { cudaStreamSynchronize(h->box_stream); cudaStreamDestroy(h->box_stream); }
-  if (h->group_stream) { cudaStreamSynchronize(h->group_stream); cudaStreamDestroy(h->group_stream); }
-  if (h->tile_stream) { cudaStreamSynchronize(h->tile_stream); cudaStreamDestroy(h->tile_stream); }
-  if (h->group_ev) cudaEventDestroy(h->group_ev);
-  if (h->tile_ev) cudaEventDestroy(h->tile_ev);
-  for (int i = 0; i < kMaxSlices; ++i) {
-    if (h->copy_ev[i]) cudaEventDestroy(h->copy_ev[i]);
-    if (h->slice_ev[i]) cudaEventDestroy(h->slice_ev[i]);
-  }
-  if (h->box_ev) cudaEventDestroy(h->box_ev);
-  cudaFree(h->d_slices);
+  delete h->pipe;
   for (int k = 0; k < 2; ++k) for (int l = 0; l <= artp::kMaxLevel; ++l) { cudaFree(h->d_T[k][l]); cudaFree(h->d_C[k][l]); }
-  cudaFree(h->d_H[0]); cudaFree(h->d_H[1]); cudaFree(h->d_ctr); cudaFree(h->d_defer); cudaFree(h->d_stage);
-  cudaFree(h->d_compact_state); cudaFree(h->d_recs); cudaFree(h->d_recs_f); cudaFree(h->d_recs_g); cudaFree(h->d_samp_layers); cudaFree(h->d_samp_scratch);
+  cudaFree(h->d_H[0]); cudaFree(h->d_H[1]); cudaFree(h->d_stage); cudaFree(h->d_samp_layers); cudaFree(h->d_samp_scratch);
   cudaFree(h->d_dist_layers); cudaFree(h->d_dist_scratch); cudaFree(h->d_basic_keep); cudaFree(h->d_simplify);
   roadmap_free(h);
   planner_free(h);
-  if (h->h_small_out) cudaFreeHost(h->h_small_out);
   if (h->h_err) cudaFreeHost(h->h_err);
-  for (int g = 0; g < 2; ++g) if (h->chain_ev[g]) cudaEventDestroy(h->chain_ev[g]);
+  for (cudaEvent_t ev : h->chain_ev) if (ev) cudaEventDestroy(ev);
   artp_cnn::destroy(h->cnn);
-  for (int i = 0; i < 6; ++i) if (h->ev[i]) cudaEventDestroy(h->ev[i]);
   delete h;
 }
 
@@ -838,39 +957,27 @@ int artp_has_map(const artp_handle* hh) {
 int artp_set_mode(artp_handle* hh, int mode) {
   LOCK_HANDLE(h, hh);
   if (mode < 0 || mode > 1) return ARTP_E_INVALID;
-  h->mode = mode;
+  h->pipe->mode = mode;
   return ARTP_OK;
 }
 
 int artp_set_timing(artp_handle* hh, int enable) {
   LOCK_HANDLE(h, hh);
   CU_TRY(h, cudaSetDevice(h->device));
-  if (enable && !h->ev[0]) for (int i = 0; i < 6; ++i) CU_TRY(h, cudaEventCreate(&h->ev[i]));
-  h->timing = enable ? 1 : 0;
-  h->ev_valid = false;
+  if (enable && !h->pipe->ev[0]) for (cudaEvent_t& ev : h->pipe->ev) CU_TRY(h, cudaEventCreate(&ev));
+  h->pipe->timing = enable ? 1 : 0;
+  h->pipe->ev_valid = false;
   return ARTP_OK;
 }
 
 int artp_get_last_timing(artp_handle* hh, float* ms3) {
   LOCK_HANDLE(h, hh);
-  if (!ms3) return ARTP_E_INVALID;
-  if (!h->timing || !h->ev_valid) { h->err = "timing not enabled or no call recorded"; return ARTP_E_INVALID; }
-  CU_TRY(h, cudaSetDevice(h->device));
-  CU_TRY(h, cudaEventSynchronize(h->ev[5]));
-  CU_TRY(h, cudaEventElapsedTime(ms3 + 0, h->ev[0], h->ev[1]));   // classify
-  CU_TRY(h, cudaEventElapsedTime(ms3 + 1, h->ev[1], h->ev[4]));   // box stages: warp + reach vertex + reach plane
-  CU_TRY(h, cudaEventElapsedTime(ms3 + 2, h->ev[4], h->ev[5]));   // plane grouping
-  return ARTP_OK;
+  return timed_round_ms(h, ms3, {{0, 1}, {1, 4}, {4, 5}});   // classify | box stages | plane grouping
 }
 
 int artp_get_last_stage_timing(artp_handle* hh, float* ms5) {
   LOCK_HANDLE(h, hh);
-  if (!ms5) return ARTP_E_INVALID;
-  if (!h->timing || !h->ev_valid) { h->err = "timing not enabled or no call recorded"; return ARTP_E_INVALID; }
-  CU_TRY(h, cudaSetDevice(h->device));
-  CU_TRY(h, cudaEventSynchronize(h->ev[5]));
-  for (int i = 0; i < 5; ++i) CU_TRY(h, cudaEventElapsedTime(ms5 + i, h->ev[i], h->ev[i + 1]));
-  return ARTP_OK;
+  return timed_round_ms(h, ms5, {{0, 1}, {1, 2}, {2, 3}, {3, 4}, {4, 5}});
 }
 
 // Pinned host memory for the adapter's staging buffers (the contiguous n x 7 state batch it gathers the OMPL states into,
@@ -891,7 +998,7 @@ int artp_poll_error(artp_handle* hh) {
 int artp_debug_set_group_capacity(artp_handle* hh, int max_triangles) {
   LOCK_HANDLE(h, hh);
   if (max_triangles < 0) return ARTP_E_INVALID;
-  h->tcap_override = max_triangles;   // takes effect at the next artp_set_map
+  h->pipe->tcap_override = max_triangles;   // takes effect at the next artp_set_map
   return ARTP_OK;
 }
 
@@ -900,10 +1007,10 @@ int artp_debug_get_reach_queue(artp_handle* hh, void* recs, size_t cap, size_t* 
   if (!n || (cap && !recs)) return ARTP_E_INVALID;
   CU_TRY(h, cudaSetDevice(h->device));
   Counters ctr{};
-  CU_TRY(h, cudaMemcpy(&ctr, h->d_ctr, sizeof(ctr), cudaMemcpyDeviceToHost));   // synchronises the device
+  CU_TRY(h, cudaMemcpy(&ctr, h->pipe->d_ctr, sizeof(ctr), cudaMemcpyDeviceToHost));   // synchronises the device
   *n = ctr.q.reach.end;
   const size_t k = std::min(cap, (size_t)ctr.q.reach.end);
-  if (k) CU_TRY(h, cudaMemcpy(recs, h->d_recs_f, k * sizeof(artp::BoxRec), cudaMemcpyDeviceToHost));
+  if (k) CU_TRY(h, cudaMemcpy(recs, h->pipe->recs[h->pipe->kReach], k * sizeof(artp::BoxRec), cudaMemcpyDeviceToHost));
   return ARTP_OK;
 }
 
@@ -912,13 +1019,13 @@ int artp_get_stats(artp_handle* hh, artp_stats* out) {
   if (!out) return ARTP_E_INVALID;
   CU_TRY(h, cudaSetDevice(h->device));
   Counters ctr{};
-  CU_TRY(h, cudaMemcpy(&ctr, h->d_ctr, sizeof(ctr), cudaMemcpyDeviceToHost));   // synchronises the device
+  CU_TRY(h, cudaMemcpy(&ctr, h->pipe->d_ctr, sizeof(ctr), cudaMemcpyDeviceToHost));   // synchronises the device
   h->stats.last_deferred = ctr.defer;
   h->stats.last_queued_boxes = ctr.q.big.end + ctr.q.reach.end + ctr.q.group.end;
   h->stats.last_queued_warp_stage = ctr.q.big.end;
   h->stats.last_queued_reach_stage = ctr.q.reach.end;
   h->stats.last_reach_plane_stage = ctr.q.group.end;
-  if (h->deferred_unread) { h->stats.poses_deferred += ctr.defer; h->deferred_unread = false; }
+  if (h->pipe->deferred_unread) { h->stats.poses_deferred += ctr.defer; h->pipe->deferred_unread = false; }
   *out = h->stats;
   return take_sticky_error(h);
 }
@@ -961,28 +1068,26 @@ int artp_api::upload_map(Handle* h, const float* elevation, const float* elevati
   f.iW = 1.0f / f.sW;
   f.iD = 1.0f / f.sD;
   f.px = (float)cx; f.py = (float)cy;
-  // K2 shared-memory plane store: bound the zone of either box by its half-diagonal; same bound -> table levels
-  int tcap = 0, kmax[2] = {0, 0};
+  // Each box's zone, bounded by its half-diagonal r: at most ceil(2 r / s) + 3 vertices along an axis of cell size s. The
+  // same bound sizes the range tables, the grouping stage's plane store and the tiles of stage B.
+  int span[2][2], kmax[2], tcap = 0;
   for (int k = 0; k < 2; ++k) {
     const float* sd = h->chk.side[k];
     const double r = 0.5 * std::sqrt((double)sd[0] * sd[0] + (double)sd[1] * sd[1] + (double)sd[2] * sd[2]);
-    const int nxm = std::min(rows, (int)std::ceil(2.0 * r * f.iW) + 4), nzm = std::min(cols, (int)std::ceil(2.0 * r * f.iD) + 4);
+    span[k][0] = (int)std::ceil(2.0 * r * f.iW); span[k][1] = (int)std::ceil(2.0 * r * f.iD);
+    const int nxm = std::min(rows, span[k][0] + 4), nzm = std::min(cols, span[k][1] + 4);
     tcap = std::max(tcap, 2 * (nxm - 1) * (nzm - 1));
     int kk = 0;
     while ((2 << kk) <= std::min(nxm, nzm) && kk < artp::kMaxLevel) ++kk;   // floor(log2(min dim bound))
     kmax[k] = kk;
   }
-  if (h->tcap_override > 0) tcap = std::min(tcap, h->tcap_override);   // test hook: force the overflow path
+  if (h->pipe->tcap_override > 0) tcap = std::min(tcap, h->pipe->tcap_override);   // test hook: force the overflow path
   tcap = (tcap + 3) & ~3;
-  const int smem = tcap * 21 + 64;
-  if (smem > 200 * 1024) {
+  const int store = tcap * 21 + 64;   // bytes of the grouping stage's plane store
+  if (store > 200 * 1024) {
     h->err = "box/map resolution combination exceeds the plane-grouping kernel's shared-memory store";
     return ARTP_E_LIMIT;
   }
-  CU_TRY(h, cudaFuncSetAttribute(artp::box_items_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  int per_sm = 0;
-  CU_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, artp::box_items_block_kernel, artp::kBlockStageThreads, smem));
-  h->k2_smem = smem; h->k2_tcap = tcap; h->k2_grid = h->sm_count * std::max(per_sm, 1);
   // upload (the previous map may still be in use by asynchronous calls on the caller's streams)
   CU_TRY(h, cudaDeviceSynchronize());
   h->chain_busy[0] = h->chain_busy[1] = false;
@@ -1063,69 +1168,7 @@ int artp_api::upload_map(Handle* h, const float* elevation, const float* elevati
   h->chk.err_word = h->d_err;
   h->chk.Lx = Lx; h->chk.Ly = Ly; h->chk.cx = cx; h->chk.cy = cy;
   h->chk.cell_margin = 0.02f + 2e-6f * (float)std::max(rows, cols);
-  // Stage B tiles (artp_tiles.cuh): a zone spans at most ceil(2 r / s) + 3 vertices per axis (r = box half-diagonal);
-  // + 3 columns because the tile starts at x0 & ~3; width rounded up to a multiple of 4 floats (16-byte rows).
-  {
-    typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                      const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                      CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn) {
-      h->err = "cuTensorMapEncodeTiled not available from the driver"; return ARTP_E_CUDA;
-    }
-    h->chk.reach_tw = 0; h->chk.reach_th = 0;
-    for (int q = 0; q < 2; ++q) {          // 0: big tiles (torso box bound), 1: small tiles (reach box bound)
-      const float* sd = h->chk.side[q];
-      const double r = 0.5 * std::sqrt((double)sd[0] * sd[0] + (double)sd[1] * sd[1] + (double)sd[2] * sd[2]);
-      int tw = ((int)std::ceil(2.0 * r * f.iW) + 3 + 3 + 3) & ~3, th = (int)std::ceil(2.0 * r * f.iD) + 3;
-      tw = std::min(tw, 256); th = std::min(th, 256);
-      artp::TileCfg tc;
-      tc.tw = tw; tc.th = th; tc.bytes = (uint32_t)tw * th * 4; tc.stride = (tc.bytes + 127u) & ~127u;
-      // big tiles: one slot per warp (three 8-warp CTAs per SM hide the copy latency better than a second 7 KB slot);
-      // small tiles: two slots, the next box's tile is in flight while this one is decided
-      tc.slots = (tc.stride > 2048) ? 1 : 2;
-      int wpc = 8;
-      while (wpc > 1 && (size_t)wpc * tc.slots * tc.stride + 128 > 72 * 1024) wpc >>= 1;
-      if ((size_t)wpc * tc.slots * tc.stride + 128 > 200 * 1024) {
-        if (q == 1) continue;              // no reach-box queue: everything takes the big-tile queue
-        // boxes this large relative to the cells: tiles capped, oversized zones go to the grouping stage
-        tc.tw = 64; tc.th = 64; tc.bytes = 64 * 64 * 4; tc.stride = tc.bytes; tc.slots = 1; wpc = 4;
-      }
-      const cuuint64_t gdim[2] = {(cuuint64_t)pitch, (cuuint64_t)cols};
-      const cuuint64_t gstr[1] = {(cuuint64_t)pitch * sizeof(float)};
-      const cuuint32_t box[2] = {(cuuint32_t)tc.tw, (cuuint32_t)tc.th};
-      const cuuint32_t one[2] = {1, 1};
-      for (int layer = 0; layer < 2; ++layer) {
-        const CUresult cr = reinterpret_cast<EncodeTiledFn>(fn)(&h->tile_map[q][layer], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, h->d_H[layer], gdim,
-                                                                gstr, box, one, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                                                                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (cr != CUDA_SUCCESS) { h->err = "cuTensorMapEncodeTiled failed (" + std::to_string((int)cr) + ")"; return ARTP_E_CUDA; }
-      }
-      tc.x_off = row0;
-      h->tile_cfg[q] = tc; h->tile_warps[q] = wpc;
-      h->tile_smem[q] = (int)((size_t)wpc * tc.slots * tc.stride + 128);
-      if (q == 1) { h->chk.reach_tw = tc.tw; h->chk.reach_th = tc.th; }
-    }
-    h->group_grid = 0;
-    if (h->chk.reach_tw && h->tile_cfg[1].tw <= 127 && h->tile_cfg[1].th <= 255) {   // task packing: 7 + 8 bits of cell coordinates
-      const int gsm = artp::kMaxTileWarps * 8 * (int)h->tile_cfg[1].stride + 128;
-      if (gsm <= 160 * 1024 && !std::getenv("ARTP_NO_GROUPS")) {   // ARTP_NO_GROUPS: every reach box takes the one-warp-per-box queue
-        CU_TRY(h, cudaFuncSetAttribute(artp::reach_groups_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, gsm));
-        int ps = 0;
-        CU_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ps, artp::reach_groups_kernel, artp::kMaxTileWarps * 32, gsm));
-        h->group_grid = h->sm_count * std::max(ps, 1);
-        h->group_smem = gsm;
-      }
-    }
-    const int smax = std::max(h->tile_smem[0], h->tile_smem[1]);
-    CU_TRY(h, cudaFuncSetAttribute(artp::box_tiles_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smax));
-    for (int q = 0; q < 2; ++q) {
-      int ps = 0;
-      CU_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ps, artp::box_tiles_warp_kernel, h->tile_warps[q] * 32, h->tile_smem[q]));
-      h->tile_grid[q] = h->sm_count * std::max(ps, 1);
-    }
-  }
+  TRY(set_shapes(h, span, tcap, store));
   h->has_map = true;
   h->map = MapState{};         // the sampler and the derived layers belong to the previous map
   h->res = res;
@@ -1170,7 +1213,7 @@ int artp_check_motions(artp_handle* hh, const double* s1, const double* s2, size
   if (n == 0) return ARTP_OK;
   if (!s1 || !s2 || !valid) return null_buffer(h);
   if (n_steps >= 0 && n * ((size_t)n_steps + 1) <= (size_t)artp::kSmallBatch && 2 * n <= (size_t)artp::kSmallBatch &&
-      !h->timing) {
+      !h->pipe->timing) {
     // latency path (a single checkMotion call): one fused launch, interpolation on the device as in the pipeline
     artp::SmallBatch sb;
     for (size_t e = 0; e < n; ++e) {

@@ -8,7 +8,6 @@
 // calls in another. It includes no kernel header: each of those defines kernels and is compiled into exactly one unit.
 #pragma once
 
-#include <cuda.h>
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -23,19 +22,7 @@
 #include "artp_cnn.h"
 #include "artp_device.cuh"
 
-namespace artp { struct BoxRec; }
-
 namespace artp_api {
-
-constexpr int kMaxSlices = 9;   // H2D slices per host-fed round: at most 8 scheduled fractions and the remainder
-
-// One box queue: the classify stage appends records up to `end`, the queue's box kernel claims them from `claim`.
-struct QueueCtr { uint32_t end, claim; };
-// The three box queues of a round (Handle::d_ctr), or the entries one slice of a host-fed round appended (Handle::d_slices).
-// One 32-byte sector each: the box kernels of consecutive slices claim from their records at the same time.
-struct alignas(32) BoxQueues { QueueCtr big, reach, group; };
-// Per-handle device counters: the round's queues, the boxes deferred to the grouping stage, and the sampler's CDF check.
-struct Counters { BoxQueues q; uint32_t defer, scratch; };
 
 // What belongs to the current map: artp_set_map_window resets all of it.
 struct Roadmap;
@@ -52,6 +39,7 @@ struct MapState {
 // Host <-> device traffic and host synchronisations of the calls that count them (artp_plan reports its own).
 struct Traffic { uint64_t h2d = 0, d2h = 0; uint32_t syncs = 0; };
 struct PlannerState;   // artp_planner_set_map / artp_plan (artp_planner.cu)
+struct Pipeline;       // the validity pipeline's queues, launch shapes, streams and events (artp_capi.cu)
 
 struct Handle {
   artp_params p;
@@ -66,35 +54,10 @@ struct Handle {
   int win_row0 = 0, win_rows = 0;   // rows held by this handle (artp_set_map_window); whole map: 0, rows
   bool has_map = false;
   MapState map;
-  Counters* d_ctr = nullptr;
-  uint32_t* d_defer = nullptr;      // deferred record list (bit 31: reach-box queue)
-  artp::BoxRec* d_recs = nullptr;   // classify -> warp-stage box queue (torso boxes, reach boxes of unusual size)
-  artp::BoxRec* d_recs_f = nullptr; // classify -> reach-box queue (one warp per box: zones with mergeable planes or not reduced by the tables)
-  artp::BoxRec* d_recs_g = nullptr; // classify -> reach-box queue of the 8-lane-group kernel (merge-free zones, with or without -inf)
-  int group_grid = 0, group_smem = 0;
-  size_t recs_cap = 0;
-  unsigned long long* d_compact_state = nullptr;   // compaction: tile counter, then one status word per tile (compact_kernel)
-  size_t compact_state_cap = 0;
-  uint32_t compact_epoch = 0;       // epoch of the last compaction's tile statuses
+  Pipeline* pipe = nullptr;         // from artp_create
   char* d_stage = nullptr;          // device staging for the host-buffer API
   size_t stage_cap = 0;
   cudaStream_t stream = nullptr;    // internal compute stream for the host-buffer API
-  cudaStream_t copy_stream = nullptr;   // H2D slices of the host-buffer API
-  cudaStream_t group_stream = nullptr;  // the 8-lane-group kernel of slice i (host-fed rounds), beside the other box kernels
-  cudaEvent_t group_ev = nullptr;
-  cudaStream_t tile_stream = nullptr;   // device rounds: the big-tile kernel, at the greatest stream priority
-  cudaEvent_t tile_ev = nullptr;
-  cudaStream_t box_stream = nullptr;    // box stages of slice i, concurrent with the copy + classify of slice i + 1
-  cudaEvent_t copy_ev[kMaxSlices] = {};    // H2D of slice i landed (the call's stream waits on it)
-  cudaEvent_t slice_ev[kMaxSlices] = {};   // classify of slice i done (box_stream waits on it)
-  cudaEvent_t box_ev = nullptr;            // box stages of a round done (stream waits on it)
-  BoxQueues* d_slices = nullptr;           // per slice of a host-fed round: its share of the three queues
-  int k2_grid = 0, k2_smem = 0, k2_tcap = 0;
-  // stage B (artp_tiles.cuh): [0] big tiles (torso queue, 4 warps per CTA), [1] small tiles (reach-box queue, 8 warps)
-  artp::TileCfg tile_cfg[2] = {};
-  int tile_grid[2] = {0, 0}, tile_smem[2] = {0, 0}, tile_warps[2] = {8, 8};
-  CUtensorMap tile_map[2][2];       // [cfg][layer]: 2-D tile maps over elevation / elevation_masked
-  int mode = 0;
   artp_cnn::State* cnn = nullptr;
   int cnn_mode = 0;
   // sampler (artp_set_sampler): device copies of the per-cell layers, scratch of the fused sample->check->compact path
@@ -117,16 +80,10 @@ struct Handle {
   Roadmap* roadmap = nullptr;       // the PRM roadmap store (artp_roadmap.cu), from the first artp_roadmap_clear
   char* d_simplify = nullptr;       // artp_simplify_path: state pool, path, round buffers (artp_path_simplify.cu)
   size_t simplify_cap = 0;
-  bool pose_states_smem = false;    // pose_states_kernel may use the latency path's dynamic shared memory
-  uint8_t* h_small_out = nullptr;   // mapped pinned host bytes the latency-path kernel writes its verdicts to
-  int timing = 0;
-  cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // classify | warp | reach vertex | reach plane | group
-  bool ev_valid = false;
-  bool deferred_unread = false;
   // Cross-stream ordering of the per-handle scratch (ADVICE r1): calls may come on different streams; every call that
   // uses a scratch group first makes its stream wait for the previous user of that group, and records an event after.
-  // group 0: d_ctr / d_recs / d_defer / d_stage / d_samp_scratch / d_dist_scratch (check, sampler, distribution);
-  // group 1: d_compact_state (compaction)
+  // group 0: the pipeline's counters and queues / d_stage / d_samp_scratch / d_dist_scratch (check, sampler, distribution);
+  // group 1: the pipeline's compaction state
   cudaEvent_t chain_ev[2] = {nullptr, nullptr};
   cudaStream_t chain_stream[2] = {nullptr, nullptr};
   bool chain_busy[2] = {false, false};
@@ -135,7 +92,6 @@ struct Handle {
   // call that caused it; device-buffer (asynchronous) calls surface it through artp_poll_error().
   uint32_t* h_err = nullptr;        // host view
   uint32_t* d_err = nullptr;        // device view of the same word
-  int tcap_override = 0;            // test hook (artp_debug_set_group_capacity)
   PlannerState* planner = nullptr;  // from the first artp_planner_set_map
   bool planner_map = false;         // the current map was installed by artp_planner_set_map
   Traffic traffic;
@@ -385,11 +341,11 @@ int simplify_path(Handle* h, const double* path, const double* d_path, size_t n,
 // order-preserving keys of float_key.
 int finite_min_max(Handle* h, const float* d_layer, size_t n, uint32_t* d_out, cudaStream_t s);
 float key_float(uint32_t key);
-// MotionCostObjective::motionCost's piece offsets of the n - 1 edges of the DEVICE path d_states (n + 0 entries, exclusive,
-// then the total) on s; *total is read back (one synchronisation). ARTP_E_INVALID for an edge of 2^32 pieces or more.
 // Planner::plan's checks of the endpoints of a device solve (start then goal, 14 doubles at d_sg) into d_out[5]: 0, -1
 // (a non-finite state), ARTP_SOLVE_INVALID_START or ARTP_SOLVE_INVALID_GOAL (outside space's bounds), then both (x, y).
 int endpoint_check(Handle* h, const double* d_sg, const artp_se3_space* space, double* d_out, cudaStream_t s);
+// MotionCostObjective::motionCost's piece offsets of the n - 1 edges of the DEVICE path d_states (n + 0 entries, exclusive,
+// then the total) on s; *total is read back (one synchronisation). ARTP_E_INVALID for an edge of 2^32 pieces or more.
 int piece_offsets(Handle* h, const double* d_states, size_t n, double max_query_edge_length, uint32_t* d_off, size_t* total,
                   cudaStream_t s);
 void planner_free(Handle* h);

@@ -519,7 +519,8 @@ int artp_set_sampler(artp_handle* hh, const artp_sampler_params* sp, const float
     h->err = "empty sampling bounds"; return ARTP_E_INVALID;
   }
   const size_t ncell = (size_t)h->rows * h->cols;
-  TRY(host_call_begin(h));
+  char* d_bad_word;   // the CDF check's verdict
+  TRY(host_call_begin(h, {sizeof(uint32_t)}, &d_bad_word));
   TRY(ensure_sampler_layers(h));
   float* base = h->d_samp_layers;
   if (host_normals) {
@@ -546,7 +547,7 @@ int artp_set_sampler(artp_handle* hh, const artp_sampler_params* sp, const float
     }
     m.cum_prob = base + 4 * ncell; m.cum_row = base + 5 * ncell;
     // the binary searches need monotone (or all-NaN) CDF rows: refuse anything else
-    uint32_t* d_bad = &h->d_ctr->scratch;
+    uint32_t* d_bad = (uint32_t*)d_bad_word;
     CU_TRY(h, cudaMemsetAsync(d_bad, 0, sizeof(uint32_t), h->stream));
     TRY(launch(h, artp::validate_cdf_kernel, (h->rows + 127) / 128, 128, 0, h->stream, m.cum_prob, h->rows, h->cols,
         (size_t)h->rows, 1, d_bad));
