@@ -21,6 +21,10 @@
 namespace artp_api {
 
 constexpr int kMaxSlices = 9;   // H2D slices per host-fed round: at most 8 scheduled fractions and the remainder
+// Dynamic shared memory caps of the per-map launch shapes, which artp_create gives the kernels as their attribute:
+// the grouping stage's plane store (upload_map refuses a map above it; the latency-path kernels share the store), a
+// box_tiles_warp_kernel CTA's tiles, and a reach_groups_kernel CTA's tiles (set_shapes).
+constexpr int kMaxStoreSmem = 200 * 1024, kMaxTileSmem = 200 * 1024, kMaxGroupsSmem = 160 * 1024;
 
 struct QueueCtr { uint32_t end, claim; };   // classify appends records up to end, the queue's box kernel claims from claim
 // The three box queues of a round (Pipeline::d_ctr), or one host-fed slice's share of them (Pipeline::d_slices). One
@@ -735,10 +739,10 @@ int timed_round_ms(Handle* h, float* ms, std::initializer_list<std::pair<int, in
   return ARTP_OK;
 }
 
-// Lets `kernel` take max_smem bytes of dynamic shared memory; out = its launch at block threads and smem bytes, full grid.
+// out = the launch of `kernel` at block threads and smem bytes of dynamic shared memory, full grid. The kernel's
+// shared-memory attribute is set once, in artp_create.
 template <typename... P>
-int fit_shape(Handle* h, void (*kernel)(P...), int block, int smem, int max_smem, Shape& out) {
-  CU_TRY(h, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+int fit_shape(Handle* h, void (*kernel)(P...), int block, int smem, Shape& out) {
   int per_sm = 0;
   CU_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, smem));
   out = {h->sm_count * std::max(per_sm, 1), block, smem};
@@ -746,10 +750,10 @@ int fit_shape(Handle* h, void (*kernel)(P...), int block, int smem, int max_smem
 }
 
 // The box kernels' launch shapes for the map just installed (h->d_H, pitch, cols, win_row0), from each box's zone bound
-// span and the grouping stage's plane store (upload_map): attributes, occupancy grids, tile maps, chk's reach tile.
+// span and the grouping stage's plane store (upload_map): occupancy grids, tile maps, chk's reach tile.
 int set_shapes(Handle* h, const int span[2][2], int tcap, int store) {
   Pipeline& p = *h->pipe;
-  TRY(fit_shape(h, artp::box_items_block_kernel, artp::kBlockStageThreads, store, store, p.grouping));
+  TRY(fit_shape(h, artp::box_items_block_kernel, artp::kBlockStageThreads, store, p.grouping));
   p.tcap = tcap;
   // Stage B tiles (artp_tiles.cuh): a zone spans at most ceil(2 r / s) + 3 vertices per axis; + 3 columns because the
   // tile starts at x0 & ~3; width rounded up to a multiple of 4 floats (16-byte rows).
@@ -768,7 +772,7 @@ int set_shapes(Handle* h, const int span[2][2], int tcap, int store) {
     tc.slots = (tc.stride > 2048) ? 1 : 2;
     int wpc = 8;
     while (wpc > 1 && (size_t)wpc * tc.slots * tc.stride + 128 > 72 * 1024) wpc >>= 1;
-    if ((size_t)wpc * tc.slots * tc.stride + 128 > 200 * 1024) {
+    if ((size_t)wpc * tc.slots * tc.stride + 128 > kMaxTileSmem) {
       if (q == 1) { p.tile[1] = Shape{}; continue; }   // no reach-box queue: everything takes the big-tile queue
       // boxes this large relative to the cells: tiles capped, oversized zones go to the grouping stage
       tc.tw = 64; tc.th = 64; tc.bytes = 64 * 64 * 4; tc.stride = tc.bytes; tc.slots = 1; wpc = 4;
@@ -791,13 +795,12 @@ int set_shapes(Handle* h, const int span[2][2], int tcap, int store) {
   p.groups = Shape{};
   if (h->chk.reach_tw && p.tile_cfg[1].tw <= 127 && p.tile_cfg[1].th <= 255) {   // task packing: 7 + 8 bits of cell coordinates
     const int gsm = artp::kMaxTileWarps * 8 * (int)p.tile_cfg[1].stride + 128;
-    if (gsm <= 160 * 1024 && !std::getenv("ARTP_NO_GROUPS")) {   // ARTP_NO_GROUPS: every reach box takes the one-warp-per-box queue
-      TRY(fit_shape(h, artp::reach_groups_kernel, artp::kMaxTileWarps * 32, gsm, gsm, p.groups));
+    if (gsm <= kMaxGroupsSmem && !std::getenv("ARTP_NO_GROUPS")) {   // ARTP_NO_GROUPS: every reach box takes the one-warp-per-box queue
+      TRY(fit_shape(h, artp::reach_groups_kernel, artp::kMaxTileWarps * 32, gsm, p.groups));
     }
   }
-  const int smax = std::max(p.tile[0].smem, p.tile[1].smem);   // one kernel runs both tile sizes
   for (Shape& t : p.tile)
-    if (t.block) TRY(fit_shape(h, artp::box_tiles_warp_kernel, t.block, t.smem, smax, t));
+    if (t.block) TRY(fit_shape(h, artp::box_tiles_warp_kernel, t.block, t.smem, t));
   return ARTP_OK;
 }
 
@@ -909,9 +912,15 @@ int artp_create(const artp_params* params, artp_handle** out) {
   if ((e = cudaMalloc(&p.d_slices, kMaxSlices * sizeof(BoxQueues))) != cudaSuccess) return fail("cudaMalloc", e);
   if ((e = cudaMalloc(&p.d_ctr, sizeof(Counters))) != cudaSuccess) return fail("cudaMalloc", e);
   if ((e = cudaHostAlloc((void**)&p.h_small_out, 64, cudaHostAllocMapped)) != cudaSuccess) return fail("cudaHostAlloc", e);
-  // the latency-path kernels' plane store (the grouping stage's, sized per map) may take up to 200 KB
-  for (const void* k : {(const void*)artp::pose_small_kernel, (const void*)artp::pose_states_kernel})
-    if ((e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)) != cudaSuccess)
+  // A kernel's max-dynamic-shared-memory attribute belongs to the kernel in the device's context, so every handle on the
+  // device shares it. Each kernel gets the most that any accepted map can ask of it, here and never per map: a handle
+  // that set it to its own map's size would lower it under the launches of a handle holding a larger map.
+  const std::pair<const void*, int> smem_caps[] = {
+      {(const void*)artp::pose_small_kernel, kMaxStoreSmem}, {(const void*)artp::pose_states_kernel, kMaxStoreSmem},
+      {(const void*)artp::box_items_block_kernel, kMaxStoreSmem}, {(const void*)artp::box_tiles_warp_kernel, kMaxTileSmem},
+      {(const void*)artp::reach_groups_kernel, kMaxGroupsSmem}};
+  for (const auto& [k, bytes] : smem_caps)
+    if ((e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)) != cudaSuccess)
       return fail("cudaFuncSetAttribute", e);
   if ((e = cudaHostAlloc((void**)&h->h_err, 64, cudaHostAllocMapped)) != cudaSuccess) return fail("cudaHostAlloc", e);
   *h->h_err = 0;
@@ -1084,7 +1093,7 @@ int artp_api::upload_map(Handle* h, const float* elevation, const float* elevati
   if (h->pipe->tcap_override > 0) tcap = std::min(tcap, h->pipe->tcap_override);   // test hook: force the overflow path
   tcap = (tcap + 3) & ~3;
   const int store = tcap * 21 + 64;   // bytes of the grouping stage's plane store
-  if (store > 200 * 1024) {
+  if (store > kMaxStoreSmem) {
     h->err = "box/map resolution combination exceeds the plane-grouping kernel's shared-memory store";
     return ARTP_E_LIMIT;
   }
