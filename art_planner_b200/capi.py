@@ -189,6 +189,10 @@ def load():
                                        C.POINTER(ArtpSimplifyInfo)]
     lib.artp_planner_set_map.argtypes = [vp, C.POINTER(ArtpPlannerParams), vp, vp, vp, vp, i32, i32, dbl, dbl, dbl,
                                          C.POINTER(ArtpPlannerMapInfo)]
+    lib.artp_planner_set_map_raw.argtypes = [vp, C.POINTER(ArtpPlannerParams), vp, vp, i32, i32, dbl, dbl, dbl,
+                                             C.POINTER(ArtpPlannerMapInfo)]
+    lib.artp_inpaint_layer.argtypes = [vp, vp, i32, i32, vp]
+    lib.artp_inpaint_layer_device.argtypes = [vp, vp, i32, i32, vp, vp]
     lib.artp_planner_get_space.argtypes = [vp, C.POINTER(ArtpSe3Space)]
     lib.artp_plan.argtypes = [vp, C.POINTER(ArtpPlannerParams), vp, vp, vp, sz, C.POINTER(sz), C.POINTER(ArtpPlanInfo)]
     lib.artp_host_alloc.restype = C.c_void_p

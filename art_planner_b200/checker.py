@@ -336,6 +336,25 @@ class StateValidityChecker:
         last poll (the affected poses were reported invalid). Synchronise the stream first."""
         self._h.check(self._h.lib.artp_poll_error(self._h.h))
 
+    def inpaint(self, layer):
+        """inpaintMatrix (art_planner/src/utils.cpp:13-63) of a rows x cols grid_map layer (NaN = unknown) on the device:
+        artp_inpaint_layer for a numpy array (returns a column-major float32 array), artp_inpaint_layer_device for a CUDA
+        tensor (column-major: a transposed contiguous cols x rows float32 tensor; returns the same layout, on the current
+        stream)."""
+        if _is_torch_cuda(layer):
+            import torch
+            rows, cols = layer.shape
+            if layer.dtype != torch.float32 or not layer.t().is_contiguous():
+                raise ValueError("inpaint: a CUDA layer must be float32 and column-major (a transposed contiguous tensor)")
+            out = torch.empty((cols, rows), dtype=torch.float32, device=layer.device).t()
+            self._h.check(self._h.lib.artp_inpaint_layer_device(self._h.h, layer.data_ptr(), rows, cols, out.data_ptr(),
+                                                                _stream_ptr()))
+            return out
+        a = np.asfortranarray(layer, dtype=np.float32)
+        out = np.empty(a.shape, np.float32, order="F")
+        self._h.check(self._h.lib.artp_inpaint_layer(self._h.h, a.ctypes.data, a.shape[0], a.shape[1], out.ctypes.data))
+        return out
+
     def debugSetGroupCapacity(self, max_triangles: int) -> None:
         self._h.check(self._h.lib.artp_debug_set_group_capacity(self._h.h, int(max_triangles)))
 
@@ -673,6 +692,17 @@ class Planner:
         mi = capi.ArtpPlannerMapInfo()
         h.check(h.lib.artp_planner_set_map(h.h, C.byref(self.parameters), *[None if a is None else a.ctypes.data for a in (e, t, ei, ti)],
                                            e.shape[0], e.shape[1], float(res), float(cx), float(cy), C.byref(mi)))
+        return {k: int(getattr(mi, k)) for k, _ in capi.ArtpPlannerMapInfo._fields_}
+
+    def setMapRaw(self, elevation, traversability, res: float, cx: float, cy: float) -> dict:
+        """setMap from the RAW layers alone (artp_planner_set_map_raw): processors::Basic's two inpaintMatrix calls run
+        on the device. traversability may be None. Returns the call's host_syncs, bytes_h2d and bytes_d2h."""
+        e = np.asfortranarray(elevation, dtype=np.float32)
+        t = None if traversability is None else np.asfortranarray(traversability, dtype=np.float32)
+        h = self._c.handle
+        mi = capi.ArtpPlannerMapInfo()
+        h.check(h.lib.artp_planner_set_map_raw(h.h, C.byref(self.parameters), e.ctypes.data, None if t is None else t.ctypes.data,
+                                               e.shape[0], e.shape[1], float(res), float(cx), float(cy), C.byref(mi)))
         return {k: int(getattr(mi, k)) for k, _ in capi.ArtpPlannerMapInfo._fields_}
 
     def space(self):

@@ -341,6 +341,9 @@ int simplify_path(Handle* h, const double* path, const double* d_path, size_t n,
 // order-preserving keys of float_key.
 int finite_min_max(Handle* h, const float* d_layer, size_t n, uint32_t* d_out, cudaStream_t s);
 float key_float(uint32_t key);
+// inpaintMatrix (artp_inpaint.cuh) of the rows x cols column-major layer d_in into d_out on s; d_mm holds the layer's
+// finite_min_max words (at least one finite cell). Scratch is stream-ordered (cudaMallocAsync).
+int inpaint_layer(Handle* h, const float* d_in, int rows, int cols, const uint32_t* d_mm, float* d_out, cudaStream_t s);
 // Planner::plan's checks of the endpoints of a device solve (start then goal, 14 doubles at d_sg) into d_out[5]: 0, -1
 // (a non-finite state), ARTP_SOLVE_INVALID_START or ARTP_SOLVE_INVALID_GOAL (outside space's bounds), then both (x, y).
 int endpoint_check(Handle* h, const double* d_sg, const artp_se3_space* space, double* d_out, cudaStream_t s);

@@ -236,17 +236,42 @@ void artp_api::planner_free(Handle* h) {
   h->planner = nullptr;
 }
 
-extern "C" {
+namespace {
 
-int artp_planner_set_map(artp_handle* hh, const artp_planner_params* pp, const float* elevation, const float* traversability,
-                         const float* elevation_inpainted, const float* traversability_inpainted, int rows, int cols,
-                         double res, double cx, double cy, artp_planner_map_info* info) {
-  LOCK_CALL(h, hh);
+// artp_planner_set_map's body. raw: the inpainted layers are made on the device from the uploaded raw ones (the
+// *_inpainted arguments are unused).
+// The two layers' marches are independent: the traversability's runs on a second stream beside the elevation's, which
+// matters when one giant component leaves most SMs idle. d_mm: the elevation's min / max words, the traversability's at +4.
+int inpaint_both(Handle* h, const float* raw_e, const float* raw_t, int rows, int cols, const uint32_t* d_mm, float* L,
+                 cudaStream_t s) {
+  if (!raw_t) return inpaint_layer(h, raw_e, rows, cols, d_mm, L, s);
+  const size_t n = (size_t)rows * cols;
+  cudaStream_t s2 = nullptr;
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  int rc = ARTP_OK;
+  auto cu = [&](cudaError_t e) { if (rc == ARTP_OK && e != cudaSuccess) { h->err = cudaGetErrorString(e); rc = ARTP_E_CUDA; } };
+  cu(cudaStreamCreateWithFlags(&s2, cudaStreamNonBlocking));
+  for (auto& e : ev) cu(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  cu(cudaEventRecord(ev[0], s));
+  cu(cudaStreamWaitEvent(s2, ev[0], 0));
+  if (rc == ARTP_OK) rc = inpaint_layer(h, raw_t, rows, cols, d_mm + 4, L + n, s2);
+  if (rc == ARTP_OK) rc = inpaint_layer(h, raw_e, rows, cols, d_mm, L, s);
+  cu(cudaEventRecord(ev[1], s2));
+  cu(cudaStreamWaitEvent(s, ev[1], 0));
+  for (auto e : ev) if (e) cudaEventDestroy(e);
+  if (s2) cudaStreamDestroy(s2);   // released once its work is done
+  return rc;
+}
+
+int set_map(Handle* h, const artp_planner_params* pp, const float* elevation, const float* traversability,
+            const float* elevation_inpainted, const float* traversability_inpainted, bool raw, int rows, int cols,
+            double res, double cx, double cy, artp_planner_map_info* info) {
   // every check before any work: a refused map leaves the previous one installed
-  if (!pp || !elevation || !elevation_inpainted) return null_buffer(h);
-  if (!traversability != !traversability_inpainted) {
+  if (!pp || !elevation || (!raw && !elevation_inpainted)) return null_buffer(h);
+  if (!raw && !traversability != !traversability_inpainted) {
     h->err = "pass both traversability layers (raw and inpainted) or neither"; return ARTP_E_INVALID;
   }
+  if (raw && (size_t)rows * cols >= 0x7FFFFFFFull) { h->err = "inpaint: rows * cols must be < 2^31"; return ARTP_E_INVALID; }
   if (rows < 2 || cols < 2 || !(res > 0) || !std::isfinite(cx) || !std::isfinite(cy)) { h->err = "bad map arguments"; return ARTP_E_INVALID; }
   TRY(plan_args(h, pp));
   TRY(map_chain_limits(h, &pp->basic, res, pp->sample_from_distribution != 0, pp->use_inverse_vertex_density != 0));
@@ -258,20 +283,23 @@ int artp_planner_set_map(artp_handle* hh, const artp_planner_params* pp, const f
   TRY(grow(h, st->d_layers, st->layers_cap, 11 * n));
   float *raw_e = st->d_layers, *raw_t = st->d_layers + n, *L = st->d_layers + 2 * n;
   TRY(copy_async(h, raw_e, elevation, lb, cudaMemcpyHostToDevice, s));
-  TRY(copy_async(h, L, elevation_inpainted, lb, cudaMemcpyHostToDevice, s));
+  if (!raw) TRY(copy_async(h, L, elevation_inpainted, lb, cudaMemcpyHostToDevice, s));
   if (traversability) {
     TRY(copy_async(h, raw_t, traversability, lb, cudaMemcpyHostToDevice, s));
-    TRY(copy_async(h, L + n, traversability_inpainted, lb, cudaMemcpyHostToDevice, s));
+    if (!raw) TRY(copy_async(h, L + n, traversability_inpainted, lb, cudaMemcpyHostToDevice, s));
   }
   // observed, and the SE(3) bounds from the RAW elevation (planner.cpp:146-156)
   TRY(launch(h, observed_kernel, grid_for(h, n, 256), 256, 0, s, raw_e, traversability ? raw_t : nullptr, n, L + 2 * n, L + n));
   if (!st->d_q) CU_TRY(h, cudaMalloc(&st->d_q, QB_SIZE * sizeof(double)));
   uint32_t* d_mm = reinterpret_cast<uint32_t*>(st->d_q + QB_MINMAX);
   TRY(finite_min_max(h, raw_e, n, d_mm, s));
-  uint32_t mm[3];
-  TRY(copy_async(h, mm, d_mm, sizeof(mm), cudaMemcpyDeviceToHost, s));
+  const bool raw_t_inpaint = raw && traversability;
+  if (raw_t_inpaint) TRY(finite_min_max(h, raw_t, n, d_mm + 4, s));   // inpaintMatrix's range of the traversability
+  uint32_t mm[8];
+  TRY(copy_async(h, mm, d_mm, (raw_t_inpaint ? 8 : 3) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
   TRY(host_call_end(h));
   if (!mm[2]) { h->err = "the elevation layer has no finite cell"; return ARTP_E_INVALID; }
+  if (raw_t_inpaint && !mm[6]) { h->err = "the traversability layer has no finite cell"; return ARTP_E_INVALID; }
   artp_se3_space sp{};
   const double Lx = rows * res, Ly = cols * res;   // grid_map getLength: the FULL length, not half of it
   sp.low[0] = cx - Lx; sp.high[0] = cx + Lx;
@@ -283,6 +311,9 @@ int artp_planner_set_map(artp_handle* hh, const artp_planner_params* pp, const f
   // failure (only a CUDA error can remain) leaves no planner map.
   h->planner_map = false;
   TRY(host_call_begin(h));
+  if (raw) {   // processors::Basic's inpaintMatrix calls (basic.cpp:42-45), from the raw layers already on the device
+    TRY(inpaint_both(h, raw_e, traversability ? raw_t : nullptr, rows, cols, d_mm, L, s));
+  }
   TRY(process_basic(h, L, rows, cols, res, &pp->basic, true, s));
   TRY(host_call_end(h));
   TRY(upload_map(h, L, L + 8 * n, true, rows, cols, res, cx, cy, 0, rows));
@@ -318,6 +349,25 @@ int artp_planner_set_map(artp_handle* hh, const artp_planner_params* pp, const f
     info->bytes_d2h = h->traffic.d2h - t0.d2h;
   }
   return ARTP_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int artp_planner_set_map(artp_handle* hh, const artp_planner_params* pp, const float* elevation, const float* traversability,
+                         const float* elevation_inpainted, const float* traversability_inpainted, int rows, int cols,
+                         double res, double cx, double cy, artp_planner_map_info* info) {
+  LOCK_CALL(h, hh);
+  return set_map(h, pp, elevation, traversability, elevation_inpainted, traversability_inpainted, false, rows, cols, res,
+                 cx, cy, info);
+}
+
+int artp_planner_set_map_raw(artp_handle* hh, const artp_planner_params* pp, const float* elevation,
+                             const float* traversability, int rows, int cols, double res, double cx, double cy,
+                             artp_planner_map_info* info) {
+  LOCK_CALL(h, hh);
+  return set_map(h, pp, elevation, traversability, nullptr, nullptr, true, rows, cols, res, cx, cy, info);
 }
 
 int artp_planner_get_space(artp_handle* hh, artp_se3_space* out) {

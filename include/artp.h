@@ -540,6 +540,16 @@ int artp_simplify_path(artp_handle* h, const double* path, size_t n, const artp_
 int artp_debug_se3_ops(artp_handle* h, const double* a, const double* b, const double* t, size_t n, double* dist,
                        double* interp);
 
+/* ---- inpaintMatrix (art_planner/src/utils.cpp:13-63) --------------------------------------------------------------
+ * The rows x cols column-major layer: its finite min / max, the NaN mask (+-inf cells are not masked), convertTo(CV_8U,
+ * 255/(max-min), -min*255/(max-min)) with the fused multiply-add, cv::inpaint(radius 3, INPAINT_TELEA) on the cols x rows
+ * image, back to float (* (max-min)/255, + min) and column / row 0 copied from column / row 1. Bit for bit with
+ * oracle/inpaint_oracle.py (DESIGN.md section 4.6, which lists its one known divergence from cv2 4.13). rows, cols >= 2, rows * cols < 2^31; a layer without a
+ * finite cell is ARTP_E_INVALID. _device: device buffers, on `stream` (a cudaStream_t cast to void*, may be NULL); one
+ * host sync reads the finite count, the rest is asynchronous. */
+int artp_inpaint_layer(artp_handle* h, const float* layer, int rows, int cols, float* out);
+int artp_inpaint_layer_device(artp_handle* h, const float* d_layer, int rows, int cols, float* d_out, void* stream);
+
 /* ---- the planner: Planner::setMap and Planner::plan + getSolutionPath for prm_motion_cost (planner.cpp:135-298) ----
  * The shipped replan (PlannerRos::updateMapAndPlanFromCurrentRobotPose, planner.name prm_motion_cost,
  * simplify_solution true) as two calls whose stages hand data to each other in device memory: no layer, state or path
@@ -556,8 +566,8 @@ int artp_debug_se3_ops(artp_handle* h, const double* a, const double* b, const d
  *                      (double)minCoeffOfFinites(raw elevation) - reach_z / 2 .. (double)maxCoeffOfFinites(..) + reach_z / 2,
  *                      from the RAW layer, before any processing; -0 is taken as +0. Min and max are order-free: exact.
  *                      A layer with no finite cell: ARTP_E_INVALID (grid_map's result there is not pinned).
- *   Basic              artp_process_basic on the INPAINTED layers (TELEA inpainting, which also quantises finite cells to
- *                      8 bits, stays with the caller: always pass inpaintMatrix's output), then the map upload of the
+ *   Basic              artp_process_basic on the INPAINTED layers (inpaintMatrix's output, which also quantises finite
+ *                      cells to 8 bits; artp_planner_set_map_raw makes them on the device), then the map upload of the
  *                      inpainted elevation and elevation_masked straight from device memory (artp_set_map's rules).
  *   the chain          artp_estimate_normals ((torso.length + torso.width) * 0.25); with sample_from_distribution the
  *                      sample filter, the distribution without vertices and its CDF; the sampler armed with the bounds' x / y;
@@ -640,6 +650,13 @@ typedef struct artp_planner_map_info {
 int artp_planner_set_map(artp_handle* h, const artp_planner_params* pp, const float* elevation, const float* traversability,
                          const float* elevation_inpainted, const float* traversability_inpainted, int rows, int cols,
                          double res, double cx, double cy, artp_planner_map_info* info);
+/* artp_planner_set_map with processors::Basic's two inpaintMatrix calls done on the device from the raw layers: only
+ * elevation and traversability (NULL: checkTraversability's 1.0 layer, not inpainted) go up. It leaves the handle in the
+ * state artp_planner_set_map leaves it in when given artp_inpaint_layer's outputs. A traversability layer without a
+ * finite cell is ARTP_E_INVALID, checked before the installed map changes. */
+int artp_planner_set_map_raw(artp_handle* h, const artp_planner_params* pp, const float* elevation,
+                             const float* traversability, int rows, int cols, double res, double cx, double cy,
+                             artp_planner_map_info* info);
 /* The artp_se3_space artp_planner_set_map installed (ARTP_E_NOMAP before). */
 int artp_planner_get_space(artp_handle* h, artp_se3_space* out);
 int artp_plan(artp_handle* h, const artp_planner_params* pp, const double* start, const double* goal, double* path,

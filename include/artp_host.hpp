@@ -518,6 +518,15 @@ enum PlannerStatus { UNKNOWN = ARTP_PLANNER_UNKNOWN, INVALID_START = ARTP_PLANNE
                      INVALID_GOAL = ARTP_PLANNER_INVALID_GOAL, NO_MAP = ARTP_PLANNER_NO_MAP,
                      NOT_SOLVED = ARTP_PLANNER_NOT_SOLVED, SOLVED = ARTP_PLANNER_SOLVED };
 
+// art_planner::inpaintMatrix (utils.cpp:13-63) on the device of `handle` (artp_inpaint_layer): the rows x cols
+// column-major layer (NaN unknown) in, the inpainted layer out, bit for bit with OpenCV's chain (DESIGN.md section 4.6).
+inline std::vector<float> inpaintMatrix(const Handle& handle, const std::vector<float>& layer, int rows, int cols) {
+  if (layer.size() != (size_t)rows * (size_t)cols) throw std::runtime_error("inpaintMatrix: layer size is not rows * cols");
+  std::vector<float> out(layer.size());
+  handle.check(artp_inpaint_layer(handle.get(), layer.data(), rows, cols, out.data()), "artp_inpaint_layer");
+  return out;
+}
+
 // art_planner::Planner for planner.name prm_motion_cost (planner.cpp:135-298) on the device: setMap is
 // artp_planner_set_map, plan is artp_plan (the simplification of getSolutionPath(true) runs inside it when
 // parameters().simplify is set), and the stages hand data to each other in device memory. The parameters start from
@@ -554,6 +563,15 @@ class Planner {
                                   traversability_inpainted.empty() ? nullptr : traversability_inpainted.data(), map.rows,
                                   map.cols, map.resolution, map.position_x, map.position_y, &map_info_),
              "artp_planner_set_map");
+  }
+  // Planner::setMap from the RAW layers alone (artp_planner_set_map_raw): processors::Basic's two inpaintMatrix calls
+  // (basic.cpp:42-45) run on the device; traversability may be empty. The handle ends in the state the overload above
+  // leaves it in when given inpaintMatrix's outputs.
+  void setMap(const Map& map, const std::vector<float>& elevation, const std::vector<float>& traversability) {
+    const auto& h = checker_->handle();
+    h->check(artp_planner_set_map_raw(h->get(), &pp_, elevation.data(), traversability.empty() ? nullptr : traversability.data(),
+                                      map.rows, map.cols, map.resolution, map.position_x, map.position_y, &map_info_),
+             "artp_planner_set_map_raw");
   }
   artp_se3_space space() const {
     artp_se3_space sp{};
