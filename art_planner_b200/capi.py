@@ -44,6 +44,14 @@ class ArtpBasicParams(C.Structure):
         "foothold_margin_min_step", "foothold_size")]
 
 
+def basic_params(b) -> ArtpBasicParams:
+    """artp_basic_params from an object with its fields (oracle.basic_oracle.BasicParams has them)."""
+    return ArtpBasicParams(float(b.traversability_thres), int(b.unknown_space_untraversable), float(b.foothold_margin),
+                           float(b.foothold_margin_max_hole_size), float(b.foothold_margin_max_drop),
+                           float(b.foothold_margin_max_drop_search_radius), float(b.foothold_margin_min_step),
+                           float(b.foothold_size))
+
+
 class ArtpSampleDistributionParams(C.Structure):
     _fields_ = [("use_inverse_vertex_density", C.c_int), ("density_blur_radius", C.c_double),
                 ("use_max_prob_unknown_samples", C.c_int), ("max_prob_unknown_samples", C.c_double)]

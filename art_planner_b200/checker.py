@@ -165,10 +165,7 @@ class StateValidityChecker:
         e = np.asfortranarray(elevation, dtype=np.float32)
         t = np.asfortranarray(traversability, dtype=np.float32)
         o = None if observed is None else np.asfortranarray(observed, dtype=np.float32)
-        p = capi.ArtpBasicParams(float(bp.traversability_thres), int(bp.unknown_space_untraversable), float(bp.foothold_margin),
-                                 float(bp.foothold_margin_max_hole_size), float(bp.foothold_margin_max_drop),
-                                 float(bp.foothold_margin_max_drop_search_radius), float(bp.foothold_margin_min_step),
-                                 float(bp.foothold_size))
+        p = capi.basic_params(bp)
         masked = np.empty(e.shape, np.float32, order="F"); thr = np.empty(e.shape, np.float32, order="F")
         self._h.check(self._h.lib.artp_process_basic(self._h.h, e.ctypes.data, t.ctypes.data, None if o is None else o.ctypes.data,
                                                      e.shape[0], e.shape[1], float(res), C.byref(p), masked.ctypes.data, thr.ctypes.data))
@@ -393,6 +390,13 @@ class StateValidityChecker:
         return self._h
 
 
+def _distribution_params(sp, rp) -> capi.ArtpSampleDistributionParams:
+    """The distribution parameters from the sampler parameters `sp` and the robot's `rp`, with the reference Planner's
+    density blur radius (planner.cpp:48)."""
+    return capi.ArtpSampleDistributionParams(int(sp.use_inverse_vertex_density), (rp.torso_length + rp.torso_width) * 0.25,
+                                             int(sp.use_max_prob_unknown_samples), float(sp.max_prob_unknown_samples))
+
+
 class SE3FromSE2Sampler:
     """art_planner::SE3FromSE2Sampler::sampleUniform (src/sampler.cpp:82-131) on the device, plus the fused
     sample -> isValid -> compact form of the rejection loops around it (prm_motion_cost.cpp:171-194).
@@ -426,10 +430,7 @@ class SE3FromSE2Sampler:
         then the sampler re-armed on the new device CDF. Parameters from `sp` (use_inverse_vertex_density,
         use_max_prob_unknown_samples, max_prob_unknown_samples) and the blur radius of planner.cpp:48."""
         h, lib = self._c.handle, self._c.handle.lib
-        rp = h.params
-        dp = capi.ArtpSampleDistributionParams(int(self._sp.use_inverse_vertex_density), (rp.torso_length + rp.torso_width) * 0.25,
-                                               int(self._sp.use_max_prob_unknown_samples), float(self._sp.max_prob_unknown_samples))
-        self._c.updateSampleDistribution(vertex_states, dp, want_host=False)
+        self._c.updateSampleDistribution(vertex_states, _distribution_params(self._sp, h.params), want_host=False)
         h.check(lib.artp_set_sampler(h.h, C.byref(self._params), *[None if a is None else a.ctypes.data for a in self._normals],
                                      None, None))
 
@@ -535,11 +536,7 @@ class PRMRoadmap:
         budget replaces max_sample_time. Returns the draws used."""
         h = self._c.handle
         p = capi.ArtpRoadmapParams(int(max_n_vertices), int(max_n_edges), int(recompute_density_after_n_samples), int(max_draws))
-        dp = None
-        if distribution:
-            sp, rp = sampler._sp, h.params
-            dp = capi.ArtpSampleDistributionParams(int(sp.use_inverse_vertex_density), (rp.torso_length + rp.torso_width) * 0.25,
-                                                   int(sp.use_max_prob_unknown_samples), float(sp.max_prob_unknown_samples))
+        dp = _distribution_params(sampler._sp, h.params) if distribution else None
         used = C.c_uint64(0)
         h.check(h.lib.artp_roadmap_sample_graph(h.h, C.byref(p), None if dp is None else C.byref(dp), sampler.seed,
                                                 int(first_sample), C.byref(used)))
@@ -675,10 +672,7 @@ class Planner:
                                                                  foothold_margin_max_drop=0.3,
                                                                  foothold_margin_max_drop_search_radius=0.16,
                                                                  foothold_margin_min_step=0.3, foothold_size=0.1))
-        p.basic = capi.ArtpBasicParams(float(b.traversability_thres), int(b.unknown_space_untraversable), float(b.foothold_margin),
-                                       float(b.foothold_margin_max_hole_size), float(b.foothold_margin_max_drop),
-                                       float(b.foothold_margin_max_drop_search_radius), float(b.foothold_margin_min_step),
-                                       float(b.foothold_size))
+        p.basic = capi.basic_params(b)
         return p
 
     def setMap(self, elevation, traversability, elevation_inpainted, traversability_inpainted, res: float, cx: float,

@@ -946,8 +946,8 @@ void artp_destroy(artp_handle* hh) {
   if (h->stream) { cudaStreamSynchronize(h->stream); cudaStreamDestroy(h->stream); }
   delete h->pipe;
   for (int k = 0; k < 2; ++k) for (int l = 0; l <= artp::kMaxLevel; ++l) { cudaFree(h->d_T[k][l]); cudaFree(h->d_C[k][l]); }
-  cudaFree(h->d_H[0]); cudaFree(h->d_H[1]); cudaFree(h->d_stage); cudaFree(h->d_samp_layers); cudaFree(h->d_samp_scratch);
-  cudaFree(h->d_dist_layers); cudaFree(h->d_dist_scratch); cudaFree(h->d_basic_keep); cudaFree(h->d_simplify);
+  cudaFree(h->d_H[0]); cudaFree(h->d_H[1]); cudaFree(h->d_stage); cudaFree(h->d_simplify);
+  sampling_free(h);
   roadmap_free(h);
   planner_free(h);
   if (h->h_err) cudaFreeHost(h->h_err);
@@ -1179,7 +1179,7 @@ int artp_api::upload_map(Handle* h, const float* elevation, const float* elevati
   h->chk.cell_margin = 0.02f + 2e-6f * (float)std::max(rows, cols);
   TRY(set_shapes(h, span, tcap, store));
   h->has_map = true;
-  h->map = MapState{};         // the sampler and the derived layers belong to the previous map
+  sampling_forget_map(h);
   h->res = res;
   return ARTP_OK;
 }

@@ -24,22 +24,13 @@
 
 namespace artp_api {
 
-// What belongs to the current map: artp_set_map_window resets all of it.
 struct Roadmap;
-
-struct MapState {
-  bool has_sampler = false;
-  bool has_device_normals = false;  // artp_estimate_normals filled normal_x/y/z/std_dev of d_samp_layers for this map
-  bool has_device_cdf = false;      // artp_compute_sample_cdf filled cum_prob / cum_row of d_samp_layers for this map
-  bool has_normals = false;         // normal_x/y/z of d_samp_layers hold this map's normals (device-estimated or the caller's)
-  bool has_sample_filter = false;   // d_dist_layers holds this map's traversability_sample_filter ...
-  bool has_dist_observed = false;   // ... and observed layer
-};
 
 // Host <-> device traffic and host synchronisations of the calls that count them (artp_plan reports its own).
 struct Traffic { uint64_t h2d = 0, d2h = 0; uint32_t syncs = 0; };
 struct PlannerState;   // artp_planner_set_map / artp_plan (artp_planner.cu)
 struct Pipeline;       // the validity pipeline's queues, launch shapes, streams and events (artp_capi.cu)
+struct Sampling;       // the sampler, the distribution, their layers and what the map has of them (artp_sampling.cu)
 
 struct Handle {
   artp_params p;
@@ -53,36 +44,20 @@ struct Handle {
   int rows = 0, cols = 0;           // full map
   int win_row0 = 0, win_rows = 0;   // rows held by this handle (artp_set_map_window); whole map: 0, rows
   bool has_map = false;
-  MapState map;
   Pipeline* pipe = nullptr;         // from artp_create
   char* d_stage = nullptr;          // device staging for the host-buffer API
   size_t stage_cap = 0;
   cudaStream_t stream = nullptr;    // internal compute stream for the host-buffer API
   artp_cnn::State* cnn = nullptr;
   int cnn_mode = 0;
-  // sampler (artp_set_sampler): device copies of the per-cell layers, scratch of the fused sample->check->compact path
-  artp::SamplerDev samp{};
-  float* d_samp_layers = nullptr;   // normal_x | normal_y | normal_z | std_dev | cum_prob | cum_row
-  size_t samp_layers_cap = 0;       // floats
-  char* d_samp_scratch = nullptr;
-  size_t samp_scratch_cap = 0;
+  Sampling* sampling = nullptr;     // from the first call that needs it
   double res = 0.0;                 // map resolution as artp_set_map received it
-  // sampling distribution (artp_distribution.cuh): the layers artp_set_sample_filter keeps for this map ...
-  float* d_dist_layers = nullptr;   // traversability_sample_filter | observed
-  size_t dist_layers_cap = 0;       // floats
-  char* d_dist_scratch = nullptr;   // n_samples | blur pass | sample_probability | cap row sums | words (artp_update_sample_distribution)
-  size_t dist_scratch_cap = 0;
-  // ... and the layers of the last artp_process_basic, its NULL-layer inputs
-  float* d_basic_keep = nullptr;    // observed | traversability_thresholded
-  size_t basic_keep_cap = 0;        // floats
-  int basic_rows = 0, basic_cols = 0;
-  bool has_basic_layers = false, has_basic_observed = false;
   Roadmap* roadmap = nullptr;       // the PRM roadmap store (artp_roadmap.cu), from the first artp_roadmap_clear
   char* d_simplify = nullptr;       // artp_simplify_path: state pool, path, round buffers (artp_path_simplify.cu)
   size_t simplify_cap = 0;
   // Cross-stream ordering of the per-handle scratch (ADVICE r1): calls may come on different streams; every call that
   // uses a scratch group first makes its stream wait for the previous user of that group, and records an event after.
-  // group 0: the pipeline's counters and queues / d_stage / d_samp_scratch / d_dist_scratch (check, sampler, distribution);
+  // group 0: the pipeline's counters and queues / d_stage / the sampling unit's scratch (check, sampler, distribution);
   // group 1: the pipeline's compaction state
   cudaEvent_t chain_ev[2] = {nullptr, nullptr};
   cudaStream_t chain_stream[2] = {nullptr, nullptr};
@@ -259,8 +234,12 @@ int compact_valid(Handle* h, const uint8_t* d_valid, size_t n, int64_t base, voi
 int check_states_cta(Handle* h, const double* d_states, const uint32_t* d_count, const uint32_t* d_stop, size_t max_n,
                      uint8_t* d_valid, cudaStream_t s);
 
-// artp_sampling.cu, for the roadmap:
-// A map and an armed sampler (ARTP_E_NOMAP otherwise).
+// artp_sampling.cu: upload_map forgets what the unit derived from the previous map; artp_destroy frees the rest.
+void sampling_forget_map(Handle* h);
+void sampling_free(Handle* h);
+// The density blur radius of the reference's Planner (planner.cpp:48).
+inline double density_blur_radius(const artp_params& p) { return (p.torso_length + p.torso_width) * 0.25; }
+// For the roadmap: a map and an armed sampler (ARTP_E_NOMAP otherwise).
 int sampler_armed(Handle* h);
 // artp_sample_valid_device's work on s, with the draw index of every kept state into d_draws (capacity entries).
 int sample_valid_draws(Handle* h, uint64_t seed, uint64_t first_sample, size_t n_draw, double* d_states_out, uint64_t* d_draws,
@@ -313,8 +292,9 @@ int process_basic(Handle* h, float* L, int rows, int cols, double res, const art
 int map_chain_limits(Handle* h, const artp_basic_params* bp, double res, bool distribution, bool inverse_density);
 int estimate_normals(Handle* h, double estimation_radius, cudaStream_t s);
 int set_sample_filter_basic(Handle* h, cudaStream_t s);   // artp_set_sample_filter(h, NULL, NULL, NULL)
-// artp_set_sampler(h, sp, NULL x 6) on the layers the device computed for this map (no CDF validation: they are cumulative).
-int arm_sampler_device(Handle* h, const artp_sampler_params* sp);
+// Points the sampler at the resident layers (the CDF too when it samples from the distribution): with sp, as
+// artp_set_sampler(h, sp, NULL x 6) without its CDF validation; without, keeping its view and parameters.
+void arm_sampler(Handle* h, const artp_sampler_params* sp);
 int ball_search(Handle* h, const double* d_centres, size_t n, const double* d_radius, uint32_t n_iter, uint64_t seed,
                 uint64_t first_draw, double* d_states_out, int32_t* d_index, cudaStream_t s);
 int pose_from_2d(Handle* h, const double* d_in, size_t n, double* d_out, uint8_t* d_inside, cudaStream_t s);

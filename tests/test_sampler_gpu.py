@@ -114,6 +114,30 @@ def test_sampler_errors(rig):
         smp.sampleUniformBatch(4)
 
 
+def test_refused_arming_keeps_the_armed_sampler(rig):
+    """artp_set_sampler refusing CDF layers that are not cumulative leaves an armed sampler as it was: still uniform, in
+    its own bounds, drawing what it drew before."""
+    ap, m, chk, L = rig
+    import copy
+    import dataclasses
+    chk2 = ap.StateValidityChecker(cases.PARAMS["yaml"], device=0)
+    chk2.setMap(m)
+    chk2.updateHeightField()
+    full = synth.sampler_params_for(m)
+    narrow = dataclasses.replace(synth.sampler_params_for(m, from_distribution=False),
+                                 low=tuple(0.75 * a + 0.25 * b for a, b in zip(full.low, full.high)),
+                                 high=tuple(0.25 * a + 0.75 * b for a, b in zip(full.low, full.high)))
+    smp = ap.SE3FromSE2Sampler(chk2, L, narrow, seed=9)
+    want = smp.sampleUniformBatch(512, first=0)
+    bad = copy.copy(L)
+    cp = L.cum_prob.copy(order="F")
+    cp[5, 10] = cp[5, 9] - 0.25                  # not a CDF any more
+    bad.cum_prob = cp
+    with pytest.raises(RuntimeError):
+        smp.setLayers(bad, full)
+    assert np.array_equal(smp.sampleUniformBatch(512, first=0), want, equal_nan=True)
+
+
 @pytest.mark.parametrize("mk", ["fbm_rough", "ramp", "fixture", "flat_holes_terrace"])
 def test_estimate_normals_bit_exact(maps, port_lib, mk):
     """artp_estimate_normals == the CPU restatement of utils.cpp:213-324, bit for bit (float32 layers)."""
