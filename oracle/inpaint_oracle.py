@@ -195,9 +195,52 @@ def to_u8(x: np.ndarray, alpha: np.float32, beta: np.float32) -> np.ndarray:
     return np.where(ok, np.clip(r, 0, 255), 0).astype(np.uint8)
 
 
-def inpaint_matrix(layer: np.ndarray) -> np.ndarray:
-    """inpaintMatrix of a rows x cols float32 grid_map layer; returns the inpainted layer (column-major, float32).
-    Raises ValueError for a layer without a finite cell (the C ABI's ARTP_E_INVALID)."""
+def interaction_components(mask: np.ndarray):
+    """The interaction components of a mask: the 8-connected components of the mask dilated by the 7 x 7 square.
+    Returns (labels, n) as scipy.ndimage.label does: 0 outside every component, ids 1..n."""
+    from scipy import ndimage
+    return ndimage.label(_dilate(np.asarray(mask) != 0, RANGE), structure=np.ones((3, 3), bool))
+
+
+def telea_by_components(img: np.ndarray, mask: np.ndarray, margin: int = 4, components=None, labels=None):
+    """telea(img, mask), one interaction component at a time: each component's cells come from telea run on the
+    component's bounding box widened by `margin` cells (clipped to the image) with only that component's mask cells.
+    Returns (result, labels); with `components` (an iterable of ids) only those components are inpainted and every
+    other mask cell keeps its input byte. `labels` may pass interaction_components(mask)[0] to skip the labelling.
+
+    Why it equals the whole-image march for any margin >= 1: the component's box already holds every cell within
+    Chebyshev distance 3 of its mask. Inpainting a cell reads f, t and the image only within distance 4 of it (the
+    radius-3 window, then one more cell for the image gradient's and FastMarching_solve's neighbours), and the outer
+    pass marches only the ring within 3 of the mask, so with margin >= 1 every read lands inside the crop and no other
+    component's cell is within reach (two components' masks are at least 8 apart). The gradient's km / kp / lm / lp
+    clamps act on a window cell in the crop's first or last row or column; a window cell is within 3 of the mask, so
+    that is the crop's edge only where the crop edge is the true image border. Within the crop, the queue's (T, push
+    order) keeps the same relative order as the whole image's: the band is pushed in raster order in both, and the
+    interleaving with other components' cells never changes what this component reads."""
+    img = np.asarray(img, np.uint8)
+    m = np.asarray(mask) != 0
+    if labels is None:
+        labels, n = interaction_components(m)
+    else:
+        n = int(labels.max())
+    from scipy import ndimage
+    boxes = ndimage.find_objects(labels)
+    out = img.copy()
+    H, W = img.shape
+    ids = range(1, n + 1) if components is None else components
+    for c in ids:
+        sy, sx = boxes[c - 1]
+        y0, y1 = max(sy.start - margin, 0), min(sy.stop + margin, H)
+        x0, x1 = max(sx.start - margin, 0), min(sx.stop + margin, W)
+        cm = m[y0:y1, x0:x1] & (labels[y0:y1, x0:x1] == c)
+        res = telea(img[y0:y1, x0:x1], cm)
+        out[y0:y1, x0:x1][cm] = res[cm]
+    return out, labels
+
+
+def to_image(layer: np.ndarray):
+    """inpaintMatrix up to the march: (NaN mask, 8-bit image, both cols x rows; the finite min; the scale back;
+    whether the finite cells are all equal, which skips the march). Raises ValueError for a layer without a finite cell (the C ABI's ARTP_E_INVALID)."""
     mat = np.asfortranarray(np.asarray(layer, np.float32))
     fin = np.isfinite(mat)
     if not fin.any():
@@ -212,10 +255,40 @@ def inpaint_matrix(layer: np.ndarray) -> np.ndarray:
         beta = f32(f32(f32(-mn) * f32(255)) / rng_)
         scale = f32(rng_ / f32(255))
     u8 = to_u8(img_f, alpha, beta) if mx != mn else np.zeros(img_f.shape, np.uint8)
-    res = telea(u8, mask) if mx != mn else u8
+    return mask, u8, mn, scale, mx == mn
+
+
+def from_image(res: np.ndarray, mn: np.float32, scale: np.float32) -> np.ndarray:
+    """inpaintMatrix after the march: the cols x rows 8-bit image back to a column-major float layer (two float
+    operations), then the column / row 0 copies."""
     with np.errstate(all="ignore"):
         back = (res.astype(np.float32) * scale) + mn           # two float operations
     out = np.asfortranarray(back.T).astype(np.float32)
     out[:, 0] = out[:, 1]
     out[0, :] = out[1, :]
     return out
+
+
+def inpaint_matrix(layer: np.ndarray) -> np.ndarray:
+    """inpaintMatrix of a rows x cols float32 grid_map layer; returns the inpainted layer (column-major, float32).
+    Raises ValueError for a layer without a finite cell (the C ABI's ARTP_E_INVALID)."""
+    mask, u8, mn, scale, const = to_image(layer)
+    return from_image(u8 if const else telea(u8, mask), mn, scale)
+
+
+def inpaint_matrix_by_components(layer: np.ndarray, margin: int = 4, components=None, labels=None):
+    """inpaint_matrix through telea_by_components. Returns (inpainted layer, labels) where labels is the interaction
+    components' label image in the layer's rows x cols shape (0 outside every component). With `components`, mask
+    cells of the other components keep the 8-bit conversion's byte of NaN (0), so only cells outside those
+    components' masks and inside the chosen ones are inpaintMatrix's. `labels` may pass layer_components(layer)."""
+    mask, u8, mn, scale, const = to_image(layer)
+    lab = interaction_components(mask)[0] if labels is None else np.ascontiguousarray(np.asarray(labels).T)
+    if const:
+        return from_image(u8, mn, scale), lab.T
+    res, lab = telea_by_components(u8, mask, margin, components, lab)
+    return from_image(res, mn, scale), lab.T
+
+
+def layer_components(layer: np.ndarray) -> np.ndarray:
+    """The interaction components of a layer's NaN cells as a rows x cols label image (0 outside every component)."""
+    return interaction_components(np.isnan(np.asarray(layer, np.float32)).T)[0].T

@@ -128,6 +128,162 @@ def profile_layer(n, pattern, frac=0.14, seed=0):
     return np.asfortranarray(a)
 
 
+# ---- map-scale layers (tests/test_inpaint_scale_gpu.py; small versions in tests/test_inpaint_components_cpu.py) ----
+
+DIRECTIONS = {"h": (0, 1), "v": (1, 0), "d": (1, 1), "a": (1, -1)}
+
+
+def hole_pair(direction, gap, block_first):
+    """Cells of a one-cell hole and a 2 x 2 hole at Chebyshev distance `gap` along `direction` (the 2 x 2 hole first
+    when `block_first`), shifted to start at row / column 0."""
+    di, dj = DIRECTIONS[direction]
+    block = [(0, 0), (0, 1), (1, 0), (1, 1)]
+    if block_first:
+        a = block
+        b = [(di * (gap + 1) if di > 0 else 0, dj * (gap + 1) if dj > 0 else dj * gap)]
+    else:
+        a = [(0, 0)]
+        b = [(di * gap + y, dj * gap + x - (1 if dj < 0 else 0)) for y, x in block]
+    cells = np.array(a + b)
+    cells -= cells.min(0)
+    na = len(a)
+    d = np.abs(cells[:na, None, :] - cells[None, na:, :]).max(-1).min()
+    assert d == gap, (direction, gap, block_first, d)
+    return cells[:na], cells[na:]
+
+
+def gap_lattice(rows=1000, cols=1000, gaps=(7, 8), tile=18, seed=10, border=False):
+    """Hole pairs on a tile x tile lattice, every (direction, gap, order) in turn in a seeded shuffle; one pair per
+    tile at the tile's origin. A pair spans at most max(gaps) + 2 cells, so with tile >= max(gaps) + 10 pairs of
+    neighbouring tiles are at least 8 apart: each pair at gap <= 7 is one interaction component, at gap >= 8 two.
+    With `border`, the layer is cropped to the holes, so pairs touch all four borders.
+    Returns (layer, pairs) with pairs = [(a cells, b cells, gap)] in layer (row, col) coordinates."""
+    assert tile >= max(gaps) + 10
+    rng = np.random.default_rng(seed)
+    kinds = [(d, g, o) for d in DIRECTIONS for g in gaps for o in (False, True)]
+    ti, tj = -(-rows // tile), -(-cols // tile)
+    pick = rng.permutation(np.arange(ti * tj) % len(kinds))
+    pairs = []
+    for t in range(ti * tj):
+        a, b = hole_pair(*kinds[pick[t]])
+        o = np.array([(t // tj) * tile, (t % tj) * tile])
+        a, b = a + o, b + o
+        if np.concatenate([a, b]).max(0)[0] < rows and np.concatenate([a, b]).max(0)[1] < cols:
+            pairs.append((a, b, kinds[pick[t]][1]))
+    a = _field(rows, cols, seed, noise=0.2)
+    for p, q, _ in pairs:
+        a[p[:, 0], p[:, 1]] = np.nan
+        a[q[:, 0], q[:, 1]] = np.nan
+    if border:
+        cells = np.concatenate([np.concatenate(p[:2]) for p in pairs])
+        hi = cells.max(0) + 1
+        a = np.asfortranarray(a[:hi[0], :hi[1]])
+    return a, pairs
+
+
+def size_ladder(rows=997, cols=613, sides=(1, 2, 6, 12, 20, 30, 50, 70, 100, 130), step=9, seed=11):
+    """One square hole of each side in `sides` (interaction components of (side + 6)^2 cells: one per power-of-two
+    size class from 2^5 up; side 130 is class 2^14), a one-cell hole in the corner (class 2^4, a clipped 4 x 4 region)
+    and two on the borders (4 x 7), then a lattice of 1- and 2-cell holes every `step` cells on the columns right
+    of the squares: several components of each small class, and more components than the march launches warps."""
+    assert step >= 9
+    a = _field(rows, cols, seed, noise=0.1)
+    rng = np.random.default_rng(seed)
+    i = 10
+    for s in sides:
+        a[i:i + s, 10:10 + s] = np.nan
+        i += s + 10
+    assert i <= rows, "the ladder does not fit"
+    a[0, 0] = np.nan
+    a[rows // 2, cols - 1] = np.nan
+    a[rows - 1, 5] = np.nan
+    j0 = 10 + max(sides) + 10
+    for ii in range(0, rows - 1, step):
+        for jj in range(j0, cols - 2, step):
+            k = rng.integers(0, 3)
+            a[ii, jj] = np.nan
+            if k == 1:
+                a[ii + 1, jj] = np.nan
+            elif k == 2:
+                a[ii, jj + 1] = np.nan
+    return a
+
+
+def long_thin(rows=800, cols=700, seed=12, spiral=61):
+    """Long components whose bounding box is far larger than their cell count: a 1-cell diagonal line, a zig-zag
+    line of 8-connected diagonal runs, and a square spiral of 1-cell arms 2 apart (a long march through many equal
+    T values)."""
+    a = _field(rows, cols, seed, noise=0.1)
+    n = min(rows, cols) // 2 - 20
+    k = np.arange(n)
+    a[10 + k, 10 + k] = np.nan
+    i = np.arange(10, rows - 10)
+    amp = max(4, (cols - n - 60) // 2)
+    tri = np.abs((i % (2 * amp)) - amp)
+    a[i, cols - 10 - tri] = np.nan
+    # the spiral: walk right, down, left, up with arm lengths shrinking by 2 every two turns
+    y, x = rows - spiral - 10, 10
+    length, d = spiral - 1, 0
+    steps = [(0, 1), (1, 0), (0, -1), (-1, 0)]
+    a[y, x] = np.nan
+    while length > 0:
+        for _ in range(length):
+            y, x = y + steps[d][0], x + steps[d][1]
+            a[y, x] = np.nan
+        if d % 2 == 1:
+            length -= 2
+        d = (d + 1) % 4
+    return a
+
+
+def thin_layer(rows, cols, seed=13):
+    """A layer 2-5 cells thin: NaN in the four corners, a hole across the whole width at both ends' second cell,
+    and 1-cell holes 8 apart along the length (as many components as the width allows) with a few gaps."""
+    a = _field(rows, cols, seed, noise=0.1)
+    t = a if rows <= cols else a.T                     # a view: thin x long
+    w, n = t.shape
+    for y in (0, w - 1):
+        for x in (0, n - 1):
+            t[y, x] = np.nan
+    t[:, 2] = np.nan
+    t[:, n - 3] = np.nan
+    rng = np.random.default_rng(seed)
+    for x in range(12, n - 12, 8):
+        if rng.random() < 0.85:
+            t[rng.integers(0, w), x] = np.nan
+    return np.asfortranarray(a)
+
+
+def scattered(rows, cols, n_holes, seed=14):
+    """Seeded 1-20-cell rectangles across the layer, plus holes in the four corners and on each border."""
+    a = _field(rows, cols, seed, noise=0.1)
+    rng = np.random.default_rng(seed)
+    h = rng.integers(1, 5, n_holes)
+    w = np.minimum(rng.integers(1, 21, n_holes), 20 // h)
+    y = rng.integers(0, rows - h + 1)
+    x = rng.integers(0, cols - w + 1)
+    for yy, xx, hh, ww in zip(y, x, h, w):
+        a[yy:yy + hh, xx:xx + ww] = np.nan
+    for yy, xx in ((0, 0), (0, cols - 2), (rows - 3, 0), (rows - 1, cols - 1)):
+        a[yy:yy + 3, xx:xx + 2] = np.nan
+    a[0, cols // 3] = a[rows - 1, cols // 2] = a[rows // 3, 0] = a[rows // 2, cols - 1] = np.nan
+    return a
+
+
+def near_constant(ulps, rows=300, cols=257, seed=15, base=np.float32(37.25)):
+    """A layer whose finite cells lie within `ulps` float steps above `base`, with scattered holes: the 8-bit
+    conversion's multiply-add then lands near byte midpoints, where a fused and an unfused one round differently."""
+    rng = np.random.default_rng(seed)
+    k = rng.integers(0, ulps + 1, (rows, cols)).astype(np.uint32)
+    k[0, 0], k[-1, -1] = 0, ulps
+    a = (np.uint32(np.float32(base).view(np.uint32)) + k).view(np.float32)
+    a = np.asfortranarray(a)
+    hole = rng.random((rows, cols)) < 0.05
+    hole[0, 0] = hole[-1, -1] = False
+    a[hole] = np.nan
+    return a
+
+
 # The one known divergence of the restatement from cv2 (DESIGN.md section 4.6): a 120 x 120 crop of the 8-bit image
 # inpaintMatrix makes from profile_layer(1000, "holes") (image rows 0-119, columns 380-499). cv2.inpaint differs from
 # oracle.inpaint_oracle.telea on 6 cells of it. The golden file stores the crop's image, mask and cv2's result.
