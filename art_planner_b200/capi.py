@@ -97,7 +97,7 @@ class ArtpPlannerParams(C.Structure):
                 ("edge_capacity", C.c_size_t), ("max_roll_pert", C.c_double), ("max_pitch_pert", C.c_double),
                 ("sample_from_distribution", C.c_int), ("use_inverse_vertex_density", C.c_int),
                 ("use_max_prob_unknown_samples", C.c_int), ("max_prob_unknown_samples", C.c_double), ("basic", ArtpBasicParams),
-                ("simplify", C.c_int), ("clear_roadmap", C.c_int), ("seed", C.c_uint64)]
+                ("simplify", C.c_int), ("clear_roadmap", C.c_int), ("seed", C.c_uint64), ("cost_map_from_raw", C.c_int)]
 
 
 class ArtpPlanInfo(C.Structure):
@@ -201,6 +201,10 @@ def load():
                                              C.POINTER(ArtpPlannerMapInfo)]
     lib.artp_inpaint_layer.argtypes = [vp, vp, i32, i32, vp]
     lib.artp_inpaint_layer_device.argtypes = [vp, vp, i32, i32, vp, vp]
+    lib.artp_cost_map_layer.argtypes = [vp, vp, i32, i32, vp]
+    lib.artp_cost_map_layer_device.argtypes = [vp, vp, i32, i32, vp, vp]
+    lib.artp_update_features_raw.argtypes = [vp, vp, i32, i32, dbl, dbl, dbl]
+    lib.artp_update_features_raw_device.argtypes = [vp, vp, i32, i32, dbl, dbl, dbl, vp]
     lib.artp_planner_get_space.argtypes = [vp, C.POINTER(ArtpSe3Space)]
     lib.artp_plan.argtypes = [vp, C.POINTER(ArtpPlannerParams), vp, vp, vp, sz, C.POINTER(sz), C.POINTER(ArtpPlanInfo)]
     lib.artp_host_alloc.restype = C.c_void_p

@@ -65,6 +65,14 @@ def _stream_ptr():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+def _column_major_cuda(layer, what: str):
+    """(rows, cols) of a column-major float32 CUDA layer (a transposed contiguous cols x rows tensor)."""
+    import torch
+    if layer.dtype != torch.float32 or not layer.t().is_contiguous():
+        raise ValueError(f"{what}: a CUDA layer must be float32 and column-major (a transposed contiguous tensor)")
+    return layer.shape
+
+
 class StateValidityChecker:
     """art_planner::StateValidityChecker on the GPU (validity_checker.cpp:9-45)."""
 
@@ -662,7 +670,7 @@ class Planner:
                  recompute_density_after_n_samples=1000, max_query_edge_length=0.5, max_draws=1 << 26, vertex_capacity=20000,
                  edge_capacity=60000, max_roll_pert=3.33 / 180 * np.pi, max_pitch_pert=10.0 / 180 * np.pi,
                  sample_from_distribution=1, use_inverse_vertex_density=1, use_max_prob_unknown_samples=1,
-                 max_prob_unknown_samples=0.1, simplify=1, clear_roadmap=0, seed=int(seed))
+                 max_prob_unknown_samples=0.1, simplify=1, clear_roadmap=0, seed=int(seed), cost_map_from_raw=0)
         basic = kw.pop("basic", None)
         d.update(kw)
         for k, v in d.items():
@@ -946,6 +954,36 @@ class MotionCostObjective:
         """CostPredictor.updateFeatures over the checker's current map (predictor.py:28-36)."""
         h = self._c.handle
         h.check(h.lib.artp_update_features(h.h))
+
+    def updateFeaturesRaw(self, layer, res: float, cx: float, cy: float) -> None:
+        """CostPredictor.updateFeatures on the map the cost server prepares from the RAW rows x cols elevation layer
+        (cost_query_server.py _elvMapProcess, artp_update_features_raw): no installed map needed; geometry res, cx, cy.
+        numpy arrays use the host entry point, CUDA tensors (column-major float32, as StateValidityChecker.inpaint) the
+        device one on the current stream."""
+        h = self._c.handle
+        if _is_torch_cuda(layer):
+            rows, cols = _column_major_cuda(layer, "updateFeaturesRaw")
+            h.check(h.lib.artp_update_features_raw_device(h.h, layer.data_ptr(), rows, cols, float(res), float(cx), float(cy),
+                                                          _stream_ptr()))
+            return
+        a = np.asfortranarray(layer, dtype=np.float32)
+        h.check(h.lib.artp_update_features_raw(h.h, a.ctypes.data, a.shape[0], a.shape[1], float(res), float(cx), float(cy)))
+
+    def costMap(self, layer):
+        """The cost server's preparation of the RAW rows x cols elevation layer (artp_cost_map_layer): the map whose
+        network input the server feeds the trunk, in grid_map layout, column-major float32. A CUDA tensor (column-major,
+        as StateValidityChecker.inpaint) gives a CUDA tensor of the same layout, on the current stream."""
+        h = self._c.handle
+        if _is_torch_cuda(layer):
+            import torch
+            rows, cols = _column_major_cuda(layer, "costMap")
+            out = torch.empty((cols, rows), dtype=torch.float32, device=layer.device).t()
+            h.check(h.lib.artp_cost_map_layer_device(h.h, layer.data_ptr(), rows, cols, out.data_ptr(), _stream_ptr()))
+            return out
+        a = np.asfortranarray(layer, dtype=np.float32)
+        out = np.empty(a.shape, np.float32, order="F")
+        h.check(h.lib.artp_cost_map_layer(h.h, a.ctypes.data, a.shape[0], a.shape[1], out.ctypes.data))
+        return out
 
     def costQuery(self, edge_matrix, out=None):
         """edge_matrix [n, 6] float32 = [tx, ty, tyaw, sx, sy, syaw] -> [n, 3] float32 (energy, time, risk)."""

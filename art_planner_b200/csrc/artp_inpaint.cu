@@ -1,7 +1,10 @@
 // art_planner_b200/csrc/artp_inpaint.cu -- inpaintMatrix on the device (artp_inpaint.cuh) behind the C ABI:
 // artp_inpaint_layer (host buffers), artp_inpaint_layer_device (device buffers), and artp_api::inpaint_layer, the body
-// artp_planner_set_map_raw runs on the layers it has uploaded.
+// artp_planner_set_map_raw runs on the layers it has uploaded. Beside it the cost server's preparation of the same raw
+// layer over the same march: artp_cost_map_layer[_device], and artp_update_features_raw[_device], which runs the trunk on
+// it (cost_map_features, also what artp_planner_set_map[_raw] run with cost_map_from_raw).
 #include <algorithm>
+#include <cmath>
 
 #include "artp_internal.h"
 #include "artp_inpaint.cuh"
@@ -11,21 +14,27 @@ using namespace artp_inpaint;
 
 namespace {
 
-int inpaint_args(Handle* h, const void* in, int rows, int cols, const void* out) {
+int inpaint_args(Handle* h, const void* in, int rows, int cols, const void* out, const char* what = "inpaint") {
   if (!in || !out) return null_buffer(h);
   if (rows < 2 || cols < 2 || (size_t)rows * cols >= 0x7FFFFFFFull) {
-    h->err = "inpaint: rows and cols must be >= 2 and rows * cols < 2^31"; return ARTP_E_INVALID;
+    h->err = std::string(what) + ": rows and cols must be >= 2 and rows * cols < 2^31"; return ARTP_E_INVALID;
   }
   return ARTP_OK;
 }
 
-}  // namespace
+// artp_update_features_raw[_device]'s checks before any work: arguments, geometry, weights.
+int features_raw_args(Handle* h, const float* raw, int rows, int cols, double res, double cx, double cy) {
+  TRY(inpaint_args(h, raw, rows, cols, raw, "cost map"));
+  if (!(res > 0) || !std::isfinite(cx) || !std::isfinite(cy)) { h->err = "bad map arguments"; return ARTP_E_INVALID; }
+  if (!artp_cnn::has_weights(h->cnn)) { h->err = "motion-cost weights not set"; return ARTP_E_NOWEIGHTS; }
+  return ARTP_OK;
+}
 
-// The march on a layer whose finite min / max keys (finite_min_max) are at d_mm; stream-ordered scratch.
-int artp_api::inpaint_layer(Handle* h, const float* d_in, int rows, int cols, const uint32_t* d_mm, float* d_out,
-                            cudaStream_t s) {
-  const size_t n = (size_t)rows * cols;
-  const int H = cols, W = rows;
+// The stages from region to march (artp_inpaint.cuh) on the H x W image that prep(img, flag) fills, then finish(img);
+// stream-ordered scratch.
+template <class Prep, class Finish>
+int march(Handle* h, int H, int W, cudaStream_t s, Prep prep, Finish finish) {
+  const size_t n = (size_t)H * W;
   // Components: their regions are disjoint and each holds the clipped 7 x 7 square around one of its mask cells, so
   // there are at most n / (min(4, H) * min(4, W)) of them.
   const size_t max_comp = n / ((size_t)std::min(4, H) * std::min(4, W)) + 1;
@@ -50,7 +59,7 @@ int artp_api::inpaint_layer(Handle* h, const float* d_in, int rows, int cols, co
   const unsigned g = grid_for(h, n, 256, 8);
   auto run = [&]() -> int {
     CU_TRY(h, cudaMemsetAsync(cnt, 0, bytes[9], s));
-    TRY(launch(h, inp_prep_kernel, g, 256, 0, s, d_in, n, d_mm, img, flag));
+    TRY(prep(img, flag));
     TRY(launch(h, inp_region_kernel, g, 256, 0, s, H, W, flag, t, label));
     TRY(launch(h, inp_union_kernel, g, 256, 0, s, H, W, label));
     TRY(launch(h, inp_root_kernel, g, 256, 0, s, n, label, slot, comps, cnt));
@@ -62,10 +71,60 @@ int artp_api::inpaint_layer(Handle* h, const float* d_in, int rows, int cols, co
     Grid gr{H, W, img, flag, t};
     TRY(launch(h, inp_march_kernel, (unsigned)h->sm_count * 8, 32 * kWarps, 0, s, gr, (const int*)label, (const Comp*)comps,
                (const int*)order, (const int*)cnt, cnt, key, cell));
-    return launch(h, inp_finish_kernel, g, 256, 0, s, (const uint8_t*)img, rows, cols, d_mm, d_out);
+    return finish((const uint8_t*)img);
   };
   rc = run();
   const cudaError_t fe = cudaFreeAsync(base, s);
+  if (rc == ARTP_OK && fe != cudaSuccess) CU_TRY(h, fe);
+  return rc;
+}
+
+}  // namespace
+
+// The march on a layer whose finite min / max keys (finite_min_max) are at d_mm, on the cols x rows image.
+int artp_api::inpaint_layer(Handle* h, const float* d_in, int rows, int cols, const uint32_t* d_mm, float* d_out,
+                            cudaStream_t s) {
+  const size_t n = (size_t)rows * cols;
+  const unsigned g = grid_for(h, n, 256, 8);
+  return march(h, cols, rows, s,
+               [&](uint8_t* img, uint8_t* flag) { return launch(h, inp_prep_kernel, g, 256, 0, s, d_in, n, d_mm, img, flag); },
+               [&](const uint8_t* img) { return launch(h, inp_finish_kernel, g, 256, 0, s, img, rows, cols, d_mm, d_out); });
+}
+
+int artp_api::cost_map_scan(Handle* h, const float* d_in, size_t n, uint32_t* d_w, cudaStream_t s) {
+  TRY(finite_min_max(h, d_in, n, d_w, s));
+  return nonfinite_any(h, d_in, n, d_w + 3, s);
+}
+
+int artp_api::cost_map_verdict(Handle* h, const uint32_t* w) {
+  if (w[4]) { h->err = "cost map: the layer has a +-inf cell"; return ARTP_E_INVALID; }
+  if (!w[2]) { h->err = "cost map: the layer has no finite cell"; return ARTP_E_INVALID; }
+  if (!w[3]) return ARTP_OK;   // no hole: the layer itself
+  const float mn = key_float(w[0]), d = key_float(w[1]) - mn;
+  if (!std::isfinite(d * 255.0f)) { h->err = "cost map: the finite range times 255 overflows float"; return ARTP_E_INVALID; }
+  return ARTP_OK;
+}
+
+int artp_api::cost_map_layer(Handle* h, const float* d_in, int rows, int cols, const uint32_t* d_w, bool holes,
+                             bool reverse_cols, float* d_out, cudaStream_t s) {
+  const size_t n = (size_t)rows * cols;
+  const unsigned g = grid_for(h, n, 256, 8);
+  if (!holes) return launch(h, cm_finish_kernel, g, 256, 0, s, (const uint8_t*)nullptr, d_in, rows, cols, d_w, reverse_cols, d_out);
+  return march(h, rows, cols, s,
+               [&](uint8_t* img, uint8_t* flag) { return launch(h, cm_prep_kernel, g, 256, 0, s, d_in, rows, cols, d_w, img, flag); },
+               [&](const uint8_t* img) {
+                 return launch(h, cm_finish_kernel, g, 256, 0, s, img, d_in, rows, cols, d_w, reverse_cols, d_out);
+               });
+}
+
+int artp_api::cost_map_features(Handle* h, const float* d_in, int rows, int cols, const uint32_t* d_w, bool holes,
+                                double res, double cx, double cy, cudaStream_t s) {
+  float* d_map = nullptr;
+  CU_TRY(h, cudaMallocAsync(reinterpret_cast<void**>(&d_map), (size_t)rows * cols * sizeof(float), s));
+  int rc = cost_map_layer(h, d_in, rows, cols, d_w, holes, true, d_map, s);
+  if (rc == ARTP_OK)
+    rc = artp_cnn::update_features(h->cnn, d_map, rows, cols, rows, res, cx, cy, s, h->cnn_mode & 1, h->err);
+  const cudaError_t fe = cudaFreeAsync(d_map, s);
   if (rc == ARTP_OK && fe != cudaSuccess) CU_TRY(h, fe);
   return rc;
 }
@@ -107,6 +166,80 @@ int artp_inpaint_layer_device(artp_handle* hh, const float* d_layer, int rows, i
   if (rc == ARTP_OK && !mm[2]) { h->err = "inpaint: the layer has no finite cell"; rc = ARTP_E_INVALID; }
   if (rc == ARTP_OK) rc = inpaint_layer(h, d_layer, rows, cols, d_mm, d_out, s);
   cudaFreeAsync(d_mm, s);
+  return rc;
+}
+
+int artp_cost_map_layer(artp_handle* hh, const float* raw, int rows, int cols, float* out) {
+  LOCK_CALL(h, hh);
+  TRY(inpaint_args(h, raw, rows, cols, out, "cost map"));
+  const size_t n = (size_t)rows * cols, lb = n * sizeof(float);
+  char* r[3];
+  TRY(host_call_begin(h, {lb, lb, 64}, r));
+  cudaStream_t s = h->stream;
+  float *d_in = (float*)r[0], *d_out = (float*)r[1];
+  uint32_t* d_w = (uint32_t*)r[2];
+  TRY(copy_async(h, d_in, raw, lb, cudaMemcpyHostToDevice, s));
+  TRY(cost_map_scan(h, d_in, n, d_w, s));
+  uint32_t w[kCostMapWords];
+  TRY(copy_async(h, w, d_w, sizeof(w), cudaMemcpyDeviceToHost, s));
+  TRY(sync_stream(h, s));
+  if (const int rc = cost_map_verdict(h, w)) { host_call_end(h); return rc; }
+  TRY(cost_map_layer(h, d_in, rows, cols, d_w, w[3] != 0, false, d_out, s));
+  TRY(copy_async(h, out, d_out, lb, cudaMemcpyDeviceToHost, s));
+  return host_call_end(h);
+}
+
+int artp_cost_map_layer_device(artp_handle* hh, const float* d_raw, int rows, int cols, float* d_out, void* stream) {
+  LOCK_CALL(h, hh);
+  TRY(inpaint_args(h, d_raw, rows, cols, d_out, "cost map"));
+  CU_TRY(h, cudaSetDevice(h->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  uint32_t* d_w = nullptr;
+  CU_TRY(h, cudaMallocAsync(reinterpret_cast<void**>(&d_w), 64, s));
+  int rc = cost_map_scan(h, d_raw, (size_t)rows * cols, d_w, s);
+  uint32_t w[kCostMapWords] = {};
+  if (rc == ARTP_OK) rc = copy_async(h, w, d_w, sizeof(w), cudaMemcpyDeviceToHost, s);
+  if (rc == ARTP_OK) rc = sync_stream(h, s);
+  if (rc == ARTP_OK) rc = cost_map_verdict(h, w);
+  if (rc == ARTP_OK) rc = cost_map_layer(h, d_raw, rows, cols, d_w, w[3] != 0, false, d_out, s);
+  cudaFreeAsync(d_w, s);
+  return rc;
+}
+
+int artp_update_features_raw(artp_handle* hh, const float* raw, int rows, int cols, double res, double cx, double cy) {
+  LOCK_CALL(h, hh);
+  TRY(features_raw_args(h, raw, rows, cols, res, cx, cy));
+  const size_t n = (size_t)rows * cols, lb = n * sizeof(float);
+  char* r[2];
+  TRY(host_call_begin(h, {lb, 64}, r));
+  cudaStream_t s = h->stream;
+  float* d_in = (float*)r[0];
+  uint32_t* d_w = (uint32_t*)r[1];
+  TRY(copy_async(h, d_in, raw, lb, cudaMemcpyHostToDevice, s));
+  TRY(cost_map_scan(h, d_in, n, d_w, s));
+  uint32_t w[kCostMapWords];
+  TRY(copy_async(h, w, d_w, sizeof(w), cudaMemcpyDeviceToHost, s));
+  TRY(sync_stream(h, s));
+  if (const int rc = cost_map_verdict(h, w)) { host_call_end(h); return rc; }
+  TRY(cost_map_features(h, d_in, rows, cols, d_w, w[3] != 0, res, cx, cy, s));
+  return host_call_end(h);
+}
+
+int artp_update_features_raw_device(artp_handle* hh, const float* d_raw, int rows, int cols, double res, double cx,
+                                    double cy, void* stream) {
+  LOCK_CALL(h, hh);
+  TRY(features_raw_args(h, d_raw, rows, cols, res, cx, cy));
+  CU_TRY(h, cudaSetDevice(h->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  uint32_t* d_w = nullptr;
+  CU_TRY(h, cudaMallocAsync(reinterpret_cast<void**>(&d_w), 64, s));
+  int rc = cost_map_scan(h, d_raw, (size_t)rows * cols, d_w, s);
+  uint32_t w[kCostMapWords] = {};
+  if (rc == ARTP_OK) rc = copy_async(h, w, d_w, sizeof(w), cudaMemcpyDeviceToHost, s);
+  if (rc == ARTP_OK) rc = sync_stream(h, s);
+  if (rc == ARTP_OK) rc = cost_map_verdict(h, w);
+  if (rc == ARTP_OK) rc = cost_map_features(h, d_raw, rows, cols, d_w, w[3] != 0, res, cx, cy, s);
+  cudaFreeAsync(d_w, s);
   return rc;
 }
 

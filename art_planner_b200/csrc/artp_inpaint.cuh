@@ -20,10 +20,27 @@
 //   inp_march_kernel     one warp per component: outer FMM, negation, TELEA march
 //   inp_finish_kernel    back to float (two float operations), column / row 0 copies
 //
+// The cost server's preparation of the same raw layer (cost_query_server.py, _elvMapProcess) reuses the stages from
+// region to march on an image of its own, with its own prep and finish (cm_prep_kernel, cm_finish_kernel). Stated once,
+// all float32 round-to-nearest with no contraction (oracle/cost_map_oracle.py restates it):
+//   1. E = layer[::-1, ::-1], rows x cols: E[r][c] = layer(rows-1-r, cols-1-c), the image the trunk reads.
+//   2. No cell NaN or +-inf: the result is E itself.
+//   3. Otherwise mn / mx = min / max over the finite cells, d = mx - mn, and on the finite cells
+//      q = trunc(((E - mn) * 255) / d) (so the max cell can land at 254; 0 / 0 when mx == mn gives byte 0, so that map
+//      comes back as mn everywhere); the mask is ~isfinite(E), and a masked cell holds 0. Both zeros are numpy's
+//      astype(uint8) of NaN on x86-64. The march reads a masked cell before filling it only through the image gradient's
+//      clamped reads at the border, so its byte matters only for components within two cells of the border.
+//   4. TELEA with radius 3 on q in E's orientation (image row r, column c: raster index r * cols + c).
+//   5. out = ((float)u * d) / 255 + mn on every cell, known cells too; no row / column 0 copies.
+// The C ABI refuses (ARTP_E_INVALID, before any work) a +-inf cell and a layer without a finite cell, where the server's
+// output is NaN, and a range whose d * 255 overflows, where it casts infinite quotients to 8 bits (undefined in numpy).
+//
 // The heap of a component is a binary min-heap on the 64-bit key (order-preserving T bits << 32 | push sequence) in global
 // memory; the initial band's sequence is its raster index (Heap->Add pushes it in raster order, all at T = 0), later
 // pushes count from N. All arithmetic uses explicit round-to-nearest intrinsics, so no contraction can change a bit.
 #pragma once
+#include <math_constants.h>
+
 #include <cstdint>
 
 namespace artp_inpaint {
@@ -426,6 +443,38 @@ __global__ void inp_finish_kernel(const uint8_t* __restrict__ img, int rows, int
     const int i = (int)(c % rows), j = (int)(c / rows);
     const size_t src = (size_t)max(j, 1) * rows + max(i, 1);
     out[c] = __fadd_rn(__fmul_rn((float)img[src], s.scale), s.mn);
+  }
+}
+
+// ---- the cost server's preparation (steps 1-5 above) --------------------------------------------------------------------
+
+// Steps 1 and 3: E's orientation, the truncating 8-bit conversion of the finite cells and the ~isfinite mask.
+__global__ void cm_prep_kernel(const float* __restrict__ layer, int rows, int cols, const uint32_t* __restrict__ mm,
+                               uint8_t* __restrict__ img, uint8_t* __restrict__ flag) {
+  const float mn = key_to_float(mm[0]), d = __fsub_rn(key_to_float(mm[1]), mn);
+  const size_t n = (size_t)rows * cols;
+  for (size_t c = blockIdx.x * (size_t)blockDim.x + threadIdx.x; c < n; c += (size_t)gridDim.x * blockDim.x) {
+    const int r = (int)(c / cols), x = (int)(c % cols);
+    const float v = layer[(size_t)(rows - 1 - r) + (size_t)(cols - 1 - x) * rows];
+    const bool known = fabsf(v) < CUDART_INF_F;
+    const float q = __fdiv_rn(__fmul_rn(__fsub_rn(v, mn), 255.0f), d);   // NaN when d = 0: byte 0
+    img[c] = known && q >= 0.0f ? (uint8_t)__float2int_rz(q) : 0;
+    flag[c] = known ? 0 : F_MASK;
+  }
+}
+
+// Step 5 (img: the marched image) or step 2 (img null: the layer itself), written as the layer P with
+// E'[r][c] = P(rows-1-r, cols-1-c): out[i + j * rows] = P(i, j), or with reverse_cols out[i + (cols-1-j) * rows], the
+// heightfield layout whose E[r][c] the trunk's SRC_MAP read takes from out[c * rows + rows-1-r] (pitch = rows).
+__global__ void cm_finish_kernel(const uint8_t* __restrict__ img, const float* __restrict__ layer, int rows, int cols,
+                                 const uint32_t* __restrict__ mm, bool reverse_cols, float* __restrict__ out) {
+  const float mn = key_to_float(mm[0]), d = __fsub_rn(key_to_float(mm[1]), mn);
+  const size_t n = (size_t)rows * cols;
+  for (size_t c = blockIdx.x * (size_t)blockDim.x + threadIdx.x; c < n; c += (size_t)gridDim.x * blockDim.x) {
+    const int i = (int)(c % rows), j = (int)(c / rows);
+    const float v = img ? __fadd_rn(__fdiv_rn(__fmul_rn((float)img[(size_t)(rows - 1 - i) * cols + (cols - 1 - j)], d), 255.0f), mn)
+                        : layer[c];
+    out[(size_t)(reverse_cols ? cols - 1 - j : j) * rows + i] = v;
   }
 }
 

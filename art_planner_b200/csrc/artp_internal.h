@@ -321,9 +321,24 @@ int simplify_path(Handle* h, const double* path, const double* d_path, size_t n,
 // order-preserving keys of float_key.
 int finite_min_max(Handle* h, const float* d_layer, size_t n, uint32_t* d_out, cudaStream_t s);
 float key_float(uint32_t key);
+// Whether any of n floats is NaN or +-inf (d_out[0]) and whether any is +-inf (d_out[1]), 0 or 1, on s.
+int nonfinite_any(Handle* h, const float* d_layer, size_t n, uint32_t* d_out, cudaStream_t s);
 // inpaintMatrix (artp_inpaint.cuh) of the rows x cols column-major layer d_in into d_out on s; d_mm holds the layer's
 // finite_min_max words (at least one finite cell). Scratch is stream-ordered (cudaMallocAsync).
 int inpaint_layer(Handle* h, const float* d_in, int rows, int cols, const uint32_t* d_mm, float* d_out, cudaStream_t s);
+// artp_inpaint.cu: the cost server's map preparation (artp_inpaint.cuh). The words of a layer are
+// {finite_min_max's three, nonfinite_any's two}: cost_map_scan enqueues them into d_w on s, and cost_map_verdict, on
+// their host copy, refuses the layers the server cannot prepare (ARTP_E_INVALID, artp.h). cost_map_layer then prepares the
+// rows x cols column-major layer d_in into d_out (its grid_map layout, or with reverse_cols the trunk's heightfield layout
+// at pitch rows); cost_map_features prepares it and runs the trunk on it (update_features's geometry and codes).
+// Scratch is stream-ordered.
+constexpr int kCostMapWords = 5;
+int cost_map_scan(Handle* h, const float* d_in, size_t n, uint32_t* d_w, cudaStream_t s);
+int cost_map_verdict(Handle* h, const uint32_t* w);
+int cost_map_layer(Handle* h, const float* d_in, int rows, int cols, const uint32_t* d_w, bool holes, bool reverse_cols,
+                   float* d_out, cudaStream_t s);
+int cost_map_features(Handle* h, const float* d_in, int rows, int cols, const uint32_t* d_w, bool holes, double res,
+                      double cx, double cy, cudaStream_t s);
 // Planner::plan's checks of the endpoints of a device solve (start then goal, 14 doubles at d_sg) into d_out[5]: 0, -1
 // (a non-finite state), ARTP_SOLVE_INVALID_START or ARTP_SOLVE_INVALID_GOAL (outside space's bounds), then both (x, y).
 int endpoint_check(Handle* h, const double* d_sg, const artp_se3_space* space, double* d_out, cudaStream_t s);

@@ -55,6 +55,22 @@ __global__ void finite_min_max_kernel(const float* __restrict__ a, size_t n, uin
   if ((threadIdx.x & 31) == 0 && cnt) { atomicMin(out, lo); atomicMax(out + 1, hi); atomicAdd(out + 2, cnt); }
 }
 
+// out[0] = 1 when a cell is NaN or +-inf, out[1] = 1 when a cell is +-inf (both zeroed first).
+__global__ void nonfinite_any_kernel(const float* __restrict__ a, size_t n, uint32_t* __restrict__ out) {
+  uint32_t nonfinite = 0u, inf = 0u;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float v = fabsf(a[i]);
+    nonfinite |= !(v < CUDART_INF_F);
+    inf |= v == CUDART_INF_F;
+  }
+  nonfinite = __reduce_or_sync(0xFFFFFFFFu, nonfinite);
+  inf = __reduce_or_sync(0xFFFFFFFFu, inf);
+  if ((threadIdx.x & 31) == 0) {
+    if (nonfinite) atomicOr(out, 1u);
+    if (inf) atomicOr(out + 1, 1u);
+  }
+}
+
 // addKnownCells (basic.cpp:25-38): observed = 1 where every basic layer ({elevation, traversability}, map.cpp:16) is finite
 // (grid_map's isValid). A missing traversability layer is checkTraversability's 1.0 (basic.cpp:13-21), written to trav_fill.
 __global__ void observed_kernel(const float* __restrict__ elevation, const float* __restrict__ traversability, size_t n,
@@ -186,6 +202,7 @@ int plan_args(Handle* h, const artp_planner_params* pp) {
   if (pp->use_max_prob_unknown_samples && !(pp->max_prob_unknown_samples >= 0.0 && pp->max_prob_unknown_samples <= 1.0)) {
     h->err = "max_prob_unknown_samples must lie in [0, 1]"; return ARTP_E_INVALID;
   }
+  if (pp->cost_map_from_raw != 0 && pp->cost_map_from_raw != 1) { h->err = "cost_map_from_raw must be 0 or 1"; return ARTP_E_INVALID; }
   return ARTP_OK;
 }
 
@@ -200,6 +217,11 @@ int artp_api::finite_min_max(Handle* h, const float* d_layer, size_t n, uint32_t
   CU_TRY(h, cudaMemsetAsync(d_out, 0xFF, sizeof(uint32_t), s));
   CU_TRY(h, cudaMemsetAsync(d_out + 1, 0, 2 * sizeof(uint32_t), s));
   return launch(h, finite_min_max_kernel, grid_for(h, n, 256, 8), 256, 0, s, d_layer, n, d_out);
+}
+
+int artp_api::nonfinite_any(Handle* h, const float* d_layer, size_t n, uint32_t* d_out, cudaStream_t s) {
+  CU_TRY(h, cudaMemsetAsync(d_out, 0, 2 * sizeof(uint32_t), s));
+  return launch(h, nonfinite_any_kernel, grid_for(h, n, 256, 8), 256, 0, s, d_layer, n, d_out);
 }
 
 float artp_api::key_float(uint32_t key) {
@@ -295,11 +317,15 @@ int set_map(Handle* h, const artp_planner_params* pp, const float* elevation, co
   TRY(finite_min_max(h, raw_e, n, d_mm, s));
   const bool raw_t_inpaint = raw && traversability;
   if (raw_t_inpaint) TRY(finite_min_max(h, raw_t, n, d_mm + 4, s));   // inpaintMatrix's range of the traversability
-  uint32_t mm[8];
-  TRY(copy_async(h, mm, d_mm, (raw_t_inpaint ? 8 : 3) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  const bool cost_map = pp->cost_map_from_raw != 0;
+  if (cost_map) TRY(cost_map_scan(h, raw_e, n, d_mm + 8, s));        // the cost server's preparation of the elevation
+  uint32_t mm[8 + kCostMapWords];
+  TRY(copy_async(h, mm, d_mm, (cost_map ? 8 + kCostMapWords : raw_t_inpaint ? 8 : 3) * sizeof(uint32_t),
+                 cudaMemcpyDeviceToHost, s));
   TRY(host_call_end(h));
   if (!mm[2]) { h->err = "the elevation layer has no finite cell"; return ARTP_E_INVALID; }
   if (raw_t_inpaint && !mm[6]) { h->err = "the traversability layer has no finite cell"; return ARTP_E_INVALID; }
+  if (cost_map) TRY(cost_map_verdict(h, mm + 8));
   artp_se3_space sp{};
   const double Lx = rows * res, Ly = cols * res;   // grid_map getLength: the FULL length, not half of it
   sp.low[0] = cx - Lx; sp.high[0] = cx + Lx;
@@ -331,12 +357,16 @@ int set_map(Handle* h, const artp_planner_params* pp, const float* elevation, co
   }
   arm_sampler(h, &smp);
   TRY(host_call_end(h));
-  // CostPredictor.updateFeatures, when a network is loaded
+  // CostPredictor.updateFeatures, when a network is loaded: on the uploaded elevation, or with cost_map_from_raw on the
+  // cost server's preparation of the raw one
   if (h->cnn && artp_cnn::network(h->cnn) >= 0) {
     CU_TRY(h, cudaSetDevice(h->device));
-    if (const int rc = artp_cnn::update_features(h->cnn, h->d_H[0], h->rows, h->cols, h->pitch, h->res, h->chk.cx, h->chk.cy,
-                                                 h->stream, h->cnn_mode & 1, h->err))
+    if (cost_map) {
+      TRY(cost_map_features(h, raw_e, rows, cols, d_mm + 8, mm[8 + 3] != 0, h->res, h->chk.cx, h->chk.cy, h->stream));
+    } else if (const int rc = artp_cnn::update_features(h->cnn, h->d_H[0], h->rows, h->cols, h->pitch, h->res, h->chk.cx,
+                                                        h->chk.cy, h->stream, h->cnn_mode & 1, h->err)) {
       return rc;
+    }
   }
   st->space = sp;
   st->generation += 1;

@@ -550,6 +550,31 @@ int artp_debug_se3_ops(artp_handle* h, const double* a, const double* b, const d
 int artp_inpaint_layer(artp_handle* h, const float* layer, int rows, int cols, float* out);
 int artp_inpaint_layer_device(artp_handle* h, const float* d_layer, int rows, int cols, float* d_out, void* stream);
 
+/* ---- the cost server's map preparation (cost_query_server.py, _elvMapProcess) -------------------------------------
+ * What the learned cost's trunk is fed by the reference: the server prepares the RAW elevation itself, not
+ * processors::Basic's output. All float32, round to nearest, no contraction (DESIGN.md section 4.7):
+ *   1. E = layer[::-1, ::-1], rows x cols: E[r][c] = layer(rows-1-r, cols-1-c) (the trunk's input orientation).
+ *   2. no cell NaN or +-inf: E itself (not quantised).
+ *   3. otherwise mn / mx = min / max of the finite cells, d = mx - mn, q = trunc(((E - mn) * 255) / d) on the finite
+ *      cells (the max cell may land at 254; mx == mn gives 0 / 0 -> byte 0, so the map is mn everywhere),
+ *      mask = ~isfinite(E), masked cells 0 (both zeros are numpy's NaN -> uint8 on x86-64);
+ *   4. cv::inpaint(q, mask, 3, INPAINT_TELEA) in E's orientation (artp_inpaint_layer's march);
+ *   5. ((float)u * d) / 255 + mn on every cell, known cells too; no row / column 0 copies.
+ * Refused with ARTP_E_INVALID before any work: a +-inf cell and a layer without a finite cell (the server's result is
+ * NaN), and a range whose d * 255 overflows float (the server casts infinite quotients to 8 bits, undefined in numpy). rows, cols >= 2 and rows * cols < 2^31.
+ * artp_cost_map_layer returns the prepared map P in grid_map layout (E'[r][c] = P(rows-1-r, cols-1-c)), so
+ * artp_set_map(P as elevation) + artp_update_features feeds the trunk what the server fed it. _device: device buffers on
+ * `stream` (may be NULL); one host sync reads the layer's range and flags, the rest is asynchronous. */
+int artp_cost_map_layer(artp_handle* h, const float* raw, int rows, int cols, float* out);
+int artp_cost_map_layer_device(artp_handle* h, const float* d_raw, int rows, int cols, float* d_out, void* stream);
+/* The preparation above, then CostPredictor.updateFeatures on it: the trunk's features and the head's geometry (res,
+ * cx, cy, rows * res x cols * res) as artp_update_features sets them from a map, but no installed map is needed or
+ * changed. Without weights: ARTP_E_NOWEIGHTS. A refused call (any code before the trunk runs, the preparation's refusals
+ * included) keeps the previous features. _device: d_raw on `stream`; the call returns when the features are made. */
+int artp_update_features_raw(artp_handle* h, const float* raw, int rows, int cols, double res, double cx, double cy);
+int artp_update_features_raw_device(artp_handle* h, const float* d_raw, int rows, int cols, double res, double cx,
+                                    double cy, void* stream);
+
 /* ---- the planner: Planner::setMap and Planner::plan + getSolutionPath for prm_motion_cost (planner.cpp:135-298) ----
  * The shipped replan (PlannerRos::updateMapAndPlanFromCurrentRobotPose, planner.name prm_motion_cost,
  * simplify_solution true) as two calls whose stages hand data to each other in device memory: no layer, state or path
@@ -571,7 +596,9 @@ int artp_inpaint_layer_device(artp_handle* h, const float* d_layer, int rows, in
  *                      inpainted elevation and elevation_masked straight from device memory (artp_set_map's rules).
  *   the chain          artp_estimate_normals ((torso.length + torso.width) * 0.25); with sample_from_distribution the
  *                      sample filter, the distribution without vertices and its CDF; the sampler armed with the bounds' x / y;
- *                      artp_update_features when weights are loaded.
+ *                      artp_update_features when weights are loaded; with cost_map_from_raw = 1 the trunk instead runs on
+ *                      the cost server's preparation of the uploaded RAW elevation (artp_update_features_raw's features,
+ *                      whose refusals are then checked with the others, before the installed map changes).
  *   generation         a map counter, +1 per installed map: it stands in for the grid_map timestamp that
  *                      PRMMotionCostMaintainer::sampleGraph compares (prm_motion_cost.cpp:146-153).
  * Layers are HOST pointers in grid_map layout (artp_set_map). Every check runs before the installed map changes, and a
@@ -625,6 +652,8 @@ typedef struct artp_planner_params {
   artp_basic_params basic;                            /* params.h:23-35 */
   int      simplify, clear_roadmap;                   /* simplify_solution; the ROS node's ss_->clear() */
   uint64_t seed;
+  int      cost_map_from_raw;                         /* 0: features from the uploaded elevation; 1: from the raw one as
+                                                         the cost server prepares it (artp_update_features_raw) */
 } artp_planner_params;
 typedef struct artp_plan_info {
   int32_t  status;                      /* ARTP_PLANNER_* */

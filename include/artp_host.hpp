@@ -528,6 +528,15 @@ inline std::vector<float> inpaintMatrix(const Handle& handle, const std::vector<
   return out;
 }
 
+// The cost server's preparation of the RAW rows x cols column-major elevation layer (cost_query_server.py _elvMapProcess,
+// artp_cost_map_layer): the layer whose network input is what the server feeds the trunk (DESIGN.md section 4.7).
+inline std::vector<float> costServerMap(const Handle& handle, const std::vector<float>& layer, int rows, int cols) {
+  if (layer.size() != (size_t)rows * (size_t)cols) throw std::runtime_error("costServerMap: layer size is not rows * cols");
+  std::vector<float> out(layer.size());
+  handle.check(artp_cost_map_layer(handle.get(), layer.data(), rows, cols, out.data()), "artp_cost_map_layer");
+  return out;
+}
+
 // art_planner::Planner for planner.name prm_motion_cost (planner.cpp:135-298) on the device: setMap is
 // artp_planner_set_map, plan is artp_plan (the simplification of getSolutionPath(true) runs inside it when
 // parameters().simplify is set), and the stages hand data to each other in device memory. The parameters start from
@@ -551,6 +560,7 @@ class Planner {
     pp_.max_prob_unknown_samples = p.sampler.max_prob_unknown_samples;
     pp_.basic = artp_basic_params{0.15f, p.planner.unknown_space_untraversable ? 1 : 0, 0.3, 0.3, 0.3, 0.16, 0.3, 0.1};
     pp_.simplify = 1; pp_.clear_roadmap = 0; pp_.seed = 0;
+    pp_.cost_map_from_raw = 0;   // 1: the trunk reads the cost server's preparation of the raw elevation
   }
   artp_planner_params& parameters() { return pp_; }
 
@@ -761,6 +771,16 @@ class MotionCostObjective {
     checker_->handle()->check(artp_set_cost_weights(checker_->handle()->get(), blob.data(), blob.size()), "artp_set_cost_weights");
   }
   void updateFeatures() { checker_->handle()->check(artp_update_features(checker_->handle()->get()), "artp_update_features"); }
+  // CostPredictor.updateFeatures on the map the cost server prepares from the RAW elevation (artp_update_features_raw):
+  // the rows x cols column-major layer, the map's resolution and position; no installed map needed.
+  void updateFeaturesRaw(const std::vector<float>& elevation, int rows, int cols, double resolution, double position_x,
+                         double position_y) {
+    if (elevation.size() != (size_t)rows * (size_t)cols)
+      throw std::runtime_error("updateFeaturesRaw: layer size is not rows * cols");
+    checker_->handle()->check(artp_update_features_raw(checker_->handle()->get(), elevation.data(), rows, cols, resolution,
+                                                       position_x, position_y),
+                              "artp_update_features_raw");
+  }
 
   double getCost(const float* e3) const {                                        // motion_cost_objective.h:54-61
     const auto& w = checker_->handle()->params().planner.prm_motion_cost.cost_weights;
