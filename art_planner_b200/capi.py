@@ -166,6 +166,8 @@ def load():
     lib.artp_find_valid_near_device.argtypes = [vp, vp, sz, vp, u32, vp, u64, u64, vp, vp, vp]
     lib.artp_ball_offsets.argtypes = [vp, u64, u64, sz, u32, vp, vp]
     lib.artp_pose_from_2d.argtypes = [vp, vp, sz, vp, vp]
+    lib.artp_valid_heading_layer.argtypes = [vp, vp, i32, vp]
+    lib.artp_valid_heading_layer_device.argtypes = [vp, vp, i32, vp, vp]
     lib.artp_path_length_cost.argtypes = [vp, vp, vp, sz, vp]
     lib.artp_path_length_cost_device.argtypes = [vp, vp, vp, sz, vp, vp]
     lib.artp_compact_valid_device.argtypes = [vp, vp, sz, C.c_int64, vp, vp, vp]

@@ -79,6 +79,7 @@ class StateValidityChecker:
     def __init__(self, params, device: int = 0, handle: _Handle | None = None):
         self._h = handle or _Handle(params, device)
         self._map = None
+        self._installed = None      # (rows, cols) of the map the handle holds, for host outputs over whole-map layers
 
     # -- reference interface ------------------------------------------------------------------
     def setMap(self, synth_map) -> None:             # validity_checker.cpp:20-23
@@ -96,6 +97,7 @@ class StateValidityChecker:
             k = np.asfortranarray(m.elevation_masked[row0:row0 + nrows, :], dtype=np.float32)
             self._h.check(self._h.lib.artp_set_map_window(self._h.h, e.ctypes.data, k.ctypes.data, m.elevation.shape[0],
                                                           m.elevation.shape[1], float(m.res), float(m.cx), float(m.cy), row0, nrows))
+            self._installed = m.elevation.shape
             return
         e = np.asfortranarray(m.elevation, dtype=np.float32)
         k = np.asfortranarray(m.elevation_masked, dtype=np.float32)
@@ -103,6 +105,7 @@ class StateValidityChecker:
             raise capi.ArtpError(capi.ARTP_E_INVALID, "layer shapes differ")
         self._h.check(self._h.lib.artp_set_map(self._h.h, e.ctypes.data, k.ctypes.data, e.shape[0], e.shape[1],
                                                float(m.res), float(m.cx), float(m.cy)))
+        self._installed = e.shape
 
     def hasMap(self) -> bool:                        # validity_checker.cpp:33-35
         return bool(self._h.lib.artp_has_map(self._h.h))
@@ -290,6 +293,26 @@ class StateValidityChecker:
         inside = np.empty(s.shape[0], np.uint8)
         self._h.check(self._h.lib.artp_pose_from_2d(self._h.h, s.ctypes.data, s.shape[0], out.ctypes.data, inside.ctypes.data))
         return out, inside
+
+    def validHeadingLayer(self, yaws, out=None):
+        """The valid-heading layer of the installed map (artp_valid_heading_layer): a uint32 [rows, cols] column-major
+        array whose bit k is set where a goal at the cell's centre with yaw yaws[k] (1 to 32 finite yaws) passes isValid
+        once projected onto the map (poseFrom2D). Needs the map's normals, as poseFrom2D does. With `out` a CUDA tensor
+        (int32 or uint32, column-major as inpaint's: a transposed contiguous cols x rows tensor) the layer is written
+        there on the current stream (artp_valid_heading_layer_device) and `out` is returned."""
+        y = np.ascontiguousarray(yaws, dtype=np.float64).reshape(-1)
+        if out is not None and _is_torch_cuda(out):
+            import torch
+            if out.dtype not in (torch.int32, torch.uint32) or out.dim() != 2 or not out.t().is_contiguous():
+                raise ValueError("validHeadingLayer: out must be a column-major int32 or uint32 CUDA tensor")
+            self._h.check(self._h.lib.artp_valid_heading_layer_device(self._h.h, y.ctypes.data, y.shape[0], out.data_ptr(),
+                                                                      _stream_ptr()))
+            return out
+        if self._installed is None:
+            raise capi.ArtpError(capi.ARTP_E_NOMAP, "no map installed")
+        mask = np.empty(self._installed, np.uint32, order="F")
+        self._h.check(self._h.lib.artp_valid_heading_layer(self._h.h, y.ctypes.data, y.shape[0], mask.ctypes.data))
+        return mask
 
     def isValidBatchBits(self, states, out_valid, out_bits):
         """One shard step of the multi-GPU path: verdict bytes + bit-packed mask (CUDA float64 states), one call."""
@@ -694,6 +717,7 @@ class Planner:
         mi = capi.ArtpPlannerMapInfo()
         h.check(h.lib.artp_planner_set_map(h.h, C.byref(self.parameters), *[None if a is None else a.ctypes.data for a in (e, t, ei, ti)],
                                            e.shape[0], e.shape[1], float(res), float(cx), float(cy), C.byref(mi)))
+        self._c._installed = e.shape
         return {k: int(getattr(mi, k)) for k, _ in capi.ArtpPlannerMapInfo._fields_}
 
     def setMapRaw(self, elevation, traversability, res: float, cx: float, cy: float) -> dict:
@@ -705,6 +729,7 @@ class Planner:
         mi = capi.ArtpPlannerMapInfo()
         h.check(h.lib.artp_planner_set_map_raw(h.h, C.byref(self.parameters), e.ctypes.data, None if t is None else t.ctypes.data,
                                                e.shape[0], e.shape[1], float(res), float(cx), float(cy), C.byref(mi)))
+        self._c._installed = e.shape
         return {k: int(getattr(mi, k)) for k, _ in capi.ArtpPlannerMapInfo._fields_}
 
     def space(self):

@@ -1,7 +1,8 @@
 // art_planner_b200/csrc/artp_internal.h -- what the three units of the C ABI share (not installed):
 //   artp_capi.cu      handle lifecycle, errors, stats and timing, map upload, the validity pipeline, pose / motion / edge
 //                     checks, compaction and bit packing
-//   artp_sampling.cu  normals and the CDF, the sampler, start / goal search, poseFrom2D, Basic, the sample distribution
+//   artp_sampling.cu  normals and the CDF, the sampler, start / goal search, poseFrom2D, the valid-heading layer, Basic,
+//                     the sample distribution
 //   artp_cost.cu      path length, the edge matrix, the learned motion cost, cost weights and features
 //   artp_planner.cu   artp_planner_set_map / artp_plan: the replan, over the lock-free bodies declared at the end
 // the handle and its lock, launch and call bookkeeping, scratch regions, argument checks, and the few functions one unit

@@ -139,14 +139,15 @@ __device__ __forceinline__ bool sample_state(const SamplerDev& m, const double u
 // Map::get3DPoseFrom2D as Planner::plan applies it to the goal (planner.cpp:223-237, map.cpp:77-90): for a state whose
 // (x, y) lies on the map, z = the cell's elevation, roll / pitch from the cell's normal seen in the state's yaw frame,
 // yaw = getYawFromSO3 (utils.h:80-88: double atan2 returned as float); x and y stay. Other states pass unchanged.
-__device__ __forceinline__ bool pose_from_2d(const SamplerDev& m, const double in[7], double out[7]) {
+// With yaw_f, *yaw_f stands for getYawFromSO3 of the state (the valid-heading layer's headings).
+__device__ __forceinline__ bool pose_from_2d(const SamplerDev& m, const double in[7], double out[7], const float* yaw_f = nullptr) {
 #pragma unroll
   for (int k = 0; k < 7; ++k) out[k] = in[k];
   int row, col;
   if (!map_cell(m, in[0], in[1], row, col)) return false;
   const size_t at = (size_t)row + (size_t)col * m.rows;
   const double nw[3] = {(double)__ldg(m.normal_x + at), (double)__ldg(m.normal_y + at), (double)__ldg(m.normal_z + at)};
-  const double yaw = (double)so3_yaw(in);
+  const double yaw = (double)(yaw_f ? *yaw_f : so3_yaw(in));
   double nb[3];
   normal_in_yaw_frame(yaw, nw, nb);
   out[2] = cell_height(m, row, col);
@@ -164,6 +165,46 @@ __global__ void pose_from_2d_kernel(SamplerDev m, const double* __restrict__ in,
 #pragma unroll
     for (int k = 0; k < 7; ++k) out[i * 7 + k] = o[k];
     if (inside) inside[i] = ok ? 1 : 0;
+  }
+}
+
+// ---- The valid-heading layer (artp_valid_heading_layer) ------------------------------------------------------------
+// Bit k of cell (row, col) is isValid of the goal projection of the cell's centre at heading k: the pose pose_from_2d
+// makes when getYawFromSO3 reads yaw[k]. Poses are numbered cell-major, heading-minor: pose i is heading i % n of cell
+// i / n, cells in the layers' column-major order.
+constexpr int kMaxHeadings = 32;
+struct Headings {
+  float yaw[kMaxHeadings];   // the caller's yaws cast to float, as getYawFromSO3 returns them
+  int n;
+};
+
+// Poses c0 * n .. c0 * n + count - 1 as float states (the cast Pose3FromSE3 applies first). The centre is
+// grid_map::getPositionFromIndex (as in sample_state), and map_cell maps every centre back to its own cell
+// (tests/test_heading_layer_cpu.py), so pose_from_2d always projects: the rest of the input state is never read.
+__global__ void heading_poses_kernel(SamplerDev m, Headings hd, size_t c0, size_t count, float* __restrict__ states_f32) {
+  const double Lx = m.rows * m.res, Ly = m.cols * m.res;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < count; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t cell = c0 + i / hd.n;
+    const int k = (int)(i % hd.n);
+    const int r = (int)(cell % m.rows), c = (int)(cell / m.rows);
+    const double in[7] = {(m.cx + (0.5 * Lx - 0.5 * m.res)) + m.res * (-(double)r),
+                          (m.cy + (0.5 * Ly - 0.5 * m.res)) + m.res * (-(double)c), 0.0, 0.0, 0.0, 0.0, 1.0};
+    const float yaw = hd.yaw[k];
+    double s[7];
+    pose_from_2d(m, in, s, &yaw);
+#pragma unroll
+    for (int j = 0; j < 7; ++j) states_f32[i * 7 + j] = (float)s[j];
+  }
+}
+
+// The masks of cells c0 .. c0 + cells - 1 from their poses' verdict bytes (pose c0 * n + i at valid[i]).
+__global__ void heading_pack_kernel(const uint8_t* __restrict__ valid, int n, size_t c0, size_t cells,
+                                    uint32_t* __restrict__ mask) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < cells; i += (size_t)gridDim.x * blockDim.x) {
+    const uint8_t* v = valid + i * n;
+    uint32_t bits = 0;
+    for (int k = 0; k < n; ++k) bits |= (v[k] ? 1u : 0u) << k;
+    mask[c0 + i] = bits;
   }
 }
 

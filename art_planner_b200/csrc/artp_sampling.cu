@@ -1,6 +1,6 @@
 // art_planner_b200/csrc/artp_sampling.cu -- the sampling half of the C ABI (include/artp.h): normals and the CDF, the
 // sampler (SE3FromSE2Sampler::sampleUniform) with its fused sample -> check -> compact path, the start / goal search,
-// poseFrom2D, Basic's masking and the sampler's distribution. It reaches the validity pipeline through check_states_f32
+// poseFrom2D and the valid-heading layer, Basic's masking and the sampler's distribution. It reaches the validity pipeline through check_states_f32
 // (artp_internal.h).
 #include <cmath>
 #include <cstdlib>
@@ -158,6 +158,47 @@ int find_valid_near(Handle* h, const double* d_centres, size_t n, const double* 
     TRY(launch(h, artp::ball_first_valid_kernel, grid_for(h, m, 256), 256, 0, s, d_val, c0, m, n_iter, d_best));
   }
   return launch(h, artp::ball_result_kernel, grid_for(h, n, 128), 128, 0, s, b, n, d_best, d_states_out, d_index);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// The valid-heading layer: isValid of the goal projection (planner.cpp:223-237) of every cell centre at each heading
+// ---------------------------------------------------------------------------------------------------------------
+// Argument checks shared by both forms, before any device work; the headings as the kernels take them into *hd.
+int heading_args(Handle* h, const double* yaw, int n_yaw, const uint32_t* mask, artp::Headings* hd) {
+  TRY(require_whole_map(h));
+  if (!sampling(h).map.has_normals) {
+    h->err = "no normal layers for this map (artp_estimate_normals or artp_set_sampler after artp_set_map)"; return ARTP_E_INVALID;
+  }
+  if (n_yaw < 1 || n_yaw > artp::kMaxHeadings) { h->err = "n_yaw must lie in 1..32"; return ARTP_E_INVALID; }
+  if (!yaw || !mask) return null_buffer(h);
+  std::memset(hd, 0, sizeof(*hd));
+  for (int k = 0; k < n_yaw; ++k) {
+    if (!std::isfinite(yaw[k])) { h->err = "yaw must be finite"; return ARTP_E_INVALID; }
+    hd->yaw[k] = (float)yaw[k];
+  }
+  hd->n = n_yaw;
+  return ARTP_OK;
+}
+
+// The layer of the current map into d_mask (rows x cols words) on s, in chunks of whole cells of at most kSampleChunk
+// poses each; arguments checked by heading_args.
+int valid_heading_layer(Handle* h, const artp::Headings& hd, uint32_t* d_mask, cudaStream_t s) {
+  const size_t ncell = (size_t)h->rows * h->cols;
+  const size_t chunk_cells = std::min(ncell, kSampleChunk / hd.n);
+  char* r[2];   // states f32 | verdicts
+  Buf<char>& scratch = sampling(h).samp_scratch;
+  TRY(carve(h, scratch.p, scratch.cap, {chunk_cells * hd.n * 7 * sizeof(float), chunk_cells * hd.n}, r));
+  float* d_sf = (float*)r[0];
+  uint8_t* d_val = (uint8_t*)r[1];
+  artp::SamplerDev m{};
+  sampler_map_view(h, m);
+  for (size_t c0 = 0; c0 < ncell; c0 += chunk_cells) {
+    const size_t cells = std::min(chunk_cells, ncell - c0), n = cells * hd.n;
+    TRY(launch(h, artp::heading_poses_kernel, grid_for(h, n, 128), 128, 0, s, m, hd, c0, n, d_sf));
+    TRY(check_states_f32(h, d_sf, n, d_val, s));
+    TRY(launch(h, artp::heading_pack_kernel, grid_for(h, cells, 256), 256, 0, s, d_val, hd.n, c0, cells, d_mask));
+  }
+  return ARTP_OK;
 }
 
 // cv::circle(kernel, (r, r), r, 255, FILLED) on a size x size zero image, r = size / 2 (utils.cpp:106-111): OpenCV's
@@ -719,6 +760,29 @@ int artp_pose_from_2d(artp_handle* hh, const double* states_in, size_t n, double
   CU_TRY(h, cudaMemcpyAsync(states_out, r[1], n * 7 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   if (inside) CU_TRY(h, cudaMemcpyAsync(inside, r[2], n, cudaMemcpyDeviceToHost, h->stream));
   return host_call_end(h);
+}
+
+int artp_valid_heading_layer(artp_handle* hh, const double* yaw, int n_yaw, uint32_t* mask) {
+  LOCK_CALL(h, hh);
+  artp::Headings hd;
+  TRY(heading_args(h, yaw, n_yaw, mask, &hd));
+  const size_t bytes = (size_t)h->rows * h->cols * sizeof(uint32_t);
+  char* d_mask;
+  TRY(host_call_begin(h, {bytes}, &d_mask));
+  TRY(valid_heading_layer(h, hd, (uint32_t*)d_mask, h->stream));
+  CU_TRY(h, cudaMemcpyAsync(mask, d_mask, bytes, cudaMemcpyDeviceToHost, h->stream));
+  return host_call_end(h, true);
+}
+
+int artp_valid_heading_layer_device(artp_handle* hh, const double* yaw, int n_yaw, uint32_t* d_mask, void* stream) {
+  LOCK_CALL(h, hh);
+  artp::Headings hd;
+  TRY(heading_args(h, yaw, n_yaw, d_mask, &hd));
+  CU_TRY(h, cudaSetDevice(h->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  ChainScope cs(h, 0, s);
+  if (cs.rc) return cs.rc;
+  return valid_heading_layer(h, hd, d_mask, s);
 }
 
 int artp_debug_circular_kernel(int size, uint8_t* out) {   // test hook: the size x size element as 0 / 1 bytes (row-major)

@@ -33,6 +33,9 @@
  *                                   each through isValid, first valid wins
  *   artp_pose_from_2d               the goal's projection in Planner::plan (planner.cpp:223-237): grid_map isInside, then
  *                                   Map::get3DPoseFrom2D (src/map/map.cpp:77-90) + setSO3FromRPY (utils.h:101-115)
+ *   artp_valid_heading_layer[_device]  no single reference call: per map cell and heading, whether Planner::plan accepts a
+ *                                   goal there without moving it, i.e. isValid of artp_pose_from_2d's projection of the
+ *                                   cell centre (GoalStateRegion's search moves x and y only, goal.cpp:11-41)
  *   artp_estimate_normals           art_planner::estimateNormals (src/utils.cpp:213-324; processors::Basic, basic.cpp:47)
  *   artp_compute_sample_cdf         computeCumulativeProbabilityDistribution
  *                                   (src/map/processors/probability_distribution.cpp:20-46)
@@ -249,6 +252,18 @@ int artp_ball_offsets(artp_handle* h, uint64_t seed, uint64_t first_draw, size_t
  * HOST buffers. Needs the normal layers of the current map (artp_estimate_normals, or artp_set_sampler with host layers),
  * else ARTP_E_INVALID; ARTP_E_INVALID on a map window. The bounds clip before it (enforceBounds) stays with OMPL. */
 int artp_pose_from_2d(artp_handle* h, const double* states_in, size_t n, double* states_out, uint8_t* inside);
+/* The valid-heading layer: which of n_yaw goal headings Planner::plan accepts on each cell of the current map as it stands.
+ * mask[r + c * rows] (grid_map layout, rows x cols words) has bit k set iff isValid(P), P = artp_pose_from_2d of the
+ * state whose (x, y) is the centre of cell (r, c) (grid_map::getPositionFromIndex) and whose getYawFromSO3 is
+ * (float)yaw[k]; bits k >= n_yaw are 0. Each bit equals artp_pose_from_2d followed by artp_check_poses on that state.
+ * GoalStateRegion's search (goal.cpp:11-41) moves only x and y, so a cell where a heading is invalid is not repaired by
+ * the planner at that heading. popcount(mask) is the number of valid headings of a cell.
+ * yaw: n_yaw HOST doubles, 1 <= n_yaw <= 32, all finite. Needs the normal layers of the current map, as
+ * artp_pose_from_2d does (artp_planner_set_map[_raw] leaves them). ARTP_E_NOMAP without a map; ARTP_E_INVALID on a map
+ * window, without normals, for n_yaw outside 1..32, a non-finite yaw or a NULL buffer, all before any device work.
+ * artp_valid_heading_layer: mask is a HOST buffer. _device: d_mask is a DEVICE buffer, written on `stream`. */
+int artp_valid_heading_layer(artp_handle* h, const double* yaw, int n_yaw, uint32_t* mask);
+int artp_valid_heading_layer_device(artp_handle* h, const double* yaw, int n_yaw, uint32_t* d_mask, void* stream);
 
 /* PathLengthObjective::motionCost for n edges -> cost[n] (double). */
 int artp_path_length_cost(artp_handle* h, const double* s1, const double* s2, size_t n, double* cost);

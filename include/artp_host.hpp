@@ -259,6 +259,17 @@ class StateValidityChecker {
     handle_->check(artp_pose_from_2d(handle_->get(), &in[0].x, in.size(), &(*out)[0].x, inside->data()), "artp_pose_from_2d");
   }
 
+  // The valid-heading layer (artp_valid_heading_layer): per cell of the map (rows x cols, column-major), bit k is set iff a
+  // goal at the cell's centre with yaw yaws[k] passes isValid once projected onto the map (1 to 32 yaws). Needs the map's
+  // normals (estimateNormals).
+  std::vector<uint32_t> validHeadingLayer(const std::vector<double>& yaws) const {
+    if (!map_) throw std::runtime_error("validHeadingLayer: no map");
+    std::vector<uint32_t> mask(static_cast<size_t>(map_->rows) * map_->cols);
+    handle_->check(artp_valid_heading_layer(handle_->get(), yaws.data(), static_cast<int>(yaws.size()), mask.data()),
+                   "artp_valid_heading_layer");
+    return mask;
+  }
+
   const HandlePtr& handle() const { return handle_; }
 
  private:
