@@ -16,7 +16,7 @@ SOURCES = [("artp_capi.cu", GEOMETRY_FLAGS), ("artp_sampling.cu", GEOMETRY_FLAGS
            ("artp_planner.cu", GEOMETRY_FLAGS), ("artp_inpaint.cu", GEOMETRY_FLAGS),
            ("artp_cnn.cu", ["-Xcompiler", "-fPIC"])]
 HEADERS = ["artp_internal.h", "artp_device.cuh", "artp_kernels.cuh", "artp_sampler.cuh", "artp_tiles.cuh", "artp_basic.cuh",
-           "artp_distribution.cuh", "artp_roadmap.cuh", "artp_roadmap_query.cuh", "artp_inpaint.cuh", "artp_cnn.h", "artp.map", os.path.join("..", "..", "include", "artp.h")]
+           "artp_distribution.cuh", "artp_roadmap.cuh", "artp_roadmap_query.cuh", "artp_inpaint.cuh", "artp.map", os.path.join("..", "..", "include", "artp.h")]
 # The library exports the C ABI (artp_*) and nothing else.
 VERSION_SCRIPT = os.path.join(CSRC, "artp.map")
 

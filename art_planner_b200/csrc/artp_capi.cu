@@ -925,7 +925,6 @@ int artp_create(const artp_params* params, artp_handle** out) {
   if ((e = cudaHostAlloc((void**)&h->h_err, 64, cudaHostAllocMapped)) != cudaSuccess) return fail("cudaHostAlloc", e);
   *h->h_err = 0;
   if ((e = cudaHostGetDevicePointer((void**)&h->d_err, h->h_err, 0)) != cudaSuccess) return fail("cudaHostGetDevicePointer", e);
-  h->cnn = artp_cnn::create(h->device, h->sm_count);
   // checker constants (float casts as the reference's ctor/Pose3FromXYZ arguments make them)
   artp::Checker& c = h->chk;
   std::memset(&c, 0, sizeof(c));
@@ -950,9 +949,9 @@ void artp_destroy(artp_handle* hh) {
   sampling_free(h);
   roadmap_free(h);
   planner_free(h);
+  cost_net_free(h);
   if (h->h_err) cudaFreeHost(h->h_err);
   for (cudaEvent_t ev : h->chain_ev) if (ev) cudaEventDestroy(ev);
-  artp_cnn::destroy(h->cnn);
   delete h;
 }
 

@@ -1,4 +1,5 @@
-// art_planner_b200/csrc/artp_cnn.cu -- the learned motion-cost network on sm_90a.
+// art_planner_b200/csrc/artp_cnn.cu -- the learned motion-cost network on sm_90a, and the unit of the C ABI that owns it:
+// its weights, features, mode and timing, and the trunk and head launches the other units run through it.
 //
 // Reference: art_planner_motion_cost/src/art_planner_motion_cost/predictor/network_light.py
 //   CNNpart :78-110  conv3x3(1->24)+BN, conv3x3(24->24)+BN+LReLU(0.3), maxpool 2/2, conv3x3(24->48)+BN+LReLU,
@@ -6,6 +7,8 @@
 //   FCpart  :113-165 and CostQuery.__call__ (cost_query.py:39-69), server centring (cost_query_server.py:160-161)
 // and the full-width network.py (same file but for the widths: 32 where light has 24, 64 where it has 48, out0 80->64,
 // out1 64->32 x 3). The weight blob's length picks the network (kNets); every kernel below is instantiated for both.
+// The tensor-core path and its fp32 CUDA-core cross-check (artp_set_cnn_mode bit 0) both run 8 trunk kernels;
+// artp_set_cost_weights runs 17 folding kernels.
 //
 // Numerics: the reference evaluates in fp16; parity here is against the fp32 evaluation of the same module to 1e-4
 // relative, so everything accumulates in fp32 and the 15x15 convolution -- 83.6 % of the FLOPs, implicit GEMM
@@ -33,28 +36,17 @@
 
 #include <cmath>
 #include <cstdint>
-#include <cstring>
 #include <string>
-#include <vector>
 
-#include "artp_cnn.h"
+#include "artp_internal.h"
 
 namespace artp_cnn {
-
-// ------------------------------------------------------------------------------------------------
-// small helpers
-// ------------------------------------------------------------------------------------------------
-#define CNN_TRY(expr)                                                              \
-  do {                                                                             \
-    cudaError_t _e = (expr);                                                       \
-    if (_e != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(_e); return -3; } \
-  } while (0)
 
 // The widths that tell the two architectures apart: c1 = init_conv1/2, c3 = init_conv3..5 and init_flatten (the
 // feature channels), nh = out0_conv1, b = out1_conv1..3 (the out2 convs read b and give 1 each).
 struct NetDims { int c1, c3, nh, b[3]; };
-constexpr NetDims kNets[kNumNetworks] = {{24, 48, 48, {24, 24, 36}},    // kNetLight: network_light.py
-                                         {32, 64, 64, {32, 32, 32}}};   // kNetFull: network.py
+constexpr NetDims kNets[2] = {{24, 48, 48, {24, 24, 36}},    // ARTP_COST_NET_LIGHT: network_light.py
+                              {32, 64, 64, {32, 32, 32}}};   // ARTP_COST_NET_FULL: network.py
 
 struct LayerDef { int cout, cin, k; bool bn; };
 // Layer l of the blob order: init_conv1..5, init_flatten, tar0_conv1, out0_conv1, out1_conv1..3, out2_conv1..3.
@@ -75,8 +67,8 @@ static const float kBnEps = 1e-5f;
 // bit order of the overflow flag the split kernels raise.
 static const char* const kSplitLayerNames[5] = {"init_conv1", "init_conv2", "init_conv3", "init_conv4", "init_conv5"};
 
-size_t blob_floats(int net) {
-  if (net < 0 || net >= kNumNetworks) return 0;
+static size_t blob_floats(int net) {
+  if (net != ARTP_COST_NET_LIGHT && net != ARTP_COST_NET_FULL) return 0;
   size_t n = 0;
   for (int i = 0; i < 14; ++i) {
     const LayerDef l = layer_def(net, i);
@@ -739,166 +731,154 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 // One tensor-core layer: weights (hi/lo), bias, and its launch geometry.
 struct TcLayer { __half *whi = nullptr, *wlo = nullptr; float* inv_scale = nullptr; int nout = 0; };
 
-struct State {
-  int device = 0, sm_count = 0;
+// The trunk's activations: h* / l* = fp16 hi / lo NHWC-64, f* = fp32 NHWC, feat = the feature map; overflow = the fp16
+// range overflow of the tensor-core path's activation splits, bit i = output of trunk layer i (kSplitLayerNames).
+struct Acts {
+  __half *h1, *l1, *hp2, *lp2, *h3, *l3, *hp4, *lp4, *h5, *l5;
+  float *f1, *f2, *fp2, *f3, *f4, *fp4, *f5, *feat;
+  unsigned* overflow;
+};
+
+}  // namespace artp_cnn
+
+using namespace artp_api;
+using namespace artp_cnn;
+
+namespace artp_api {
+
+struct CostNet {
+  int mode = 0;   // artp_set_cnn_mode
   bool has_weights = false, has_features = false;
-  // The loaded network (-1: none yet). Weight buffers, activation buffers, tensor maps and kernel attributes are all
-  // sized for it and are released when a blob of the other network arrives.
+  // The loaded network (-1: none yet). The weights, the activations, the tensor maps and the kernel attributes are laid
+  // out for it.
   int net = -1;
   LayerDef layers[14];
-  float* d_blob = nullptr;
   size_t layer_off[14];
-  float* d_wf[5] = {};     // folded fp32 3x3 weights [9][cin][cout] (layer 0 always; 1..4 for the CUDA-core check path)
-  float* d_bias[6] = {};   // folded biases (layers 0..5)
-  float* d_wf6 = nullptr;  // folded fp32 15x15 weights [225][c3][c3] (CUDA-core check path only)
-  TcLayer tc[6];           // tensor-core weights of layers 1..5 (index = layer)
-  float* d_head = nullptr;
+  // The weights, one scratch group (carve): the blob, the head's layer offsets in it, the folded head, and per trunk
+  // layer l the folded fp32 weights [k*k][cin][cout] (layer 0 always, 1..5 for the CUDA-core path) and bias, and for
+  // l = 1..5 the tensor-core weights.
+  char* d_w = nullptr;
+  size_t w_cap = 0;
+  float* d_blob = nullptr;
   size_t* d_offs = nullptr;
-  // activations (sized for the current map and network); h* / l* = fp16 hi / lo NHWC-64, f* = fp32 NHWC
+  float* d_head = nullptr;
+  float* d_wf[6] = {};
+  float* d_bias[6] = {};
+  TcLayer tc[6];
+  // The activations, another scratch group, laid out for the map of rows x cols.
+  char* d_act = nullptr;
+  size_t act_cap = 0;
+  Acts a{};
   int rows = 0, cols = 0;
-  __half *h1 = nullptr, *l1 = nullptr, *hp2 = nullptr, *lp2 = nullptr, *h3 = nullptr, *l3 = nullptr, *hp4 = nullptr,
-         *lp4 = nullptr, *h5 = nullptr, *l5 = nullptr;
-  float *f1 = nullptr, *f2 = nullptr, *fp2 = nullptr, *f3 = nullptr, *f4 = nullptr, *fp4 = nullptr, *f5 = nullptr, *feat = nullptr;
   int Hf = 0, Wf = 0;
   double res = 0, Lx = 0, Ly = 0, cx = 0, cy = 0;
   EncodeTiledFn encode = nullptr;
-  CUtensorMap maps[6][4];      // per tensor-core layer: activation hi/lo, weight hi/lo (rebuilt when buffers change)
+  // Per tensor-core layer: activation hi/lo, weight hi/lo. Valid while the map size and the network stay, which is also
+  // while the regions they address stay where they are.
+  CUtensorMap maps[6][4];
   bool maps_valid = false;
   bool attrs_set = false;
   float last_ms[3] = {0, 0, 0};
   cudaEvent_t ev[4] = {};
-  // fp16 range overflow of the tensor-core path's activation splits: bit i = output of trunk layer i (kSplitLayerNames)
-  unsigned* d_overflow = nullptr;
   unsigned* h_overflow = nullptr;   // pinned
 };
 
-State* create(int device, int sm_count) {
-  State* s = new State();
-  s->device = device;
-  s->sm_count = sm_count;
-  return s;
-}
+}  // namespace artp_api
 
-static void free_acts(State* s) {
-  void* ptrs[] = {s->h1, s->l1, s->hp2, s->lp2, s->h3, s->l3, s->hp4, s->lp4, s->h5, s->l5,
-                  s->f1, s->f2, s->fp2, s->f3, s->f4, s->fp4, s->f5, s->feat};
-  for (void* p : ptrs) cudaFree(p);
-  s->h1 = s->l1 = s->hp2 = s->lp2 = s->h3 = s->l3 = s->hp4 = s->lp4 = s->h5 = s->l5 = nullptr;
-  s->f1 = s->f2 = s->fp2 = s->f3 = s->f4 = s->fp4 = s->f5 = s->feat = nullptr;
-}
+namespace {
 
-static void free_weights(State* s) {
-  cudaFree(s->d_blob);
-  for (auto& p : s->d_wf) { cudaFree(p); p = nullptr; }
-  for (auto& p : s->d_bias) { cudaFree(p); p = nullptr; }
-  for (auto& t : s->tc) { cudaFree(t.whi); cudaFree(t.wlo); cudaFree(t.inv_scale); t = TcLayer(); }
-  cudaFree(s->d_wf6); cudaFree(s->d_head); cudaFree(s->d_offs);
-  s->d_blob = s->d_wf6 = s->d_head = nullptr;
-  s->d_offs = nullptr;
+// A handle without the state reads as one without weights.
+const CostNet& view(const Handle* h) {
+  static const CostNet none{};
+  return h->cost_net ? *h->cost_net : none;
 }
-
-void destroy(State* s) {
-  if (!s) return;
-  free_acts(s);
-  free_weights(s);
-  for (auto e : s->ev) if (e) cudaEventDestroy(e);
-  cudaFree(s->d_overflow);
-  cudaFreeHost(s->h_overflow);
-  delete s;
+CostNet& state(Handle* h) {
+  if (!h->cost_net) h->cost_net = new CostNet();
+  return *h->cost_net;
 }
-
-bool has_features(const State* s) { return s->has_features; }
-bool has_weights(const State* s) { return s->has_weights; }
-int network(const State* s) { return s->has_weights ? s->net : -1; }
-void last_times(const State* s, float* ms3) { ms3[0] = s->last_ms[0]; ms3[1] = s->last_ms[1]; ms3[2] = s->last_ms[2]; }
 
 // wgmma N of tensor-core layer l (1..5): Cout rounded up to a multiple of 16 (light init_conv2: 24 -> 32)
-static int tc_nout(const LayerDef& l) { return (l.cout + 15) / 16 * 16; }
+int tc_nout(const LayerDef& l) { return (l.cout + 15) / 16 * 16; }
 
-static int head_floats(int net) {
+int head_floats(int net) {
   const NetDims& d = kNets[net];
-  return head_floats(d.c3, d.nh, d.b[0], d.b[1], d.b[2]);
+  return artp_cnn::head_floats(d.c3, d.nh, d.b[0], d.b[1], d.b[2]);
 }
 
-int set_weights(State* s, const float* blob, size_t n, cudaStream_t st, std::string& err) {
+int set_weights(Handle* h, const float* blob, size_t n) {
   int net = -1;
-  for (int k = 0; k < kNumNetworks; ++k) if (n == blob_floats(k)) net = k;
-  if (net < 0) { err = "weight blob has the wrong number of floats (neither network_light nor network)"; return -1; }
-  CNN_TRY(cudaSetDevice(s->device));
-  if (s->net != net) {
-    // Another architecture: every buffer, tensor map and kernel attribute sized for the old one goes.
-    CNN_TRY(cudaStreamSynchronize(st));
-    free_weights(s);
-    free_acts(s);
-    s->rows = s->cols = 0;
-    s->maps_valid = false;
-    s->attrs_set = false;
-    s->has_weights = s->has_features = false;
-    s->net = net;
-    for (int l = 0; l < 14; ++l) s->layers[l] = layer_def(net, l);
+  for (int k : {ARTP_COST_NET_LIGHT, ARTP_COST_NET_FULL}) if (n == blob_floats(k)) net = k;
+  if (net < 0) { h->err = "weight blob has the wrong number of floats (neither network_light nor network)"; return ARTP_E_INVALID; }
+  CU_TRY(h, cudaSetDevice(h->device));
+  CostNet& c = state(h);
+  cudaStream_t st = h->stream;
+  if (c.net != net) {
+    // Another architecture: the features, tensor maps and kernel attributes of the old one go.
+    c.maps_valid = false;
+    c.attrs_set = false;
+    c.has_weights = c.has_features = false;
+    c.net = net;
+    for (int l = 0; l < 14; ++l) c.layers[l] = layer_def(net, l);
   }
-  const LayerDef* L = s->layers;
-  if (!s->d_blob) {
-    CNN_TRY(cudaMalloc(&s->d_blob, n * sizeof(float)));
-    for (int l = 0; l < 5; ++l) CNN_TRY(cudaMalloc(&s->d_wf[l], (size_t)9 * L[l].cin * L[l].cout * sizeof(float)));
-    for (int l = 0; l < 6; ++l) CNN_TRY(cudaMalloc(&s->d_bias[l], L[l].cout * sizeof(float)));
-    CNN_TRY(cudaMalloc(&s->d_wf6, (size_t)225 * L[5].cin * L[5].cout * sizeof(float)));
-    for (int l = 1; l < 6; ++l) {
-      s->tc[l].nout = tc_nout(L[l]);
-      const size_t cnt = (size_t)L[l].k * L[l].k * s->tc[l].nout * 64;
-      CNN_TRY(cudaMalloc(&s->tc[l].whi, cnt * sizeof(__half)));
-      CNN_TRY(cudaMalloc(&s->tc[l].wlo, cnt * sizeof(__half)));
-      CNN_TRY(cudaMalloc(&s->tc[l].inv_scale, L[l].cout * sizeof(float)));
-    }
-    CNN_TRY(cudaMalloc(&s->d_head, head_floats(net) * sizeof(float)));
-    CNN_TRY(cudaMalloc(&s->d_offs, 8 * sizeof(size_t)));
-  }
+  const LayerDef* L = c.layers;
+  auto wf = [&](int l) { return (size_t)L[l].k * L[l].k * L[l].cin * L[l].cout * sizeof(float); };
+  auto tc = [&](int l) { return (size_t)L[l].k * L[l].k * tc_nout(L[l]) * 64 * sizeof(__half); };
+  auto ch = [&](int l) { return L[l].cout * sizeof(float); };
+  char* r[30];   // blob | offsets | head | wf[0..5] | bias[0..5] | whi[1..5] | wlo[1..5] | inv_scale[1..5]
+  TRY(carve(h, c.d_w, c.w_cap,
+            {n * sizeof(float), 8 * sizeof(size_t), head_floats(net) * sizeof(float), wf(0), wf(1), wf(2), wf(3), wf(4),
+             wf(5), ch(0), ch(1), ch(2), ch(3), ch(4), ch(5), tc(1), tc(2), tc(3), tc(4), tc(5), tc(1), tc(2), tc(3), tc(4),
+             tc(5), ch(1), ch(2), ch(3), ch(4), ch(5)},
+            r));
+  c.d_blob = (float*)r[0];
+  c.d_offs = (size_t*)r[1];
+  c.d_head = (float*)r[2];
+  for (int l = 0; l < 6; ++l) { c.d_wf[l] = (float*)r[3 + l]; c.d_bias[l] = (float*)r[9 + l]; }
+  for (int l = 1; l < 6; ++l) c.tc[l] = {(__half*)r[14 + l], (__half*)r[19 + l], (float*)r[24 + l], tc_nout(L[l])};
   size_t off = 0;
   for (int l = 0; l < 14; ++l) {
-    s->layer_off[l] = off;
+    c.layer_off[l] = off;
     off += (size_t)L[l].cout * L[l].cin * L[l].k * L[l].k + (L[l].bn ? 4 * L[l].cout : L[l].cout);
   }
-  CNN_TRY(cudaMemcpyAsync(s->d_blob, blob, n * sizeof(float), cudaMemcpyHostToDevice, st));
-  CNN_TRY(cudaMemcpyAsync(s->d_offs, s->layer_off + 6, 8 * sizeof(size_t), cudaMemcpyHostToDevice, st));
+  TRY(copy_async(h, c.d_blob, blob, n * sizeof(float), cudaMemcpyHostToDevice, st));
+  TRY(copy_async(h, c.d_offs, c.layer_off + 6, 8 * sizeof(size_t), cudaMemcpyHostToDevice, st));
   for (int l = 0; l < 6; ++l) {
     const int kk = L[l].k * L[l].k;
-    const float* w = s->d_blob + s->layer_off[l];
+    const float* w = c.d_blob + c.layer_off[l];
     const float* bn = w + (size_t)L[l].cout * L[l].cin * kk;
-    // fp32 folded weights (first layer + the CUDA-core check path) and biases
-    fold_conv_kernel<<<256, 256, 0, st>>>(w, bn, L[l].cout, L[l].cin, kk, l < 5 ? s->d_wf[l] : s->d_wf6, s->d_bias[l]);
+    // fp32 folded weights (first layer + the CUDA-core path) and biases
+    TRY(launch(h, fold_conv_kernel, 256, 256, 0, st, w, bn, L[l].cout, L[l].cin, kk, c.d_wf[l], c.d_bias[l]));
     if (l >= 1) {
-      tc_scale_kernel<<<L[l].cout, 256, 0, st>>>(w, bn, L[l].cout, L[l].cin, kk, s->tc[l].inv_scale);
-      fold_tc_kernel<<<256, 256, 0, st>>>(w, bn, L[l].cout, L[l].cin, kk, s->tc[l].nout, s->tc[l].inv_scale, s->tc[l].whi,
-                                          s->tc[l].wlo, s->d_bias[l]);
+      TRY(launch(h, tc_scale_kernel, L[l].cout, 256, 0, st, w, bn, L[l].cout, L[l].cin, kk, c.tc[l].inv_scale));
+      TRY(launch(h, fold_tc_kernel, 256, 256, 0, st, w, bn, L[l].cout, L[l].cin, kk, c.tc[l].nout,
+                 c.tc[l].inv_scale, c.tc[l].whi, c.tc[l].wlo, c.d_bias[l]));
     }
   }
   HeadDims hd;
   for (int l = 0; l < 8; ++l) { hd.cin[l] = L[6 + l].cin; hd.cout[l] = L[6 + l].cout; }
-  fold_head_kernel<<<1, 256, 0, st>>>(s->d_blob, s->d_offs, hd, s->d_head);
-  CNN_TRY(cudaGetLastError());
-  CNN_TRY(cudaStreamSynchronize(st));
-  s->has_weights = true;
-  s->has_features = false;
-  return 0;
+  TRY(launch(h, fold_head_kernel, 1, 256, 0, st, c.d_blob, c.d_offs, hd, c.d_head));
+  TRY(sync_stream(h, st));
+  c.has_weights = true;
+  c.has_features = false;
+  return ARTP_OK;
 }
 
-static int get_encoder(State* s, std::string& err) {
-  if (s->encode) return 0;
+int get_encoder(Handle* h, CostNet& c) {
+  if (c.encode) return ARTP_OK;
   void* fn = nullptr;
   cudaDriverEntryPointQueryResult qres;
   if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn) {
-    err = "cuTensorMapEncodeTiled not available from the driver";
-    return -3;
+    h->err = "cuTensorMapEncodeTiled not available from the driver";
+    return ARTP_E_CUDA;
   }
-  s->encode = reinterpret_cast<EncodeTiledFn>(fn);
-  return 0;
+  c.encode = reinterpret_cast<EncodeTiledFn>(fn);
+  return ARTP_OK;
 }
 
 // maps[0..1]: activations hi/lo [H][W][64] fp16, box (64, brick_x, brick_y); maps[2..3]: weights [taps*nout][64], box (64, nout)
-static int encode_layer_maps(State* s, CUtensorMap* maps, __half* ahi, __half* alo, int H, int W, int brick_x, int brick_y,
-                             __half* whi, __half* wlo, int taps, int nout, std::string& err) {
-  int rc = get_encoder(s, err);
-  if (rc) return rc;
+int encode_layer_maps(Handle* h, CostNet& c, CUtensorMap* maps, __half* ahi, __half* alo, int H, int W, int brick_x,
+                      int brick_y, __half* whi, __half* wlo, int taps, int nout) {
+  TRY(get_encoder(h, c));
   const cuuint64_t adim[3] = {64, (cuuint64_t)W, (cuuint64_t)H};
   const cuuint64_t astr[2] = {128, (cuuint64_t)W * 128};
   const cuuint32_t abox[3] = {64, (cuuint32_t)brick_x, (cuuint32_t)brick_y};
@@ -910,33 +890,29 @@ static int encode_layer_maps(State* s, CUtensorMap* maps, __half* ahi, __half* a
   for (int i = 0; i < 4; ++i) {
     CUresult r;
     if (i < 2)
-      r = s->encode(&maps[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, ptrs[i], adim, astr, abox, one3, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      r = c.encode(&maps[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, ptrs[i], adim, astr, abox, one3, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     else
-      r = s->encode(&maps[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, ptrs[i], wdim, wstr, wbox, one3, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { err = "cuTensorMapEncodeTiled failed (" + std::to_string((int)r) + ")"; return -3; }
+      r = c.encode(&maps[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, ptrs[i], wdim, wstr, wbox, one3, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { h->err = "cuTensorMapEncodeTiled failed (" + std::to_string((int)r) + ")"; return ARTP_E_CUDA; }
   }
-  return 0;
+  return ARTP_OK;
 }
 
 template <int KS, int KSTEPS, int NOUT, int NMAIN, bool SPLIT>
-static int launch_tc(State* s, int layer, __half* ahi, __half* alo, int H, int W, float* out, __half* ohi, __half* olo,
-                     cudaStream_t st, std::string& err) {
+int launch_tc(Handle* h, CostNet& c, int layer, __half* ahi, __half* alo, int H, int W, float* out, __half* ohi, __half* olo,
+              cudaStream_t st) {
   using Cfg = ConvCfg<KS, NOUT>;
-  CUtensorMap* maps = s->maps[layer];
-  if (!s->maps_valid) {
-    int rc = encode_layer_maps(s, maps, ahi, alo, H, W, Cfg::kBrickX, Cfg::kBrickY, s->tc[layer].whi, s->tc[layer].wlo, KS * KS, NOUT, err);
-    if (rc) return rc;
-  }
+  CUtensorMap* maps = c.maps[layer];
+  if (!c.maps_valid)
+    TRY(encode_layer_maps(h, c, maps, ahi, alo, H, W, Cfg::kBrickX, Cfg::kBrickY, c.tc[layer].whi, c.tc[layer].wlo, KS * KS, NOUT));
   auto kern = conv_wgmma_kernel<KS, KSTEPS, NOUT, NMAIN, SPLIT>;
-  if (!s->attrs_set) CNN_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
+  if (!c.attrs_set) CU_TRY(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
   const int OH = H - KS + 1, OW = W - KS + 1;
   const dim3 grid((OW + kTileX - 1) / kTileX, (OH + kTileY - 1) / kTileY);
-  kern<<<grid, kConvThreads, Cfg::kSmem, st>>>(maps[0], maps[1], maps[2], maps[3], s->d_bias[layer], s->tc[layer].inv_scale, out,
-                                               ohi, olo, OH, OW, s->layers[layer].cout, s->d_overflow, 1u << layer);
-  CNN_TRY(cudaGetLastError());
-  return 0;
+  return launch(h, kern, grid, kConvThreads, Cfg::kSmem, st, maps[0], maps[1], maps[2], maps[3], c.d_bias[layer],
+                c.tc[layer].inv_scale, out, ohi, olo, OH, OW, c.layers[layer].cout, c.a.overflow, 1u << layer);
 }
 
 // Extents of every trunk activation for a rows x cols map.
@@ -952,140 +928,208 @@ struct TrunkDims {
 // The trunk's launches for one network: C1 channels after init_conv1/2, C3 after init_conv3..5 and init_flatten. Events
 // ev[0..3] bracket the 3x3 stack and the 15x15 layer.
 template <int NET>
-static int run_trunk(State* s, const float* d_layer, int pitch, const TrunkDims& d, cudaStream_t st, int use_cuda_core_path,
-                     std::string& err) {
+int run_trunk(Handle* h, CostNet& c, const float* d_layer, int pitch, const TrunkDims& d, cudaStream_t st) {
   constexpr int C1 = kNets[NET].c1, C3 = kNets[NET].c3;
   constexpr int K2 = (C1 + 15) / 16, N2 = 16 * K2, K4 = C3 / 16;   // wgmma K steps / N of init_conv2 and the C3 layers
   static_assert(C3 % 16 == 0, "C3 channels are whole K = 16 steps");
   auto grid2 = [](int oh, int ow) { return dim3((ow + 15) / 16, (oh + 15) / 16); };
-  const int g1 = s->sm_count * 8;
-  CNN_TRY(cudaEventRecord(s->ev[0], st));
-  if (use_cuda_core_path) {
-    conv3x3_kernel<1, C1, 1, false, true><<<grid2(d.H1, d.W1), 256, 0, st>>>(d_layer, d.H0, d.W0, pitch, s->d_wf[0], s->d_bias[0], s->f1);
-    conv3x3_kernel<C1, C1, 8, true, false><<<grid2(d.H2, d.W2), 256, 0, st>>>(s->f1, d.H1, d.W1, 0, s->d_wf[1], s->d_bias[1], s->f2);
-    maxpool_kernel<<<g1, 256, 0, st>>>(s->f2, d.H2, d.W2, C1, 2, 2, s->fp2, d.HP2, d.WP2);
-    conv3x3_kernel<C1, C3, 8, true, false><<<grid2(d.H3, d.W3), 256, 0, st>>>(s->fp2, d.HP2, d.WP2, 0, s->d_wf[2], s->d_bias[2], s->f3);
-    conv3x3_kernel<C3, C3, 8, true, false><<<grid2(d.H4, d.W4), 256, 0, st>>>(s->f3, d.H3, d.W3, 0, s->d_wf[3], s->d_bias[3], s->f4);
-    maxpool_kernel<<<g1, 256, 0, st>>>(s->f4, d.H4, d.W4, C3, 3, 1, s->fp4, d.HP4, d.WP4);
-    conv3x3_kernel<C3, C3, 8, true, false><<<grid2(d.H5, d.W5), 256, 0, st>>>(s->fp4, d.HP4, d.WP4, 0, s->d_wf[4], s->d_bias[4], s->f5);
-    CNN_TRY(cudaGetLastError());
-    CNN_TRY(cudaEventRecord(s->ev[1], st));
-    CNN_TRY(cudaEventRecord(s->ev[2], st));
-    conv15_reference_kernel<C3><<<(d.H6 * d.W6 * C3 + 255) / 256, 256, 0, st>>>(s->f5, d.H5, d.W5, s->d_wf6, s->d_bias[5], s->feat);
-    CNN_TRY(cudaGetLastError());
+  const unsigned g1 = h->sm_count * 8;
+  const Acts& a = c.a;
+  CU_TRY(h, cudaEventRecord(c.ev[0], st));
+  if (c.mode & 1) {   // the fp32 CUDA-core path
+    TRY(launch(h, conv3x3_kernel<1, C1, 1, false, true>, grid2(d.H1, d.W1), 256, 0, st, d_layer, d.H0, d.W0, pitch,
+               c.d_wf[0], c.d_bias[0], a.f1));
+    TRY(launch(h, conv3x3_kernel<C1, C1, 8, true, false>, grid2(d.H2, d.W2), 256, 0, st, a.f1, d.H1, d.W1, 0,
+               c.d_wf[1], c.d_bias[1], a.f2));
+    TRY(launch(h, maxpool_kernel, g1, 256, 0, st, a.f2, d.H2, d.W2, C1, 2, 2, a.fp2, d.HP2, d.WP2));
+    TRY(launch(h, conv3x3_kernel<C1, C3, 8, true, false>, grid2(d.H3, d.W3), 256, 0, st, a.fp2, d.HP2, d.WP2, 0,
+               c.d_wf[2], c.d_bias[2], a.f3));
+    TRY(launch(h, conv3x3_kernel<C3, C3, 8, true, false>, grid2(d.H4, d.W4), 256, 0, st, a.f3, d.H3, d.W3, 0,
+               c.d_wf[3], c.d_bias[3], a.f4));
+    TRY(launch(h, maxpool_kernel, g1, 256, 0, st, a.f4, d.H4, d.W4, C3, 3, 1, a.fp4, d.HP4, d.WP4));
+    TRY(launch(h, conv3x3_kernel<C3, C3, 8, true, false>, grid2(d.H5, d.W5), 256, 0, st, a.fp4, d.HP4, d.WP4, 0,
+               c.d_wf[4], c.d_bias[4], a.f5));
+    CU_TRY(h, cudaEventRecord(c.ev[1], st));
+    CU_TRY(h, cudaEventRecord(c.ev[2], st));
+    TRY(launch(h, conv15_reference_kernel<C3>, (d.H6 * d.W6 * C3 + 255) / 256, 256, 0, st, a.f5, d.H5, d.W5,
+               c.d_wf[5], c.d_bias[5], a.feat));
   } else {
-    int rc;
-    conv1_split_kernel<C1><<<g1, 256, 0, st>>>(d_layer, d.H0, d.W0, pitch, s->d_wf[0], s->d_bias[0], s->h1, s->l1,
-                                               s->d_overflow);
-    if ((rc = launch_tc<3, K2, N2, 1, false>(s, 1, s->h1, s->l1, d.H1, d.W1, s->f2, nullptr, nullptr, st, err))) return rc;
-    maxpool_split_kernel<<<g1, 256, 0, st>>>(s->f2, d.H2, d.W2, C1, 2, 2, s->hp2, s->lp2, d.HP2, d.WP2, s->d_overflow, 1u << 1);
-    if ((rc = launch_tc<3, K2, C3, 1, true>(s, 2, s->hp2, s->lp2, d.HP2, d.WP2, nullptr, s->h3, s->l3, st, err))) return rc;
-    if ((rc = launch_tc<3, K4, C3, 1, false>(s, 3, s->h3, s->l3, d.H3, d.W3, s->f4, nullptr, nullptr, st, err))) return rc;
-    maxpool_split_kernel<<<g1, 256, 0, st>>>(s->f4, d.H4, d.W4, C3, 3, 1, s->hp4, s->lp4, d.HP4, d.WP4, s->d_overflow, 1u << 3);
-    if ((rc = launch_tc<3, K4, C3, 1, true>(s, 4, s->hp4, s->lp4, d.HP4, d.WP4, nullptr, s->h5, s->l5, st, err))) return rc;
-    CNN_TRY(cudaGetLastError());
-    CNN_TRY(cudaEventRecord(s->ev[1], st));
-    CNN_TRY(cudaEventRecord(s->ev[2], st));
-    if ((rc = launch_tc<15, K4, C3, 2, false>(s, 5, s->h5, s->l5, d.H5, d.W5, s->feat, nullptr, nullptr, st, err))) return rc;
-    s->maps_valid = true;
-    s->attrs_set = true;
+    TRY(launch(h, conv1_split_kernel<C1>, g1, 256, 0, st, d_layer, d.H0, d.W0, pitch, c.d_wf[0],
+               c.d_bias[0], a.h1, a.l1, a.overflow));
+    TRY((launch_tc<3, K2, N2, 1, false>(h, c, 1, a.h1, a.l1, d.H1, d.W1, a.f2, nullptr, nullptr, st)));
+    TRY(launch(h, maxpool_split_kernel, g1, 256, 0, st, a.f2, d.H2, d.W2, C1, 2, 2, a.hp2, a.lp2, d.HP2, d.WP2,
+               a.overflow, 1u << 1));
+    TRY((launch_tc<3, K2, C3, 1, true>(h, c, 2, a.hp2, a.lp2, d.HP2, d.WP2, nullptr, a.h3, a.l3, st)));
+    TRY((launch_tc<3, K4, C3, 1, false>(h, c, 3, a.h3, a.l3, d.H3, d.W3, a.f4, nullptr, nullptr, st)));
+    TRY(launch(h, maxpool_split_kernel, g1, 256, 0, st, a.f4, d.H4, d.W4, C3, 3, 1, a.hp4, a.lp4, d.HP4, d.WP4,
+               a.overflow, 1u << 3));
+    TRY((launch_tc<3, K4, C3, 1, true>(h, c, 4, a.hp4, a.lp4, d.HP4, d.WP4, nullptr, a.h5, a.l5, st)));
+    CU_TRY(h, cudaEventRecord(c.ev[1], st));
+    CU_TRY(h, cudaEventRecord(c.ev[2], st));
+    TRY((launch_tc<15, K4, C3, 2, false>(h, c, 5, a.h5, a.l5, d.H5, d.W5, a.feat, nullptr, nullptr, st)));
+    c.maps_valid = true;
+    c.attrs_set = true;
   }
-  return 0;
+  return ARTP_OK;
 }
 
-// CostPredictor.updateFeatures (predictor.py:28-36): the CNN trunk over the `elevation` layer currently uploaded.
-// use_cuda_core_path: fp32 CUDA-core direct convolutions for every layer (the in-library cross-check of the tensor path).
-int update_features(State* s, const float* d_layer, int rows, int cols, int pitch, double res, double cx, double cy,
-                    cudaStream_t st, int use_cuda_core_path, std::string& err) {
-  if (!s->has_weights) { err = "motion-cost weights not set"; return -5; }
-  if (rows < 64 || cols < 64) { err = "map too small for the motion-cost network (needs >= 64 x 64 cells)"; return -1; }
-  CNN_TRY(cudaSetDevice(s->device));
+}  // namespace
+
+int artp_api::cost_network(const Handle* h) {
+  const CostNet& c = view(h);
+  return c.has_weights ? c.net : -1;
+}
+
+int artp_api::check_cost_weights(Handle* h) {
+  if (cost_network(h) < 0) { h->err = "motion-cost weights not set"; return ARTP_E_NOWEIGHTS; }
+  return ARTP_OK;
+}
+
+int artp_api::check_cost_net(Handle* h) {
+  TRY(check_cost_weights(h));
+  if (!view(h).has_features) {
+    h->err = "features not computed (call artp_update_features after artp_set_map)";
+    return ARTP_E_NOWEIGHTS;
+  }
+  return ARTP_OK;
+}
+
+// CostPredictor.updateFeatures (predictor.py:28-36): the CNN trunk over the layer, one synchronisation of st.
+int artp_api::update_features(Handle* h, const float* d_layer, int rows, int cols, int pitch, double res, double cx,
+                              double cy, cudaStream_t st) {
+  if (rows < 64 || cols < 64) { h->err = "map too small for the motion-cost network (needs >= 64 x 64 cells)"; return ARTP_E_INVALID; }
+  CU_TRY(h, cudaSetDevice(h->device));
+  CostNet& c = *h->cost_net;
+  c.has_features = false;
   const TrunkDims d(rows, cols);
-  if (rows != s->rows || cols != s->cols) {
-    free_acts(s);
-    auto hl = [&](__half** h, __half** l, int hh, int ww) -> cudaError_t {
-      cudaError_t e = cudaMalloc(h, (size_t)hh * ww * 64 * 2);
-      return e != cudaSuccess ? e : cudaMalloc(l, (size_t)hh * ww * 64 * 2);
-    };
-    const size_t c1 = s->layers[0].cout, c3 = s->layers[2].cout;
-    CNN_TRY(hl(&s->h1, &s->l1, d.H1, d.W1));
-    CNN_TRY(hl(&s->hp2, &s->lp2, d.HP2, d.WP2));
-    CNN_TRY(hl(&s->h3, &s->l3, d.H3, d.W3));
-    CNN_TRY(hl(&s->hp4, &s->lp4, d.HP4, d.WP4));
-    CNN_TRY(hl(&s->h5, &s->l5, d.H5, d.W5));
-    CNN_TRY(cudaMalloc(&s->f1, (size_t)d.H1 * d.W1 * c1 * 4));
-    CNN_TRY(cudaMalloc(&s->f2, (size_t)d.H2 * d.W2 * c1 * 4));
-    CNN_TRY(cudaMalloc(&s->fp2, (size_t)d.HP2 * d.WP2 * c1 * 4));
-    CNN_TRY(cudaMalloc(&s->f3, (size_t)d.H3 * d.W3 * c3 * 4));
-    CNN_TRY(cudaMalloc(&s->f4, (size_t)d.H4 * d.W4 * c3 * 4));
-    CNN_TRY(cudaMalloc(&s->fp4, (size_t)d.HP4 * d.WP4 * c3 * 4));
-    CNN_TRY(cudaMalloc(&s->f5, (size_t)d.H5 * d.W5 * c3 * 4));
-    CNN_TRY(cudaMalloc(&s->feat, (size_t)d.H6 * d.W6 * c3 * 4));
-    s->rows = rows; s->cols = cols;
-    s->maps_valid = false;
+  const size_t c1 = c.layers[0].cout, c3 = c.layers[2].cout;
+  auto split = [](int hh, int ww) { return (size_t)hh * ww * 64 * sizeof(__half); };
+  auto f32 = [](int hh, int ww, size_t ch) { return (size_t)hh * ww * ch * sizeof(float); };
+  char* r[19];   // the members of Acts in order
+  TRY(carve(h, c.d_act, c.act_cap,
+            {split(d.H1, d.W1), split(d.H1, d.W1), split(d.HP2, d.WP2), split(d.HP2, d.WP2), split(d.H3, d.W3),
+             split(d.H3, d.W3), split(d.HP4, d.WP4), split(d.HP4, d.WP4), split(d.H5, d.W5), split(d.H5, d.W5),
+             f32(d.H1, d.W1, c1), f32(d.H2, d.W2, c1), f32(d.HP2, d.WP2, c1), f32(d.H3, d.W3, c3), f32(d.H4, d.W4, c3),
+             f32(d.HP4, d.WP4, c3), f32(d.H5, d.W5, c3), f32(d.H6, d.W6, c3), sizeof(unsigned)},
+            r));
+  c.a = {(__half*)r[0], (__half*)r[1], (__half*)r[2], (__half*)r[3], (__half*)r[4], (__half*)r[5], (__half*)r[6],
+         (__half*)r[7], (__half*)r[8], (__half*)r[9], (float*)r[10], (float*)r[11], (float*)r[12], (float*)r[13],
+         (float*)r[14], (float*)r[15], (float*)r[16], (float*)r[17], (unsigned*)r[18]};
+  if (rows != c.rows || cols != c.cols) {
+    c.rows = rows; c.cols = cols;
+    c.maps_valid = false;
   }
-  if (!s->ev[0]) for (auto& e : s->ev) CNN_TRY(cudaEventCreate(&e));
-  if (!s->d_overflow) {
-    CNN_TRY(cudaMalloc(&s->d_overflow, sizeof(unsigned)));
-    CNN_TRY(cudaMallocHost(&s->h_overflow, sizeof(unsigned)));
-  }
-  s->has_features = false;
-  CNN_TRY(cudaMemsetAsync(s->d_overflow, 0, sizeof(unsigned), st));
-  const int rc = s->net == kNetFull ? run_trunk<kNetFull>(s, d_layer, pitch, d, st, use_cuda_core_path, err)
-                                    : run_trunk<kNetLight>(s, d_layer, pitch, d, st, use_cuda_core_path, err);
-  if (rc) return rc;
-  CNN_TRY(cudaEventRecord(s->ev[3], st));
-  CNN_TRY(cudaMemcpyAsync(s->h_overflow, s->d_overflow, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-  CNN_TRY(cudaStreamSynchronize(st));
-  if (*s->h_overflow) {
+  if (!c.ev[0]) for (auto& e : c.ev) CU_TRY(h, cudaEventCreate(&e));
+  if (!c.h_overflow) CU_TRY(h, cudaMallocHost(&c.h_overflow, sizeof(unsigned)));
+  CU_TRY(h, cudaMemsetAsync(c.a.overflow, 0, sizeof(unsigned), st));
+  TRY(c.net == ARTP_COST_NET_FULL ? run_trunk<ARTP_COST_NET_FULL>(h, c, d_layer, pitch, d, st)
+                                  : run_trunk<ARTP_COST_NET_LIGHT>(h, c, d_layer, pitch, d, st));
+  CU_TRY(h, cudaEventRecord(c.ev[3], st));
+  TRY(copy_async(h, c.h_overflow, c.a.overflow, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+  TRY(sync_stream(h, st));
+  if (*c.h_overflow) {
     // The tensor-core path holds activations as fp16 hi + lo: beyond 65504 the split has no representation, and the
     // features would silently be inf / NaN. The CUDA-core path (artp_set_cnn_mode bit 0) has fp32 range throughout.
     int l = 0;
-    while (!(*s->h_overflow & (1u << l))) ++l;
-    err = std::string("motion-cost trunk: an activation of ") + kSplitLayerNames[l] +
-          " exceeds the fp16 range (65504) of the tensor-core path's hi/lo split; the elevation or weight scale is out of "
-          "range for it (the CUDA-core path, artp_set_cnn_mode bit 0, has fp32 range)";
-    return -4;
+    while (!(*c.h_overflow & (1u << l))) ++l;
+    h->err = std::string("motion-cost trunk: an activation of ") + kSplitLayerNames[l] +
+             " exceeds the fp16 range (65504) of the tensor-core path's hi/lo split; the elevation or weight scale is out "
+             "of range for it (the CUDA-core path, artp_set_cnn_mode bit 0, has fp32 range)";
+    return ARTP_E_LIMIT;
   }
-  cudaEventElapsedTime(&s->last_ms[0], s->ev[0], s->ev[1]);   // layers 1..5
-  cudaEventElapsedTime(&s->last_ms[1], s->ev[2], s->ev[3]);   // 15x15 layer
-  cudaEventElapsedTime(&s->last_ms[2], s->ev[0], s->ev[3]);   // whole trunk
-  s->Hf = d.H6; s->Wf = d.W6;
-  s->res = res; s->Lx = rows * res; s->Ly = cols * res; s->cx = cx; s->cy = cy;
-  s->has_features = true;
-  return 0;
+  cudaEventElapsedTime(&c.last_ms[0], c.ev[0], c.ev[1]);   // layers 1..5
+  cudaEventElapsedTime(&c.last_ms[1], c.ev[2], c.ev[3]);   // 15x15 layer
+  cudaEventElapsedTime(&c.last_ms[2], c.ev[0], c.ev[3]);   // whole trunk
+  c.Hf = d.H6; c.Wf = d.W6;
+  c.res = res; c.Lx = rows * res; c.Ly = cols * res; c.cx = cx; c.cy = cy;
+  c.has_features = true;
+  return ARTP_OK;
 }
 
-int motion_cost(State* s, const float* d_edges, size_t n, float* d_cost3, cudaStream_t st, std::string& err) {
-  if (!s->has_weights) { err = "motion-cost weights not set"; return -5; }
-  if (!s->has_features) { err = "features not computed (call artp_update_features after artp_set_map)"; return -5; }
-  if (n == 0) return 0;
-  CNN_TRY(cudaSetDevice(s->device));
+int artp_api::map_features(Handle* h) {
+  // The resolution as artp_set_map received it: the head's row / column bias truncates (rows * res) / res like the
+  // reference, and Lx / rows may differ from res in the last bit, which moves that truncation (e.g. 116 rows at 0.04).
+  return update_features(h, h->d_H[0], h->rows, h->cols, h->pitch, h->res, h->chk.cx, h->chk.cy, h->stream);
+}
+
+int artp_api::cost_head(Handle* h, const float* d_edges, size_t n, float* d_cost3, cudaStream_t st) {
+  if (n == 0) return ARTP_OK;
+  CU_TRY(h, cudaSetDevice(h->device));
+  const CostNet& c = *h->cost_net;
   // One thread per query. Small batches (config 4: 4096 queries) use one-warp CTAs so that the batch spreads over the
   // SMs (128 CTAs instead of 32: 39 -> ~10 us); big batches amortise the 29 KB weight load over 128 queries per CTA.
-  const int bt = n <= (size_t)s->sm_count * 128 ? 32 : 128;
+  const int bt = n <= (size_t)h->sm_count * 128 ? 32 : 128;
   const unsigned grid = (unsigned)((n + bt - 1) / bt);
-  const size_t smem = head_floats(s->net) * sizeof(float);   // 30 KB light, 46.8 KB full: under the 48 KB default
-  if (s->net == kNetFull) {
-    constexpr NetDims D = kNets[kNetFull];
-    head_kernel<D.c3, D.nh, D.b[0], D.b[1], D.b[2]><<<grid, bt, smem, st>>>(s->feat, s->Hf, s->Wf, s->d_head, d_edges, n, d_cost3,
-                                                                           s->res, s->Lx, s->Ly, s->cx, s->cy);
-  } else {
-    constexpr NetDims D = kNets[kNetLight];
-    head_kernel<D.c3, D.nh, D.b[0], D.b[1], D.b[2]><<<grid, bt, smem, st>>>(s->feat, s->Hf, s->Wf, s->d_head, d_edges, n, d_cost3,
-                                                                           s->res, s->Lx, s->Ly, s->cx, s->cy);
-  }
-  CNN_TRY(cudaGetLastError());
-  return 0;
+  const size_t smem = head_floats(c.net) * sizeof(float);   // 30 KB light, 46.8 KB full: under the 48 KB default
+  constexpr NetDims L = kNets[ARTP_COST_NET_LIGHT], F = kNets[ARTP_COST_NET_FULL];
+  auto kern = c.net == ARTP_COST_NET_FULL ? head_kernel<F.c3, F.nh, F.b[0], F.b[1], F.b[2]>
+                                          : head_kernel<L.c3, L.nh, L.b[0], L.b[1], L.b[2]>;
+  return launch(h, kern, grid, bt, smem, st, c.a.feat, c.Hf, c.Wf, c.d_head, d_edges, n, d_cost3,
+                c.res, c.Lx, c.Ly, c.cx, c.cy);
 }
 
-int copy_features(State* s, float* host_out, size_t n_floats, std::string& err) {
-  if (!s->has_features) { err = "features not computed"; return -5; }
-  if (n_floats != (size_t)s->Hf * s->Wf * s->layers[5].cout) { err = "feature buffer size mismatch"; return -1; }
-  CNN_TRY(cudaMemcpy(host_out, s->feat, n_floats * sizeof(float), cudaMemcpyDeviceToHost));
-  return 0;
+void artp_api::cost_net_free(Handle* h) {
+  CostNet* c = h->cost_net;
+  if (!c) return;
+  cudaFree(c->d_w);
+  cudaFree(c->d_act);
+  for (cudaEvent_t e : c->ev) if (e) cudaEventDestroy(e);
+  cudaFreeHost(c->h_overflow);
+  delete c;
 }
 
-void feature_shape(const State* s, int* hf, int* wf) { *hf = s->Hf; *wf = s->Wf; }
+extern "C" {
 
-}  // namespace artp_cnn
+size_t artp_cost_weights_size(void) { return blob_floats(ARTP_COST_NET_LIGHT); }
+
+size_t artp_cost_weights_size_for(int network) { return blob_floats(network); }
+
+int artp_get_cost_network(artp_handle* hh, int* network) {
+  LOCK_HANDLE(h, hh);
+  if (!network) return ARTP_E_INVALID;
+  *network = cost_network(h);
+  return check_cost_weights(h);
+}
+
+int artp_set_cost_weights(artp_handle* hh, const float* blob, size_t n_floats) {
+  LOCK_CALL(h, hh);
+  if (!blob) return ARTP_E_INVALID;
+  return set_weights(h, blob, n_floats);
+}
+
+int artp_update_features(artp_handle* hh) {
+  LOCK_CALL(h, hh);
+  TRY(require_whole_map(h));
+  TRY(check_cost_weights(h));
+  return map_features(h);
+}
+
+int artp_get_features(artp_handle* hh, float* out, size_t n_floats, int* hf, int* wf) {
+  LOCK_HANDLE(h, hh);
+  if (!hf || !wf) return ARTP_E_INVALID;
+  const CostNet& c = view(h);
+  *hf = c.Hf;
+  *wf = c.Wf;
+  if (!out) return ARTP_OK;
+  TRY(check_cost_net(h));
+  if (n_floats != (size_t)c.Hf * c.Wf * c.layers[5].cout) { h->err = "feature buffer size mismatch"; return ARTP_E_INVALID; }
+  CU_TRY(h, cudaMemcpy(out, c.a.feat, n_floats * sizeof(float), cudaMemcpyDeviceToHost));
+  return ARTP_OK;
+}
+
+int artp_set_cnn_mode(artp_handle* hh, int mode) {
+  LOCK_HANDLE(h, hh);
+  if (mode & ~1) { h->err = "unknown motion-cost network mode (bit 0 is the only mode bit)"; return ARTP_E_INVALID; }
+  state(h).mode = mode;
+  return ARTP_OK;
+}
+
+int artp_get_cnn_timing(artp_handle* hh, float* ms3) {
+  LOCK_HANDLE(h, hh);
+  if (!ms3) return ARTP_E_INVALID;
+  const CostNet& c = view(h);
+  for (int i = 0; i < 3; ++i) ms3[i] = c.last_ms[i];
+  return ARTP_OK;
+}
+
+}  // extern "C"

@@ -1,6 +1,6 @@
 // art_planner_b200/csrc/artp_cost.cu -- the cost half of the C ABI (include/artp.h): PathLengthObjective::motionCost, the
-// MotionCostFunc edge matrix, the learned motion cost of edge rows, of states and of whole edges split the way
-// MotionCostObjective::motionCost splits them, and the network's weights, features and mode (artp_cnn.cu runs the network).
+// MotionCostFunc edge matrix, and the learned motion cost of edge rows, of states and of whole edges split the way
+// MotionCostObjective::motionCost splits them (artp_cnn.cu runs the network).
 // Compiled without FMA contraction like artp_capi.cu, so that the rows and costs built here equal the host's bit for bit.
 #include <cmath>
 #include <vector>
@@ -142,12 +142,6 @@ __global__ void split_reduce_kernel(const float* __restrict__ cost3, const uint3
   }
 }
 
-// The network's head over n edge rows on s, counted as one launch.
-int launch_cost_head(Handle* h, const float* d_edges, size_t n, float* d_cost3, cudaStream_t s) {
-  const int rc = artp_cnn::motion_cost(h->cnn, d_edges, n, d_cost3, s, h->err);
-  return rc || n == 0 ? rc : count_launch(h);
-}
-
 }  // namespace
 
 int artp_api::path_length_cost(Handle* h, const double* d_s1, const double* d_s2, size_t n, double* d_cost, cudaStream_t s) {
@@ -155,20 +149,11 @@ int artp_api::path_length_cost(Handle* h, const double* d_s1, const double* d_s2
                 h->p.max_lon_vel, h->p.max_lat_vel, h->p.max_ang_vel);
 }
 
-int artp_api::check_cost_net(Handle* h) {
-  if (!artp_cnn::has_weights(h->cnn)) { h->err = "motion-cost weights not set"; return ARTP_E_NOWEIGHTS; }
-  if (!artp_cnn::has_features(h->cnn)) {
-    h->err = "features not computed (call artp_update_features after artp_set_map)";
-    return ARTP_E_NOWEIGHTS;
-  }
-  return ARTP_OK;
-}
-
 int artp_api::motion_cost_split(Handle* h, const double* d_s1, const double* d_s2, size_t n, const uint32_t* d_piece_off, size_t total_pieces,
                                  float* d_rows, float* d_cost3, double* d_cost, cudaStream_t s) {
   TRY(launch(h, split_rows_kernel, grid_for(h, total_pieces, 256, 8), 256, 0, s, d_s1, d_s2, (uint32_t)n, d_piece_off,
              total_pieces, d_rows));
-  TRY(launch_cost_head(h, d_rows, total_pieces, d_cost3, s));
+  TRY(cost_head(h, d_rows, total_pieces, d_cost3, s));
   return launch(h, split_reduce_kernel, grid_for(h, n, 256, 8), 256, 0, s, d_cost3, d_piece_off, n, h->p.cost_w_energy,
                 h->p.cost_w_time, h->p.cost_w_risk, h->p.risk_threshold, d_cost);
 }
@@ -196,13 +181,10 @@ int artp_api::price_store_edges(Handle* h, const double* d_states, const uint32_
   if (n == 0) return ARTP_OK;
   const unsigned grid = grid_for(h, n, 256, 8);
   TRY(launch(h, store_rows_kernel, grid, 256, 0, s, d_states, d_edges, d_list, d_count, n, d_rows));
-  TRY(launch_cost_head(h, d_rows, n, d_cost3, s));
+  TRY(cost_head(h, d_rows, n, d_cost3, s));
   return launch(h, store_cost_kernel, grid, 256, 0, s, (const float*)d_cost3, d_list, d_count, n, h->p.cost_w_energy,
                 h->p.cost_w_time, h->p.cost_w_risk, h->p.risk_threshold, d_ecost, d_eflag);
 }
-
-static_assert(ARTP_COST_NET_LIGHT == artp_cnn::kNetLight && ARTP_COST_NET_FULL == artp_cnn::kNetFull,
-              "the ABI's network numbers are the library's");
 
 extern "C" {
 
@@ -229,7 +211,8 @@ int artp_motion_cost_states(artp_handle* hh, const double* s_start, const double
   CU_TRY(h, cudaMemcpyAsync(r[1], s_target, sb, cudaMemcpyHostToDevice, h->stream));
   const unsigned grid = grid_for(h, n, 256, 8);
   TRY(launch(h, edge_matrix_kernel, grid, 256, 0, h->stream, (const double*)r[0], (const double*)r[1], n, d_edges));
-  TRY(launch_cost_head(h, d_edges, n, d_c3, h->stream));
+  TRY(check_cost_net(h));
+  TRY(cost_head(h, d_edges, n, d_c3, h->stream));
   TRY(launch(h, combine_cost_kernel, grid, 256, 0, h->stream, d_c3, n, h->p.cost_w_energy, h->p.cost_w_time, h->p.cost_w_risk,
       h->p.risk_threshold, (double*)r[4], (uint8_t*)r[5]));
   CU_TRY(h, cudaMemcpyAsync(cost, r[4], n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
@@ -261,37 +244,11 @@ int artp_path_length_cost(artp_handle* hh, const double* s1, const double* s2, s
   return host_call_end(h);
 }
 
-size_t artp_cost_weights_size(void) { return artp_cnn::blob_floats(ARTP_COST_NET_LIGHT); }
-
-size_t artp_cost_weights_size_for(int network) { return artp_cnn::blob_floats(network); }
-
-int artp_get_cost_network(artp_handle* hh, int* network) {
-  LOCK_HANDLE(h, hh);
-  if (!network) return ARTP_E_INVALID;
-  *network = artp_cnn::network(h->cnn);
-  if (*network < 0) { h->err = "motion-cost weights not set"; return ARTP_E_NOWEIGHTS; }
-  return ARTP_OK;
-}
-
-int artp_set_cost_weights(artp_handle* hh, const float* blob, size_t n_floats) {
-  LOCK_HANDLE(h, hh);
-  if (!blob) return ARTP_E_INVALID;
-  return artp_cnn::set_weights(h->cnn, blob, n_floats, h->stream, h->err);
-}
-
-int artp_update_features(artp_handle* hh) {
-  LOCK_HANDLE(h, hh);
-  TRY(require_whole_map(h));
-  // The resolution as artp_set_map received it: the head's row / column bias truncates (rows * res) / res like the
-  // reference, and Lx / rows may differ from res in the last bit, which moves that truncation (e.g. 116 rows at 0.04).
-  return artp_cnn::update_features(h->cnn, h->d_H[0], h->rows, h->cols, h->pitch, h->res, h->chk.cx, h->chk.cy,
-                                   h->stream, h->cnn_mode & 1, h->err);
-}
-
 int artp_motion_cost_device(artp_handle* hh, const float* d_edges, size_t n, float* d_cost3, void* stream) {
   LOCK_CALL(h, hh);
   if (n && (!d_edges || !d_cost3)) return null_buffer(h);
-  return launch_cost_head(h, d_edges, n, d_cost3, (cudaStream_t)stream);
+  TRY(check_cost_net(h));
+  return cost_head(h, d_edges, n, d_cost3, (cudaStream_t)stream);
 }
 
 int artp_motion_cost(artp_handle* hh, const float* edges, size_t n, float* cost3) {
@@ -301,7 +258,8 @@ int artp_motion_cost(artp_handle* hh, const float* edges, size_t n, float* cost3
   char* r[2];   // edges | cost3
   TRY(host_call_begin(h, {n * 6 * sizeof(float), n * 3 * sizeof(float)}, r));
   CU_TRY(h, cudaMemcpyAsync(r[0], edges, n * 6 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-  TRY(launch_cost_head(h, (const float*)r[0], n, (float*)r[1], h->stream));
+  TRY(check_cost_net(h));
+  TRY(cost_head(h, (const float*)r[0], n, (float*)r[1], h->stream));
   CU_TRY(h, cudaMemcpyAsync(cost3, r[1], n * 3 * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
   return host_call_end(h);
 }
@@ -356,28 +314,6 @@ int artp_motion_cost_split(artp_handle* hh, const double* s1, const double* s2, 
       (float*)r[4], (double*)r[5], h->stream));
   CU_TRY(h, cudaMemcpyAsync(cost, r[5], n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   return host_call_end(h);   // `off` outlives its H2D copy: the call synchronises before it returns
-}
-
-int artp_get_features(artp_handle* hh, float* out, size_t n_floats, int* hf, int* wf) {
-  LOCK_HANDLE(h, hh);
-  if (!hf || !wf) return ARTP_E_INVALID;
-  artp_cnn::feature_shape(h->cnn, hf, wf);
-  if (!out) return ARTP_OK;
-  return artp_cnn::copy_features(h->cnn, out, n_floats, h->err);
-}
-
-int artp_set_cnn_mode(artp_handle* hh, int mode) {
-  LOCK_HANDLE(h, hh);
-  if (mode & ~1) { h->err = "unknown motion-cost network mode (bit 0 is the only mode bit)"; return ARTP_E_INVALID; }
-  h->cnn_mode = mode;
-  return ARTP_OK;
-}
-
-int artp_get_cnn_timing(artp_handle* hh, float* ms3) {
-  LOCK_HANDLE(h, hh);
-  if (!ms3) return ARTP_E_INVALID;
-  artp_cnn::last_times(h->cnn, ms3);
-  return ARTP_OK;
 }
 
 }  // extern "C"

@@ -26,8 +26,7 @@ int inpaint_args(Handle* h, const void* in, int rows, int cols, const void* out,
 int features_raw_args(Handle* h, const float* raw, int rows, int cols, double res, double cx, double cy) {
   TRY(inpaint_args(h, raw, rows, cols, raw, "cost map"));
   if (!(res > 0) || !std::isfinite(cx) || !std::isfinite(cy)) { h->err = "bad map arguments"; return ARTP_E_INVALID; }
-  if (!artp_cnn::has_weights(h->cnn)) { h->err = "motion-cost weights not set"; return ARTP_E_NOWEIGHTS; }
-  return ARTP_OK;
+  return check_cost_weights(h);
 }
 
 // The stages from region to march (artp_inpaint.cuh) on the H x W image that prep(img, flag) fills, then finish(img);
@@ -123,7 +122,7 @@ int artp_api::cost_map_features(Handle* h, const float* d_in, int rows, int cols
   CU_TRY(h, cudaMallocAsync(reinterpret_cast<void**>(&d_map), (size_t)rows * cols * sizeof(float), s));
   int rc = cost_map_layer(h, d_in, rows, cols, d_w, holes, true, d_map, s);
   if (rc == ARTP_OK)
-    rc = artp_cnn::update_features(h->cnn, d_map, rows, cols, rows, res, cx, cy, s, h->cnn_mode & 1, h->err);
+    rc = update_features(h, d_map, rows, cols, rows, res, cx, cy, s);
   const cudaError_t fe = cudaFreeAsync(d_map, s);
   if (rc == ARTP_OK && fe != cudaSuccess) CU_TRY(h, fe);
   return rc;

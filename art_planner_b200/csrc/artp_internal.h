@@ -1,9 +1,10 @@
-// art_planner_b200/csrc/artp_internal.h -- what the three units of the C ABI share (not installed):
+// art_planner_b200/csrc/artp_internal.h -- what the units of the C ABI share (not installed):
 //   artp_capi.cu      handle lifecycle, errors, stats and timing, map upload, the validity pipeline, pose / motion / edge
 //                     checks, compaction and bit packing
 //   artp_sampling.cu  normals and the CDF, the sampler, start / goal search, poseFrom2D, the valid-heading layer, Basic,
 //                     the sample distribution
-//   artp_cost.cu      path length, the edge matrix, the learned motion cost, cost weights and features
+//   artp_cost.cu      path length, the edge matrix, the learned motion cost of edge rows, states and split edges
+//   artp_cnn.cu       the motion-cost network: its weights, features, mode and timing, the trunk and the head
 //   artp_planner.cu   artp_planner_set_map / artp_plan: the replan, over the lock-free bodies declared at the end
 // the handle and its lock, launch and call bookkeeping, scratch regions, argument checks, and the few functions one unit
 // calls in another. It includes no kernel header: each of those defines kernels and is compiled into exactly one unit.
@@ -20,7 +21,6 @@
 #include <vector>
 
 #include "../../include/artp.h"
-#include "artp_cnn.h"
 #include "artp_device.cuh"
 
 namespace artp_api {
@@ -32,6 +32,7 @@ struct Traffic { uint64_t h2d = 0, d2h = 0; uint32_t syncs = 0; };
 struct PlannerState;   // artp_planner_set_map / artp_plan (artp_planner.cu)
 struct Pipeline;       // the validity pipeline's queues, launch shapes, streams and events (artp_capi.cu)
 struct Sampling;       // the sampler, the distribution, their layers and what the map has of them (artp_sampling.cu)
+struct CostNet;        // the motion-cost network's weights, activations, features, mode and timing (artp_cnn.cu)
 
 struct Handle {
   artp_params p;
@@ -49,9 +50,8 @@ struct Handle {
   char* d_stage = nullptr;          // device staging for the host-buffer API
   size_t stage_cap = 0;
   cudaStream_t stream = nullptr;    // internal compute stream for the host-buffer API
-  artp_cnn::State* cnn = nullptr;
-  int cnn_mode = 0;
   Sampling* sampling = nullptr;     // from the first call that needs it
+  CostNet* cost_net = nullptr;      // from the first call that needs it
   double res = 0.0;                 // map resolution as artp_set_map received it
   Roadmap* roadmap = nullptr;       // the PRM roadmap store (artp_roadmap.cu), from the first artp_roadmap_clear
   char* d_simplify = nullptr;       // artp_simplify_path: state pool, path, round buffers (artp_path_simplify.cu)
@@ -263,8 +263,6 @@ int price_store_edges(Handle* h, const double* d_states, const uint32_t* d_edges
 // artp_cost.cu, for the path simplifier:
 // PathLengthObjective::motionCost of n edges (d_s1[i] -> d_s2[i]) into d_cost on s.
 int path_length_cost(Handle* h, const double* d_s1, const double* d_s2, size_t n, double* d_cost, cudaStream_t s);
-// ARTP_E_NOWEIGHTS unless the network has weights and features.
-int check_cost_net(Handle* h);
 // MotionCostObjective::motionCost of n edges with the piece offsets d_piece_off (n + 1, total_pieces in all) on s: piece
 // rows, the head, the per-edge reduction (artp_motion_cost_split_device's work).
 int motion_cost_split(Handle* h, const double* d_s1, const double* d_s2, size_t n, const uint32_t* d_piece_off,
@@ -276,6 +274,22 @@ int cost_piece_offsets(Handle* h, const double* s1, const double* s2, size_t n, 
 
 // artp_roadmap.cu: releases the roadmap store (artp_destroy).
 void roadmap_free(Handle* h);
+
+// artp_cnn.cu: the motion-cost network.
+// The loaded network (ARTP_COST_NET_*), -1 without weights. check_cost_weights: ARTP_E_NOWEIGHTS without weights;
+// check_cost_net: without weights and features.
+int cost_network(const Handle* h);
+int check_cost_weights(Handle* h);
+int check_cost_net(Handle* h);
+// CostPredictor.updateFeatures after check_cost_weights: the trunk over the rows x cols heightfield layer d_layer (as
+// artp_set_map stores one, at `pitch`) on s, one synchronisation of s; the head then reads the map's geometry res, cx,
+// cy. map_features: over the installed map's elevation on h->stream.
+int update_features(Handle* h, const float* d_layer, int rows, int cols, int pitch, double res, double cx, double cy,
+                    cudaStream_t s);
+int map_features(Handle* h);
+// The head over n edge rows d_edges (n x 6) into d_cost3 (n x 3) on s, after check_cost_net: one launch, none for n = 0.
+int cost_head(Handle* h, const float* d_edges, size_t n, float* d_cost3, cudaStream_t s);
+void cost_net_free(Handle* h);
 
 // ---- the bodies of public entry points, without the lock, for artp_plan / artp_planner_set_map (artp_planner.cu) ----
 // artp_capi.cu: artp_set_map_window's work. device_src: the two layers are DEVICE pointers (rows x cols, grid_map layout)

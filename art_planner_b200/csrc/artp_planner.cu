@@ -359,14 +359,10 @@ int set_map(Handle* h, const artp_planner_params* pp, const float* elevation, co
   TRY(host_call_end(h));
   // CostPredictor.updateFeatures, when a network is loaded: on the uploaded elevation, or with cost_map_from_raw on the
   // cost server's preparation of the raw one
-  if (h->cnn && artp_cnn::network(h->cnn) >= 0) {
+  if (cost_network(h) >= 0) {
     CU_TRY(h, cudaSetDevice(h->device));
-    if (cost_map) {
-      TRY(cost_map_features(h, raw_e, rows, cols, d_mm + 8, mm[8 + 3] != 0, h->res, h->chk.cx, h->chk.cy, h->stream));
-    } else if (const int rc = artp_cnn::update_features(h->cnn, h->d_H[0], h->rows, h->cols, h->pitch, h->res, h->chk.cx,
-                                                        h->chk.cy, h->stream, h->cnn_mode & 1, h->err)) {
-      return rc;
-    }
+    if (cost_map) TRY(cost_map_features(h, raw_e, rows, cols, d_mm + 8, mm[8 + 3] != 0, h->res, h->chk.cx, h->chk.cy, h->stream));
+    else TRY(map_features(h));
   }
   st->space = sp;
   st->generation += 1;

@@ -8,7 +8,7 @@ import torch.nn.functional as F
 m = cases.c4_map()
 chk = ap.StateValidityChecker(synth.PARAMS_YAML, device=0); chk.setMap(m); chk.updateHeightField()
 obj = ap.MotionCostObjective(chk); sd = costnet.make_state_dict(5); obj.setWeights(sd)
-for mode in (0,4,8,12,1):
+for mode in (0, 1):
     obj.setMode(mode)
     ts=[]
     for i in range(6):
