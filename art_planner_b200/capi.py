@@ -11,6 +11,19 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libartp.so")
 
 ARTP_OK, ARTP_E_INVALID, ARTP_E_NOMAP, ARTP_E_CUDA, ARTP_E_LIMIT, ARTP_E_NOWEIGHTS, ARTP_E_WINDOW = 0, -1, -2, -3, -4, -5, -6
+# artp_box_verdicts words: box k = 0 torso, 1..4 the reach boxes (+,+), (+,-), (-,+), (-,-)
+ARTP_BOX_TORSO, ARTP_BOX_FOOT_PP, ARTP_BOX_FOOT_PM, ARTP_BOX_FOOT_MP, ARTP_BOX_FOOT_MM = 0, 1, 2, 3, 4
+ARTP_BOX_FAIL_MASK, ARTP_BOX_OUTSIDE_MASK = 0x001F, 0x1F00
+
+
+def ARTP_BOX_FAILS(k: int) -> int:
+    return 1 << k
+
+
+def ARTP_BOX_OUTSIDE(k: int) -> int:
+    return 1 << (8 + k)
+
+
 
 
 class ArtpError(RuntimeError):
@@ -142,6 +155,8 @@ def load():
     lib.artp_has_map.argtypes = [vp]
     lib.artp_check_poses.argtypes = [vp, vp, sz, vp]
     lib.artp_check_poses_device.argtypes = [vp, vp, sz, vp, vp]
+    lib.artp_box_verdicts.argtypes = [vp, vp, sz, vp]
+    lib.artp_box_verdicts_device.argtypes = [vp, vp, sz, vp, vp]
     lib.artp_check_poses_f32.argtypes = [vp, vp, sz, vp]
     lib.artp_check_poses_f32_device.argtypes = [vp, vp, sz, vp, vp]
     lib.artp_check_motions.argtypes = [vp, vp, vp, sz, i32, vp]
@@ -168,6 +183,8 @@ def load():
     lib.artp_pose_from_2d.argtypes = [vp, vp, sz, vp, vp]
     lib.artp_valid_heading_layer.argtypes = [vp, vp, i32, vp]
     lib.artp_valid_heading_layer_device.argtypes = [vp, vp, i32, vp, vp]
+    lib.artp_box_verdict_layer.argtypes = [vp, C.c_double, vp]
+    lib.artp_box_verdict_layer_device.argtypes = [vp, C.c_double, vp, vp]
     lib.artp_path_length_cost.argtypes = [vp, vp, vp, sz, vp]
     lib.artp_path_length_cost_device.argtypes = [vp, vp, vp, sz, vp, vp]
     lib.artp_compact_valid_device.argtypes = [vp, vp, sz, C.c_int64, vp, vp, vp]

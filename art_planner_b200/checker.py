@@ -137,6 +137,36 @@ class StateValidityChecker:
         h.check(fn(h.h, s.ctypes.data, n, out.ctypes.data))
         return out
 
+    def boxVerdicts(self, states, out=None):
+        """Why each state passes or fails isValid (artp_box_verdicts): states [n, 7] float64 -> uint16 [n] words, bit k set
+        when box k fails (0 torso, 1..4 the reach boxes (+,+), (+,-), (-,+), (-,-)) and bit 8 + k when box k's centre is off
+        the map (capi.ARTP_BOX_*). Every box is decided, so (word & 0x1F) == 0 exactly where isValidBatch gives 1. A CUDA
+        float64 tensor takes the device form on the current stream, into `out` (a CUDA int16 or uint16 tensor of n words,
+        same bits) or a new uint16 tensor."""
+        lib, h = self._h.lib, self._h
+        if _is_torch_cuda(states):
+            import torch
+            if states.dtype != torch.float64 or not states.is_contiguous() or states.dim() != 2 or states.shape[1] != 7:
+                raise ValueError("boxVerdicts: states must be a contiguous [n, 7] float64 CUDA tensor")
+            n = states.shape[0]
+            if out is None:
+                out = torch.empty(n, dtype=torch.uint16, device=states.device)
+            if out.dtype not in (torch.int16, torch.uint16) or not out.is_cuda or not out.is_contiguous() or out.numel() != n:
+                raise ValueError("boxVerdicts: out must be a contiguous int16 or uint16 CUDA tensor of n words")
+            h.check(lib.artp_box_verdicts_device(h.h, C.c_void_p(states.data_ptr()), n, C.c_void_p(out.data_ptr()),
+                                                 _stream_ptr()))
+            return out
+        s = np.ascontiguousarray(states, dtype=np.float64)
+        if s.ndim != 2 or s.shape[1] != 7:
+            raise ValueError("boxVerdicts: states must be [n, 7]")
+        n = s.shape[0]
+        if out is None:
+            out = np.empty(n, dtype=np.uint16)
+        if out.dtype != np.uint16 or out.shape != (n,) or not out.flags.c_contiguous:
+            raise ValueError("boxVerdicts: out must be a contiguous uint16 array of n words")
+        h.check(lib.artp_box_verdicts(h.h, s.ctypes.data, n, out.ctypes.data))
+        return out
+
     def sampleValidBatch(self, sampler, n_wanted: int, batch: int = 65536, max_draws: int = 1 << 24):
         """The rejection-sampling loop `do sampleUniform(s) while (!isValid(s))` (prm_motion_cost.cpp:171-194,
         lazy_prm_star_min_update.cpp:549-556) in batches: sampler(m) -> [m, 7] candidates; valid ones are kept in draw
@@ -313,6 +343,24 @@ class StateValidityChecker:
         mask = np.empty(self._installed, np.uint32, order="F")
         self._h.check(self._h.lib.artp_valid_heading_layer(self._h.h, y.ctypes.data, y.shape[0], mask.ctypes.data))
         return mask
+
+    def boxVerdictLayer(self, yaw: float, out=None):
+        """The box-verdict layer of the installed map (artp_box_verdict_layer): a uint16 [rows, cols] column-major array of
+        the boxVerdicts word of the goal a cell's centre projects to (poseFrom2D) at heading `yaw` -- the pose
+        validHeadingLayer checks. Needs the map's normals. With `out` a CUDA tensor (int16 or uint16, column-major: a
+        transposed contiguous cols x rows tensor) the layer is written there on the current stream
+        (artp_box_verdict_layer_device) and `out` is returned."""
+        if out is not None and _is_torch_cuda(out):
+            import torch
+            if out.dtype not in (torch.int16, torch.uint16) or out.dim() != 2 or not out.t().is_contiguous():
+                raise ValueError("boxVerdictLayer: out must be a column-major int16 or uint16 CUDA tensor")
+            self._h.check(self._h.lib.artp_box_verdict_layer_device(self._h.h, float(yaw), out.data_ptr(), _stream_ptr()))
+            return out
+        if self._installed is None:
+            raise capi.ArtpError(capi.ARTP_E_NOMAP, "no map installed")
+        words = np.empty(self._installed, np.uint16, order="F")
+        self._h.check(self._h.lib.artp_box_verdict_layer(self._h.h, float(yaw), words.ctypes.data))
+        return words
 
     def isValidBatchBits(self, states, out_valid, out_bits):
         """One shard step of the multi-GPU path: verdict bytes + bit-packed mask (CUDA float64 states), one call."""

@@ -417,51 +417,60 @@ __global__ void close_slice_kernel(const BoxQueues* round, BoxQueues* slices, in
   slices[i].big = {round->big.end, prev.big.end};
 }
 
-// Stage launchers shared by both rounds. Each launches its kernel over the items [lo, hi) of w (items).
-artp::Work items(artp::Work w, size_t lo, size_t hi) {
+// Stage launchers shared by both rounds. Each launches its kernel over the items [lo, hi) of w (items); W is artp::Work,
+// or artp::WhyWork for the explain form of the kernels (artp_box_verdicts).
+template <class W>
+constexpr bool kWhyOf = std::is_same_v<W, artp::WhyWork>;
+template <class W>
+W items(W w, size_t lo, size_t hi) {
   w.item_base = (uint32_t)lo;
   w.n_items = (uint32_t)hi;
   return w;
 }
-int launch_classify(Handle* h, const artp::Work& w, size_t lo, size_t hi, BoxQueues* q, cudaStream_t s) {
+template <class W>
+int launch_classify(Handle* h, const W& w, size_t lo, size_t hi, BoxQueues* q, cudaStream_t s) {
   const Pipeline& p = *h->pipe;
-  return launch(h, artp::classify_items_kernel, (unsigned)((hi - lo + artp::kClassifyItems - 1) / artp::kClassifyItems),
+  return launch(h, artp::classify_items_kernel<kWhyOf<W>>, (unsigned)((hi - lo + artp::kClassifyItems - 1) / artp::kClassifyItems),
                 artp::kClassifyItems, 0, s, h->chk, items(w, lo, hi), p.recs[p.kBig], p.recs[p.kReach],
                 p.groups.grid ? p.recs[p.kGroup] : nullptr, &q->big.end, &q->reach.end, &q->group.end, p.mode == 1);
 }
 
 // Classify appends to the queues q, each box kernel takes its queue's entries: the big-tile queue and the two reach-box
 // queues (one warp per box; 8-lane groups), which exist only for some box sizes. reach_cap caps both reach grids.
-int launch_big_tile(Handle* h, const artp::Work& w, size_t lo, size_t hi, BoxQueues* q, cudaStream_t s) {
+template <class W>
+int launch_big_tile(Handle* h, const W& w, size_t lo, size_t hi, BoxQueues* q, cudaStream_t s) {
   Pipeline& p = *h->pipe;
   const int wpc = p.tile[0].block / 32;   // no more CTAs than there can be boxes: up to five big-tile boxes per item
   const unsigned grid = (unsigned)std::min<size_t>((size_t)p.tile[0].grid, (5 * (hi - lo) + wpc - 1) / wpc);
-  return launch(h, artp::box_tiles_warp_kernel, grid, p.tile[0].block, p.tile[0].smem, s, h->chk, p.tile_map[0][0],
+  return launch(h, artp::box_tiles_warp_kernel<kWhyOf<W>>, grid, p.tile[0].block, p.tile[0].smem, s, h->chk, p.tile_map[0][0],
                 p.tile_map[0][1], p.tile_cfg[0], items(w, lo, hi), p.recs[p.kBig], &q->big.end, &q->big.claim, &p.d_ctr->defer,
                 p.d_defer, 0u, p.mode == 1);
 }
-int launch_reach_warp(Handle* h, const artp::Work& w, size_t lo, size_t hi, BoxQueues* q, cudaStream_t s, unsigned reach_cap) {
+template <class W>
+int launch_reach_warp(Handle* h, const W& w, size_t lo, size_t hi, BoxQueues* q, cudaStream_t s, unsigned reach_cap) {
   if (!h->chk.reach_tw) return ARTP_OK;
   Pipeline& p = *h->pipe;
   const int wpc = p.tile[1].block / 32;
   const unsigned grid = (unsigned)std::min<size_t>({(size_t)p.tile[1].grid, (4 * (hi - lo) + wpc - 1) / wpc, reach_cap});
-  return launch(h, artp::box_tiles_warp_kernel, grid, p.tile[1].block, p.tile[1].smem, s, h->chk, p.tile_map[1][1],
+  return launch(h, artp::box_tiles_warp_kernel<kWhyOf<W>>, grid, p.tile[1].block, p.tile[1].smem, s, h->chk, p.tile_map[1][1],
                 p.tile_map[1][1], p.tile_cfg[1], items(w, lo, hi), p.recs[p.kReach], &q->reach.end, &q->reach.claim,
                 &p.d_ctr->defer, p.d_defer, artp::kDeferReachBit, p.mode == 1);
 }
-int launch_reach_groups(Handle* h, const artp::Work& w, size_t lo, size_t hi, BoxQueues* q, cudaStream_t s, unsigned reach_cap) {
+template <class W>
+int launch_reach_groups(Handle* h, const W& w, size_t lo, size_t hi, BoxQueues* q, cudaStream_t s, unsigned reach_cap) {
   const Pipeline& p = *h->pipe;
   if (!p.groups.grid) return ARTP_OK;
   const unsigned grid = (unsigned)std::min<size_t>({(size_t)p.groups.grid, (hi - lo + 7) / 8, reach_cap});
-  return launch(h, artp::reach_groups_kernel, grid, p.groups.block, p.groups.smem, s, h->chk, p.tile_map[1][1], p.tile_cfg[1],
+  return launch(h, artp::reach_groups_kernel<kWhyOf<W>>, grid, p.groups.block, p.groups.smem, s, h->chk, p.tile_map[1][1], p.tile_cfg[1],
                 items(w, lo, hi), p.recs[p.kGroup], &q->group.end, &q->group.claim);
 }
 
 // The plane-grouping stage over every box the round [lo, hi) deferred.
-int launch_grouping(Handle* h, const artp::Work& w, size_t lo, size_t hi, cudaStream_t s) {
+template <class W>
+int launch_grouping(Handle* h, const W& w, size_t lo, size_t hi, cudaStream_t s) {
   const Pipeline& p = *h->pipe;
   const unsigned grid = (unsigned)std::min<size_t>((size_t)p.grouping.grid, 5 * (hi - lo));
-  return launch(h, artp::box_items_block_kernel, grid, p.grouping.block, p.grouping.smem, s, h->chk, items(w, lo, hi),
+  return launch(h, artp::box_items_block_kernel<kWhyOf<W>>, grid, p.grouping.block, p.grouping.smem, s, h->chk, items(w, lo, hi),
                 p.recs[p.kBig], p.recs[p.kReach], &p.d_ctr->defer, p.d_defer, p.tcap, h->d_err);
 }
 
@@ -472,7 +481,8 @@ int launch_grouping(Handle* h, const artp::Work& w, size_t lo, size_t hi, cudaSt
 // 8-lane kernel in about half of the steps and ended last). The grouping stage waits for tile_stream and box_stream only;
 // group_stream joins s after it. With stage timing on, everything runs in order on s, and a timed round records the
 // per-stage events.
-int run_round_device(Handle* h, const artp::Work& w, cudaStream_t s, size_t base, size_t end, bool timed) {
+template <class W>
+int run_round_device(Handle* h, const W& w, cudaStream_t s, size_t base, size_t end, bool timed) {
   Pipeline& p = *h->pipe;
   CU_TRY(h, cudaMemsetAsync(p.d_ctr, 0, sizeof(Counters), s));
   if (timed) CU_TRY(h, cudaEventRecord(p.ev[0], s));
@@ -568,13 +578,15 @@ int run_round_piped(Handle* h, const artp::Work& w, cudaStream_t s, const HostFe
 // work items (bounds the box queues), and count the items in stats.poses_checked. With a host feed, a round larger than
 // one slice is piped; any other round (and every round while stage timing is on) has its states copied on s and runs as
 // a device round.
-int run_items(Handle* h, artp::Work w, cudaStream_t s, const HostFeed* feed = nullptr) {
+// The explain form (W = artp::WhyWork) has no piped round: its host feed is copied round by round.
+template <class W>
+int run_items(Handle* h, W w, cudaStream_t s, const HostFeed* feed = nullptr) {
   const size_t n_total = w.n_items;
   TRY(ensure_queues(h, n_total));
   for (size_t base = 0; base < n_total; base += kChunkItems) {
     const size_t end = std::min(n_total, base + kChunkItems);
-    if (feed && feed->slice_items < end - base && !h->pipe->timing) {
-      TRY(run_round_piped(h, w, s, *feed, base, end));
+    if (!kWhyOf<W> && feed && feed->slice_items < end - base && !h->pipe->timing) {
+      if constexpr (!kWhyOf<W>) TRY(run_round_piped(h, w, s, *feed, base, end));
     } else {
       if (feed)
         CU_TRY(h, cudaMemcpyAsync(feed->dev + base * feed->bytes_per_item, feed->host + base * feed->bytes_per_item,
@@ -628,6 +640,28 @@ int check_states(Handle* h, const T* d_states, size_t n, uint8_t* d_valid, cudaS
   w.valid = d_valid;
   w.n_items = (uint32_t)n;
   return run_items(h, w, s, feed);
+}
+
+// The explain form of check_states: every box of each of the n states decided, the ARTP_BOX_* words into d_why, on s.
+template <typename T>
+int box_verdicts_on(Handle* h, const T* d_states, size_t n, uint16_t* d_why, cudaStream_t s) {
+  // the explain form's kernels get artp_create's shared-memory limits at their first use, not at artp_create: a handle
+  // that never explains never loads them
+  const std::pair<const void*, int> caps[] = {{(const void*)artp::box_items_block_kernel<true>, kMaxStoreSmem},
+                                              {(const void*)artp::box_tiles_warp_kernel<true>, kMaxTileSmem},
+                                              {(const void*)artp::reach_groups_kernel<true>, kMaxGroupsSmem}};
+  for (const auto& [k, bytes] : caps) CU_TRY(h, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  artp::WhyWork w;
+  if constexpr (std::is_same_v<T, float>) w.s2f = d_states; else w.s2 = d_states;
+  w.why = d_why;
+  w.n_items = (uint32_t)n;
+  return run_items(h, w, s);
+}
+
+// artp_box_verdicts[_device]'s refusals before the null-buffer check: those of artp_check_poses, and a map window.
+int box_verdict_args(Handle* h, size_t n) {
+  TRY(check_common(h, n));
+  return require_whole_map(h);
 }
 
 // The pose entry points. A float state gives the same verdict as the double one while the H2D stream is 28 B/pose
@@ -753,7 +787,7 @@ int fit_shape(Handle* h, void (*kernel)(P...), int block, int smem, Shape& out) 
 // span and the grouping stage's plane store (upload_map): occupancy grids, tile maps, chk's reach tile.
 int set_shapes(Handle* h, const int span[2][2], int tcap, int store) {
   Pipeline& p = *h->pipe;
-  TRY(fit_shape(h, artp::box_items_block_kernel, artp::kBlockStageThreads, store, p.grouping));
+  TRY(fit_shape(h, artp::box_items_block_kernel<false>, artp::kBlockStageThreads, store, p.grouping));
   p.tcap = tcap;
   // Stage B tiles (artp_tiles.cuh): a zone spans at most ceil(2 r / s) + 3 vertices per axis; + 3 columns because the
   // tile starts at x0 & ~3; width rounded up to a multiple of 4 floats (16-byte rows).
@@ -796,11 +830,11 @@ int set_shapes(Handle* h, const int span[2][2], int tcap, int store) {
   if (h->chk.reach_tw && p.tile_cfg[1].tw <= 127 && p.tile_cfg[1].th <= 255) {   // task packing: 7 + 8 bits of cell coordinates
     const int gsm = artp::kMaxTileWarps * 8 * (int)p.tile_cfg[1].stride + 128;
     if (gsm <= kMaxGroupsSmem && !std::getenv("ARTP_NO_GROUPS")) {   // ARTP_NO_GROUPS: every reach box takes the one-warp-per-box queue
-      TRY(fit_shape(h, artp::reach_groups_kernel, artp::kMaxTileWarps * 32, gsm, p.groups));
+      TRY(fit_shape(h, artp::reach_groups_kernel<false>, artp::kMaxTileWarps * 32, gsm, p.groups));
     }
   }
   for (Shape& t : p.tile)
-    if (t.block) TRY(fit_shape(h, artp::box_tiles_warp_kernel, t.block, t.smem, t));
+    if (t.block) TRY(fit_shape(h, artp::box_tiles_warp_kernel<false>, t.block, t.smem, t));
   return ARTP_OK;
 }
 
@@ -824,6 +858,10 @@ int artp_api::take_sticky_error(Handle* h) {
 
 int artp_api::check_states_f32(Handle* h, const float* d_states, size_t n, uint8_t* d_valid, cudaStream_t s) {
   return check_states(h, d_states, n, d_valid, s);
+}
+
+int artp_api::box_verdicts_f32(Handle* h, const float* d_states, size_t n, uint16_t* d_why, cudaStream_t s) {
+  return box_verdicts_on(h, d_states, n, d_why, s);
 }
 
 int artp_api::check_states_cta(Handle* h, const double* d_states, const uint32_t* d_count, const uint32_t* d_stop, size_t max_n,
@@ -894,7 +932,7 @@ int artp_create(const artp_params* params, artp_handle** out) {
   if ((e = cudaGetDeviceProperties(&prop, h->device)) != cudaSuccess) return fail("cudaGetDeviceProperties", e);
   h->sm_count = prop.multiProcessorCount;
   cudaFuncAttributes fa;
-  if ((e = cudaFuncGetAttributes(&fa, artp::box_tiles_warp_kernel)) != cudaSuccess)
+  if ((e = cudaFuncGetAttributes(&fa, artp::box_tiles_warp_kernel<false>)) != cudaSuccess)
     return fail("no usable kernel image (built for sm_90a)", e);
   int prio_least = 0, prio_greatest = 0;
   if ((e = cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest)) != cudaSuccess) return fail("cudaDeviceGetStreamPriorityRange", e);
@@ -917,8 +955,8 @@ int artp_create(const artp_params* params, artp_handle** out) {
   // that set it to its own map's size would lower it under the launches of a handle holding a larger map.
   const std::pair<const void*, int> smem_caps[] = {
       {(const void*)artp::pose_small_kernel, kMaxStoreSmem}, {(const void*)artp::pose_states_kernel, kMaxStoreSmem},
-      {(const void*)artp::box_items_block_kernel, kMaxStoreSmem}, {(const void*)artp::box_tiles_warp_kernel, kMaxTileSmem},
-      {(const void*)artp::reach_groups_kernel, kMaxGroupsSmem}};
+      {(const void*)artp::box_items_block_kernel<false>, kMaxStoreSmem}, {(const void*)artp::box_tiles_warp_kernel<false>, kMaxTileSmem},
+      {(const void*)artp::reach_groups_kernel<false>, kMaxGroupsSmem}};
   for (const auto& [k, bytes] : smem_caps)
     if ((e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)) != cudaSuccess)
       return fail("cudaFuncSetAttribute", e);
@@ -1200,6 +1238,31 @@ int artp_check_poses_device(artp_handle* hh, const double* d_states, size_t n, u
 int artp_check_poses_f32_device(artp_handle* hh, const float* d_states, size_t n, uint8_t* d_valid, void* stream) {
   LOCK_CALL(h, hh);
   return check_poses(h, d_states, n, d_valid, true, (cudaStream_t)stream);
+}
+
+int artp_box_verdicts(artp_handle* hh, const double* states, size_t n, uint16_t* why) {
+  LOCK_CALL(h, hh);
+  TRY(box_verdict_args(h, n));
+  if (n == 0) return ARTP_OK;
+  if (!states || !why) return null_buffer(h);
+  const size_t sb = n * 7 * sizeof(double), wb = n * sizeof(uint16_t);
+  char* r[2];   // states | words
+  TRY(host_call_begin(h, {sb, wb}, r));
+  TRY(copy_async(h, r[0], states, sb, cudaMemcpyHostToDevice, h->stream));
+  TRY(box_verdicts_on(h, (const double*)r[0], n, (uint16_t*)r[1], h->stream));
+  TRY(copy_async(h, why, r[1], wb, cudaMemcpyDeviceToHost, h->stream));
+  return host_call_end(h, true);
+}
+int artp_box_verdicts_device(artp_handle* hh, const double* d_states, size_t n, uint16_t* d_why, void* stream) {
+  LOCK_CALL(h, hh);
+  TRY(box_verdict_args(h, n));
+  if (n == 0) return ARTP_OK;
+  if (!d_states || !d_why) return null_buffer(h);
+  CU_TRY(h, cudaSetDevice(h->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  ChainScope cs(h, 0, s);
+  if (cs.rc) return cs.rc;
+  return box_verdicts_on(h, d_states, n, d_why, s);
 }
 
 int artp_check_motions_device(artp_handle* hh, const double* d_s1, const double* d_s2, size_t n, int n_steps,

@@ -1,8 +1,8 @@
 // art_planner_b200/csrc/artp_internal.h -- what the units of the C ABI share (not installed):
 //   artp_capi.cu      handle lifecycle, errors, stats and timing, map upload, the validity pipeline, pose / motion / edge
-//                     checks, compaction and bit packing
-//   artp_sampling.cu  normals and the CDF, the sampler, start / goal search, poseFrom2D, the valid-heading layer, Basic,
-//                     the sample distribution
+//                     checks, box verdicts, compaction and bit packing
+//   artp_sampling.cu  normals and the CDF, the sampler, start / goal search, poseFrom2D, the valid-heading and box-verdict
+//                     layers, Basic, the sample distribution
 //   artp_cost.cu      path length, the edge matrix, the learned motion cost of edge rows, states and split edges
 //   artp_cnn.cu       the motion-cost network: its weights, features, mode and timing, the trunk and the head
 //   artp_planner.cu   artp_planner_set_map / artp_plan: the replan, over the lock-free bodies declared at the end
@@ -223,9 +223,11 @@ inline int host_call_end(Handle* h, bool pipeline = false) {
   return pipeline ? take_sticky_error(h) : ARTP_OK;
 }
 
-// artp_capi.cu, for the sampler and the start / goal search:
+// artp_capi.cu, for the sampler, the start / goal search and the map layers:
 // The validity pipeline over n float states on the device (Pose3FromSE3's cast already applied) into d_valid, on s.
 int check_states_f32(Handle* h, const float* d_states, size_t n, uint8_t* d_valid, cudaStream_t s);
+// Its explain form: the ARTP_BOX_* word of each state into d_why (artp_box_verdicts), on s.
+int box_verdicts_f32(Handle* h, const float* d_states, size_t n, uint16_t* d_why, cudaStream_t s);
 // Ordered compaction of the n flags d_valid (bit-packed with `bits`) into the indices base + i of the set ones and their
 // count, int64_t indices or, with `u32`, uint32_t ones. Uses scratch group 1.
 int compact_valid(Handle* h, const uint8_t* d_valid, size_t n, int64_t base, void* d_indices, uint32_t* d_count, cudaStream_t s,

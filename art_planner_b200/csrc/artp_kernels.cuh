@@ -16,7 +16,10 @@
 //      order-dependent epsilon grouping, with all planes staged in shared memory.
 // The pose result is a pure AND over its boxes (torso free, every reach box touching), so B and C only ever
 // clear the provisional 1 that A wrote. All three are bit-exact against oracle/ (tests/test_pose_gpu.py).
+// Each stage also has an explain form (kWhy, WhyWork): every box of every item is decided and records its own bit.
 #pragma once
+
+#include <type_traits>
 
 #include "artp_device.cuh"
 
@@ -60,6 +63,26 @@ struct Work {
   // segments: item k of edge e is interpolate(s1, s2, (k + 1) / nd_e) for k < nd_e - 1 and s2 itself for k = nd_e - 1.
   int quotient = 0;
 };
+
+// The explain form of the pose pipeline (artp_box_verdicts, POSE mode only): instead of one verdict byte per item, why[i]
+// receives the item's ARTP_BOX_* word -- bit k when box k fails, bit 8 + k when box k's centre is off the map -- with
+// every box decided (no item leaves the pipeline at its first failing box). valid is not used.
+struct WhyWork : Work {
+  uint16_t* why = nullptr;
+};
+template <bool kWhy>
+using WorkOf = std::conditional_t<kWhy, WhyWork, Work>;
+
+// Sets bit k of a why word. The boxes of one item are decided by different threads, possibly in kernels that run side
+// by side: a 16-bit compare-and-swap loop (one per failing box), so no store reaches past the caller's buffer.
+__device__ __forceinline__ void why_set(uint16_t* why, uint32_t slot, int k) {
+  unsigned short* p = reinterpret_cast<unsigned short*>(why + slot);
+  unsigned short old = *(volatile unsigned short*)p, seen;
+  do {
+    seen = old;
+    old = atomicCAS(p, seen, (unsigned short)(seen | (1u << k)));
+  } while (old != seen);
+}
 
 __device__ __forceinline__ uint32_t bloom_hash(int kx, int kz) {
   return (((uint32_t)kx * 0x9E3779B1u) ^ ((uint32_t)kz * 0x85EBCA77u)) >> 20;   // 12 bits
@@ -873,6 +896,9 @@ struct ClassifyShared {
   uint32_t base[3];
 };
 static_assert(kClassifyItems <= 256, "emit packs the item index into 8 bits");
+struct ClassifySharedWhy : ClassifyShared {               // the explain form: each item's word of the boxes decided here
+  uint16_t why[kClassifyItems];
+};
 
 __device__ __forceinline__ void load_pose(const ClassifyShared& s, int i, float t[3], float R[9], float R1[9]) {
 #pragma unroll
@@ -923,11 +949,14 @@ __device__ __forceinline__ int cta_compact(ClassifyShared& s, uint16_t* list, bo
   return total;
 }
 
+// Explain form (kWhy): s.valid stays 1 for every item in range, so every wave takes every item and every undecided box is
+// queued; a decided box sets its bits in s.why instead of clearing s.valid, and the word goes to w.why.
+template <bool kWhy>
 __global__ void __launch_bounds__(kClassifyItems, 16)
-classify_items_kernel(const Checker c, const Work w, BoxRec* __restrict__ recs_w, BoxRec* __restrict__ recs_f,
+classify_items_kernel(const Checker c, const WorkOf<kWhy> w, BoxRec* __restrict__ recs_w, BoxRec* __restrict__ recs_f,
                       BoxRec* __restrict__ recs_g, uint32_t* __restrict__ count_w, uint32_t* __restrict__ count_f,
                       uint32_t* __restrict__ count_g, int force_all) {   // force_all: every in-map box goes to the grouping stage (artp_set_mode 1)
-  __shared__ ClassifyShared s;
+  __shared__ std::conditional_t<kWhy, ClassifySharedWhy, ClassifyShared> s;
   const int tid = threadIdx.x;
   const uint32_t item0 = w.item_base + blockIdx.x * kClassifyItems;
   const bool in_range = item0 + tid < w.n_items;
@@ -947,6 +976,7 @@ classify_items_kernel(const Checker c, const Work w, BoxRec* __restrict__ recs_w
     for (int j = 0; j < 3; ++j) { s.pose[12 + j][tid] = -Rb[j]; s.pose[15 + j][tid] = Rb[6 + j]; s.pose[18 + j][tid] = Rb[3 + j]; }
   }
   s.valid[tid] = in_range ? 1 : 0;
+  if constexpr (kWhy) s.why[tid] = 0;
 #pragma unroll
   for (int k = 0; k < 5; ++k) s.pend[k][tid] = 0;
 
@@ -965,7 +995,8 @@ classify_items_kernel(const Checker c, const Work w, BoxRec* __restrict__ recs_w
       int r = box_geometry(c, R, R1, t, k, b);
       if (r == -1) r = zone_classify(c, b, k, force_all, fl);
       if (r == kBoxOutside || r == kBoxOutsideWindow) {
-        if (outside_fails(c, foot, r, true)) s.valid[i] = 0;
+        if constexpr (kWhy) s.why[i] |= (uint16_t)((1u << (8 + k)) | (outside_fails(c, foot, r, true) ? 1u << k : 0u));
+        else if (outside_fails(c, foot, r, true)) s.valid[i] = 0;
       } else if (r == -1) {
         // reach boxes go to their own queue (small TMA tiles); the torso -- and a reach box whose zone would not fit the
         // small tile -- to the big-tile queue
@@ -983,7 +1014,8 @@ classify_items_kernel(const Checker c, const Work w, BoxRec* __restrict__ recs_w
           s.probe_i[0][tid] = b.x0; s.probe_i[1][tid] = b.x1; s.probe_i[2][tid] = b.z0; s.probe_i[3][tid] = b.z1;
         }
       } else if (box_fails(foot, r)) {
-        s.valid[i] = 0;
+        if constexpr (kWhy) s.why[i] |= (uint16_t)(1u << k);
+        else s.valid[i] = 0;
       }
     }
     if (!foot) break;
@@ -1005,7 +1037,8 @@ classify_items_kernel(const Checker c, const Work w, BoxRec* __restrict__ recs_w
   const bool valid = s.valid[tid] != 0;
   if (in_range) {
     const uint32_t slot = item_slot(w, item0 + tid);
-    if (w.edge_mode) { if (!valid) w.valid[slot] = 0; }
+    if constexpr (kWhy) w.why[slot] = s.why[tid];
+    else if (w.edge_mode) { if (!valid) w.valid[slot] = 0; }
     else w.valid[slot] = (uint8_t)valid;
   }
   // records of the undecided boxes of valid items: per queue, 21-bit counts packed into one scan
@@ -1222,8 +1255,9 @@ groups_done:
 }
 
 constexpr int kBlockStageThreads = 256;   // threads per deferred box in the grouping stage
+template <bool kWhy>
 __global__ void __launch_bounds__(kBlockStageThreads)
-box_items_block_kernel(const Checker c, const Work w, const BoxRec* __restrict__ recs, const BoxRec* __restrict__ recs_f,
+box_items_block_kernel(const Checker c, const WorkOf<kWhy> w, const BoxRec* __restrict__ recs, const BoxRec* __restrict__ recs_f,
                        const uint32_t* __restrict__ defer_count, const uint32_t* __restrict__ defer_list, int T_cap,
                        uint32_t* __restrict__ overflow) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -1242,8 +1276,13 @@ box_items_block_kernel(const Checker c, const Work w, const BoxRec* __restrict__
     if (threadIdx.x == 0) {
       // a zone that does not fit the plane store cannot be decided: fail closed (item invalid) and raise the sticky
       // error word (mapped host memory; the host returns ARTP_E_LIMIT from the call / artp_poll_error)
-      if (res == R_DEFER) { *(volatile uint32_t*)overflow = 1u; w.valid[slot] = 0; }
-      else if (box_fails(foot, res)) w.valid[slot] = 0;
+      if constexpr (kWhy) {
+        if (res == R_DEFER) *(volatile uint32_t*)overflow = 1u;
+        if (res == R_DEFER || box_fails(foot, res)) why_set(w.why, slot, (int)(r.flags & 7));
+      } else {
+        if (res == R_DEFER) { *(volatile uint32_t*)overflow = 1u; w.valid[slot] = 0; }
+        else if (box_fails(foot, res)) w.valid[slot] = 0;
+      }
     }
     __syncthreads();
   }

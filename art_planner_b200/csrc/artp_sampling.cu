@@ -1,7 +1,7 @@
 // art_planner_b200/csrc/artp_sampling.cu -- the sampling half of the C ABI (include/artp.h): normals and the CDF, the
 // sampler (SE3FromSE2Sampler::sampleUniform) with its fused sample -> check -> compact path, the start / goal search,
-// poseFrom2D and the valid-heading layer, Basic's masking and the sampler's distribution. It reaches the validity pipeline through check_states_f32
-// (artp_internal.h).
+// poseFrom2D with the valid-heading and box-verdict layers, Basic's masking and the sampler's distribution. It reaches the
+// validity pipeline through check_states_f32 and box_verdicts_f32 (artp_internal.h).
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -163,12 +163,18 @@ int find_valid_near(Handle* h, const double* d_centres, size_t n, const double* 
 // ---------------------------------------------------------------------------------------------------------------
 // The valid-heading layer: isValid of the goal projection (planner.cpp:223-237) of every cell centre at each heading
 // ---------------------------------------------------------------------------------------------------------------
-// Argument checks shared by both forms, before any device work; the headings as the kernels take them into *hd.
-int heading_args(Handle* h, const double* yaw, int n_yaw, const uint32_t* mask, artp::Headings* hd) {
+// What the goal projection (poseFrom2D and the layers built on it) needs: the whole map, with its normals.
+int projection_map_args(Handle* h) {
   TRY(require_whole_map(h));
   if (!sampling(h).map.has_normals) {
     h->err = "no normal layers for this map (artp_estimate_normals or artp_set_sampler after artp_set_map)"; return ARTP_E_INVALID;
   }
+  return ARTP_OK;
+}
+
+// Argument checks shared by both forms, before any device work; the headings as the kernels take them into *hd.
+int heading_args(Handle* h, const double* yaw, int n_yaw, const uint32_t* mask, artp::Headings* hd) {
+  TRY(projection_map_args(h));
   if (n_yaw < 1 || n_yaw > artp::kMaxHeadings) { h->err = "n_yaw must lie in 1..32"; return ARTP_E_INVALID; }
   if (!yaw || !mask) return null_buffer(h);
   std::memset(hd, 0, sizeof(*hd));
@@ -197,6 +203,37 @@ int valid_heading_layer(Handle* h, const artp::Headings& hd, uint32_t* d_mask, c
     TRY(launch(h, artp::heading_poses_kernel, grid_for(h, n, 128), 128, 0, s, m, hd, c0, n, d_sf));
     TRY(check_states_f32(h, d_sf, n, d_val, s));
     TRY(launch(h, artp::heading_pack_kernel, grid_for(h, cells, 256), 256, 0, s, d_val, hd.n, c0, cells, d_mask));
+  }
+  return ARTP_OK;
+}
+
+// The box-verdict layer: the ARTP_BOX_* word of the same goal projection at one heading. The argument checks of both
+// forms, before any device work; the heading as heading_poses_kernel takes it into *hd.
+int box_layer_args(Handle* h, double yaw, const uint16_t* out, artp::Headings* hd) {
+  TRY(projection_map_args(h));
+  if (!std::isfinite(yaw)) { h->err = "yaw must be finite"; return ARTP_E_INVALID; }
+  if (!out) return null_buffer(h);
+  std::memset(hd, 0, sizeof(*hd));
+  hd->yaw[0] = (float)yaw;
+  hd->n = 1;
+  return ARTP_OK;
+}
+
+// The layer of the current map into d_out (rows x cols words) on s: one pose per cell, cell-major as the layer, in
+// chunks of at most kSampleChunk cells, each chunk's words written in place; arguments checked by box_layer_args.
+int box_verdict_layer(Handle* h, const artp::Headings& hd, uint16_t* d_out, cudaStream_t s) {
+  const size_t ncell = (size_t)h->rows * h->cols;
+  const size_t chunk = std::min(ncell, kSampleChunk);
+  char* r[1];   // states f32
+  Buf<char>& scratch = sampling(h).samp_scratch;
+  TRY(carve(h, scratch.p, scratch.cap, {chunk * 7 * sizeof(float)}, r));
+  float* d_sf = (float*)r[0];
+  artp::SamplerDev m{};
+  sampler_map_view(h, m);
+  for (size_t c0 = 0; c0 < ncell; c0 += chunk) {
+    const size_t n = std::min(chunk, ncell - c0);
+    TRY(launch(h, artp::heading_poses_kernel, grid_for(h, n, 128), 128, 0, s, m, hd, c0, n, d_sf));
+    TRY(box_verdicts_f32(h, d_sf, n, d_out + c0, s));
   }
   return ARTP_OK;
 }
@@ -747,10 +784,7 @@ int artp_ball_offsets(artp_handle* hh, uint64_t seed, uint64_t first_draw, size_
 
 int artp_pose_from_2d(artp_handle* hh, const double* states_in, size_t n, double* states_out, uint8_t* inside) {
   LOCK_CALL(h, hh);
-  TRY(require_whole_map(h));
-  if (!sampling(h).map.has_normals) {
-    h->err = "no normal layers for this map (artp_estimate_normals or artp_set_sampler after artp_set_map)"; return ARTP_E_INVALID;
-  }
+  TRY(projection_map_args(h));
   if (n == 0) return ARTP_OK;
   if (!states_in || !states_out) return null_buffer(h);
   char* r[3];   // states in | states out | inside
@@ -783,6 +817,29 @@ int artp_valid_heading_layer_device(artp_handle* hh, const double* yaw, int n_ya
   ChainScope cs(h, 0, s);
   if (cs.rc) return cs.rc;
   return valid_heading_layer(h, hd, d_mask, s);
+}
+
+int artp_box_verdict_layer(artp_handle* hh, double yaw, uint16_t* out) {
+  LOCK_CALL(h, hh);
+  artp::Headings hd;
+  TRY(box_layer_args(h, yaw, out, &hd));
+  const size_t bytes = (size_t)h->rows * h->cols * sizeof(uint16_t);
+  char* d_out;
+  TRY(host_call_begin(h, {bytes}, &d_out));
+  TRY(box_verdict_layer(h, hd, (uint16_t*)d_out, h->stream));
+  TRY(copy_async(h, out, d_out, bytes, cudaMemcpyDeviceToHost, h->stream));
+  return host_call_end(h, true);
+}
+
+int artp_box_verdict_layer_device(artp_handle* hh, double yaw, uint16_t* d_out, void* stream) {
+  LOCK_CALL(h, hh);
+  artp::Headings hd;
+  TRY(box_layer_args(h, yaw, d_out, &hd));
+  CU_TRY(h, cudaSetDevice(h->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  ChainScope cs(h, 0, s);
+  if (cs.rc) return cs.rc;
+  return box_verdict_layer(h, hd, d_out, s);
 }
 
 int artp_debug_circular_kernel(int size, uint8_t* out) {   // test hook: the size x size element as 0 / 1 bytes (row-major)

@@ -69,9 +69,11 @@ __device__ __forceinline__ unsigned char* warp_tile_slots(unsigned char* smem, c
 }
 
 // map0 / map1: tiles of `elevation` / `elevation_masked` (same tile extent). queue_bit tags defer-list entries.
+// Explain form (kWhy): no box is skipped for a dead item, and a failing box sets its bit of the item's word.
+template <bool kWhy>
 __global__ void __launch_bounds__(kMaxTileWarps * 32, 3)
 box_tiles_warp_kernel(const Checker c, const __grid_constant__ CUtensorMap map0, const __grid_constant__ CUtensorMap map1,
-                      const TileCfg tc, const Work w, const BoxRec* __restrict__ recs, const uint32_t* __restrict__ rec_count,
+                      const TileCfg tc, const WorkOf<kWhy> w, const BoxRec* __restrict__ recs, const uint32_t* __restrict__ rec_count,
                       uint32_t* __restrict__ work_counter, uint32_t* __restrict__ defer_count, uint32_t* __restrict__ defer_list,
                       uint32_t queue_bit, int force_defer) {
   extern __shared__ __align__(128) unsigned char tile_smem[];
@@ -132,8 +134,10 @@ box_tiles_warp_kernel(const Checker c, const __grid_constant__ CUtensorMap map0,
       const bool foot = (r.flags & 7) != 0;
       // another box of the item (or state of the edge) already failed: nothing can change the verdict (perf only)
       int dead = 0;
-      if (lane == 0) dead = (*(volatile const uint8_t*)(w.valid + slot_item) == 0);
-      dead = __shfl_sync(kFull, dead, 0);
+      if constexpr (!kWhy) {
+        if (lane == 0) dead = (*(volatile const uint8_t*)(w.valid + slot_item) == 0);
+        dead = __shfl_sync(kFull, dead, 0);
+      }
       mbar_wait(&bars[wid][slot], phase[slot]);       // the tile must land before its slot can be reused
       phase[slot] ^= 1u;
       if (dead) continue;
@@ -149,7 +153,10 @@ box_tiles_warp_kernel(const Checker c, const __grid_constant__ CUtensorMap map0,
       }
       if (lane == 0) {
         if (res == R_DEFER) defer_list[atomicAdd(defer_count, 1u)] = ri | queue_bit;
-        else if (box_fails(foot, res)) w.valid[slot_item] = 0;
+        else if (box_fails(foot, res)) {
+          if constexpr (kWhy) why_set(w.why, slot_item, (int)(r.flags & 7));
+          else w.valid[slot_item] = 0;
+        }
       }
     }
   }
@@ -169,8 +176,10 @@ box_tiles_warp_kernel(const Checker c, const __grid_constant__ CUtensorMap map0,
 constexpr int kGroupRounds = 8;      // a warp claims 4 * kGroupRounds records per atomic
 constexpr int kGroupTasks = 64;      // candidate (cell, triangle) tasks per box: 8 corners x 4 cells x 2
 
+// Explain form (kWhy): every record is alive, and a failing box sets its bit of the item's word.
+template <bool kWhy>
 __global__ void __launch_bounds__(kMaxTileWarps * 32, 3)
-reach_groups_kernel(const Checker c, const __grid_constant__ CUtensorMap map1, const TileCfg tc, const Work w,
+reach_groups_kernel(const Checker c, const __grid_constant__ CUtensorMap map1, const TileCfg tc, const WorkOf<kWhy> w,
                     const BoxRec* __restrict__ recs, const uint32_t* __restrict__ rec_count, uint32_t* __restrict__ work_counter) {
   extern __shared__ __align__(128) unsigned char tile_smem[];
   __shared__ uint64_t bars[kMaxTileWarps][2];
@@ -224,8 +233,12 @@ reach_groups_kernel(const Checker c, const __grid_constant__ CUtensorMap map1, c
       if (act) r = load_rec(recs + ri);
       if (round + 1 < nrounds) { __syncwarp(); prefetch(r0 + 4u * (uint32_t)(round + 1), slot ^ 1); }
       int alive = 0;
-      if (act && gl == 0) alive = (*(volatile const uint8_t*)(w.valid + r.item) != 0);
-      alive = __shfl_sync(kFull, alive, 0, 8);
+      if constexpr (kWhy) {
+        alive = act;
+      } else {
+        if (act && gl == 0) alive = (*(volatile const uint8_t*)(w.valid + r.item) != 0);
+        alive = __shfl_sync(kFull, alive, 0, 8);
+      }
       mbar_wait(&bars[wid][slot], (phase >> slot) & 1u);
       phase ^= 1u << slot;
       __syncwarp();                        // lanes leave the barrier poll at different times
@@ -356,7 +369,10 @@ reach_groups_kernel(const Checker c, const __grid_constant__ CUtensorMap map1, c
         hit_groups = __reduce_or_sync(kFull, hit_groups);
         if ((hit_groups >> g) & 1u) ghit = true;
       }
-      if (gl == 0 && act && alive && box_fails(true, ghit ? R_HIT : R_FREE)) w.valid[r.item] = 0;
+      if (gl == 0 && act && alive && box_fails(true, ghit ? R_HIT : R_FREE)) {
+        if constexpr (kWhy) why_set(w.why, r.item, (int)(r.flags & 7));
+        else w.valid[r.item] = 0;
+      }
       __syncwarp();
     }
   }

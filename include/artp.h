@@ -36,6 +36,10 @@
  *   artp_valid_heading_layer[_device]  no single reference call: per map cell and heading, whether Planner::plan accepts a
  *                                   goal there without moving it, i.e. isValid of artp_pose_from_2d's projection of the
  *                                   cell centre (GoalStateRegion's search moves x and y only, goal.cpp:11-41)
+ *   artp_box_verdicts[_device]      no single reference call: why isValid (validity_checker.cpp:39-45) fails -- each of its
+ *                                   five boxes decided on its own, ValidityCheckerBody::isValid (validity_checker_body.cpp:
+ *                                   27-42) for the torso and boxIsValidAtPose (validity_checker_feet.cpp:32-70) per foot
+ *   artp_box_verdict_layer[_device] the same words for artp_pose_from_2d's projection of every cell centre at one heading
  *   artp_estimate_normals           art_planner::estimateNormals (src/utils.cpp:213-324; processors::Basic, basic.cpp:47)
  *   artp_compute_sample_cdf         computeCumulativeProbabilityDistribution
  *                                   (src/map/processors/probability_distribution.cpp:20-46)
@@ -133,6 +137,32 @@ void  artp_host_free(void* p);
  * first; results are identical to the double entry points at half the host<->device traffic. */
 int artp_check_poses_f32(artp_handle* h, const float* states, size_t n, uint8_t* valid);
 int artp_check_poses_f32_device(artp_handle* h, const float* d_states, size_t n, uint8_t* d_valid, void* stream);
+
+/* Box verdicts: why a state passes or fails isValid. For state s the five boxes are those isValid places, in its order:
+ * k = 0 the torso box at s * (torso offset), k = 1..4 the reach boxes at the foot offsets (+,+), (+,-), (-,+), (-,-), all
+ * with the one rotation dBodySetRotation orthogonalises for them. why[i] is a word of
+ *   bit k      (ARTP_BOX_FAILS(k))    box k fails. The torso: its centre is on the map (grid_map isInside) and
+ *                                     dCollide(torso, elevation) != 0. A reach box: its centre is on the map and
+ *                                     dCollide(reach, elevation_masked) == 0, or it is off the map and
+ *                                     unknown_space_untraversable is set.
+ *   bit 8 + k  (ARTP_BOX_OUTSIDE(k))  box k's centre is off the map (isInside false), whatever bit k says.
+ * and 0 in every other bit. Every box is decided (no short-circuit), so (why[i] & ARTP_BOX_FAIL_MASK) == 0 exactly when
+ * artp_check_poses reports state i valid, and the lowest set fail bit is the box where isValid's && chain stops. A box
+ * whose zone exceeds the plane-grouping store counts as failing and the call returns ARTP_E_LIMIT, as artp_check_poses
+ * does (the _device form through artp_poll_error). states: n x 7 doubles as artp_check_poses takes them.
+ * ARTP_E_NOMAP without a map; ARTP_E_INVALID on a map window (a whole-map diagnostic) and for a NULL buffer (n > 0).
+ * artp_box_verdicts: HOST buffers. _device: DEVICE buffers, asynchronous on `stream`. The planner never calls these. */
+#define ARTP_BOX_TORSO        0
+#define ARTP_BOX_FOOT_PP      1   /* reach box at (+feet_off_x, +feet_off_y) */
+#define ARTP_BOX_FOOT_PM      2   /* (+, -) */
+#define ARTP_BOX_FOOT_MP      3   /* (-, +) */
+#define ARTP_BOX_FOOT_MM      4   /* (-, -) */
+#define ARTP_BOX_FAILS(k)     (1u << (k))
+#define ARTP_BOX_OUTSIDE(k)   (1u << (8 + (k)))
+#define ARTP_BOX_FAIL_MASK    0x001Fu
+#define ARTP_BOX_OUTSIDE_MASK 0x1F00u
+int artp_box_verdicts(artp_handle* h, const double* states, size_t n, uint16_t* why);
+int artp_box_verdicts_device(artp_handle* h, const double* d_states, size_t n, uint16_t* d_why, void* stream);
 
 /* Edge validity: valid(s2) && valid(interp(s1,s2,j/(n_steps+1))) for j = 1..n_steps (n_steps >= 0). */
 int artp_check_motions(artp_handle* h, const double* s1, const double* s2, size_t n, int n_steps, uint8_t* valid);
@@ -264,6 +294,15 @@ int artp_pose_from_2d(artp_handle* h, const double* states_in, size_t n, double*
  * artp_valid_heading_layer: mask is a HOST buffer. _device: d_mask is a DEVICE buffer, written on `stream`. */
 int artp_valid_heading_layer(artp_handle* h, const double* yaw, int n_yaw, uint32_t* mask);
 int artp_valid_heading_layer_device(artp_handle* h, const double* yaw, int n_yaw, uint32_t* d_mask, void* stream);
+/* The box-verdict layer: why a goal at each cell of the current map fails at one heading. out[r + c * rows] (grid_map
+ * layout, rows x cols words) is the artp_box_verdicts word of the pose artp_pose_from_2d makes from the centre of cell
+ * (r, c) with getYawFromSO3 = (float)yaw: the pose artp_valid_heading_layer checks, so (out & ARTP_BOX_FAIL_MASK) == 0
+ * exactly where that layer's bit for the same single yaw is set. Maps of any size (up to 4000 x 4000 measured) run in
+ * chunks. ARTP_E_NOMAP without a map; ARTP_E_INVALID on a map window, without normals, for a non-finite yaw or a NULL
+ * buffer, all before any device work; ARTP_E_LIMIT as artp_box_verdicts.
+ * artp_box_verdict_layer: out is a HOST buffer. _device: d_out is a DEVICE buffer, written on `stream`. */
+int artp_box_verdict_layer(artp_handle* h, double yaw, uint16_t* out);
+int artp_box_verdict_layer_device(artp_handle* h, double yaw, uint16_t* d_out, void* stream);
 
 /* PathLengthObjective::motionCost for n edges -> cost[n] (double). */
 int artp_path_length_cost(artp_handle* h, const double* s1, const double* s2, size_t n, double* cost);

@@ -173,6 +173,16 @@ class StateValidityChecker {
     handle_->check(artp_check_poses_f32(handle_->get(), buf.data(), states.size(), valid->data()), "artp_check_poses_f32");
   }
 
+  // Why each state passes or fails isValid (artp_box_verdicts): one word per state, bit k set when box k fails (0 torso,
+  // 1..4 the reach boxes), bit 8 + k when box k's centre is off the map (ARTP_BOX_*). (word & ARTP_BOX_FAIL_MASK) == 0
+  // exactly where isValid is true. The lowest fail bit is the box where isValid stops.
+  std::vector<uint16_t> boxVerdicts(const std::vector<State>& states) const {
+    std::vector<uint16_t> why(states.size());
+    if (states.empty()) return why;
+    handle_->check(artp_box_verdicts(handle_->get(), &states[0].x, states.size(), why.data()), "artp_box_verdicts");
+    return why;
+  }
+
   // computeCumulativeProbabilityDistribution (probability_distribution.cpp:20-46) on the device: fills the map's cum_prob /
   // cum_prob_rowwise layers from `sample_probability` (rows x cols, column-major) and keeps them resident for the sampler.
   void computeSampleCdf(const std::vector<float>& sample_probability) {
@@ -268,6 +278,15 @@ class StateValidityChecker {
     handle_->check(artp_valid_heading_layer(handle_->get(), yaws.data(), static_cast<int>(yaws.size()), mask.data()),
                    "artp_valid_heading_layer");
     return mask;
+  }
+
+  // The box-verdict layer (artp_box_verdict_layer): per cell of the map (rows x cols, column-major), the boxVerdicts word
+  // of a goal at the cell's centre with yaw `yaw` once projected onto the map. Needs the map's normals (estimateNormals).
+  std::vector<uint16_t> boxVerdictLayer(double yaw) const {
+    if (!map_) throw std::runtime_error("boxVerdictLayer: no map");
+    std::vector<uint16_t> words(static_cast<size_t>(map_->rows) * map_->cols);
+    handle_->check(artp_box_verdict_layer(handle_->get(), yaw, words.data()), "artp_box_verdict_layer");
+    return words;
   }
 
   const HandlePtr& handle() const { return handle_; }
