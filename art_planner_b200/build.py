@@ -9,10 +9,10 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libartp.so")
 # (source, extra flags): the geometric kernels need bit-exact fp32 (no FMA contraction, SURVEY.md section 7);
 # the motion-cost network does not.
-# The six units of the C ABI all build rows, costs and states that must equal the host's bit for bit.
+# The eight units built with these flags all build heights, rows, costs and states that must equal the host's bit for bit.
 GEOMETRY_FLAGS = ["-fmad=false", "-Xcompiler", "-fPIC,-ffp-contract=off"]
-SOURCES = [("artp_capi.cu", GEOMETRY_FLAGS), ("artp_sampling.cu", GEOMETRY_FLAGS), ("artp_cost.cu", GEOMETRY_FLAGS),
-           ("artp_roadmap.cu", GEOMETRY_FLAGS), ("artp_path_simplify.cu", GEOMETRY_FLAGS),
+SOURCES = [("artp_capi.cu", GEOMETRY_FLAGS), ("artp_map.cu", GEOMETRY_FLAGS), ("artp_sampling.cu", GEOMETRY_FLAGS),
+           ("artp_cost.cu", GEOMETRY_FLAGS), ("artp_roadmap.cu", GEOMETRY_FLAGS), ("artp_path_simplify.cu", GEOMETRY_FLAGS),
            ("artp_planner.cu", GEOMETRY_FLAGS), ("artp_inpaint.cu", GEOMETRY_FLAGS),
            ("artp_cnn.cu", ["-Xcompiler", "-fPIC"])]
 HEADERS = ["artp_internal.h", "artp_device.cuh", "artp_kernels.cuh", "artp_sampler.cuh", "artp_tiles.cuh", "artp_basic.cuh",

@@ -1049,7 +1049,8 @@ int artp_api::update_features(Handle* h, const float* d_layer, int rows, int col
 int artp_api::map_features(Handle* h) {
   // The resolution as artp_set_map received it: the head's row / column bias truncates (rows * res) / res like the
   // reference, and Lx / rows may differ from res in the last bit, which moves that truncation (e.g. 116 rows at 0.04).
-  return update_features(h, h->d_H[0], h->rows, h->cols, h->pitch, h->res, h->chk.cx, h->chk.cy, h->stream);
+  return update_features(h, h->map.H[0], h->map.rows, h->map.cols, h->map.pitch, h->map.res, h->chk.cx, h->chk.cy,
+                         h->stream);
 }
 
 int artp_api::cost_head(Handle* h, const float* d_edges, size_t n, float* d_cost3, cudaStream_t st) {

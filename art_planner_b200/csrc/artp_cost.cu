@@ -142,6 +142,41 @@ __global__ void split_reduce_kernel(const float* __restrict__ cost3, const uint3
   }
 }
 
+// MotionCostObjective::motionCost's split of the n - 1 edges of a path (artp::cost_pieces); off = their exclusive prefix
+// sums (n entries, the last = total).
+// res[0] = the total (64 bits), res[1] = 1 when an edge has 2^32 pieces or more. One CTA.
+constexpr int kOffThreads = 1024;
+__global__ void __launch_bounds__(kOffThreads)
+piece_offsets_kernel(const double* __restrict__ st, size_t n, double mql, uint32_t* __restrict__ off,
+                     unsigned long long* __restrict__ res) {
+  __shared__ unsigned long long part[kOffThreads];
+  __shared__ int bad;
+  const size_t ne = n - 1, per = (ne + kOffThreads - 1) / kOffThreads;
+  const size_t e0 = threadIdx.x * per, e1 = min(ne, e0 + per);
+  if (threadIdx.x == 0) bad = 0;
+  __syncthreads();
+  auto pieces = [&](size_t e) -> unsigned long long {
+    const uint64_t p = artp::cost_pieces(st + 7 * e, st + 7 * (e + 1), mql);
+    if (!p) bad = 1;
+    return p;
+  };
+  unsigned long long sum = 0;
+  for (size_t e = e0; e < e1; ++e) sum += pieces(e);
+  part[threadIdx.x] = sum;
+  __syncthreads();
+  if (threadIdx.x == 0) {   // exclusive scan of the 1024 chunk sums
+    unsigned long long run = 0;
+    for (int t = 0; t < kOffThreads; ++t) { const unsigned long long v = part[t]; part[t] = run; run += v; }
+    res[0] = run;
+    off[ne] = (uint32_t)run;
+  }
+  __syncthreads();
+  unsigned long long run = part[threadIdx.x];
+  for (size_t e = e0; e < e1; ++e) { off[e] = (uint32_t)run; run += pieces(e); }
+  __syncthreads();
+  if (threadIdx.x == 0) res[1] = bad;
+}
+
 }  // namespace
 
 int artp_api::path_length_cost(Handle* h, const double* d_s1, const double* d_s2, size_t n, double* d_cost, cudaStream_t s) {
@@ -171,6 +206,20 @@ int artp_api::cost_piece_offsets(Handle* h, const double* s1, const double* s2, 
   }
   off[n] = (uint32_t)t;
   *total = t;
+  return ARTP_OK;
+}
+
+int artp_api::piece_offsets(Handle* h, const double* d_states, size_t n, double max_query_edge_length, uint32_t* d_off,
+                            size_t* total, cudaStream_t s) {
+  char* r[1];
+  TRY(carve(h, h->d_stage, h->stage_cap, {2 * sizeof(unsigned long long)}, r));
+  TRY(launch(h, piece_offsets_kernel, 1, kOffThreads, 0, s, d_states, n, max_query_edge_length, d_off, (unsigned long long*)r[0]));
+  unsigned long long res[2];
+  TRY(copy_async(h, res, r[0], sizeof(res), cudaMemcpyDeviceToHost, s));
+  TRY(sync_stream(h, s));
+  if (res[1]) { h->err = "path edge too long for the learned cost"; return ARTP_E_INVALID; }
+  if (res[0] > 0xFFFFFFFFull) { h->err = "too many cost pieces (>= 2^32)"; return ARTP_E_INVALID; }
+  *total = (size_t)res[0];
   return ARTP_OK;
 }
 

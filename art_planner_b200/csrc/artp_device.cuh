@@ -1,7 +1,8 @@
 // art_planner_b200/csrc/artp_device.cuh
-// Exact fp32 building blocks of the box-vs-heightfield decision, shared by the warp kernel and the
-// block-level grouping kernel. Arithmetic contract (SURVEY.md Appendix A): IEEE fp32, round-to-nearest,
-// NO FMA contraction, left-to-right association exactly as the reference's ODE source writes it.
+// Exact fp32 building blocks of the box-vs-heightfield decision, shared by the warp kernel, the
+// block-level grouping kernel and the map's plane tables (artp_map.cu). Arithmetic contract (SURVEY.md
+// Appendix A): IEEE fp32, round-to-nearest, NO FMA contraction, left-to-right association exactly as the
+// reference's ODE source writes it.
 // This translation unit is compiled with -fmad=false and default -prec-div/-prec-sqrt/-ftz=false;
 // 1/sqrt is spelled as two correctly rounded operations (ode/include/ode/common.h:285).
 #pragma once
@@ -462,5 +463,27 @@ __device__ __forceinline__ bool on_tri(const Field& f, bool isUp, int cx, int cz
 }
 
 __device__ __forceinline__ bool finitef(float h) { return fabsf(h) < CUDART_INF_F; }   // no NaN by contract
+
+// Heights of the four corners of cell (cx, cz): A(x,z) B(x+1,z) C(x,z+1) D(x+1,z+1).
+__device__ __forceinline__ void load_cell(const Field& f, int cx, int cz, float& hA, float& hB, float& hC, float& hD) {
+  const float* p = f.H + (size_t)cz * f.pitch + cx;
+  hA = __ldg(p); hB = __ldg(p + 1); hC = __ldg(p + f.pitch); hD = __ldg(p + f.pitch + 1);
+}
+
+// Exact plane of the Up / Down triangle of cell (cx, cz).
+__device__ __forceinline__ void cell_plane(const Field& f, bool isUp, int cx, int cz, float hA, float hB, float hC,
+                                           float hD, float pl[4]) {
+  const float xA = cx * f.sW, xB = (cx + 1) * f.sW, zA = cz * f.sD, zC = (cz + 1) * f.sD;
+  // (A, B, C) or (D, B, C): one instruction stream for both (lanes holding an Up and a Down triangle do not diverge)
+  tri_plane(isUp, isUp ? xA : xB, isUp ? hA : hD, isUp ? zA : zC, xB, hB, zA, xA, hC, zC, pl);
+}
+
+// Bucket keys of the plane screens and of the map's plane tables: nkey buckets a normal component (n0 or n2, in [-1, 1]),
+// dkey a plane offset d. A key shifted by a margin is the key of the shifted component, e.g. nkey(n0 - kKeyMargin).
+constexpr float kKeyScale = 16384.0f;   // bucket width 2^-14 on n0, n2 in [-1, 1]
+constexpr float kKeyMargin = 4e-6f;     // > eps + rsqrt.approx error + quantisation error (see DESIGN.md)
+constexpr float kDScale = 524288.0f;    // bucket width 2^-19 on d (> 2 eps, so |d_m - d_c| < eps spans <= 2 buckets)
+__device__ __forceinline__ int nkey(float n) { return (int)floorf((n + 1.0f) * kKeyScale); }
+__device__ __forceinline__ int dkey(float d) { return (int)floorf(fminf(fmaxf(d, -2000.0f), 2000.0f) * kDScale); }
 
 }  // namespace artp

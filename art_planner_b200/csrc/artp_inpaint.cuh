@@ -66,7 +66,7 @@ __device__ __forceinline__ uint8_t to_u8(float x, float a, float b) {   // satur
   return (uint8_t)min(255, max(0, r));
 }
 
-// min / max from finite_min_max's keys (artp_planner.cu)
+// min / max from finite_min_max's keys (artp_map.cu)
 __device__ __forceinline__ float key_to_float(uint32_t key) {
   return __uint_as_float((key & 0x80000000u) ? (key & 0x7FFFFFFFu) : ~key);
 }

@@ -99,14 +99,6 @@ __device__ __forceinline__ uint32_t magic_for(int n) {
   return n <= 1 ? 0u : (n <= 128 ? kMagicTab.v[n] : 0xFFFFFFFFu / (uint32_t)n + 1u);
 }
 
-// Bucket keys of the plane screens and of the map's plane tables: nkey buckets a normal component (n0 or n2, in [-1, 1]),
-// dkey a plane offset d. A key shifted by a margin is the key of the shifted component, e.g. nkey(n0 - kKeyMargin).
-constexpr float kKeyScale = 16384.0f;   // bucket width 2^-14 on n0, n2 in [-1, 1]
-constexpr float kKeyMargin = 4e-6f;     // > eps + rsqrt.approx error + quantisation error (see DESIGN.md)
-constexpr float kDScale = 524288.0f;    // bucket width 2^-19 on d (> 2 eps, so |d_m - d_c| < eps spans <= 2 buckets)
-__device__ __forceinline__ int nkey(float n) { return (int)floorf((n + 1.0f) * kKeyScale); }
-__device__ __forceinline__ int dkey(float d) { return (int)floorf(fminf(fmaxf(d, -2000.0f), 2000.0f) * kDScale); }
-
 // EDGE-mode state j of the edge (s1, s2) with `steps` interior steps: s2 itself for j == 0, else
 // interpolate(s1, s2, j / (steps + 1)).
 __device__ __forceinline__ void edge_state(const double* s1, const double* s2, uint32_t j, int steps, double s[7]) {
@@ -156,20 +148,6 @@ __device__ __forceinline__ void load_item_state(const Work& w, uint32_t item, do
 
 __device__ __forceinline__ uint32_t item_slot(const Work& w, uint32_t item) {
   return w.edge_mode ? item / ((uint32_t)w.steps + 1u) : item;
-}
-
-// Heights of the four corners of cell (cx, cz): A(x,z) B(x+1,z) C(x,z+1) D(x+1,z+1).
-__device__ __forceinline__ void load_cell(const Field& f, int cx, int cz, float& hA, float& hB, float& hC, float& hD) {
-  const float* p = f.H + (size_t)cz * f.pitch + cx;
-  hA = __ldg(p); hB = __ldg(p + 1); hC = __ldg(p + f.pitch); hD = __ldg(p + f.pitch + 1);
-}
-
-// Exact plane of the Up / Down triangle of cell (cx, cz).
-__device__ __forceinline__ void cell_plane(const Field& f, bool isUp, int cx, int cz, float hA, float hB, float hC,
-                                           float hD, float pl[4]) {
-  const float xA = cx * f.sW, xB = (cx + 1) * f.sW, zA = cz * f.sD, zC = (cz + 1) * f.sD;
-  // (A, B, C) or (D, B, C): one instruction stream for both (lanes holding an Up and a Down triangle do not diverge)
-  tri_plane(isUp, isUp ? xA : xB, isUp ? hA : hD, isUp ? zA : zC, xB, hB, zA, xA, hC, zC, pl);
 }
 
 // The collider's rules for one cell (heightfield.cpp:1306-1441) against a box bottom minB: a vertex collides when it is

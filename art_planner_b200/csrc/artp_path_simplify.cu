@@ -20,6 +20,15 @@
 
 #include "artp_internal.h"
 
+namespace artp_api {
+
+struct Simplify {
+  char* d_scratch = nullptr;   // the control block, state pool, path and round buffers of a call (carve)
+  size_t cap = 0;
+};
+
+}  // namespace artp_api
+
 using namespace artp_api;
 
 namespace {
@@ -712,6 +721,13 @@ int artp_simplify_path(artp_handle* hh, const double* path, size_t n, const artp
 
 }  // extern "C"
 
+void artp_api::simplify_free(Handle* h) {
+  if (!h->simplify) return;
+  cudaFree(h->simplify->d_scratch);
+  delete h->simplify;
+  h->simplify = nullptr;
+}
+
 int artp_api::simplify_path(Handle* h, const double* path, const double* d_path, size_t n, const artp_se3_space* space,
                             int objective, double max_query_edge_length, uint64_t seed, double* out, size_t capacity,
                             size_t* n_out, artp_simplify_info* info) {
@@ -739,7 +755,8 @@ int artp_api::simplify_path(Handle* h, const double* path, const double* d_path,
   d.pcap = (uint32_t)(512 * n + 64);
   const size_t pairs = n * (n - 1) / 2 + 1;
   char* r[14];
-  TRY(carve(h, h->d_simplify, h->simplify_cap,
+  if (!h->simplify) h->simplify = new Simplify();
+  TRY(carve(h, h->simplify->d_scratch, h->simplify->cap,
             {sizeof(SimpCtl), (size_t)d.pcap * 7 * sizeof(double), (size_t)d.ncap * sizeof(uint32_t),
              (size_t)d.ncap * sizeof(uint32_t), (size_t)d.ncap * sizeof(uint32_t), pairs * sizeof(double),
              (size_t)d.ncap * sizeof(double), kAttempts * sizeof(Att), kBatch * 14 * sizeof(double),

@@ -1,11 +1,10 @@
 // art_planner_b200/csrc/artp_planner.cu -- Planner::setMap and Planner::plan + getSolutionPath for prm_motion_cost
 // (art_planner/src/planner.cpp:135-298) as two calls of the C ABI (include/artp.h): artp_planner_set_map and artp_plan.
 // The stages are the ones the public entry points run (their bodies without the lock, artp_internal.h); between them every
-// layer, state and path stays in device memory. The kernels here are the pieces no entry point had: the finite range of a
-// layer, the "observed" layer, the goal's bounds clip, the endpoints' check and the learned cost's piece offsets.
+// layer, state and path stays in device memory. The kernels here are the planner's own: the "observed" layer and the
+// goal's bounds clip.
 #include <cfloat>
 #include <cmath>
-#include <cstring>
 
 #include "artp_internal.h"
 
@@ -36,40 +35,6 @@ enum : size_t {
   QB_START = 0, QB_GOAL = 7, QB_CLIPPED = 14, QB_PROJECTED = 21, QB_REPAIRED = 28 /* start, goal: 14 */, QB_RADIUS = 42,
   QB_FLAGS = 44 /* inside byte, clipped byte, two int32 ball indices */, QB_MINMAX = 46, QB_SIZE = 64
 };
-
-__device__ __forceinline__ uint32_t float_key(float f) {   // order-preserving: a < b <=> key(a) < key(b)
-  const uint32_t u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
-// minCoeffOfFinites / maxCoeffOfFinites: min and max over the finite cells, -0 taken as +0 (the two compare equal).
-__global__ void finite_min_max_kernel(const float* __restrict__ a, size_t n, uint32_t* __restrict__ out) {
-  uint32_t lo = 0xFFFFFFFFu, hi = 0u, cnt = 0u;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const float v = a[i] + 0.0f;
-    if (fabsf(v) < CUDART_INF_F) { const uint32_t k = float_key(v); lo = min(lo, k); hi = max(hi, k); ++cnt; }
-  }
-  lo = __reduce_min_sync(0xFFFFFFFFu, lo);
-  hi = __reduce_max_sync(0xFFFFFFFFu, hi);
-  cnt = __reduce_add_sync(0xFFFFFFFFu, cnt);
-  if ((threadIdx.x & 31) == 0 && cnt) { atomicMin(out, lo); atomicMax(out + 1, hi); atomicAdd(out + 2, cnt); }
-}
-
-// out[0] = 1 when a cell is NaN or +-inf, out[1] = 1 when a cell is +-inf (both zeroed first).
-__global__ void nonfinite_any_kernel(const float* __restrict__ a, size_t n, uint32_t* __restrict__ out) {
-  uint32_t nonfinite = 0u, inf = 0u;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const float v = fabsf(a[i]);
-    nonfinite |= !(v < CUDART_INF_F);
-    inf |= v == CUDART_INF_F;
-  }
-  nonfinite = __reduce_or_sync(0xFFFFFFFFu, nonfinite);
-  inf = __reduce_or_sync(0xFFFFFFFFu, inf);
-  if ((threadIdx.x & 31) == 0) {
-    if (nonfinite) atomicOr(out, 1u);
-    if (inf) atomicOr(out + 1, 1u);
-  }
-}
 
 // addKnownCells (basic.cpp:25-38): observed = 1 where every basic layer ({elevation, traversability}, map.cpp:16) is finite
 // (grid_map's isValid). A missing traversability layer is checkTraversability's 1.0 (basic.cpp:13-21), written to trav_fill.
@@ -110,55 +75,6 @@ __global__ void goal_clip_kernel(const double* __restrict__ in, artp_se3_space s
   }
   for (int k = 0; k < 7; ++k) out[k] = s[k];
   *clipped = ok ? 0 : 1;
-}
-
-// artp_roadmap_solve's checks of its endpoints, on the device: any non-finite state (-1), then start, then goal outside
-// the bounds (no slack: the position inside the RealVectorBounds); then both (x, y).
-__global__ void endpoint_check_kernel(const double* __restrict__ sg, artp_se3_space sp, double* __restrict__ out) {
-  double verdict = 0.0;
-  for (int k = 0; k < 14; ++k)
-    if (!isfinite(sg[k])) verdict = -1.0;
-  if (verdict == 0.0)
-    for (int w = 0; w < 2 && verdict == 0.0; ++w)
-      for (int i = 0; i < 3; ++i)
-        if (sg[7 * w + i] < sp.low[i] || sg[7 * w + i] > sp.high[i]) { verdict = w ? ARTP_SOLVE_INVALID_GOAL : ARTP_SOLVE_INVALID_START; break; }
-  out[0] = verdict;
-  out[1] = sg[0]; out[2] = sg[1]; out[3] = sg[7]; out[4] = sg[8];
-}
-
-// MotionCostObjective::motionCost's split of the n - 1 edges of a path (artp::cost_pieces); off = their exclusive prefix
-// sums (n entries, the last = total).
-// res[0] = the total (64 bits), res[1] = 1 when an edge has 2^32 pieces or more. One CTA.
-constexpr int kOffThreads = 1024;
-__global__ void __launch_bounds__(kOffThreads)
-piece_offsets_kernel(const double* __restrict__ st, size_t n, double mql, uint32_t* __restrict__ off,
-                     unsigned long long* __restrict__ res) {
-  __shared__ unsigned long long part[kOffThreads];
-  __shared__ int bad;
-  const size_t ne = n - 1, per = (ne + kOffThreads - 1) / kOffThreads;
-  const size_t e0 = threadIdx.x * per, e1 = min(ne, e0 + per);
-  if (threadIdx.x == 0) bad = 0;
-  __syncthreads();
-  auto pieces = [&](size_t e) -> unsigned long long {
-    const uint64_t p = artp::cost_pieces(st + 7 * e, st + 7 * (e + 1), mql);
-    if (!p) bad = 1;
-    return p;
-  };
-  unsigned long long sum = 0;
-  for (size_t e = e0; e < e1; ++e) sum += pieces(e);
-  part[threadIdx.x] = sum;
-  __syncthreads();
-  if (threadIdx.x == 0) {   // exclusive scan of the 1024 chunk sums
-    unsigned long long run = 0;
-    for (int t = 0; t < kOffThreads; ++t) { const unsigned long long v = part[t]; part[t] = run; run += v; }
-    res[0] = run;
-    off[ne] = (uint32_t)run;
-  }
-  __syncthreads();
-  unsigned long long run = part[threadIdx.x];
-  for (size_t e = e0; e < e1; ++e) { off[e] = (uint32_t)run; run += pieces(e); }
-  __syncthreads();
-  if (threadIdx.x == 0) res[1] = bad;
 }
 
 int planner_status(int32_t solve_status) {   // planner.cpp:254-261
@@ -212,42 +128,6 @@ int record(Handle* h, PlannerState* st, int i) {
 }
 
 }  // namespace
-
-int artp_api::finite_min_max(Handle* h, const float* d_layer, size_t n, uint32_t* d_out, cudaStream_t s) {
-  CU_TRY(h, cudaMemsetAsync(d_out, 0xFF, sizeof(uint32_t), s));
-  CU_TRY(h, cudaMemsetAsync(d_out + 1, 0, 2 * sizeof(uint32_t), s));
-  return launch(h, finite_min_max_kernel, grid_for(h, n, 256, 8), 256, 0, s, d_layer, n, d_out);
-}
-
-int artp_api::nonfinite_any(Handle* h, const float* d_layer, size_t n, uint32_t* d_out, cudaStream_t s) {
-  CU_TRY(h, cudaMemsetAsync(d_out, 0, 2 * sizeof(uint32_t), s));
-  return launch(h, nonfinite_any_kernel, grid_for(h, n, 256, 8), 256, 0, s, d_layer, n, d_out);
-}
-
-float artp_api::key_float(uint32_t key) {
-  const uint32_t u = (key & 0x80000000u) ? (key & 0x7FFFFFFFu) : ~key;
-  float f;
-  std::memcpy(&f, &u, sizeof(f));
-  return f;
-}
-
-int artp_api::endpoint_check(Handle* h, const double* d_sg, const artp_se3_space* space, double* d_out, cudaStream_t s) {
-  return launch(h, endpoint_check_kernel, 1, 1, 0, s, d_sg, *space, d_out);
-}
-
-int artp_api::piece_offsets(Handle* h, const double* d_states, size_t n, double max_query_edge_length, uint32_t* d_off,
-                            size_t* total, cudaStream_t s) {
-  char* r[1];
-  TRY(carve(h, h->d_stage, h->stage_cap, {2 * sizeof(unsigned long long)}, r));
-  TRY(launch(h, piece_offsets_kernel, 1, kOffThreads, 0, s, d_states, n, max_query_edge_length, d_off, (unsigned long long*)r[0]));
-  unsigned long long res[2];
-  TRY(copy_async(h, res, r[0], sizeof(res), cudaMemcpyDeviceToHost, s));
-  TRY(sync_stream(h, s));
-  if (res[1]) { h->err = "path edge too long for the learned cost"; return ARTP_E_INVALID; }
-  if (res[0] > 0xFFFFFFFFull) { h->err = "too many cost pieces (>= 2^32)"; return ARTP_E_INVALID; }
-  *total = (size_t)res[0];
-  return ARTP_OK;
-}
 
 void artp_api::planner_free(Handle* h) {
   PlannerState* st = h->planner;
@@ -361,7 +241,7 @@ int set_map(Handle* h, const artp_planner_params* pp, const float* elevation, co
   // cost server's preparation of the raw one
   if (cost_network(h) >= 0) {
     CU_TRY(h, cudaSetDevice(h->device));
-    if (cost_map) TRY(cost_map_features(h, raw_e, rows, cols, d_mm + 8, mm[8 + 3] != 0, h->res, h->chk.cx, h->chk.cy, h->stream));
+    if (cost_map) TRY(cost_map_features(h, raw_e, rows, cols, d_mm + 8, mm[8 + 3] != 0, h->map.res, h->chk.cx, h->chk.cy, h->stream));
     else TRY(map_features(h));
   }
   st->space = sp;
@@ -414,7 +294,9 @@ int artp_plan(artp_handle* hh, const artp_planner_params* pp, const double* star
   artp_plan_info o{};
   o.solve.path_vertices = info ? info->solve.path_vertices : nullptr;
   o.start_index = o.goal_index = -1;
-  if (h->has_map && h->win_rows != h->rows) { h->err = "not available on a map window (artp_set_map_window)"; return ARTP_E_INVALID; }
+  if (h->map.has_map && h->map.win_rows != h->map.rows) {
+    h->err = "not available on a map window (artp_set_map_window)"; return ARTP_E_INVALID;
+  }
   if (!h->planner_map) {                                   // planner.cpp:197-200
     o.status = ARTP_PLANNER_NO_MAP;
     if (info) *info = o;

@@ -120,6 +120,20 @@ int stopped_full(Handle* h, const Roadmap* r) {
   return ARTP_OK;
 }
 
+// artp_roadmap_solve's checks of its endpoints, on the device: any non-finite state (-1), then start, then goal outside
+// the bounds (no slack: the position inside the RealVectorBounds); then both (x, y).
+__global__ void endpoint_check_kernel(const double* __restrict__ sg, artp_se3_space sp, double* __restrict__ out) {
+  double verdict = 0.0;
+  for (int k = 0; k < 14; ++k)
+    if (!isfinite(sg[k])) verdict = -1.0;
+  if (verdict == 0.0)
+    for (int w = 0; w < 2 && verdict == 0.0; ++w)
+      for (int i = 0; i < 3; ++i)
+        if (sg[7 * w + i] < sp.low[i] || sg[7 * w + i] > sp.high[i]) { verdict = w ? ARTP_SOLVE_INVALID_GOAL : ARTP_SOLVE_INVALID_START; break; }
+  out[0] = verdict;
+  out[1] = sg[0]; out[2] = sg[1]; out[3] = sg[7]; out[4] = sg[8];
+}
+
 // The call's end: the control block back to the host with the stop rules off, then host_call_end.
 int finish(Handle* h, Roadmap* r, int rc) {
   const int rc_end = host_call_end(h, true);
@@ -217,7 +231,7 @@ int artp_api::roadmap_sample_graph(Handle* h, const artp_roadmap_params* rp, con
   }
   Roadmap* r = h->roadmap;
   // every sampled milestone lies on the map (the sampler's map_cell test)
-  const double Lx = h->rows * h->res, Ly = h->cols * h->res;
+  const double Lx = h->map.rows * h->map.res, Ly = h->map.cols * h->map.res;
   grow_box(r, h->chk.cx - 0.5 * Lx, h->chk.cy - 0.5 * Ly, h->chk.cx + 0.5 * Lx, h->chk.cy + 0.5 * Ly);
   TRY(fit_interior(h, r));
   TRY(host_call_begin(h));
@@ -306,11 +320,11 @@ int artp_api::roadmap_solve(Handle* h, const double* start, const double* goal, 
   artp_roadmap_solve_info out{};
   out.path_vertices = info ? info->path_vertices : nullptr;
   double xy[4];   // (x, y) of start and goal
-  if (d_sg) {      // the device's verdict (endpoint_check) and the (x, y) that size the interior-state buffer
+  if (d_sg) {      // the device's verdict (endpoint_check_kernel) and the (x, y) that size the interior-state buffer
     double* d_chk;
     double chk[5];
     TRY(host_call_begin(h, {sizeof(chk)}, (char**)&d_chk));
-    TRY(endpoint_check(h, d_sg, space, d_chk, h->stream));
+    TRY(launch(h, endpoint_check_kernel, 1, 1, 0, h->stream, d_sg, *space, d_chk));
     TRY(copy_async(h, chk, d_chk, sizeof(chk), cudaMemcpyDeviceToHost, h->stream));
     TRY(host_call_end(h));
     if (chk[0] == -1.0) { h->err = "non-finite start or goal"; return ARTP_E_INVALID; }

@@ -60,14 +60,14 @@ Sampling& sampling(Handle* h) {
   if (!h->sampling) h->sampling = new Sampling();
   return *h->sampling;
 }
-Layers sampler_layers(Handle* h) { return {sampling(h).samp_layers.p, (size_t)h->rows * h->cols}; }
+Layers sampler_layers(Handle* h) { return {sampling(h).samp_layers.p, (size_t)h->map.rows * h->map.cols}; }
 
 // ---------------------------------------------------------------------------------------------------------------
 // Sampler: SE3FromSE2Sampler::sampleUniform on the device (artp_sampler.cuh)
 // ---------------------------------------------------------------------------------------------------------------
 int ensure_sampler_layers(Handle* h) {
   Sampling& S = sampling(h);
-  const size_t need = samp_layers_floats(h->rows, h->cols);
+  const size_t need = samp_layers_floats(h->map.rows, h->map.cols);
   if (S.samp_layers.cap < need)   // the layers computed on the device go with the old buffer
     S.map.has_device_normals = S.map.has_device_cdf = S.map.has_normals = false;
   return grow(h, S.samp_layers.p, S.samp_layers.cap, need);
@@ -76,18 +76,18 @@ int ensure_sampler_layers(Handle* h) {
 // The map fields of the sampler's view (geometry, elevation, the normal-plane layers).
 void sampler_map_view(Handle* h, artp::SamplerDev& m) {
   const Layers L = sampler_layers(h);
-  m.elevation_rev = h->d_H[0]; m.pitch = h->pitch;
+  m.elevation_rev = h->map.H[0]; m.pitch = h->map.pitch;
   m.normal_x = L[kNormalX]; m.normal_y = L[kNormalY]; m.normal_z = L[kNormalZ]; m.std_dev = L[kStdDev];
-  m.rows = h->rows; m.cols = h->cols;
-  m.res = h->chk.Lx / h->rows; m.cx = h->chk.cx; m.cy = h->chk.cy;
+  m.rows = h->map.rows; m.cols = h->map.cols;
+  m.res = h->chk.Lx / h->map.rows; m.cx = h->chk.cx; m.cy = h->chk.cy;
 }
 
 // computeCumulativeProbabilityDistribution of a device-resident probability layer into cum_prob / cum_row
 // (ensure_sampler_layers first). Two launches on s.
 int launch_sample_cdf(Handle* h, const float* d_prob, cudaStream_t s) {
   const Layers L = sampler_layers(h);
-  TRY(launch(h, artp::cdf_rows_kernel, (h->rows + 63) / 64, 64, 0, s, d_prob, h->rows, h->cols, L[kCumProb], L[kCumRow]));
-  return launch(h, artp::cdf_rowwise_kernel, 1, 32, 0, s, L[kCumRow], h->rows);
+  TRY(launch(h, artp::cdf_rows_kernel, (h->map.rows + 63) / 64, 64, 0, s, d_prob, h->map.rows, h->map.cols, L[kCumProb], L[kCumRow]));
+  return launch(h, artp::cdf_rowwise_kernel, 1, 32, 0, s, L[kCumRow], h->map.rows);
 }
 
 // running total += chunk count (device-side, stream ordered)
@@ -189,7 +189,7 @@ int heading_args(Handle* h, const double* yaw, int n_yaw, const uint32_t* mask, 
 // The layer of the current map into d_mask (rows x cols words) on s, in chunks of whole cells of at most kSampleChunk
 // poses each; arguments checked by heading_args.
 int valid_heading_layer(Handle* h, const artp::Headings& hd, uint32_t* d_mask, cudaStream_t s) {
-  const size_t ncell = (size_t)h->rows * h->cols;
+  const size_t ncell = (size_t)h->map.rows * h->map.cols;
   const size_t chunk_cells = std::min(ncell, kSampleChunk / hd.n);
   char* r[2];   // states f32 | verdicts
   Buf<char>& scratch = sampling(h).samp_scratch;
@@ -222,7 +222,7 @@ int box_layer_args(Handle* h, double yaw, const uint16_t* out, artp::Headings* h
 // The layer of the current map into d_out (rows x cols words) on s: one pose per cell, cell-major as the layer, in
 // chunks of at most kSampleChunk cells, each chunk's words written in place; arguments checked by box_layer_args.
 int box_verdict_layer(Handle* h, const artp::Headings& hd, uint16_t* d_out, cudaStream_t s) {
-  const size_t ncell = (size_t)h->rows * h->cols;
+  const size_t ncell = (size_t)h->map.rows * h->map.cols;
   const size_t chunk = std::min(ncell, kSampleChunk);
   char* r[1];   // states f32
   Buf<char>& scratch = sampling(h).samp_scratch;
@@ -344,7 +344,7 @@ int distribution_args(Handle* h, const artp_sample_distribution_params* dp, Blur
     if (!(dp->density_blur_radius > 0.0 && std::isfinite(dp->density_blur_radius))) {
       h->err = "density_blur_radius must be finite and > 0"; return ARTP_E_INVALID;
     }
-    TRY(blur_size(h, dp->density_blur_radius, h->res, blur));
+    TRY(blur_size(h, dp->density_blur_radius, h->map.res, blur));
   }
   if (dp->use_max_prob_unknown_samples) {
     if (!(dp->max_prob_unknown_samples >= 0.0 && dp->max_prob_unknown_samples <= 1.0)) {
@@ -363,7 +363,7 @@ int update_distribution(Handle* h, const artp_sample_distribution_params* dp, co
                         cudaStream_t s, float** d_prob = nullptr) {
   TRY(ensure_sampler_layers(h));
   Sampling& S = sampling(h);
-  const int rows = h->rows, cols = h->cols;
+  const int rows = h->map.rows, cols = h->map.cols;
   const size_t ncell = (size_t)rows * cols, lb = ncell * sizeof(float), rb = (size_t)rows * sizeof(double);
   char* r[7];   // n_samples | blur pass | sample_probability | known row sums | unknown row sums | max bits | cap multipliers
   TRY(carve(h, S.dist_scratch.p, S.dist_scratch.cap, {lb, lb, lb, rb, rb, sizeof(unsigned int), 2 * sizeof(float)}, r));
@@ -407,9 +407,9 @@ int update_distribution(Handle* h, const artp_sample_distribution_params* dp, co
 // basic_fits: the last Basic ran on a map of this size.
 int sample_filter(Handle* h, const float* d_thr, const float* observed, bool basic_fits, cudaStream_t s) {
   FilterElements f;
-  TRY(sample_filter_sizes(h, h->res, &f));
+  TRY(sample_filter_sizes(h, h->map.res, &f));
   Sampling& S = sampling(h);
-  const int rows = h->rows, cols = h->cols;
+  const int rows = h->map.rows, cols = h->map.cols;
   const bool basic_observed = !observed && basic_fits && S.has_basic_observed;
   const size_t n = (size_t)rows * cols, lb = n * sizeof(float);
   char* r[2];   // dilated | closed
@@ -484,10 +484,10 @@ int artp_api::sampler_armed(Handle* h) {
 int artp_api::estimate_normals(Handle* h, double estimation_radius, cudaStream_t s) {
   TRY(ensure_sampler_layers(h));
   const Layers L = sampler_layers(h);
-  const double res = h->chk.Lx / h->rows;
+  const double res = h->chk.Lx / h->map.rows;
   const int r_cells = (int)(estimation_radius / res), r_diag = (int)(estimation_radius * 0.70710678118 / res);   // utils.cpp:226-227
-  TRY(launch(h, artp::estimate_normals_kernel, grid_for(h, L.ncell, 128, 32), 128, 0, s, h->d_H[0], h->pitch, h->rows,
-      h->cols, res, h->chk.cx, h->chk.cy, r_cells, r_diag, L[kNormalX], L[kNormalY], L[kNormalZ], L[kStdDev]));
+  TRY(launch(h, artp::estimate_normals_kernel, grid_for(h, L.ncell, 128, 32), 128, 0, s, h->map.H[0], h->map.pitch, h->map.rows,
+      h->map.cols, res, h->chk.cx, h->chk.cy, r_cells, r_diag, L[kNormalX], L[kNormalY], L[kNormalZ], L[kStdDev]));
   Sampling::MapFlags& f = sampling(h).map;
   f.has_device_normals = f.has_normals = true;
   f.has_sampler = false;      // the sampler must be (re)armed with artp_set_sampler
@@ -590,7 +590,7 @@ int artp_compute_sample_cdf(artp_handle* hh, const float* sample_probability, fl
   LOCK_CALL(h, hh);
   TRY(require_whole_map(h));
   if (!sample_probability) return null_buffer(h);
-  const size_t ncell = (size_t)h->rows * h->cols;
+  const size_t ncell = (size_t)h->map.rows * h->map.cols;
   char* d_prob;
   TRY(host_call_begin(h, {ncell * sizeof(float)}, &d_prob));
   TRY(ensure_sampler_layers(h));
@@ -599,7 +599,7 @@ int artp_compute_sample_cdf(artp_handle* hh, const float* sample_probability, fl
   TRY(launch_sample_cdf(h, (const float*)d_prob, h->stream));
   if (cum_prob) CU_TRY(h, cudaMemcpyAsync(cum_prob, L[kCumProb], ncell * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
   if (cum_prob_rowwise)
-    CU_TRY(h, cudaMemcpyAsync(cum_prob_rowwise, L[kCumRow], (size_t)h->rows * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(h, cudaMemcpyAsync(cum_prob_rowwise, L[kCumRow], (size_t)h->map.rows * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
   TRY(host_call_end(h));
   sampling(h).map.has_device_cdf = true;
   sampling(h).map.has_sampler = false;      // the sampler must be (re)armed with artp_set_sampler
@@ -643,16 +643,16 @@ int artp_set_sampler(artp_handle* hh, const artp_sampler_params* sp, const float
   if (sp->sample_from_distribution) {
     if (host_cdf) {
       CU_TRY(h, cudaMemcpyAsync(L[kCumProb], cum_prob, L.ncell * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-      CU_TRY(h, cudaMemcpyAsync(L[kCumRow], cum_prob_rowwise, (size_t)h->rows * sizeof(float), cudaMemcpyHostToDevice,
+      CU_TRY(h, cudaMemcpyAsync(L[kCumRow], cum_prob_rowwise, (size_t)h->map.rows * sizeof(float), cudaMemcpyHostToDevice,
                                 h->stream));
       S.map.has_device_cdf = false;   // overwritten by the caller's layers
     }
     // the binary searches need monotone (or all-NaN) CDF rows: refuse anything else
     uint32_t* d_bad = (uint32_t*)d_bad_word;
     CU_TRY(h, cudaMemsetAsync(d_bad, 0, sizeof(uint32_t), h->stream));
-    TRY(launch(h, artp::validate_cdf_kernel, (h->rows + 127) / 128, 128, 0, h->stream, L[kCumProb], h->rows, h->cols,
-        (size_t)h->rows, 1, d_bad));
-    TRY(launch(h, artp::validate_cdf_kernel, 1, 32, 0, h->stream, L[kCumRow], 1, h->rows, 1, 0, d_bad));
+    TRY(launch(h, artp::validate_cdf_kernel, (h->map.rows + 127) / 128, 128, 0, h->stream, L[kCumProb], h->map.rows, h->map.cols,
+        (size_t)h->map.rows, 1, d_bad));
+    TRY(launch(h, artp::validate_cdf_kernel, 1, 32, 0, h->stream, L[kCumRow], 1, h->map.rows, 1, 0, d_bad));
     CU_TRY(h, cudaMemcpyAsync(&bad, d_bad, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
   }
   TRY(host_call_end(h));
@@ -800,7 +800,7 @@ int artp_valid_heading_layer(artp_handle* hh, const double* yaw, int n_yaw, uint
   LOCK_CALL(h, hh);
   artp::Headings hd;
   TRY(heading_args(h, yaw, n_yaw, mask, &hd));
-  const size_t bytes = (size_t)h->rows * h->cols * sizeof(uint32_t);
+  const size_t bytes = (size_t)h->map.rows * h->map.cols * sizeof(uint32_t);
   char* d_mask;
   TRY(host_call_begin(h, {bytes}, &d_mask));
   TRY(valid_heading_layer(h, hd, (uint32_t*)d_mask, h->stream));
@@ -823,7 +823,7 @@ int artp_box_verdict_layer(artp_handle* hh, double yaw, uint16_t* out) {
   LOCK_CALL(h, hh);
   artp::Headings hd;
   TRY(box_layer_args(h, yaw, out, &hd));
-  const size_t bytes = (size_t)h->rows * h->cols * sizeof(uint16_t);
+  const size_t bytes = (size_t)h->map.rows * h->map.cols * sizeof(uint16_t);
   char* d_out;
   TRY(host_call_begin(h, {bytes}, &d_out));
   TRY(box_verdict_layer(h, hd, (uint16_t*)d_out, h->stream));
@@ -875,14 +875,14 @@ int artp_set_sample_filter(artp_handle* hh, const float* traversability_threshol
                            float* traversability_sample_filter) {
   LOCK_CALL(h, hh);
   TRY(require_whole_map(h));
-  const int rows = h->rows, cols = h->cols;
+  const int rows = h->map.rows, cols = h->map.cols;
   const Sampling& S = sampling(h);
   const bool basic_fits = S.has_basic_layers && S.basic_rows == rows && S.basic_cols == cols;
   if (!traversability_thresholded && !basic_fits) {
     h->err = "no traversability_thresholded layer: pass it, or run artp_process_basic on a map of this size first";
     return ARTP_E_INVALID;
   }
-  TRY(sample_filter_sizes(h, h->res));
+  TRY(sample_filter_sizes(h, h->map.res));
   const size_t n = (size_t)rows * cols, lb = n * sizeof(float);
   char* r[1];   // caller's traversability_thresholded
   TRY(host_call_begin(h, {lb}, r));
@@ -919,7 +919,7 @@ int artp_update_sample_distribution(artp_handle* hh, const artp_sample_distribut
   Blur blur;
   TRY(distribution_args(h, dp, &blur));
   if (n && !vertex_states) return null_buffer(h);
-  const size_t sb = n * 7 * sizeof(double), ncell = (size_t)h->rows * h->cols;
+  const size_t sb = n * 7 * sizeof(double), ncell = (size_t)h->map.rows * h->map.cols;
   char* r[1];
   TRY(host_call_begin(h, {sb}, r));
   if (n) CU_TRY(h, cudaMemcpyAsync(r[0], vertex_states, sb, cudaMemcpyHostToDevice, h->stream));
@@ -930,7 +930,7 @@ int artp_update_sample_distribution(artp_handle* hh, const artp_sample_distribut
   const Layers L = sampler_layers(h);
   if (cum_prob) CU_TRY(h, cudaMemcpyAsync(cum_prob, L[kCumProb], ncell * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
   if (cum_prob_rowwise)
-    CU_TRY(h, cudaMemcpyAsync(cum_prob_rowwise, L[kCumRow], (size_t)h->rows * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(h, cudaMemcpyAsync(cum_prob_rowwise, L[kCumRow], (size_t)h->map.rows * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
   return host_call_end(h);
 }
 

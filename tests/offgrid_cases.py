@@ -109,7 +109,7 @@ def se3_bounds(m, reach_z):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# The classify stage's path choice, restated (artp_kernels.cuh zone_classify, artp_capi.cu artp_set_map_window)
+# The classify stage's path choice, restated (artp_kernels.cuh zone_classify, artp_map.cu artp_set_map_window)
 # ---------------------------------------------------------------------------------------------------------------------
 K_MAX_LEVEL = 6
 

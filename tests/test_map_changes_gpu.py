@@ -29,7 +29,7 @@ KB = 1024
 STATE_TOL = 1e-9        # roadmap interpolation: CUDA vs numpy sin / cos / acos of the slerp; vertex kinds and edges are exact
 
 
-# ---- the per-map launch shapes, restated from upload_map and set_shapes (artp_capi.cu) ----------------------------------
+# ---- the per-map launch shapes, restated from upload_map (artp_map.cu) and set_shapes (artp_capi.cu) -------------------
 @dataclasses.dataclass
 class Tile:
     tw: int
