@@ -500,12 +500,7 @@ int check_poses(Handle* h, const T* states, size_t n, uint8_t* valid, bool on_de
   TRY(check_common(h, n));
   if (n == 0) return ARTP_OK;
   if (!states || !valid) return null_buffer(h);
-  if (on_device) {
-    CU_TRY(h, cudaSetDevice(h->device));
-    ChainScope cs(h, 0, stream);
-    if (cs.rc) return cs.rc;
-    return check_states(h, states, n, valid, stream);
-  }
+  if (on_device) return device_call(h, stream, [&](cudaStream_t s) { return check_states(h, states, n, valid, s); });
   if (n <= (size_t)artp::kSmallBatch && !h->pipe->timing) {
     artp::SmallBatch sb;
     for (size_t i = 0; i < n * 7; ++i) (&sb.s[0][0])[i] = (double)states[i];   // exact; a float state is cast back in the kernel
@@ -553,17 +548,15 @@ int check_items_prefix(Handle* h, const double* d_s1, const double* d_s2, size_t
     return null_buffer(h);
   }
   if (n >= 0xFFFFFFFFull) { h->err = "too many edges"; return ARTP_E_INVALID; }
-  CU_TRY(h, cudaSetDevice(h->device));
-  cudaStream_t s = (cudaStream_t)stream;
-  ChainScope cs(h, 0, s);
-  if (cs.rc) return cs.rc;
-  if (total_items) {
-    artp::Work w;
-    w.s1 = d_s1; w.s2 = d_s2; w.valid = d_item_valid; w.n_items = (uint32_t)total_items;
-    w.item_off = d_item_off; w.n_edges = (uint32_t)n; w.quotient = quotient;
-    TRY(run_items(h, w, s));
-  }
-  return launch(h, edge_prefix_kernel, grid_for(h, n, 256, 8), 256, 0, s, d_item_valid, d_item_off, n, d_valid_prefix);
+  return device_call(h, stream, [&](cudaStream_t s) {
+    if (total_items) {
+      artp::Work w;
+      w.s1 = d_s1; w.s2 = d_s2; w.valid = d_item_valid; w.n_items = (uint32_t)total_items;
+      w.item_off = d_item_off; w.n_edges = (uint32_t)n; w.quotient = quotient;
+      TRY(run_items(h, w, s));
+    }
+    return launch(h, edge_prefix_kernel, grid_for(h, n, 256, 8), 256, 0, s, d_item_valid, d_item_off, n, d_valid_prefix);
+  });
 }
 
 // check_items_prefix over host buffers: the n = off.size() - 1 edges (s1[e], s2[e]) with their item offsets `off`;
@@ -944,11 +937,7 @@ int artp_box_verdicts_device(artp_handle* hh, const double* d_states, size_t n, 
   TRY(box_verdict_args(h, n));
   if (n == 0) return ARTP_OK;
   if (!d_states || !d_why) return null_buffer(h);
-  CU_TRY(h, cudaSetDevice(h->device));
-  cudaStream_t s = (cudaStream_t)stream;
-  ChainScope cs(h, 0, s);
-  if (cs.rc) return cs.rc;
-  return box_verdicts_on(h, d_states, n, d_why, s);
+  return device_call(h, stream, [&](cudaStream_t s) { return box_verdicts_on(h, d_states, n, d_why, s); });
 }
 
 int artp_check_motions_device(artp_handle* hh, const double* d_s1, const double* d_s2, size_t n, int n_steps,
@@ -957,11 +946,7 @@ int artp_check_motions_device(artp_handle* hh, const double* d_s1, const double*
   TRY(motion_items(h, n, n_steps));
   if (n == 0) return ARTP_OK;
   if (!d_s1 || !d_s2 || !d_valid) return null_buffer(h);
-  CU_TRY(h, cudaSetDevice(h->device));
-  cudaStream_t s = (cudaStream_t)stream;
-  ChainScope cs(h, 0, s);
-  if (cs.rc) return cs.rc;
-  return check_motions_on(h, d_s1, d_s2, n, n_steps, d_valid, s);
+  return device_call(h, stream, [&](cudaStream_t s) { return check_motions_on(h, d_s1, d_s2, n, n_steps, d_valid, s); });
 }
 
 int artp_check_motions(artp_handle* hh, const double* s1, const double* s2, size_t n, int n_steps, uint8_t* valid) {

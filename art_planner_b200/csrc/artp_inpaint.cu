@@ -78,6 +78,44 @@ int march(Handle* h, int H, int W, cudaStream_t s, Prep prep, Finish finish) {
   return rc;
 }
 
+// The body both forms of an entry point share, on s: scan the rows x cols layer d_in into the words at d_w (64 bytes of
+// device memory), read them back (one synchronisation of s), then refuse the layer or run the work. A host-buffer call
+// (host_call) ends (host_call_end) before it returns a refusal; on an error it returns at once.
+int inpaint_body(Handle* h, const float* d_in, int rows, int cols, uint32_t* d_mm, float* d_out, cudaStream_t s,
+                 bool host_call) {
+  TRY(finite_min_max(h, d_in, (size_t)rows * cols, d_mm, s));
+  uint32_t mm[3];
+  TRY(copy_async(h, mm, d_mm, sizeof(mm), cudaMemcpyDeviceToHost, s));
+  TRY(sync_stream(h, s));
+  if (!mm[2]) { if (host_call) host_call_end(h); h->err = "inpaint: the layer has no finite cell"; return ARTP_E_INVALID; }
+  return inpaint_layer(h, d_in, rows, cols, d_mm, d_out, s);
+}
+
+// The cost-map pairs' scan, read-back and verdict (cost_map_verdict) into w.
+int cost_map_check(Handle* h, const float* d_in, int rows, int cols, uint32_t* d_w, uint32_t (&w)[kCostMapWords],
+                   cudaStream_t s, bool host_call) {
+  TRY(cost_map_scan(h, d_in, (size_t)rows * cols, d_w, s));
+  TRY(copy_async(h, w, d_w, sizeof(w), cudaMemcpyDeviceToHost, s));
+  TRY(sync_stream(h, s));
+  const int rc = cost_map_verdict(h, w);
+  if (rc && host_call) host_call_end(h);
+  return rc;
+}
+
+int cost_map_body(Handle* h, const float* d_in, int rows, int cols, uint32_t* d_w, float* d_out, cudaStream_t s,
+                  bool host_call) {
+  uint32_t w[kCostMapWords];
+  TRY(cost_map_check(h, d_in, rows, cols, d_w, w, s, host_call));
+  return cost_map_layer(h, d_in, rows, cols, d_w, w[3] != 0, false, d_out, s);
+}
+
+int features_raw_body(Handle* h, const float* d_in, int rows, int cols, uint32_t* d_w, double res, double cx, double cy,
+                      cudaStream_t s, bool host_call) {
+  uint32_t w[kCostMapWords];
+  TRY(cost_map_check(h, d_in, rows, cols, d_w, w, s, host_call));
+  return cost_map_features(h, d_in, rows, cols, d_w, w[3] != 0, res, cx, cy, s);
+}
+
 }  // namespace
 
 // The march on a layer whose finite min / max keys (finite_min_max) are at d_mm, on the cols x rows image.
@@ -136,17 +174,10 @@ int artp_inpaint_layer(artp_handle* hh, const float* layer, int rows, int cols, 
   const size_t n = (size_t)rows * cols, lb = n * sizeof(float);
   char* r[3];
   TRY(host_call_begin(h, {lb, lb, 64}, r));
-  cudaStream_t s = h->stream;
   float *d_in = (float*)r[0], *d_out = (float*)r[1];
-  uint32_t* d_mm = (uint32_t*)r[2];
-  TRY(copy_async(h, d_in, layer, lb, cudaMemcpyHostToDevice, s));
-  TRY(finite_min_max(h, d_in, n, d_mm, s));
-  uint32_t mm[3];
-  TRY(copy_async(h, mm, d_mm, sizeof(mm), cudaMemcpyDeviceToHost, s));
-  TRY(sync_stream(h, s));
-  if (!mm[2]) { host_call_end(h); h->err = "inpaint: the layer has no finite cell"; return ARTP_E_INVALID; }
-  TRY(inpaint_layer(h, d_in, rows, cols, d_mm, d_out, s));
-  TRY(copy_async(h, out, d_out, lb, cudaMemcpyDeviceToHost, s));
+  TRY(copy_async(h, d_in, layer, lb, cudaMemcpyHostToDevice, h->stream));
+  TRY(inpaint_body(h, d_in, rows, cols, (uint32_t*)r[2], d_out, h->stream, true));
+  TRY(copy_async(h, out, d_out, lb, cudaMemcpyDeviceToHost, h->stream));
   return host_call_end(h);
 }
 
@@ -155,15 +186,9 @@ int artp_inpaint_layer_device(artp_handle* hh, const float* d_layer, int rows, i
   TRY(inpaint_args(h, d_layer, rows, cols, d_out));
   CU_TRY(h, cudaSetDevice(h->device));
   cudaStream_t s = (cudaStream_t)stream;
-  const size_t n = (size_t)rows * cols;
   uint32_t* d_mm = nullptr;
   CU_TRY(h, cudaMallocAsync(reinterpret_cast<void**>(&d_mm), 64, s));
-  int rc = finite_min_max(h, d_layer, n, d_mm, s);
-  uint32_t mm[3] = {0, 0, 0};
-  if (rc == ARTP_OK) rc = copy_async(h, mm, d_mm, sizeof(mm), cudaMemcpyDeviceToHost, s);
-  if (rc == ARTP_OK) rc = sync_stream(h, s);
-  if (rc == ARTP_OK && !mm[2]) { h->err = "inpaint: the layer has no finite cell"; rc = ARTP_E_INVALID; }
-  if (rc == ARTP_OK) rc = inpaint_layer(h, d_layer, rows, cols, d_mm, d_out, s);
+  const int rc = inpaint_body(h, d_layer, rows, cols, d_mm, d_out, s, false);
   cudaFreeAsync(d_mm, s);
   return rc;
 }
@@ -174,17 +199,10 @@ int artp_cost_map_layer(artp_handle* hh, const float* raw, int rows, int cols, f
   const size_t n = (size_t)rows * cols, lb = n * sizeof(float);
   char* r[3];
   TRY(host_call_begin(h, {lb, lb, 64}, r));
-  cudaStream_t s = h->stream;
   float *d_in = (float*)r[0], *d_out = (float*)r[1];
-  uint32_t* d_w = (uint32_t*)r[2];
-  TRY(copy_async(h, d_in, raw, lb, cudaMemcpyHostToDevice, s));
-  TRY(cost_map_scan(h, d_in, n, d_w, s));
-  uint32_t w[kCostMapWords];
-  TRY(copy_async(h, w, d_w, sizeof(w), cudaMemcpyDeviceToHost, s));
-  TRY(sync_stream(h, s));
-  if (const int rc = cost_map_verdict(h, w)) { host_call_end(h); return rc; }
-  TRY(cost_map_layer(h, d_in, rows, cols, d_w, w[3] != 0, false, d_out, s));
-  TRY(copy_async(h, out, d_out, lb, cudaMemcpyDeviceToHost, s));
+  TRY(copy_async(h, d_in, raw, lb, cudaMemcpyHostToDevice, h->stream));
+  TRY(cost_map_body(h, d_in, rows, cols, (uint32_t*)r[2], d_out, h->stream, true));
+  TRY(copy_async(h, out, d_out, lb, cudaMemcpyDeviceToHost, h->stream));
   return host_call_end(h);
 }
 
@@ -195,12 +213,7 @@ int artp_cost_map_layer_device(artp_handle* hh, const float* d_raw, int rows, in
   cudaStream_t s = (cudaStream_t)stream;
   uint32_t* d_w = nullptr;
   CU_TRY(h, cudaMallocAsync(reinterpret_cast<void**>(&d_w), 64, s));
-  int rc = cost_map_scan(h, d_raw, (size_t)rows * cols, d_w, s);
-  uint32_t w[kCostMapWords] = {};
-  if (rc == ARTP_OK) rc = copy_async(h, w, d_w, sizeof(w), cudaMemcpyDeviceToHost, s);
-  if (rc == ARTP_OK) rc = sync_stream(h, s);
-  if (rc == ARTP_OK) rc = cost_map_verdict(h, w);
-  if (rc == ARTP_OK) rc = cost_map_layer(h, d_raw, rows, cols, d_w, w[3] != 0, false, d_out, s);
+  const int rc = cost_map_body(h, d_raw, rows, cols, d_w, d_out, s, false);
   cudaFreeAsync(d_w, s);
   return rc;
 }
@@ -211,16 +224,9 @@ int artp_update_features_raw(artp_handle* hh, const float* raw, int rows, int co
   const size_t n = (size_t)rows * cols, lb = n * sizeof(float);
   char* r[2];
   TRY(host_call_begin(h, {lb, 64}, r));
-  cudaStream_t s = h->stream;
   float* d_in = (float*)r[0];
-  uint32_t* d_w = (uint32_t*)r[1];
-  TRY(copy_async(h, d_in, raw, lb, cudaMemcpyHostToDevice, s));
-  TRY(cost_map_scan(h, d_in, n, d_w, s));
-  uint32_t w[kCostMapWords];
-  TRY(copy_async(h, w, d_w, sizeof(w), cudaMemcpyDeviceToHost, s));
-  TRY(sync_stream(h, s));
-  if (const int rc = cost_map_verdict(h, w)) { host_call_end(h); return rc; }
-  TRY(cost_map_features(h, d_in, rows, cols, d_w, w[3] != 0, res, cx, cy, s));
+  TRY(copy_async(h, d_in, raw, lb, cudaMemcpyHostToDevice, h->stream));
+  TRY(features_raw_body(h, d_in, rows, cols, (uint32_t*)r[1], res, cx, cy, h->stream, true));
   return host_call_end(h);
 }
 
@@ -232,12 +238,7 @@ int artp_update_features_raw_device(artp_handle* hh, const float* d_raw, int row
   cudaStream_t s = (cudaStream_t)stream;
   uint32_t* d_w = nullptr;
   CU_TRY(h, cudaMallocAsync(reinterpret_cast<void**>(&d_w), 64, s));
-  int rc = cost_map_scan(h, d_raw, (size_t)rows * cols, d_w, s);
-  uint32_t w[kCostMapWords] = {};
-  if (rc == ARTP_OK) rc = copy_async(h, w, d_w, sizeof(w), cudaMemcpyDeviceToHost, s);
-  if (rc == ARTP_OK) rc = sync_stream(h, s);
-  if (rc == ARTP_OK) rc = cost_map_verdict(h, w);
-  if (rc == ARTP_OK) rc = cost_map_features(h, d_raw, rows, cols, d_w, w[3] != 0, res, cx, cy, s);
+  const int rc = features_raw_body(h, d_raw, rows, cols, d_w, res, cx, cy, s, false);
   cudaFreeAsync(d_w, s);
   return rc;
 }

@@ -237,6 +237,15 @@ inline int host_call_end(Handle* h, bool pipeline = false) {
   h->chain_busy[0] = false;
   return pipeline ? take_sticky_error(h) : ARTP_OK;
 }
+// Device-buffer calls that use scratch group 0 run on the caller's stream: device_call sets the device, then returns
+// run(s) on that stream s as the group's user (ChainScope, so the group's next user waits for run's work).
+template <class Run>
+int device_call(Handle* h, void* stream, Run run) {
+  CU_TRY(h, cudaSetDevice(h->device));
+  const cudaStream_t s = (cudaStream_t)stream;
+  const ChainScope cs(h, 0, s);
+  return cs.rc ? cs.rc : run(s);
+}
 
 // Functions one unit calls in another, by the unit that defines them. A function named after an entry point is that entry
 // point's body without the lock; artp_planner_set_map and artp_plan chain them.

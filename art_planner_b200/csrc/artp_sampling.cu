@@ -82,12 +82,29 @@ void sampler_map_view(Handle* h, artp::SamplerDev& m) {
   m.res = h->chk.Lx / h->map.rows; m.cx = h->chk.cx; m.cy = h->chk.cy;
 }
 
+// The armed sampler's states of draws first_sample .. first_sample + n - 1 on s (artp_sampler.cuh: d_u, d_states_f32
+// and d_rowcol are nullable).
+int sample_states(Handle* h, const double* d_u, uint64_t seed, uint64_t first_sample, size_t n, double* d_states,
+                  float* d_states_f32, int32_t* d_rowcol, cudaStream_t s) {
+  return launch(h, artp::sample_states_kernel, grid_for(h, n, 128), 128, 0, s, sampling(h).samp, d_u, seed, first_sample, n,
+                d_states, d_states_f32, d_rowcol);
+}
+
 // computeCumulativeProbabilityDistribution of a device-resident probability layer into cum_prob / cum_row
 // (ensure_sampler_layers first). Two launches on s.
 int launch_sample_cdf(Handle* h, const float* d_prob, cudaStream_t s) {
   const Layers L = sampler_layers(h);
   TRY(launch(h, artp::cdf_rows_kernel, (h->map.rows + 63) / 64, 64, 0, s, d_prob, h->map.rows, h->map.cols, L[kCumProb], L[kCumRow]));
   return launch(h, artp::cdf_rowwise_kernel, 1, 32, 0, s, L[kCumRow], h->map.rows);
+}
+// cum_prob and cum_row to the HOST buffers cum_prob and cum_prob_rowwise (each nullable) on h->stream.
+int copy_cdf_out(Handle* h, float* cum_prob, float* cum_prob_rowwise) {
+  const Layers L = sampler_layers(h);
+  const size_t ncell = L.ncell;
+  if (cum_prob) CU_TRY(h, cudaMemcpyAsync(cum_prob, L[kCumProb], ncell * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  if (cum_prob_rowwise)
+    CU_TRY(h, cudaMemcpyAsync(cum_prob_rowwise, L[kCumRow], (size_t)h->map.rows * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  return ARTP_OK;
 }
 
 // running total += chunk count (device-side, stream ordered)
@@ -543,8 +560,7 @@ int artp_api::sample_valid_draws(Handle* h, uint64_t seed, uint64_t first_sample
   uint32_t* d_cnt = (uint32_t*)r[4];
   for (size_t done = 0; done < n_draw; done += chunk) {
     const size_t m = std::min(chunk, n_draw - done);
-    TRY(launch(h, artp::sample_states_kernel, grid_for(h, m, 128), 128, 0, s, S.samp, nullptr, seed, first_sample + done, m,
-        d_st, d_sf, nullptr));
+    TRY(sample_states(h, nullptr, seed, first_sample + done, m, d_st, d_sf, nullptr, s));
     TRY(check_states_f32(h, d_sf, m, d_val, s));
     // rejected (outside-map) candidates carry NaN states
     if (!S.samp.from_distribution) TRY(launch(h, artp::reject_nan_kernel, grid_for(h, m, 256), 256, 0, s, d_st, m, d_val));
@@ -594,12 +610,9 @@ int artp_compute_sample_cdf(artp_handle* hh, const float* sample_probability, fl
   char* d_prob;
   TRY(host_call_begin(h, {ncell * sizeof(float)}, &d_prob));
   TRY(ensure_sampler_layers(h));
-  const Layers L = sampler_layers(h);
   CU_TRY(h, cudaMemcpyAsync(d_prob, sample_probability, ncell * sizeof(float), cudaMemcpyHostToDevice, h->stream));
   TRY(launch_sample_cdf(h, (const float*)d_prob, h->stream));
-  if (cum_prob) CU_TRY(h, cudaMemcpyAsync(cum_prob, L[kCumProb], ncell * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  if (cum_prob_rowwise)
-    CU_TRY(h, cudaMemcpyAsync(cum_prob_rowwise, L[kCumRow], (size_t)h->map.rows * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  TRY(copy_cdf_out(h, cum_prob, cum_prob_rowwise));
   TRY(host_call_end(h));
   sampling(h).map.has_device_cdf = true;
   sampling(h).map.has_sampler = false;      // the sampler must be (re)armed with artp_set_sampler
@@ -679,8 +692,7 @@ int artp_sample_states_device(artp_handle* hh, const double* d_u, uint64_t seed,
   if (n == 0) return ARTP_OK;
   if (!d_states) return null_buffer(h);
   CU_TRY(h, cudaSetDevice(h->device));
-  return launch(h, artp::sample_states_kernel, grid_for(h, n, 128), 128, 0, (cudaStream_t)stream, sampling(h).samp, d_u, seed, first_sample, n,
-                d_states, nullptr, d_rowcol);
+  return sample_states(h, d_u, seed, first_sample, n, d_states, nullptr, d_rowcol, (cudaStream_t)stream);
 }
 
 int artp_sample_states(artp_handle* hh, const double* u, uint64_t seed, uint64_t first_sample, size_t n, double* states,
@@ -692,8 +704,8 @@ int artp_sample_states(artp_handle* hh, const double* u, uint64_t seed, uint64_t
   char* r[3];   // u | states | rowcol
   TRY(host_call_begin(h, {n * 6 * sizeof(double), n * 7 * sizeof(double), n * 2 * sizeof(int32_t)}, r));
   if (u) CU_TRY(h, cudaMemcpyAsync(r[0], u, n * 6 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-  TRY(launch(h, artp::sample_states_kernel, grid_for(h, n, 128), 128, 0, h->stream, sampling(h).samp, u ? (const double*)r[0] : nullptr,
-      seed, first_sample, n, (double*)r[1], nullptr, rowcol ? (int32_t*)r[2] : nullptr));
+  TRY(sample_states(h, u ? (const double*)r[0] : nullptr, seed, first_sample, n, (double*)r[1], nullptr,
+                    rowcol ? (int32_t*)r[2] : nullptr, h->stream));
   CU_TRY(h, cudaMemcpyAsync(states, r[1], n * 7 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   if (rowcol) CU_TRY(h, cudaMemcpyAsync(rowcol, r[2], n * 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream));
   return host_call_end(h);
@@ -704,11 +716,9 @@ int artp_sample_valid_device(artp_handle* hh, uint64_t seed, uint64_t first_samp
   LOCK_CALL(h, hh);
   TRY(sampler_armed(h));
   if (!d_count || (capacity && !d_states_out)) return null_buffer(h);
-  CU_TRY(h, cudaSetDevice(h->device));
-  cudaStream_t s = (cudaStream_t)stream;
-  ChainScope cs(h, 0, s);
-  if (cs.rc) return cs.rc;
-  return sample_valid_draws(h, seed, first_sample, n_draw, d_states_out, nullptr, capacity, d_count, s);
+  return device_call(h, stream, [&](cudaStream_t s) {
+    return sample_valid_draws(h, seed, first_sample, n_draw, d_states_out, nullptr, capacity, d_count, s);
+  });
 }
 
 int artp_sample_valid(artp_handle* hh, uint64_t seed, uint64_t first_sample, size_t n_draw, double* states, size_t capacity,
@@ -740,11 +750,9 @@ int artp_find_valid_near_device(artp_handle* hh, const double* d_centres, size_t
   TRY(ball_search_args(h, n, n_iter, nullptr));
   if (n == 0) return ARTP_OK;
   if (!d_centres || !d_radius || !d_states_out || !d_index) return null_buffer(h);
-  CU_TRY(h, cudaSetDevice(h->device));
-  cudaStream_t s = (cudaStream_t)stream;
-  ChainScope cs(h, 0, s);
-  if (cs.rc) return cs.rc;
-  return find_valid_near(h, d_centres, n, d_radius, n_iter, d_offsets, seed, first_draw, d_states_out, d_index, s);
+  return device_call(h, stream, [&](cudaStream_t s) {
+    return find_valid_near(h, d_centres, n, d_radius, n_iter, d_offsets, seed, first_draw, d_states_out, d_index, s);
+  });
 }
 
 int artp_find_valid_near(artp_handle* hh, const double* centres, size_t n, const double* radius, uint32_t n_iter,
@@ -812,11 +820,7 @@ int artp_valid_heading_layer_device(artp_handle* hh, const double* yaw, int n_ya
   LOCK_CALL(h, hh);
   artp::Headings hd;
   TRY(heading_args(h, yaw, n_yaw, d_mask, &hd));
-  CU_TRY(h, cudaSetDevice(h->device));
-  cudaStream_t s = (cudaStream_t)stream;
-  ChainScope cs(h, 0, s);
-  if (cs.rc) return cs.rc;
-  return valid_heading_layer(h, hd, d_mask, s);
+  return device_call(h, stream, [&](cudaStream_t s) { return valid_heading_layer(h, hd, d_mask, s); });
 }
 
 int artp_box_verdict_layer(artp_handle* hh, double yaw, uint16_t* out) {
@@ -835,11 +839,7 @@ int artp_box_verdict_layer_device(artp_handle* hh, double yaw, uint16_t* d_out, 
   LOCK_CALL(h, hh);
   artp::Headings hd;
   TRY(box_layer_args(h, yaw, d_out, &hd));
-  CU_TRY(h, cudaSetDevice(h->device));
-  cudaStream_t s = (cudaStream_t)stream;
-  ChainScope cs(h, 0, s);
-  if (cs.rc) return cs.rc;
-  return box_verdict_layer(h, hd, d_out, s);
+  return device_call(h, stream, [&](cudaStream_t s) { return box_verdict_layer(h, hd, d_out, s); });
 }
 
 int artp_debug_circular_kernel(int size, uint8_t* out) {   // test hook: the size x size element as 0 / 1 bytes (row-major)
@@ -906,11 +906,7 @@ int artp_update_sample_distribution_device(artp_handle* hh, const artp_sample_di
   Blur blur;
   TRY(distribution_args(h, dp, &blur));
   if (n && !d_vertex_states) return null_buffer(h);
-  CU_TRY(h, cudaSetDevice(h->device));
-  cudaStream_t s = (cudaStream_t)stream;
-  ChainScope cs(h, 0, s);
-  if (cs.rc) return cs.rc;
-  return update_distribution(h, dp, blur, d_vertex_states, n, s);
+  return device_call(h, stream, [&](cudaStream_t s) { return update_distribution(h, dp, blur, d_vertex_states, n, s); });
 }
 
 int artp_update_sample_distribution(artp_handle* hh, const artp_sample_distribution_params* dp, const double* vertex_states,
@@ -927,10 +923,7 @@ int artp_update_sample_distribution(artp_handle* hh, const artp_sample_distribut
   TRY(update_distribution(h, dp, blur, (const double*)r[0], n, h->stream, &d_prob));
   if (sample_probability)
     CU_TRY(h, cudaMemcpyAsync(sample_probability, d_prob, ncell * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  const Layers L = sampler_layers(h);
-  if (cum_prob) CU_TRY(h, cudaMemcpyAsync(cum_prob, L[kCumProb], ncell * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  if (cum_prob_rowwise)
-    CU_TRY(h, cudaMemcpyAsync(cum_prob_rowwise, L[kCumRow], (size_t)h->map.rows * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  TRY(copy_cdf_out(h, cum_prob, cum_prob_rowwise));
   return host_call_end(h);
 }
 
